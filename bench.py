@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- DSMIL aggregator forward throughput on B200 (BASELINE.json metric).
+"""bench.py -- DSMIL aggregator forward throughput on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 metric  : patches/sec of the DSMIL forward (MILNet.forward, dsmil.py:70-74) at N=10 000, D=512, C=2.
 step    : one pass over a stream of `--bags` synthetic bags (default 16 x 10 000 x 512 fp32 = 328 MB,
-          larger than the 126 MB L2, so every bag is read from HBM: "inputs larger than L2").
+          larger than the 50 MB L2, so every bag is read from HBM: "inputs larger than L2").
 N GPUs  : weak scaling -- every bag is a giant bag of 10 000*N rows row-sharded over the N ranks
           (each rank keeps 10 000 rows per bag); two NCCL all-gathers per step carry the per-class
           critical-instance candidates and the softmax/partial-sum records (SURVEY §8e).
@@ -21,6 +21,9 @@ extras  : torch_eager_gpu (the unmodified reference module through PyTorch eager
           to beat), single-call milnet(x) latency, N=8 192 forward, N=15 000 C=1 forward+backward+Adam
           (train_tcga.py:67-73), and the N=100 000 giant-bag STRONG-scaling workload (BASELINE configs 1,2,4).
 `--impl reference` times the reference's CPU implementation alone.
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step returned to its caller as
+          DIR/<name>.npy (float32; indices as float64; a fixed-seed row sample when the whole exceeds 64 MB).  The
+          inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import contextlib
@@ -95,7 +98,34 @@ def load_peaks():
     if os.path.exists(path):
         pk = json.load(open(path))
         return float(pk["hbm_gbs"]), float(pk.get("bf16_tflops", 1590.0)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, 989.0, "fallback (H100 SXM data sheet: HBM3, dense BF16)"
+
+
+def _named_arrays(out, prefix=""):
+    """(name, tensor) for every tensor of a step's result: forward_bags' packed outputs by their names, tuples and
+    lists by position."""
+    if hasattr(out, "packed"):
+        return list(zip(("classes", "prediction_bag", "A", "B"), out.packed))
+    if torch.is_tensor(out):
+        return [(prefix or "out", out)]
+    if isinstance(out, (tuple, list)):
+        return [item for i, o in enumerate(out) for item in _named_arrays(o, f"{prefix}{'_' if prefix else 'out'}{i}")]
+    return []
+
+
+def dump_outputs(out, outdir, budget=64 << 20):
+    """Writes the arrays the timed step returned to its caller as outdir/<name>.npy: floating point as float32,
+    integers (indices) as float64.  Arrays beyond an equal share of `budget` keep a fixed, seeded sample of rows."""
+    os.makedirs(outdir, exist_ok=True)
+    named = _named_arrays(out)
+    share = budget // max(len(named), 1)
+    for name, t in named:
+        a = t.detach().cpu().numpy()
+        a = a.astype(np.float32 if np.issubdtype(a.dtype, np.floating) else np.float64)
+        if a.nbytes > share and a.ndim > 0:
+            keep = max(1, share // max(a.nbytes // a.shape[0], 1))
+            a = a[np.sort(np.random.default_rng(0).choice(a.shape[0], keep, replace=False))]
+        np.save(os.path.join(outdir, name + ".npy"), a)
 
 
 def warmup_plan(world: int, warmup: int):
@@ -107,7 +137,7 @@ def warmup_plan(world: int, warmup: int):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -522,7 +552,7 @@ def run_ours(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py needs a CUDA device: the DSMIL B200 path has no CPU fallback")
+        raise RuntimeError("bench.py needs a CUDA device: the DSMIL H100 path has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -604,10 +634,13 @@ def run_ours(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     e0.record()
+    out = None
     for _ in range(args.steps):
-        step()
+        out = step()
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
     launches = int(lib.dsmil_launch_count() - l0)
     ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
     if world > 1:
@@ -629,7 +662,7 @@ def run_ours(args):
     n_tag = (ctypes.c_uint64 * 8)()
     lib.dsmil_profile_read(ms_tag, n_tag)
     lib.dsmil_profile_enable(0)
-    tags = ["scores", "q_mlp", "attend", "finalize", "fused_sm100"]
+    tags = ["scores", "q_mlp", "attend", "finalize", "fused_sm90"]
     per = {t: (ms_tag[i] / n_tag[i] if n_tag[i] else None) for i, t in enumerate(tags)}
     dom = max((t for t in tags if per[t]), key=lambda t: per[t] * n_tag[tags.index(t)])
     launches_dom = int(n_tag[tags.index(dom)])
@@ -638,12 +671,6 @@ def run_ours(args):
     dom_ms = per[dom]
     achieved = alg_step / (ms_per_step / 1e3) / 1e9     # whole forward: every kernel and gap of the step is charged
     traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if os.path.exists(tpath):     # dram__bytes_read+write of the step's kernels from the committed ncu --set full capture
-        tj = json.load(open(tpath))
-        traffic = tj.get("dram_bytes_per_step_16x10k")
-        if traffic is not None and nb != 16:
-            traffic = traffic * nb / 16.0
     tflops = tensor_flops_fwd(NBAG * nb, D) / (ms_per_step / 1e3) / 1e12
     roofline = {"bound": "hbm", "kernel": "whole forward step (all kernels of forward_bags)", "achieved": achieved,
                 "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak, "traffic": traffic,
@@ -882,7 +909,7 @@ def run_ours(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--bags", type=int, default=16, help="bags per step (16 x 20.5 MB > L2)")
@@ -892,7 +919,11 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip the extra workloads (eager-GPU baseline, N=8192, "
                     "N=15000 training step, N=100k strong scaling, multi-rank parity check)")
     ap.add_argument("--giant-bags", type=int, default=32, help="N=100 000 bags per step of the strong-scaling workload")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,4 +1,4 @@
-"""dsmil_wsi_b200 -- B200-native DSMIL aggregator hot path (see DESIGN.md).
+"""dsmil_wsi_b200 -- H100-native DSMIL aggregator hot path (see DESIGN.md).
 
 Public surface == the reference's dsmil.py: FCLayer, IClassifier, BClassifier, MILNet.
 """

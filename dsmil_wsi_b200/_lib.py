@@ -45,7 +45,6 @@ SIGNATURES = {
                                           C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, c_i64, C.c_void_p]),
     "dsmil_profile_enable": (C.c_int, [C.c_int]),
     "dsmil_profile_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),
-    "dsmil_debug_set_trace": (C.c_int, [C.c_void_p]),
     "dsmil_forward_path": (C.c_int, [C.POINTER(DsmilParams), c_i64]),
     "dsmil_forward_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), c_i64]),
     "dsmil_forward": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, c_i64,
@@ -111,7 +110,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"libdsmil_b200.so not found at {LIB_PATH}. Build it with `python -m dsmil_wsi_b200.build` "
-            "(nvcc, sm_100a). There is no CPU or PyTorch fallback for the DSMIL hot path.")
+            "(nvcc, sm_90a). There is no CPU or PyTorch fallback for the DSMIL hot path.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the header and the library disagree

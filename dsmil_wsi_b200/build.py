@@ -1,4 +1,4 @@
-"""Builds libdsmil_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo).
+"""Builds libdsmil_b200.so in-tree with nvcc for sm_90a (no JIT cache: the .so is built next to the sources).
 
     python -m dsmil_wsi_b200.build          # or: from dsmil_wsi_b200.build import build_library
 """
@@ -16,7 +16,7 @@ SOURCES = ["abi.cu"]
 HOST_CSRC = os.path.join(HERE, "csrc_host")
 HOST_LIB = os.path.join(LIBDIR, "libdsmil_host.so")
 HOST_SOURCES = ["bagcsv.c", "jpegparse.c"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _nvcc():

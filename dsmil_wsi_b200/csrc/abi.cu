@@ -1,6 +1,6 @@
 // extern "C" entry points of libdsmil_b200.so (see include/dsmil_b200.h for the contract and the
 // reference spans each call replaces).  Host orchestration only; kernels live in *_kernels.cuh
-// and fwd_sm100.cuh.
+// and fwd_sm90.cuh.
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
@@ -13,9 +13,8 @@
 #include "gemm_generic.cuh"
 #include "fwd_kernels.cuh"
 #include "bwd_kernels.cuh"
-#include "fwd_sm100.cuh"
+#include "fwd_sm90.cuh"
 #include "fwd_batched.cuh"
-#include "fwd_pair.cuh"
 #include "embed_kernels.cuh"
 #include "jpeg_kernels.cuh"
 
@@ -36,8 +35,6 @@ int cuda_fail(cudaError_t e, const char* what) {
   return DSMIL_ERR_CUDA;
 }
 void count_launch(int n) { g_launches.fetch_add(static_cast<uint64_t>(n), std::memory_order_relaxed); }
-
-namespace sm100 { long long* g_trace_buf = nullptr; }
 
 // train_tcga.py:78-83 dropout_patches: `feats[random_indices]` -- a row gather.  One warp per output row.
 __global__ void __launch_bounds__(256)
@@ -109,7 +106,7 @@ static int check_params(const dsmil_params_t* p, bool need_scores = false) {
 
 static inline int attend_ctas(int64_t N) {
   const int64_t tiles = (N + kAttendRows - 1) / kAttendRows;
-  return static_cast<int>(tiles < 296 ? (tiles < 1 ? 1 : tiles) : 296);
+  return static_cast<int>(tiles < kSplits ? (tiles < 1 ? 1 : tiles) : kSplits);
 }
 
 struct FwdWs {
@@ -132,7 +129,7 @@ static FwdWs carve_fwd(const dsmil_params_t* p, int64_t N, void* ws, size_t cap,
   w.crit = c.take<int64_t>(kMaxC);
   w.recs = c.take<float>(static_cast<size_t>(attend_ctas(N)) * rec_floats(p->C, p->D));
   w.rec = c.take<float>(rec_floats(p->C, p->D));
-  w.wimg = sm100::qmlp_supported(p) ? c.take<uint8_t>(sm100::wimg_bytes(p->D) + 1024 + 256) : nullptr;
+  w.wimg = sm90::qmlp_supported(p) ? c.take<uint8_t>(sm90::wimg_bytes(p->D) + 1024 + 256) : nullptr;
   w.bytes = c.off;
   *ok = c.ok();
   return w;
@@ -146,7 +143,7 @@ static int launch_scores(const dsmil_params_t* p, const float* X, int64_t N, flo
   const size_t smem = sizeof(float) * C * D;
   const bool vec = (D % 4 == 0) && ((reinterpret_cast<uintptr_t>(X) & 15) == 0);
   const int mode = !vec ? 0 : (D % 64 == 0 ? 2 : 1);
-  const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, mode == 2 ? 16 : 8), 148 * 8));
+  const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, mode == 2 ? 64 : 8), kSms * 8));
   prof_begin(PROF_SCORES, st);
   if (mode == 2) {
     if (smem > 48 * 1024) DSMIL_CUDA_OK(cudaFuncSetAttribute(k_scores<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -166,18 +163,18 @@ static int launch_scores(const dsmil_params_t* p, const float* X, int64_t N, flo
 static int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kSms;
   if (!cached[dev]) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kSms;
     cached[dev] = n;
   }
   return cached[dev];
 }
-static bool use_sm100(const dsmil_params_t* p) {
+static bool use_sm90(const dsmil_params_t* p) {
   static int disabled = -1;
   if (disabled < 0) { const char* e = getenv("DSMIL_B200_GENERIC"); disabled = (e && e[0] == '1') ? 1 : 0; }
-  return !disabled && sm100::qmlp_supported(p);
+  return !disabled && sm90::qmlp_supported(p);
 }
 
 // Under stream capture (CUDA-graph serving loops) the pageable host->device copies of the bag table cannot be
@@ -194,36 +191,29 @@ static int blocked_q_mode() {
   if (mode < 0) { const char* e = getenv("DSMIL_B200_QPRE"); mode = (e && e[0] == '0') ? 1 : 2; }
   return mode;
 }
-static bool use_pair(const dsmil_params_t* p) {
-  // CTA-pair phase 1 (fwd_pair.cuh): parity-green, but not yet faster than k_qmlp_sm100 (profiles/r2_bench_history.md),
-  // so it is opt-in: DSMIL_B200_PAIR=1
-  static int enabled = -1;
-  if (enabled < 0) { const char* e = getenv("DSMIL_B200_PAIR"); enabled = (e && e[0] == '1') ? 1 : 0; }
-  return enabled && use_sm100(p) && pair::pair_supported(p);
-}
 
 static int phase1_impl(const dsmil_params_t* p, const float* X, const float* xv, const float* classes_in,
                        int64_t N, int64_t row_offset, float* classes, float* Q, float* H1, float* V,
                        float* cand, unsigned long long* keys, uint8_t* wimg, cudaStream_t st) {
   const int C = p->C, D = p->D;
   DSMIL_CUDA_OK(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * kMaxC, st));
-  if (N > 0 && use_sm100(p) && wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0) {
+  if (N > 0 && use_sm90(p) && wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0) {
     // tensor-core path: scores + arg-max + Q-MLP in one persistent kernel
     int rc;
     if (classes_in) {
       if (classes && classes != classes_in)
         DSMIL_CUDA_OK(cudaMemcpyAsync(classes, classes_in, sizeof(float) * N * C, cudaMemcpyDeviceToDevice, st));
-      const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), 296));
+      const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
       k_argmax<<<grid, 256, 0, st>>>(classes_in, N, C, keys);
       DSMIL_LAUNCH_OK("k_argmax");
     }
     uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wimg) + 1023) & ~uintptr_t(1023));
-    sm100::BagDev* tbl = reinterpret_cast<sm100::BagDev*>(img + sm100::wimg_bytes(D));
-    sm100::BagDev one{X, N, 0, 0, 0, 1, 0};
+    sm90::BagDev* tbl = reinterpret_cast<sm90::BagDev*>(img + sm90::wimg_bytes(D));
+    sm90::BagDev one{X, N, 0, 0, 0, 1, 0};
     DSMIL_CUDA_OK(cudaMemcpyAsync(tbl, &one, sizeof(one), cudaMemcpyHostToDevice, st));
-    if ((rc = sm100::launch_prep_wimg(p, img, st))) return rc;
-    const int ntiles = static_cast<int>((N + sm100::kTileM - 1) / sm100::kTileM);
-    if ((rc = sm100::launch_qmlp(p, tbl, 0, 1, 0, ntiles, classes_in ? nullptr : classes, keys, Q, H1, img, num_sms(), st)))
+    if ((rc = sm90::launch_prep_wimg(p, img, st))) return rc;
+    const int ntiles = static_cast<int>((N + sm90::kTileM - 1) / sm90::kTileM);
+    if ((rc = sm90::launch_qmlp(p, tbl, 0, 1, 0, ntiles, classes_in ? nullptr : classes, keys, Q, H1, img, num_sms(), st)))
       return rc;
     if (p->passing_v) {
       if ((rc = launch_linear<ACT_RELU, false>(xv ? xv : X, N, D, p->Wv, p->bv, D, V, nullptr, 0, st))) return rc;
@@ -232,7 +222,7 @@ static int phase1_impl(const dsmil_params_t* p, const float* X, const float* xv,
     if (classes_in) {
       if (classes && classes != classes_in)
         DSMIL_CUDA_OK(cudaMemcpyAsync(classes, classes_in, sizeof(float) * N * C, cudaMemcpyDeviceToDevice, st));
-      const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), 296));
+      const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
       k_argmax<<<grid, 256, 0, st>>>(classes_in, N, C, keys);
       DSMIL_LAUNCH_OK("k_argmax");
     } else {
@@ -306,7 +296,7 @@ static int phase2_impl(const dsmil_params_t* p, const float* V, const float* Q, 
 
 static int phase3_impl(const dsmil_params_t* p, int64_t N, const float* rec, float* A, float* B, float* pred,
                        cudaStream_t st) {
-  const int grid = static_cast<int>(std::min<int64_t>(std::max<int64_t>(ceil_div(N * p->C, 256), 1), 296));
+  const int grid = static_cast<int>(std::min<int64_t>(std::max<int64_t>(ceil_div(N * p->C, 256), 1), kSplits));
   prof_begin(PROF_FINAL, st);
   k_finalize<<<grid, 256, 0, st>>>(rec, N, p->C, p->D, p->Wf, p->bf, A, B, pred);
   prof_end(PROF_FINAL, st);
@@ -330,7 +320,7 @@ static int forward_impl(const dsmil_params_t* p, const float* X, const float* xv
     return DSMIL_ERR_EMPTY;
   }
   DSMIL_REQUIRE(X && pred && A && B && (classes || classes_in), "NULL tensor pointer");
-  if (use_sm100(p) && sm100::batched_supported(p) && (reinterpret_cast<uintptr_t>(X) & 15) == 0)
+  if (use_sm90(p) && sm90::batched_supported(p) && (reinterpret_cast<uintptr_t>(X) & 15) == 0)
     return forward_bags_impl(p, &X, &N, 1, classes_in, classes, pred, A, B, crit_idx, save_Q, save_H1, ws, ws_bytes, st);
   bool ok;
   FwdWs w = carve_fwd(p, N, ws, ws_bytes, &ok);
@@ -353,8 +343,7 @@ static int forward_impl(const dsmil_params_t* p, const float* X, const float* xv
 
 // ---- batched forward: a stream of bags in a handful of launches (tensor-core path only) -----------
 struct BagsWs {
-  sm100::BagDev* table;
-  CUtensorMap* tmaps;       // one per bag (pair kernel: X of the bag as a 2-D TMA tensor)
+  sm90::BagDev* table;
   unsigned long long* keys;
   float* Q;
   uint8_t* wimg;
@@ -364,8 +353,8 @@ struct BagsWs {
   size_t bytes;
 };
 static inline int recs_for_bag(int64_t N) {
-  const int64_t t = (N + sm100::kAttRows - 1) / sm100::kAttRows;
-  return static_cast<int>(t < sm100::kMaxRecPerBag ? (t < 1 ? 1 : t) : sm100::kMaxRecPerBag);
+  const int64_t t = (N + sm90::kAttRows - 1) / sm90::kAttRows;
+  return static_cast<int>(t < sm90::kMaxRecPerBag ? (t < 1 ? 1 : t) : sm90::kMaxRecPerBag);
 }
 static BagsWs carve_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, bool need_Q, void* ws, size_t cap,
                          bool* ok) {
@@ -373,19 +362,18 @@ static BagsWs carve_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, boo
   BagsWs w;
   int64_t total = 0, nrec = 0;
   for (int b = 0; b < nb; ++b) { total += Ns[b]; nrec += recs_for_bag(Ns[b]); }
-  w.table = c.take<sm100::BagDev>(nb);
-  w.tmaps = c.take<CUtensorMap>(nb);
+  w.table = c.take<sm90::BagDev>(nb);
   // keys and the finalize arrival counters are zeroed together (one memset): keep them adjacent
   w.keys = c.take<unsigned long long>(static_cast<size_t>(nb) * (kMaxC + 1));
   w.counters = reinterpret_cast<unsigned int*>(w.keys ? w.keys + static_cast<size_t>(nb) * kMaxC : nullptr);
-  w.pred_part = c.take<float>(static_cast<size_t>(nb) * sm100::kFinSlices * kMaxC);
+  w.pred_part = c.take<float>(static_cast<size_t>(nb) * sm90::kFinSlices * kMaxC);
   {   // tile-blocked Q: one 128x128 block per 128-row tile
     int64_t tiles = 0;
-    for (int b = 0; b < nb; ++b) tiles += (Ns[b] + sm100::kTileM - 1) / sm100::kTileM;
-    w.Q = need_Q ? c.take<float>(static_cast<size_t>(tiles) * sm100::kTileM * kQ) : nullptr;
+    for (int b = 0; b < nb; ++b) tiles += (Ns[b] + sm90::kTileM - 1) / sm90::kTileM;
+    w.Q = need_Q ? c.take<float>(static_cast<size_t>(tiles) * sm90::kTileM * kQ) : nullptr;
   }
   (void)total;
-  w.wimg = c.take<uint8_t>(sm100::wimg_bytes(p->D) + 1024);
+  w.wimg = c.take<uint8_t>(sm90::wimg_bytes(p->D) + 1024);
   w.recs = c.take<float>(static_cast<size_t>(nrec) * rec_floats(p->C, p->D));
   w.bytes = c.off;
   *ok = c.ok();
@@ -415,48 +403,28 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
     set_error("workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
     return DSMIL_ERR_WORKSPACE;
   }
-  std::vector<sm100::BagDev> tbl(nb);
+  std::vector<sm90::BagDev> tbl(nb);
   long long row = 0;
   int tile = 0, rec = 0;
-  // inference (Q stays in the tile-blocked workspace) on D <= 512, opt-in: the CTA-pair phase-1 kernel (fwd_pair.cuh)
-  const bool pair_path = save_Q == nullptr && save_H1 == nullptr && use_pair(p);
   for (int b = 0; b < nb; ++b) {
     DSMIL_REQUIRE(Ns[b] >= 1 && Ns[b] < 0xffffffffll && Xs[b], "bag %d: empty or NULL", b);
     DSMIL_REQUIRE((reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0, "bag %d: features must be 16-byte aligned", b);
     const int nrec = recs_for_bag(Ns[b]);
-    tbl[b] = sm100::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
+    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
     row += Ns[b];
-    tile += static_cast<int>((Ns[b] + sm100::kTileM - 1) / sm100::kTileM);
+    tile += static_cast<int>((Ns[b] + sm90::kTileM - 1) / sm90::kTileM);
     rec += nrec;
   }
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm100::BagDev) * nb, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
   DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
   uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(w.wimg) + 1023) & ~uintptr_t(1023));
   int rc;
-  if (pair_path) {
-    std::vector<CUtensorMap> maps(nb);
-    for (int b = 0; b < nb; ++b)
-      if ((rc = pair::encode_bag_tmap(&maps[b], Xs[b], Ns[b], D))) return rc;
-    DSMIL_CUDA_OK(cudaMemcpyAsync(w.tmaps, maps.data(), sizeof(CUtensorMap) * nb, cudaMemcpyHostToDevice, st));
-    if ((rc = pair::launch_prep_wimg_pair(p, img, st))) return rc;
-  } else {
-    if ((rc = sm100::launch_prep_wimg(p, img, st))) return rc;
-  }
+  if ((rc = sm90::launch_prep_wimg(p, img, st))) return rc;
   float* Q = save_Q ? save_Q : w.Q;
   if (classes_in) {   // bag form: arg-max of the given scores (single bag only)
-    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(Ns[0], 256), 296));
+    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(Ns[0], 256), kSplits));
     k_argmax<<<grid, 256, 0, st>>>(classes_in, Ns[0], C, w.keys);
     DSMIL_LAUNCH_OK("k_argmax");
-  }
-  if (pair_path) {
-    if ((rc = pair::launch_fwd_pair(p, w.table, w.tmaps, nb, tile, classes_in ? nullptr : classes, w.keys, Q, img,
-                                    num_sms(), st)))
-      return rc;
-    sm100::AttendArgs aa{w.table, 0, nb, 0, D, C, Q, 1, w.keys, A, w.recs, nullptr};
-    if ((rc = sm100::launch_attend_b(aa, rec, st))) return rc;
-    sm100::FinalizeArgs fa{w.table, 0, D, C, w.recs, w.keys, p->Wf, p->bf, A, B, pred,
-                           reinterpret_cast<long long*>(crit), w.pred_part, w.counters, nullptr, 0, 0};
-    return sm100::launch_finalize_b(fa, nb, st);
   }
   // sub-batches sized so that a sub-batch's features (+Q) are still in L2 when the attend pass re-reads them
   const size_t budget = l2_budget_bytes();
@@ -475,14 +443,14 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
     const int r0 = tbl[b0].rec_off;
     const int r1 = (b1 < nb) ? tbl[b1].rec_off : rec;
     const int q_blocked = save_Q ? 0 : blocked_q_mode();   // training keeps Q (after tanh) row-major for the backward kernels
-    if ((rc = sm100::launch_qmlp(p, w.table, b0, b1 - b0, t0, t1 - t0, classes_in ? nullptr : classes, w.keys, Q,
+    if ((rc = sm90::launch_qmlp(p, w.table, b0, b1 - b0, t0, t1 - t0, classes_in ? nullptr : classes, w.keys, Q,
                                  save_H1, img, num_sms(), st, q_blocked)))
       return rc;
-    sm100::AttendArgs aa{w.table, b0, b1 - b0, r0, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr};
-    if ((rc = sm100::launch_attend_b(aa, r1 - r0, st))) return rc;
-    sm100::FinalizeArgs fa{w.table, b0, D, C, w.recs, w.keys, p->Wf, p->bf, A, B, pred,
+    sm90::AttendArgs aa{w.table, b0, b1 - b0, r0, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr};
+    if ((rc = sm90::launch_attend_b(aa, r1 - r0, st))) return rc;
+    sm90::FinalizeArgs fa{w.table, b0, D, C, w.recs, w.keys, p->Wf, p->bf, A, B, pred,
                            reinterpret_cast<long long*>(crit), w.pred_part, w.counters, nullptr, 0, 0};
-    if ((rc = sm100::launch_finalize_b(fa, b1 - b0, st))) return rc;
+    if ((rc = sm90::launch_finalize_b(fa, b1 - b0, st))) return rc;
     b0 = b1;
   }
   return 0;
@@ -507,7 +475,7 @@ static ShardBagsWs carve_shard_bags(const dsmil_params_t* p, const int64_t* Ns, 
   *ok = c.ok();
   return s;
 }
-static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::vector<sm100::BagDev>& tbl, int* tiles,
+static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::vector<sm90::BagDev>& tbl, int* tiles,
                        int* recs) {
   long long row = 0;
   int tile = 0, rec = 0;
@@ -516,9 +484,9 @@ static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::v
     DSMIL_REQUIRE(Ns[b] >= 1 && Ns[b] < 0xffffffffll && Xs[b], "bag %d: empty or NULL (sharded batches need >= 1 row per rank)", b);
     DSMIL_REQUIRE((reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0, "bag %d: features must be 16-byte aligned", b);
     const int nrec = recs_for_bag(Ns[b]);
-    tbl[b] = sm100::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
+    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
     row += Ns[b];
-    tile += static_cast<int>((Ns[b] + sm100::kTileM - 1) / sm100::kTileM);
+    tile += static_cast<int>((Ns[b] + sm90::kTileM - 1) / sm90::kTileM);
     rec += nrec;
   }
   *tiles = tile;
@@ -537,19 +505,14 @@ const char* dsmil_last_error(void) { return g_err; }
 uint64_t dsmil_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 int dsmil_forward_path(const dsmil_params_t* p, int64_t N) {
   (void)N;
-  return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && use_sm100(p)) ? 2 : 1;
+  return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && use_sm90(p)) ? 2 : 1;
 }
 
-/* Debug: CTA-0 timeline of the tensor-core kernel (clock64 stamps).  buf = device int64[3*8*64] or NULL. */
-int dsmil_debug_set_trace(void* buf) {
-  sm100::g_trace_buf = static_cast<long long*>(buf);
-  return 0;
-}
 
 int dsmil_gather_rows(const float* X, int64_t N, int32_t D, const int64_t* idx, int64_t M, float* out, void* stream) {
   DSMIL_REQUIRE(N >= 0 && M >= 0 && D >= 1 && (M == 0 || (X && idx && out)), "bad arguments");
   if (M == 0) return 0;
-  const int grid = static_cast<int>(std::min<int64_t>((M + 7) / 8, 148 * 8));
+  const int grid = static_cast<int>(std::min<int64_t>((M + 7) / 8, kSms * 8));
   k_gather_rows<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(X, D, reinterpret_cast<const long long*>(idx), M, out);
   DSMIL_LAUNCH_OK("k_gather_rows");
   return 0;
@@ -559,7 +522,7 @@ int dsmil_patches_u8_to_f32(const uint8_t* in, int64_t B, int32_t H, int32_t W, 
   DSMIL_REQUIRE(B >= 0 && H >= 1 && W >= 1 && Cc >= 1 && Cc <= 4 && (B == 0 || (in && out)), "bad arguments");
   if (B == 0) return 0;
   const long long total = static_cast<long long>(B) * H * W;
-  const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 148 * 16));
+  const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, kSms * 16));
   k_u8hwc_to_f32chw<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(in, B, H, W, Cc, out);
   DSMIL_LAUNCH_OK("k_u8hwc_to_f32chw");
   return 0;
@@ -657,7 +620,7 @@ size_t dsmil_forward_workspace_bytes(const dsmil_params_t* p, int64_t N) {
   if (!p || p->C < 1 || p->C > DSMIL_MAX_C || p->D < 1 || p->D > DSMIL_MAX_D || N < 0) return 0;
   bool ok;
   size_t a = carve_fwd(p, N, nullptr, 0, &ok).bytes;
-  if (sm100::batched_supported(p) && N > 0) a = std::max(a, carve_bags(p, &N, 1, true, nullptr, 0, &ok).bytes);
+  if (sm90::batched_supported(p) && N > 0) a = std::max(a, carve_bags(p, &N, 1, true, nullptr, 0, &ok).bytes);
   return a;
 }
 
@@ -669,7 +632,7 @@ size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t
   int64_t mx = 0;
   for (int b = 0; b < nb; ++b) mx = std::max<int64_t>(mx, Ns[b]);
   size_t bytes = carve_fwd(p, mx, nullptr, 0, &ok).bytes;
-  if (sm100::batched_supported(p)) bytes = std::max(bytes, carve_bags(p, Ns, nb, true, nullptr, 0, &ok).bytes);
+  if (sm90::batched_supported(p)) bytes = std::max(bytes, carve_bags(p, Ns, nb, true, nullptr, 0, &ok).bytes);
   return bytes;
 }
 
@@ -689,7 +652,7 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
   }
   bool aligned = true;
   for (int b = 0; b < nb; ++b) aligned = aligned && Xs[b] && (reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0 && Ns[b] >= 1;
-  if (use_sm100(p) && sm100::batched_supported(p) && aligned)
+  if (use_sm90(p) && sm90::batched_supported(p) && aligned)
     return forward_bags_impl(p, Xs, Ns, nb, nullptr, classes, pred, A, B, crit_idx, nullptr, nullptr, workspace,
                              workspace_bytes, st);
   // shapes the tensor-core kernels do not take: same packed outputs, one bag at a time
@@ -750,8 +713,8 @@ int dsmil_shard_phase1(const dsmil_params_t* p, const float* X, const float* x_f
     set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes);
     return DSMIL_ERR_WORKSPACE;
   }
-  // the tensor-core path keeps H1 in TMEM; the generic path (also taken for an unaligned X) needs a buffer
-  const bool tc = use_sm100(p) && w.wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
+  // the tensor-core path keeps H1 in registers; the generic path (also taken for an unaligned X) needs a buffer
+  const bool tc = use_sm90(p) && w.wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
   float* h1 = p->nonlinear ? (H1 ? H1 : (tc ? nullptr : w.H1)) : nullptr;
   return phase1_impl(p, X, x_for_v, classes_in, N_local, row_offset, classes, Q, h1, V, cand_rec, w.keys, w.wimg,
                      static_cast<cudaStream_t>(stream));
@@ -808,7 +771,7 @@ static BwdWs carve_bwd(const dsmil_params_t* p, int64_t N, int need_gX, void* ws
   const int64_t n = N > 0 ? N : 1;
   w.dB = c.take<float>(static_cast<size_t>(C) * D);
   w.dA = c.take<float>(n * C);
-  w.tpart = c.take<float>(296 * kMaxC);
+  w.tpart = c.take<float>(kSplits * kMaxC);
   w.dqm = c.take<float>(static_cast<size_t>(C) * kQ);
   w.dz2 = c.take<float>(n * kQ);
   w.dz1 = p->nonlinear ? c.take<float>(n * kQ) : nullptr;
@@ -818,7 +781,7 @@ static BwdWs carve_bwd(const dsmil_params_t* p, int64_t N, int need_gX, void* ws
   tn = std::max(tn, tn_partial_floats(C, D, N));
   if (p->passing_v) tn = std::max(tn, tn_partial_floats(D, D, N));
   w.tnpart = c.take<float>(tn);
-  w.cspart = c.take<float>(static_cast<size_t>(296) * std::max(D, kQ));
+  w.cspart = c.take<float>(static_cast<size_t>(kSplits) * std::max(D, kQ));
   w.dzv = p->passing_v ? c.take<float>(n * D) : nullptr;
   w.tmp = (p->passing_v && need_gX) ? c.take<float>(n * D) : nullptr;
   w.bytes = c.off;
@@ -852,7 +815,7 @@ int dsmil_backward(const dsmil_params_t* p, const float* X, const float* x_for_v
   }
   const float* Vv = p->passing_v ? V : X;
   const float* Xv = x_for_v ? x_for_v : X;
-  const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), 296));
+  const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
 
   // bag classifier (dsmil.py:59-61) and B
   k_bwd_bag<<<ceil_div(static_cast<int64_t>(C) * D, 256), 256, 0, st>>>(p->Wf, B, d_pred, d_B, C, D, w.dB, g->gWf,
@@ -872,7 +835,7 @@ int dsmil_backward(const dsmil_params_t* p, const float* X, const float* x_for_v
     const size_t smem = sizeof(float) * C * D;
     if (smem > 48 * 1024)
       DSMIL_CUDA_OK(cudaFuncSetAttribute(k_rowdot, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 8), 148 * 8));
+    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 8), kSms * 8));
     k_rowdot<<<grid, 256, smem, st>>>(Vv, N, D, w.dB, C, d_A, w.dA);
     DSMIL_LAUNCH_OK("k_rowdot");
   }
@@ -884,7 +847,7 @@ int dsmil_backward(const dsmil_params_t* p, const float* X, const float* x_for_v
   // dq_max = dL^T Q  (dsmil.py:55), then dQ rows (+ the critical rows' share, dsmil.py:53-54)
   if ((rc = launch_gemm_tn(dL, C, Q, kQ, N, w.tnpart, w.dqm, st))) return rc;
   {
-    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N * kQ, 256), 148 * 8));
+    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N * kQ, 256), kSms * 8));
     k_bwd_dq<<<grid, 256, 0, st>>>(dL, Q, w.dqm, crit_idx, N, C, p->nonlinear, w.dz2);
     DSMIL_LAUNCH_OK("k_bwd_dq");
   }
@@ -898,7 +861,7 @@ int dsmil_backward(const dsmil_params_t* p, const float* X, const float* x_for_v
   if (g->gW1 && (rc = launch_gemm_tn(dz1, kQ, X, D, N, w.tnpart, g->gW1, st))) return rc;
   if (g->gb1 && (rc = launch_colsum(dz1, kQ, N, w.cspart, g->gb1, st))) return rc;
 
-  const int ge = static_cast<int>(std::min<int64_t>(ceil_div(N * D, 256), 148 * 8));
+  const int ge = static_cast<int>(std::min<int64_t>(ceil_div(N * D, 256), kSms * 8));
   if (p->passing_v) {
     k_bwd_dzv<<<ge, 256, 0, st>>>(A, w.dB, V, N, C, D, w.dzv);
     DSMIL_LAUNCH_OK("k_bwd_dzv");
@@ -958,10 +921,10 @@ int dsmil_shard_backward_phase1(const dsmil_params_t* p, const float* X, int64_t
   const size_t smem = sizeof(float) * C * D;
   if (smem > 48 * 1024)
     DSMIL_CUDA_OK(cudaFuncSetAttribute(k_rowdot, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 8), 148 * 8));
+  const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 8), kSms * 8));
   k_rowdot<<<grid, 256, smem, st>>>(X, N, D, w.dB, C, nullptr, dA);
   DSMIL_LAUNCH_OK("k_rowdot");
-  const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), 296));
+  const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
   k_bwd_t_partial<<<gs, 256, 0, st>>>(A, dA, N, C, w.tpart);
   DSMIL_LAUNCH_OK("k_bwd_t_partial");
   k_sum_partials<<<1, 256, 0, st>>>(w.tpart, gs, C, t_local);
@@ -980,7 +943,7 @@ int dsmil_shard_backward_phase2(const dsmil_params_t* p, int64_t N, const float*
   BwdWs w;
   if ((rc = shard_bwd_ws(p, N, workspace, workspace_bytes, &w))) return rc;
   if (N > 0) {
-    const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), 296));
+    const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
     k_bwd_dL<<<gs, 256, 0, st>>>(A, dA, N, C, t_global, 1);
     DSMIL_LAUNCH_OK("k_bwd_dL");
   }
@@ -1001,7 +964,7 @@ int dsmil_shard_backward_phase3(const dsmil_params_t* p, const float* X, int64_t
   if ((rc = shard_bwd_ws(p, N, workspace, workspace_bytes, &w))) return rc;
   const float* dz1 = w.dz2;
   if (N > 0) {
-    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N * kQ, 256), 148 * 8));
+    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N * kQ, 256), kSms * 8));
     k_bwd_dq_shard<<<grid, 256, 0, st>>>(dL, Q, q_max, dqm_global, crit_idx, N, row_offset, C, p->nonlinear, w.dz2);
     DSMIL_LAUNCH_OK("k_bwd_dq_shard");
   }
@@ -1025,7 +988,7 @@ int dsmil_instance_scores_backward(const dsmil_params_t* p, const float* X, int6
   const int C = p->C, D = p->D;
   Carver c(workspace, workspace_bytes);
   float* tnpart = c.take<float>(tn_partial_floats(C, D, N));
-  float* cspart = c.take<float>(static_cast<size_t>(296) * kMaxC);
+  float* cspart = c.take<float>(static_cast<size_t>(kSplits) * kMaxC);
   if (!workspace || !c.ok()) {
     set_error("workspace too small: need %zu bytes, got %zu", c.off, workspace_bytes);
     return DSMIL_ERR_WORKSPACE;
@@ -1034,7 +997,7 @@ int dsmil_instance_scores_backward(const dsmil_params_t* p, const float* X, int6
   if (gWi && (rc = launch_gemm_tn(d_classes, C, X, D, N, tnpart, gWi, st))) return rc;
   if (gbi && (rc = launch_colsum(d_classes, C, N, cspart, gbi, st))) return rc;
   if (gX) {
-    const int ge = static_cast<int>(std::min<int64_t>(ceil_div(N * D, 256), 148 * 8));
+    const int ge = static_cast<int>(std::min<int64_t>(ceil_div(N * D, 256), kSms * 8));
     k_bwd_dx_extra<<<ge, 256, 0, st>>>(d_classes, p->Wi, nullptr, nullptr, N, C, D, 0, gX);
     DSMIL_LAUNCH_OK("k_bwd_dx_extra");
   }
@@ -1043,8 +1006,8 @@ int dsmil_instance_scores_backward(const dsmil_params_t* p, const float* X, int6
 
 // ---- sharded batch ABI ---------------------------------------------------------------------------
 int dsmil_shard_bags_supported(const dsmil_params_t* p) {
-  return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && use_sm100(p) &&
-          sm100::batched_supported(p)) ? 1 : 0;
+  return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && use_sm90(p) &&
+          sm90::batched_supported(p)) ? 1 : 0;
 }
 size_t dsmil_shard_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
   if (!dsmil_shard_bags_supported(p) || !Ns || nb < 1) return 0;
@@ -1062,21 +1025,21 @@ int dsmil_shard_bags_phase1(const dsmil_params_t* p, const float* const* Xs, con
   bool ok;
   ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
   if (!workspace || !ok) { set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes); return DSMIL_ERR_WORKSPACE; }
-  std::vector<sm100::BagDev> tbl;
+  std::vector<sm90::BagDev> tbl;
   int tiles = 0, recs = 0;
   if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;
   if (!stream_is_capturing(st)) {
-    DSMIL_CUDA_OK(cudaMemcpyAsync(w.base.table, tbl.data(), sizeof(sm100::BagDev) * nb, cudaMemcpyHostToDevice, st));
+    DSMIL_CUDA_OK(cudaMemcpyAsync(w.base.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
     DSMIL_CUDA_OK(cudaMemcpyAsync(w.row_offsets, row_offsets, sizeof(long long) * nb, cudaMemcpyHostToDevice, st));
   }
   DSMIL_CUDA_OK(cudaMemsetAsync(w.base.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
   uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(w.base.wimg) + 1023) & ~uintptr_t(1023));
   // (a captured serving loop also reuses the weight images of the preceding eager call: re-capture after a weight update)
-  if (!stream_is_capturing(st) && (rc = sm100::launch_prep_wimg(p, img, st))) return rc;
-  if ((rc = sm100::launch_qmlp(p, w.base.table, 0, nb, 0, tiles, classes, w.base.keys, w.base.Q, nullptr, img, num_sms(), st,
+  if (!stream_is_capturing(st) && (rc = sm90::launch_prep_wimg(p, img, st))) return rc;
+  if ((rc = sm90::launch_qmlp(p, w.base.table, 0, nb, 0, tiles, classes, w.base.keys, w.base.Q, nullptr, img, num_sms(), st,
                                blocked_q_mode())))
     return rc;
-  sm100::k_gather_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(w.base.table, w.base.keys, classes, w.base.Q, blocked_q_mode(), w.row_offsets, p->C,
+  sm90::k_gather_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(w.base.table, w.base.keys, classes, w.base.Q, blocked_q_mode(), w.row_offsets, p->C,
                                                         cand_recs);
   DSMIL_LAUNCH_OK("k_gather_cand_b");
   return 0;
@@ -1092,31 +1055,31 @@ int dsmil_shard_bags_phase2(const dsmil_params_t* p, const float* const* Xs, con
   bool ok;
   ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
   if (!workspace || !ok) { set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes); return DSMIL_ERR_WORKSPACE; }
-  std::vector<sm100::BagDev> tbl;
+  std::vector<sm90::BagDev> tbl;
   int tiles = 0, recs = 0;
   if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
-  sm100::k_merge_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(cands_all, G, nb, p->C, w.qmax, reinterpret_cast<long long*>(crit_idx));
+  sm90::k_merge_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(cands_all, G, nb, p->C, w.qmax, reinterpret_cast<long long*>(crit_idx));
   DSMIL_LAUNCH_OK("k_merge_cand_b");
-  sm100::AttendArgs aa{w.base.table, 0, nb, 0, p->D, p->C, w.base.Q, blocked_q_mode(), w.base.keys, A, w.base.recs, w.qmax};
-  if ((rc = sm100::launch_attend_b(aa, recs, st))) return rc;
-  sm100::FinalizeArgs fa{w.base.table, 0, p->D, p->C, w.base.recs, w.base.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
+  sm90::AttendArgs aa{w.base.table, 0, nb, 0, p->D, p->C, w.base.Q, blocked_q_mode(), w.base.keys, A, w.base.recs, w.qmax};
+  if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
+  sm90::FinalizeArgs fa{w.base.table, 0, p->D, p->C, w.base.recs, w.base.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
                          w.base.pred_part, w.base.counters, recs_out, 0, 0};
-  return sm100::launch_finalize_b(fa, nb, st);
+  return sm90::launch_finalize_b(fa, nb, st);
 }
 int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                             const float* recs_all, int32_t G, float* A, float* B, float* pred, void* workspace,
                             size_t workspace_bytes, void* stream) {
   int rc = check_params(p, true);
   if (rc) return rc;
-  DSMIL_REQUIRE(dsmil_shard_bags_supported(p) && Xs && Ns && nb >= 1 && recs_all && G >= 1 && G <= sm100::kMaxRecPerBag && A && B && pred,
+  DSMIL_REQUIRE(dsmil_shard_bags_supported(p) && Xs && Ns && nb >= 1 && recs_all && G >= 1 && G <= sm90::kMaxRecPerBag && A && B && pred,
                 "bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
   ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
   if (!workspace || !ok) { set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes); return DSMIL_ERR_WORKSPACE; }
-  sm100::FinalizeArgs fa{w.base.table, 0, p->D, p->C, recs_all, w.base.keys, p->Wf, p->bf, A, B, pred, nullptr,
+  sm90::FinalizeArgs fa{w.base.table, 0, p->D, p->C, recs_all, w.base.keys, p->Wf, p->bf, A, B, pred, nullptr,
                          w.base.pred_part, w.base.counters, nullptr, G, nb};
-  return sm100::launch_finalize_b(fa, nb, st);
+  return sm90::launch_finalize_b(fa, nb, st);
 }
 
 }  // extern "C"

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libdsmil_b200 (sm_100a only).
+// Shared device/host helpers for libdsmil_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -12,6 +12,12 @@ constexpr int kQ = DSMIL_Q;
 constexpr int kMaxC = DSMIL_MAX_C;
 // dsmil.py:56 divides by sqrt(float32(128)); this is that fp32 value.
 constexpr float kScale = 11.313708305358887f;
+// SMs of an H100 SXM: sizes the grids of the grid-stride kernels (kSms * 8 CTAs)
+constexpr int kSms = 132;
+// Largest number of partial sums of a split reduction (attention records, column sums, TN GEMM splits): it fixes the
+// fp32 summation order, so it does not follow the SM count -- results are the same on every GPU.  The workspace
+// sizes depend on it.
+constexpr int kSplits = 296;
 
 // ---- host-side error plumbing -------------------------------------------------------------
 void set_error(const char* fmt, ...);

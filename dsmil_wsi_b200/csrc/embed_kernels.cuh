@@ -10,9 +10,8 @@
 //   k_instnorm_warp    one WARP per plane of <= 1024 elements (56x56 is handled by the CTA kernel; 28x28, 14x14, 7x7
 //                      here): the plane lives in registers, 8 planes per CTA
 //
-//   k_instnorm_nhwc    the channels-last form (cuDNN's NHWC convolution kernels run the ResNet-18 convolutions 1.5x
-//                      faster than its NCHW ones on B200: 2.43 vs 3.70 ms per 128-patch batch, profiles/
-//                      r2_exp_channels_last.json).  Memory is [n][HW][C]; one CTA per (sample, 32-channel group),
+//   k_instnorm_nhwc    the channels-last form (the embedding loop runs the ResNet-18 convolutions in cuDNN's NHWC
+//                      kernels, tools/exp_channels_last.py compares the two layouts).  Memory is [n][HW][C]; one CTA per (sample, 32-channel group),
 //                      lane = channel, warps stride over the pixels, so every warp load is one 128-byte row segment.
 //                      Statistics in ONE pass as shifted sums (x - x0, x0 = the channel's first pixel: no
 //                      catastrophic cancellation for activations whose mean is far from 0), second pass normalises;

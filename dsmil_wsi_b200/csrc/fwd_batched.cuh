@@ -1,4 +1,4 @@
-// Batched (bag-table) phase 2/3 kernels used with the tensor-core phase 1 (fwd_sm100.cuh).
+// Batched (bag-table) phase 2/3 kernels used with the tensor-core phase 1 (fwd_sm90.cuh).
 //   k_attend_b     dsmil.py:53-57  per (bag, CTA): q_max = Q[critical rows], logits -> A (unnormalised),
 //                                  online softmax over the instance axis, partial bag vector
 //   k_finalize_b   dsmil.py:56-61  per bag: combine partial records, normalise A, B, Conv1d bag logits,
@@ -7,10 +7,10 @@
 #pragma once
 #include "common.cuh"
 #include "fwd_kernels.cuh"
-#include "fwd_sm100.cuh"
+#include "fwd_sm90.cuh"
 
 namespace dsmil {
-namespace sm100 {
+namespace sm90 {
 
 constexpr int kAttRows = 128;          // rows per attend tile (same tiling as phase 1)
 constexpr int kMaxRecPerBag = 128;
@@ -30,8 +30,8 @@ struct AttendArgs {
 
 // CT = classes rounded up to 1,2,4; NJ = float4 column groups per thread (D <= 512*NJ)
 // Occupancy: the D <= 512, C <= 2 instantiations fit 48 registers without spills, i.e. 5 CTAs per SM instead of 4.
-// One CTA per 128-row tile makes the 16 x 10 000-row step 1264 CTAs: 2.14 waves of 592 slots (three rounds) become
-// 1.71 waves of 740 (two rounds) -- see DESIGN.md §8-1b.  Wider variants keep the default bound (they would spill).
+// One CTA per 128-row tile makes the 16 x 10 000-row step 1264 CTAs: on 132 SMs 2.39 waves of 528 slots (three
+// rounds) become 1.92 waves of 660 (two rounds).  Wider variants keep the default bound (they would spill).
 template <int CT, int NJ>
 __global__ void __launch_bounds__(256, (NJ == 1 && CT <= 2) ? 5 : 0)
 k_attend_b(const AttendArgs a) {
@@ -274,8 +274,7 @@ constexpr int kFinSlices = 32;
 // rows of A, combines its share of the B columns -- eight threads per column, each summing every eighth record with
 // all its loads in flight, partials added in a fixed order (deterministic) -- and contributes a partial Conv1d dot
 // product; the last CTA of the bag to finish adds the kFinSlices partials in slice order (dsmil.py:59-61) and writes
-// the critical indices.  (r1 ran 8 slices with two threads per column: 128 CTAs of latency-bound serial work, 19-21 us
-// for a 16-bag step; profiles/r2_bench_history.md.)
+// the critical indices.
 __global__ void __launch_bounds__(256)
 k_finalize_b(const FinalizeArgs a) {
   __shared__ float sw[kMaxRecPerBag][kMaxC];
@@ -479,5 +478,5 @@ inline int launch_finalize_b(const FinalizeArgs& a, int nb, cudaStream_t st) {
   return 0;
 }
 
-}  // namespace sm100
+}  // namespace sm90
 }  // namespace dsmil

@@ -13,9 +13,9 @@ namespace dsmil {
 
 // ------------------------------------------------------------------------------------------
 // scores: one warp per row (grid-stride), Wi staged in shared memory, float4 loads when legal.
-// MODE 0: scalar loads (any D).  MODE 1: float4, one warp per row.  MODE 2 (D % 64 == 0): float4, HALF a
-// warp per row with exactly the summation order of the tensor-core kernel's fused scores
-// (fwd_sm100.cuh: lane `seg` takes float4 #seg of every 64-float chunk, then xor-shuffles 8,4,2,1), so
+// MODE 0: scalar loads (any D).  MODE 1: float4, one warp per row.  MODE 2 (D % 64 == 0): float4, FOUR lanes
+// per row with exactly the summation order of the tensor-core kernel's fused scores
+// (fwd_sm90.cuh: lane `seg` takes float4 #seg, #seg+4, ... of the row, then xor-shuffles 2,1), so
 // FCLayer/IClassifier scores are bit-identical whichever kernel produced them.
 template <int MODE>
 __global__ void __launch_bounds__(256)
@@ -30,9 +30,9 @@ k_scores(const float* __restrict__ X, int64_t N, int D, const float* __restrict_
   unsigned long long best[kMaxC];
 #pragma unroll
   for (int k = 0; k < kMaxC; ++k) best[k] = 0ull;
-  constexpr int RPW = (MODE == 2) ? 2 : 1;  // rows per warp per iteration
-  const int sub = (MODE == 2) ? (lane >> 4) : 0;
-  const int seg = (MODE == 2) ? (lane & 15) : lane;
+  constexpr int RPW = (MODE == 2) ? 8 : 1;  // rows per warp per iteration
+  const int sub = (MODE == 2) ? (lane >> 2) : 0;
+  const int seg = (MODE == 2) ? (lane & 3) : lane;
   const int64_t stride = static_cast<int64_t>(gridDim.x) * 8 * RPW;
   for (int64_t n0 = (static_cast<int64_t>(blockIdx.x) * 8 + warp) * RPW; n0 < N; n0 += stride) {
     const int64_t n = n0 + sub;
@@ -44,7 +44,7 @@ k_scores(const float* __restrict__ X, int64_t N, int D, const float* __restrict_
     if (MODE >= 1) {
       const float4* r4 = reinterpret_cast<const float4*>(row);
       const int D4 = D >> 2;
-      const int step = (MODE == 2) ? 16 : 32;
+      const int step = (MODE == 2) ? 4 : 32;
       for (int j = seg; j < D4; j += step) {
         const float4 x = __ldg(r4 + j);
 #pragma unroll
@@ -70,8 +70,6 @@ k_scores(const float* __restrict__ X, int64_t N, int D, const float* __restrict_
       if (k < C) {
         float v = acc[k];
         if (MODE == 2) {
-          v += __shfl_xor_sync(0xffffffffu, v, 8);
-          v += __shfl_xor_sync(0xffffffffu, v, 4);
           v += __shfl_xor_sync(0xffffffffu, v, 2);
           v += __shfl_xor_sync(0xffffffffu, v, 1);
         } else {
@@ -87,7 +85,7 @@ k_scores(const float* __restrict__ X, int64_t N, int D, const float* __restrict_
   }
 #pragma unroll
   for (int k = 0; k < kMaxC; ++k) {
-    best[k] = warp_max_u64(best[k]);   // MODE 2 keeps two partial bests per warp (lanes 0 and 16)
+    best[k] = warp_max_u64(best[k]);   // MODE 2 keeps eight partial bests per warp (lanes 0, 4, ..., 28)
     if (lane == 0) sbest[warp][k] = best[k];
   }
   __syncthreads();

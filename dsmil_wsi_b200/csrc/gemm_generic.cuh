@@ -1,5 +1,5 @@
 // Generic fp32 FFMA GEMM building blocks (any N, K, M; no alignment assumptions).
-// Used by the generic forward for shapes the tcgen05 kernel does not take (D % 64 != 0, e.g. the
+// Used by the generic forward for shapes the wgmma kernel does not take (D % 128 != 0, e.g. the
 // classic-MIL 166/230 features of train_mil.py:127-141), by the V projection (dsmil.py:35-39) and
 // by the backward GEMMs.  Deterministic: split reductions go through partial buffers summed in a
 // fixed order, never float atomics.
@@ -295,11 +295,11 @@ inline bool tn_use_gemv(int M1, int M2) { return M1 <= kGemvMaxM1 && (M2 & 3) ==
 inline int tn_splits(int M1, int M2, int64_t N) {
   int s, maxs;
   if (tn_use_gemv(M1, M2)) {
-    s = 296;
+    s = kSplits;
     maxs = ceil_div(N, 64);
   } else {
     const int tiles = ceil_div(M1, TBM) * ceil_div(M2, TBM);
-    s = 296 / (tiles > 0 ? tiles : 1);
+    s = kSplits / (tiles > 0 ? tiles : 1);
     maxs = ceil_div(N, 128);
   }
   if (s > maxs) s = maxs;
@@ -332,7 +332,7 @@ inline int launch_gemm_tn(const float* P, int M1, const float* R, int M2, int64_
   int Sg = S;
   if (tn_use_gemv(M1, M2)) {                                 // unaligned operand: the tile kernel, within the same budget
     const int tiles = ceil_div(M1, TBM) * ceil_div(M2, TBM);
-    Sg = std::max(1, std::min(S, 296 / tiles));
+    Sg = std::max(1, std::min(S, kSplits / tiles));
   }
   int64_t rps = (N + Sg - 1) / Sg;
   rps = (rps + TBK - 1) / TBK * TBK;
@@ -343,7 +343,7 @@ inline int launch_gemm_tn(const float* P, int M1, const float* R, int M2, int64_
 }
 inline int colsum_splits(int64_t N) {
   int s = ceil_div(N, 64);
-  return s > 296 ? 296 : (s < 1 ? 1 : s);
+  return s > kSplits ? kSplits : (s < 1 ? 1 : s);
 }
 inline int launch_colsum(const float* P, int M, int64_t N, float* part, float* out, cudaStream_t st) {
   if (N <= 0) {

@@ -1,4 +1,4 @@
-"""The patch-embedding loop (SURVEY §8 a13; reference compute_feats.py:19-82), B200-side re-design.
+"""The patch-embedding loop (SURVEY §8 a13; reference compute_feats.py:19-82), H100-side re-design.
 
 Reference loop per bag: DataLoader(batch 128, 4 workers: PIL open + VF.to_tensor) -> `.float().cuda()`
 (synchronous, pageable, 77 MB per batch) -> `i_classifier(patches)` -> `.cpu().numpy()` (a sync per batch)
@@ -268,7 +268,7 @@ def embed_bag(paths: Sequence[str], i_classifier, batch_size: int = 128, num_wor
         fuse_instance_norm(fe)                               # (idempotent; leaves parameters / state_dict untouched)
     fmt = torch.contiguous_format
     if fe is not None and os.environ.get("DSMIL_B200_NHWC", "1") != "0" and any(isinstance(m, torch.nn.Conv2d) for m in fe.modules()):
-        # cuDNN's channels-last kernels run this backbone's convolutions 1.5x faster on B200; values and state_dict are
+        # cuDNN's channels-last kernels for this backbone's convolutions (tools/exp_channels_last.py); values and state_dict are
         # unchanged (only the strides of the 4-D weights), the decoded batch is produced in that layout directly
         fmt = torch.channels_last
         if not getattr(fe, "_dsmil_channels_last", False):

@@ -2,8 +2,8 @@
 ResNet built with `norm_layer=nn.InstanceNorm2d` (compute_feats.py:146-170).  The convolutions stay cuDNN library
 GEMMs; everything between them -- instance norm, the residual add and the ReLU, which the framework runs as two or three
 memory-bound passes per convolution -- goes through ONE kernel of libdsmil_b200.so (`dsmil_instnorm_act`,
-csrc/embed_kernels.cuh), in NCHW or in channels-last memory (`dsmil_instnorm_act_nhwc`): cuDNN runs this backbone's
-convolutions 1.5x faster in channels-last on B200, so `embed.embed_bag` switches the backbone and its input to it.
+csrc/embed_kernels.cuh), in NCHW or in channels-last memory (`dsmil_instnorm_act_nhwc`): `embed.embed_bag`
+switches the backbone and its input to channels-last (tools/exp_channels_last.py times both layouts).
 
     fuse_instance_norm(resnet)   rewires the blocks of a torchvision ResNet in place (parameters, buffers and
                                  state_dict keys untouched, so the reference's embedder checkpoints still load);

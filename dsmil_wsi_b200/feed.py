@@ -40,7 +40,7 @@ def dropout_patches(feats: torch.Tensor, p: float, generator: Optional[torch.Gen
 
 
 class DeviceBagStore:
-    """Bags resident in HBM (180 GB holds thousands of 15 000 x 512 bags), in the `.pt` cache layout."""
+    """Bags resident in HBM (80 GB holds thousands of 15 000 x 512 bags), in the `.pt` cache layout."""
 
     def __init__(self, feats_size: int, device="cuda"):
         self.D = feats_size

@@ -35,7 +35,7 @@ def _f32c(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
 def require_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise RuntimeError(
-            f"dsmil_b200: {what} is on '{t.device}'. The B200-native DSMIL path runs on CUDA only "
+            f"dsmil_b200: {what} is on '{t.device}'. The H100-native DSMIL path runs on CUDA only "
             "(no CPU fallback); move the module and the bag to a CUDA device.")
 
 

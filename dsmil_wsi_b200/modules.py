@@ -83,7 +83,7 @@ class BClassifier(nn.Module):
                 and isinstance(q[1], nn.ReLU) and isinstance(q[2], nn.Linear) and isinstance(q[3], nn.Tanh)):
             return q[0].weight, q[0].bias, q[2].weight, q[2].bias
         raise TypeError("BClassifier.q must be Linear(D,128) or Sequential(Linear, ReLU, Linear, Tanh) "
-                        "(dsmil.py:31,33); other structures have no B200 kernel")
+                        "(dsmil.py:31,33); other structures have no H100 kernel")
 
     def _v_params(self):
         v = self.v

@@ -23,8 +23,7 @@ class HostBagPipeline:
         with torch.cuda.device(self.dev):
             self.slots = [torch.empty(max_rows, feature_size, dtype=torch.float32, device=self.dev)
                           for _ in range(depth)]
-            # two H2D streams, four slots: consecutive bags are in flight on two copy engines (measured on the B200 box:
-            # 51.4 GB/s with one stream / two slots, 52.6-53.5 GB/s with two streams / 4-6 slots -- the link is the bound)
+            # two H2D streams, four slots: consecutive bags are in flight on two copy engines (the host link is the bound)
             self.copy_streams = [torch.cuda.Stream(device=self.dev) for _ in range(max(1, copy_streams))]
             self.h2d_done = [torch.cuda.Event() for _ in range(depth)]
             self.slot_free = [torch.cuda.Event() for _ in range(depth)]

@@ -1,5 +1,5 @@
 /*
- * dsmil_b200.h -- C ABI of libdsmil_b200.so: the DSMIL per-slide aggregator hot path on B200 (sm_100a).
+ * dsmil_b200.h -- C ABI of libdsmil_b200.so: the DSMIL per-slide aggregator hot path on H100 (sm_90a).
  *
  * The reference (binli123/dsmil-wsi) is pure Python/PyTorch and has no FFI of its own; the
  * "interface" each entry point replaces is therefore a span of reference Python, cited per
@@ -90,8 +90,8 @@ int dsmil_patches_u8_to_f32(const uint8_t* in, int64_t B, int32_t H, int32_t W, 
  * HW <= 16384. */
 int dsmil_instnorm_act(const float* x, const float* residual, float* y, int64_t planes, int32_t HW, float eps,
                        int32_t relu, void* stream);
-/* The same operator on channels-last memory, [N][HW][C] fp32 (torch.channels_last: the layout in which cuDNN's
- * convolutions of this backbone run fastest on B200).  C a multiple of 32; statistics per (sample, channel) over HW. */
+/* The same operator on channels-last memory, [N][HW][C] fp32 (torch.channels_last: the layout the embedding loop
+ * runs this backbone's cuDNN convolutions in).  C a multiple of 32; statistics per (sample, channel) over HW. */
 int dsmil_instnorm_act_nhwc(const float* x, const float* residual, float* y, int64_t N, int32_t HW, int32_t C, float eps,
                             int32_t relu, void* stream);
 
@@ -115,13 +115,10 @@ int dsmil_jpeg_decode_batch(const uint8_t* blob, int64_t blob_bytes, const void*
 /* Live per-kernel timing for the roofline report (bench.py): when enabled, tagged launches are
  * bracketed by CUDA events on the launching stream.  dsmil_profile_read synchronises those events,
  * returns summed milliseconds and launch counts per tag (arrays of 8: 0 scores, 1 q-mlp, 2 attend,
- * 3 finalize, 4 fused tcgen05 kernel) and resets the log.  Not thread-safe; bench use only. */
+ * 3 finalize, 4 fused wgmma kernel) and resets the log.  Not thread-safe; bench use only. */
 int dsmil_profile_enable(int on);
 int dsmil_profile_read(double* ms_per_tag, uint64_t* launches_per_tag);
-/* Debug aid: when buf (device int64[3*8*64]) is non-NULL, CTA 0 of the tensor-core kernel stores clock64
- * stamps of its pipeline events there (tools/ktrace.py decodes them).  NULL disables. */
-int dsmil_debug_set_trace(void* buf);
-/* Which kernel family the forward would use for (D,C): 1 = generic fp32 FFMA, 2 = sm_100a tcgen05. */
+/* Which kernel family the forward would use for (D,C): 1 = generic fp32 FFMA, 2 = sm_90a wgmma. */
 int dsmil_forward_path(const dsmil_params_t* p, int64_t N);
 
 /* ---- single-device forward ------------------------------------------------------------

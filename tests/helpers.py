@@ -59,7 +59,7 @@ def pred_tolerance_ok(pred, ref_pred, p: orc.Params, B_ref, tol):
 
 
 def scores_close(a, b, tol=2e-6):
-    """Instance scores from two DIFFERENT kernels (pair kernel / k_qmlp_sm100 / k_scores: each sums the D products of a
+    """Instance scores from two DIFFERENT kernels (k_qmlp_sm90 / k_scores: each sums the D products of a
     row in its own fixed order): equal to the tolerance every path is held to against the reference (2e-6 of the
     largest score); the arg-max they select is asserted bit-exact separately."""
     a = a.detach().float().cpu().numpy().astype(np.float64)

@@ -115,7 +115,7 @@ def test_size_arithmetic():
 
 
 def test_path_selector_is_pure_and_consistent():
-    """dsmil_forward_path: which kernel family a shape takes (1 generic fp32 FFMA, 2 sm_100a tcgen05)."""
+    """dsmil_forward_path: which kernel family a shape takes (1 generic fp32 FFMA, 2 sm_90a wgmma)."""
     import os
     lib = _lib.load()
     if os.environ.get("DSMIL_B200_GENERIC") == "1":

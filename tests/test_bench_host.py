@@ -23,7 +23,7 @@ def test_algorithmic_bytes_match_baseline_md():
 
 def test_warmup_is_rank_invariant_under_torchrun():
     """Every bench step contains two all-gathers when WORLD_SIZE > 1: a time-based warm-up count differs
-    between ranks and deadlocks them (this happened once: profiles/r1_bench_history.md)."""
+    between ranks and deadlocks them."""
     for world in (2, 4, 8):
         fixed, timed, extra = bench.warmup_plan(world, 3)
         assert timed == 0.0 and fixed >= 3 and extra > 0

@@ -265,7 +265,7 @@ def test_errors_are_loud():
 
 @pytest.mark.parametrize("name", ["shipped_tcga", "shipped_c16", "rand_d512_c2", "rand_d512_c1", "tree_d1024_c2"])
 def test_tensor_core_q_mlp_matches_fp64(name):
-    """Phase 1 on the tcgen05 path (3xBF16 split, fp32 accumulate in TMEM): Q, H1-derived outputs and the
+    """Phase 1 on the wgmma path (3xBF16 split, fp32 accumulate): Q, H1-derived outputs and the
     fused instance scores against the fp64 oracle.  Q is tanh-bounded, so the tolerance is absolute."""
     import ctypes
     from dsmil_wsi_b200 import _lib
@@ -318,7 +318,7 @@ def test_forward_bags_generic_shapes_loop():
                                         (1024, 2, 640, "uniform"), (2048, 1, 300, "normal"), (2048, 2, 129, "uniform"),
                                         (512, 2, 1, "normal"), (512, 1, 2, "uniform"), (640, 2, 200, "normal")])
 def test_tensor_core_path_shapes_vs_oracle(D, C, N, kind):
-    """Every (D % 128 == 0, C <= 4) configuration of the tcgen05 path, incl. classes padded to 4 (C = 3), the
+    """Every (D % 128 == 0, C <= 4) configuration of the wgmma path, incl. classes padded to 4 (C = 3), the
     widest feature size of the reference backbones (2048, ResNet-50/101), two-chunk D = 128 and one-row bags."""
     import ctypes
     from dsmil_wsi_b200 import _lib
@@ -342,7 +342,7 @@ def test_tensor_core_path_shapes_vs_oracle(D, C, N, kind):
 
 
 def test_training_step_on_tensor_core_path_matches_oracle_grads():
-    """fwd (tcgen05, Q/H1 saved row-major) + bwd on D=512, C=2, N=3000 against the fp64 manual backward."""
+    """fwd (wgmma, Q/H1 saved row-major) + bwd on D=512, C=2, N=3000 against the fp64 manual backward."""
     p = orc.random_params(512, 2, 55, scale=1.0)
     X = orc.synthetic_bag(3000, 512, 56, "normal")
     y = np.array([0.0, 1.0], np.float32)

@@ -85,10 +85,19 @@ def test_tree_loop_reproduces_reference_csv(gold, tmp_path, monkeypatch, mode):
     # the golden CSV holds 4 decimals of the reference's fp32 result
     assert np.abs(got["feats"].numpy() - want).max() <= 5.1e-5
     csv = os.path.join(str(tmp_path), "c0", "slideT.csv")                           # compute_feats.py:123-125
-    assert np.array_equal(F.read_bag_csv(csv), want.astype(np.float32))
+    vals = F.read_bag_csv(csv)
+    feats = got["feats"].numpy()
+    # the CSV is exactly '%.4f' of our fp32 features ...
+    assert np.array_equal(vals, np.array([[float("%.4f" % v) for v in row] for row in feats], np.float32))
+    # ... and equal to the reference's 4 decimals, except where a feature lies within 2e-6 of a rounding midpoint:
+    # there the fp32 results of two CPUs' convolution kernels (last bits) may round to either neighbour
+    f = feats.astype(np.float64) * 1e4
+    tie = np.abs(f - np.floor(f) - 0.5) < 2e-2
+    w32 = want.astype(np.float32)
+    assert np.all((vals == w32) | (tie & (np.abs(vals.astype(np.float64) - w32) <= 1.01e-4))), (vals, w32)
     exact, _ = F.read_bag_bin(os.path.join(str(tmp_path), "c0", "slideT.bin"))
     assert torch.equal(exact, got["feats"])
-    if np.array_equal(want, gold[f"feats_{mode}"]):     # same listing order as at generation time: same text
+    if np.array_equal(want, gold[f"feats_{mode}"]) and np.array_equal(vals, w32):   # same listing order: same text
         assert open(csv).read() == str(gold[f"csv_{mode}"])
 
 

@@ -1,7 +1,7 @@
 """Experiment: where does the ResNet-18-InstanceNorm embedder spend its time, and would channels_last help?"""
-import sys, json
+import os, sys, json
 import torch, torchvision.models as models
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench
 dev = torch.device('cuda', 0)
 torch.cuda.set_device(0)

@@ -19,7 +19,7 @@ def main():
     net = make_net(Weights(0), dev)
     lib = _lib.load()
     ops = CudaShardOps(milnet_params(net))
-    tags = ["scores", "q_mlp", "attend", "finalize", "fused_sm100"]
+    tags = ["scores", "q_mlp", "attend", "finalize", "fused_sm90"]
     for N in Ns:
         x = torch.rand(N, 512, device=dev)
         flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)

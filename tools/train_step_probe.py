@@ -2,7 +2,7 @@
 how long, and how much of the step is GPU time at all."""
 import sys, os, json
 import torch
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench
 import dsmil as mil
 dev = torch.device('cuda', 0); torch.cuda.set_device(0)
