@@ -171,11 +171,6 @@ static int num_sms() {
   }
   return cached[dev];
 }
-static bool use_sm90(const dsmil_params_t* p) {
-  static int disabled = -1;
-  if (disabled < 0) { const char* e = getenv("DSMIL_B200_GENERIC"); disabled = (e && e[0] == '1') ? 1 : 0; }
-  return !disabled && sm90::qmlp_supported(p);
-}
 
 // Under stream capture (CUDA-graph serving loops) the pageable host->device copies of the bag table cannot be
 // recorded; the captured call then reuses the table that the preceding EAGER call with the same arguments wrote into
@@ -185,51 +180,36 @@ static bool stream_is_capturing(cudaStream_t st) {
   return cudaStreamIsCapturing(st, &cs) == cudaSuccess && cs != cudaStreamCaptureStatusNone;
 }
 
-// tile-blocked Q holds the pre-activation, tanh applied by its readers (DSMIL_B200_QPRE=0: r1 behaviour, tanh in phase 1)
-static int blocked_q_mode() {
-  static int mode = -1;
-  if (mode < 0) { const char* e = getenv("DSMIL_B200_QPRE"); mode = (e && e[0] == '0') ? 1 : 2; }
-  return mode;
-}
-
 static int phase1_impl(const dsmil_params_t* p, const float* X, const float* xv, const float* classes_in,
                        int64_t N, int64_t row_offset, float* classes, float* Q, float* H1, float* V,
                        float* cand, unsigned long long* keys, uint8_t* wimg, cudaStream_t st) {
   const int C = p->C, D = p->D;
   DSMIL_CUDA_OK(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * kMaxC, st));
-  if (N > 0 && use_sm90(p) && wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0) {
+  if (N > 0 && classes_in) {   // bag form: arg-max of the given scores
+    if (classes && classes != classes_in)
+      DSMIL_CUDA_OK(cudaMemcpyAsync(classes, classes_in, sizeof(float) * N * C, cudaMemcpyDeviceToDevice, st));
+    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
+    k_argmax<<<grid, 256, 0, st>>>(classes_in, N, C, keys);
+    DSMIL_LAUNCH_OK("k_argmax");
+  }
+  if (N > 0 && sm90::qmlp_supported(p) && wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0) {
     // tensor-core path: scores + arg-max + Q-MLP in one persistent kernel
     int rc;
-    if (classes_in) {
-      if (classes && classes != classes_in)
-        DSMIL_CUDA_OK(cudaMemcpyAsync(classes, classes_in, sizeof(float) * N * C, cudaMemcpyDeviceToDevice, st));
-      const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
-      k_argmax<<<grid, 256, 0, st>>>(classes_in, N, C, keys);
-      DSMIL_LAUNCH_OK("k_argmax");
-    }
     uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wimg) + 1023) & ~uintptr_t(1023));
     sm90::BagDev* tbl = reinterpret_cast<sm90::BagDev*>(img + sm90::wimg_bytes(D));
     sm90::BagDev one{X, N, 0, 0, 0, 1, 0};
     DSMIL_CUDA_OK(cudaMemcpyAsync(tbl, &one, sizeof(one), cudaMemcpyHostToDevice, st));
     if ((rc = sm90::launch_prep_wimg(p, img, st))) return rc;
     const int ntiles = static_cast<int>((N + sm90::kTileM - 1) / sm90::kTileM);
-    if ((rc = sm90::launch_qmlp(p, tbl, 0, 1, 0, ntiles, classes_in ? nullptr : classes, keys, Q, H1, img, num_sms(), st)))
+    if ((rc = sm90::launch_qmlp(p, tbl, 1, ntiles, classes_in ? nullptr : classes, keys, Q, H1, img, num_sms(), st,
+                                false)))
       return rc;
     if (p->passing_v) {
       if ((rc = launch_linear<ACT_RELU, false>(xv ? xv : X, N, D, p->Wv, p->bv, D, V, nullptr, 0, st))) return rc;
     }
   } else if (N > 0) {
-    if (classes_in) {
-      if (classes && classes != classes_in)
-        DSMIL_CUDA_OK(cudaMemcpyAsync(classes, classes_in, sizeof(float) * N * C, cudaMemcpyDeviceToDevice, st));
-      const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
-      k_argmax<<<grid, 256, 0, st>>>(classes_in, N, C, keys);
-      DSMIL_LAUNCH_OK("k_argmax");
-    } else {
-      int rcs = launch_scores(p, X, N, classes, keys, st);
-      if (rcs) return rcs;
-    }
     int rc;
+    if (!classes_in && (rc = launch_scores(p, X, N, classes, keys, st))) return rc;
     prof_begin(PROF_QMLP, st);
     if (p->nonlinear) {
       if ((rc = launch_linear<ACT_RELU, false>(X, N, D, p->W1, p->b1, kQ, H1, nullptr, 0, st))) return rc;
@@ -320,7 +300,7 @@ static int forward_impl(const dsmil_params_t* p, const float* X, const float* xv
     return DSMIL_ERR_EMPTY;
   }
   DSMIL_REQUIRE(X && pred && A && B && (classes || classes_in), "NULL tensor pointer");
-  if (use_sm90(p) && sm90::batched_supported(p) && (reinterpret_cast<uintptr_t>(X) & 15) == 0)
+  if (sm90::batched_supported(p) && (reinterpret_cast<uintptr_t>(X) & 15) == 0)
     return forward_bags_impl(p, &X, &N, 1, classes_in, classes, pred, A, B, crit_idx, save_Q, save_H1, ws, ws_bytes, st);
   bool ok;
   FwdWs w = carve_fwd(p, N, ws, ws_bytes, &ok);
@@ -333,7 +313,7 @@ static int forward_impl(const dsmil_params_t* p, const float* X, const float* xv
   float* V = p->passing_v ? (save_V ? save_V : w.V) : nullptr;
   if ((rc = phase1_impl(p, X, xv, classes_in, N, 0, classes, Q, H1, V, w.cand, w.keys, w.wimg, st))) return rc;
   int64_t* crit = crit_idx ? crit_idx : w.crit;
-  k_merge_cand<<<p->C, kQ, 0, st>>>(w.cand, 1, p->C, w.qmax, crit);
+  k_merge_cand<<<p->C, kQ, 0, st>>>(w.cand, 1, 1, p->C, w.qmax, crit);
   DSMIL_LAUNCH_OK("k_merge_cand");
   const float* Vv = p->passing_v ? V : X;
   if ((rc = phase2_impl(p, Vv, Q, N, w.qmax, A, w.rec, w.recs, st))) return rc;
@@ -379,17 +359,24 @@ static BagsWs carve_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, boo
   *ok = c.ok();
   return w;
 }
-static size_t l2_budget_bytes() {
-  static size_t v = 0;
-  if (!v) {
-    const char* e = getenv("DSMIL_B200_L2_MB");
-    // Default: no sub-batching.  At the kernels' current speed a second HBM read of X (3 us per 10k-row bag)
-    // costs less than the wave quantisation of small launches; set e.g. DSMIL_B200_L2_MB=72 to keep each
-    // sub-batch L2-resident between phase 1 and phase 2 instead.
-    const long mb = e ? atol(e) : (1l << 20);
-    v = static_cast<size_t>(mb > 0 ? mb : (1l << 20)) << 20;
+// Host copy of the bag table: each bag's first row, 128-row tile and partial record, numbered across the batch.
+static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::vector<sm90::BagDev>& tbl, int* tiles,
+                       int* recs) {
+  long long row = 0;
+  int tile = 0, rec = 0;
+  tbl.resize(nb);
+  for (int b = 0; b < nb; ++b) {
+    DSMIL_REQUIRE(Ns[b] >= 1 && Ns[b] < 0xffffffffll && Xs[b], "bag %d: empty or NULL", b);
+    DSMIL_REQUIRE((reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0, "bag %d: features must be 16-byte aligned", b);
+    const int nrec = recs_for_bag(Ns[b]);
+    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
+    row += Ns[b];
+    tile += static_cast<int>((Ns[b] + sm90::kTileM - 1) / sm90::kTileM);
+    rec += nrec;
   }
-  return v;
+  *tiles = tile;
+  *recs = rec;
+  return 0;
 }
 
 static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
@@ -403,22 +390,12 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
     set_error("workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
     return DSMIL_ERR_WORKSPACE;
   }
-  std::vector<sm90::BagDev> tbl(nb);
-  long long row = 0;
-  int tile = 0, rec = 0;
-  for (int b = 0; b < nb; ++b) {
-    DSMIL_REQUIRE(Ns[b] >= 1 && Ns[b] < 0xffffffffll && Xs[b], "bag %d: empty or NULL", b);
-    DSMIL_REQUIRE((reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0, "bag %d: features must be 16-byte aligned", b);
-    const int nrec = recs_for_bag(Ns[b]);
-    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
-    row += Ns[b];
-    tile += static_cast<int>((Ns[b] + sm90::kTileM - 1) / sm90::kTileM);
-    rec += nrec;
-  }
+  std::vector<sm90::BagDev> tbl;
+  int tiles = 0, recs = 0, rc;
+  if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;
   DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
   DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
   uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(w.wimg) + 1023) & ~uintptr_t(1023));
-  int rc;
   if ((rc = sm90::launch_prep_wimg(p, img, st))) return rc;
   float* Q = save_Q ? save_Q : w.Q;
   if (classes_in) {   // bag form: arg-max of the given scores (single bag only)
@@ -426,34 +403,15 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
     k_argmax<<<grid, 256, 0, st>>>(classes_in, Ns[0], C, w.keys);
     DSMIL_LAUNCH_OK("k_argmax");
   }
-  // sub-batches sized so that a sub-batch's features (+Q) are still in L2 when the attend pass re-reads them
-  const size_t budget = l2_budget_bytes();
-  int b0 = 0;
-  while (b0 < nb) {
-    int b1 = b0;
-    size_t bytes = 0;
-    while (b1 < nb) {
-      const size_t add = static_cast<size_t>(Ns[b1]) * (D + kQ) * sizeof(float);
-      if (b1 > b0 && bytes + add > budget) break;
-      bytes += add;
-      ++b1;
-    }
-    const int t0 = tbl[b0].tile_off;
-    const int t1 = (b1 < nb) ? tbl[b1].tile_off : tile;
-    const int r0 = tbl[b0].rec_off;
-    const int r1 = (b1 < nb) ? tbl[b1].rec_off : rec;
-    const int q_blocked = save_Q ? 0 : blocked_q_mode();   // training keeps Q (after tanh) row-major for the backward kernels
-    if ((rc = sm90::launch_qmlp(p, w.table, b0, b1 - b0, t0, t1 - t0, classes_in ? nullptr : classes, w.keys, Q,
-                                 save_H1, img, num_sms(), st, q_blocked)))
-      return rc;
-    sm90::AttendArgs aa{w.table, b0, b1 - b0, r0, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr};
-    if ((rc = sm90::launch_attend_b(aa, r1 - r0, st))) return rc;
-    sm90::FinalizeArgs fa{w.table, b0, D, C, w.recs, w.keys, p->Wf, p->bf, A, B, pred,
-                           reinterpret_cast<long long*>(crit), w.pred_part, w.counters, nullptr, 0, 0};
-    if ((rc = sm90::launch_finalize_b(fa, b1 - b0, st))) return rc;
-    b0 = b1;
-  }
-  return 0;
+  const bool q_blocked = save_Q == nullptr;   // training keeps Q (after tanh) row-major for the backward kernels
+  if ((rc = sm90::launch_qmlp(p, w.table, nb, tiles, classes_in ? nullptr : classes, w.keys, Q, save_H1, img, num_sms(),
+                              st, q_blocked)))
+    return rc;
+  sm90::AttendArgs aa{w.table, nb, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr};
+  if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
+  sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, p->Wf, p->bf, A, B, pred, reinterpret_cast<long long*>(crit),
+                         w.pred_part, w.counters, nullptr, 0, 0};
+  return sm90::launch_finalize_b(fa, nb, st);
 }
 
 
@@ -475,24 +433,6 @@ static ShardBagsWs carve_shard_bags(const dsmil_params_t* p, const int64_t* Ns, 
   *ok = c.ok();
   return s;
 }
-static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::vector<sm90::BagDev>& tbl, int* tiles,
-                       int* recs) {
-  long long row = 0;
-  int tile = 0, rec = 0;
-  tbl.resize(nb);
-  for (int b = 0; b < nb; ++b) {
-    DSMIL_REQUIRE(Ns[b] >= 1 && Ns[b] < 0xffffffffll && Xs[b], "bag %d: empty or NULL (sharded batches need >= 1 row per rank)", b);
-    DSMIL_REQUIRE((reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0, "bag %d: features must be 16-byte aligned", b);
-    const int nrec = recs_for_bag(Ns[b]);
-    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
-    row += Ns[b];
-    tile += static_cast<int>((Ns[b] + sm90::kTileM - 1) / sm90::kTileM);
-    rec += nrec;
-  }
-  *tiles = tile;
-  *recs = rec;
-  return 0;
-}
 
 }  // namespace dsmil
 
@@ -505,7 +445,7 @@ const char* dsmil_last_error(void) { return g_err; }
 uint64_t dsmil_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 int dsmil_forward_path(const dsmil_params_t* p, int64_t N) {
   (void)N;
-  return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && use_sm90(p)) ? 2 : 1;
+  return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && sm90::qmlp_supported(p)) ? 2 : 1;
 }
 
 
@@ -627,8 +567,8 @@ size_t dsmil_forward_workspace_bytes(const dsmil_params_t* p, int64_t N) {
 size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
   if (!p || !Ns || nb < 1 || p->C < 1 || p->C > DSMIL_MAX_C || p->D < 1 || p->D > DSMIL_MAX_D) return 0;
   bool ok;
-  // dsmil_forward_bags may take either route (tensor-core batch, or the per-bag generic loop when
-  // DSMIL_B200_GENERIC=1 / a bag is not 16-byte aligned): the workspace must cover both layouts.
+  // Even on a shape of the tensor-core batch, a bag that is not 16-byte aligned sends dsmil_forward_bags down the
+  // per-bag loop: the workspace must cover both layouts.
   int64_t mx = 0;
   for (int b = 0; b < nb; ++b) mx = std::max<int64_t>(mx, Ns[b]);
   size_t bytes = carve_fwd(p, mx, nullptr, 0, &ok).bytes;
@@ -643,6 +583,16 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
   if (rc) return rc;
   DSMIL_REQUIRE(Xs && Ns && nb >= 1 && classes && pred && A && B, "NULL pointer or nb < 1");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  bool aligned = true;
+  for (int b = 0; b < nb; ++b) {
+    DSMIL_REQUIRE(Ns[b] >= 0 && Ns[b] < 0xffffffffll, "bag %d: N=%lld out of range", b, (long long)Ns[b]);
+    if (Ns[b] == 0) {
+      set_error("bag %d: empty bag (N == 0): the reference raises IndexError at dsmil.py:53", b);
+      return DSMIL_ERR_EMPTY;
+    }
+    DSMIL_REQUIRE(Xs[b], "bag %d: NULL features", b);
+    aligned = aligned && (reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0;
+  }
   {   // one contract for both routes below: the size dsmil_forward_bags_workspace_bytes reports
     const size_t need = dsmil_forward_bags_workspace_bytes(p, Ns, nb);
     if (!workspace || workspace_bytes < need) {
@@ -650,9 +600,7 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
       return DSMIL_ERR_WORKSPACE;
     }
   }
-  bool aligned = true;
-  for (int b = 0; b < nb; ++b) aligned = aligned && Xs[b] && (reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0 && Ns[b] >= 1;
-  if (use_sm90(p) && sm90::batched_supported(p) && aligned)
+  if (sm90::batched_supported(p) && aligned)
     return forward_bags_impl(p, Xs, Ns, nb, nullptr, classes, pred, A, B, crit_idx, nullptr, nullptr, workspace,
                              workspace_bytes, st);
   // shapes the tensor-core kernels do not take: same packed outputs, one bag at a time
@@ -714,7 +662,7 @@ int dsmil_shard_phase1(const dsmil_params_t* p, const float* X, const float* x_f
     return DSMIL_ERR_WORKSPACE;
   }
   // the tensor-core path keeps H1 in registers; the generic path (also taken for an unaligned X) needs a buffer
-  const bool tc = use_sm90(p) && w.wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
+  const bool tc = sm90::qmlp_supported(p) && w.wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
   float* h1 = p->nonlinear ? (H1 ? H1 : (tc ? nullptr : w.H1)) : nullptr;
   return phase1_impl(p, X, x_for_v, classes_in, N_local, row_offset, classes, Q, h1, V, cand_rec, w.keys, w.wimg,
                      static_cast<cudaStream_t>(stream));
@@ -723,7 +671,7 @@ int dsmil_shard_phase1(const dsmil_params_t* p, const float* X, const float* x_f
 int dsmil_shard_merge_candidates(int32_t C, const float* cand_recs, int32_t G, float* q_max, int64_t* crit_idx,
                                  void* stream) {
   DSMIL_REQUIRE(C >= 1 && C <= DSMIL_MAX_C && G >= 1 && cand_recs && q_max && crit_idx, "bad arguments");
-  k_merge_cand<<<C, kQ, 0, static_cast<cudaStream_t>(stream)>>>(cand_recs, G, C, q_max, crit_idx);
+  k_merge_cand<<<C, kQ, 0, static_cast<cudaStream_t>(stream)>>>(cand_recs, G, 1, C, q_max, crit_idx);
   DSMIL_LAUNCH_OK("k_merge_cand");
   return 0;
 }
@@ -1006,8 +954,7 @@ int dsmil_instance_scores_backward(const dsmil_params_t* p, const float* X, int6
 
 // ---- sharded batch ABI ---------------------------------------------------------------------------
 int dsmil_shard_bags_supported(const dsmil_params_t* p) {
-  return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && use_sm90(p) &&
-          sm90::batched_supported(p)) ? 1 : 0;
+  return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && sm90::batched_supported(p)) ? 1 : 0;
 }
 size_t dsmil_shard_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
   if (!dsmil_shard_bags_supported(p) || !Ns || nb < 1) return 0;
@@ -1036,10 +983,10 @@ int dsmil_shard_bags_phase1(const dsmil_params_t* p, const float* const* Xs, con
   uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(w.base.wimg) + 1023) & ~uintptr_t(1023));
   // (a captured serving loop also reuses the weight images of the preceding eager call: re-capture after a weight update)
   if (!stream_is_capturing(st) && (rc = sm90::launch_prep_wimg(p, img, st))) return rc;
-  if ((rc = sm90::launch_qmlp(p, w.base.table, 0, nb, 0, tiles, classes, w.base.keys, w.base.Q, nullptr, img, num_sms(), st,
-                               blocked_q_mode())))
+  if ((rc = sm90::launch_qmlp(p, w.base.table, nb, tiles, classes, w.base.keys, w.base.Q, nullptr, img, num_sms(), st,
+                              true)))
     return rc;
-  sm90::k_gather_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(w.base.table, w.base.keys, classes, w.base.Q, blocked_q_mode(), w.row_offsets, p->C,
+  sm90::k_gather_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(w.base.table, w.base.keys, classes, w.base.Q, true, w.row_offsets, p->C,
                                                         cand_recs);
   DSMIL_LAUNCH_OK("k_gather_cand_b");
   return 0;
@@ -1058,11 +1005,11 @@ int dsmil_shard_bags_phase2(const dsmil_params_t* p, const float* const* Xs, con
   std::vector<sm90::BagDev> tbl;
   int tiles = 0, recs = 0;
   if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
-  sm90::k_merge_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(cands_all, G, nb, p->C, w.qmax, reinterpret_cast<long long*>(crit_idx));
-  DSMIL_LAUNCH_OK("k_merge_cand_b");
-  sm90::AttendArgs aa{w.base.table, 0, nb, 0, p->D, p->C, w.base.Q, blocked_q_mode(), w.base.keys, A, w.base.recs, w.qmax};
+  k_merge_cand<<<dim3(p->C, nb), kQ, 0, st>>>(cands_all, G, nb, p->C, w.qmax, crit_idx);
+  DSMIL_LAUNCH_OK("k_merge_cand");
+  sm90::AttendArgs aa{w.base.table, nb, p->D, p->C, w.base.Q, true, w.base.keys, A, w.base.recs, w.qmax};
   if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
-  sm90::FinalizeArgs fa{w.base.table, 0, p->D, p->C, w.base.recs, w.base.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
+  sm90::FinalizeArgs fa{w.base.table, p->D, p->C, w.base.recs, w.base.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
                          w.base.pred_part, w.base.counters, recs_out, 0, 0};
   return sm90::launch_finalize_b(fa, nb, st);
 }
@@ -1077,7 +1024,7 @@ int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, con
   bool ok;
   ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
   if (!workspace || !ok) { set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes); return DSMIL_ERR_WORKSPACE; }
-  sm90::FinalizeArgs fa{w.base.table, 0, p->D, p->C, recs_all, w.base.keys, p->Wf, p->bf, A, B, pred, nullptr,
+  sm90::FinalizeArgs fa{w.base.table, p->D, p->C, recs_all, w.base.keys, p->Wf, p->bf, A, B, pred, nullptr,
                          w.base.pred_part, w.base.counters, nullptr, G, nb};
   return sm90::launch_finalize_b(fa, nb, st);
 }

@@ -17,11 +17,10 @@ constexpr int kMaxRecPerBag = 128;
 
 struct AttendArgs {
   const BagDev* bags;
-  int bag0, nb;
-  int rec0;                 // first record index covered by this launch (== blockIdx.x 0)
+  int nb;
   int D, C;
   const float* Q;           // packed [sumN,128] row-major, or tile-blocked column-major (q_blocked)
-  int q_blocked;            // 0 row-major Q; 1 tile blocks of Q; 2 tile blocks of the pre-activation (tanh applied on read)
+  bool q_blocked;           // false: row-major Q; true: tile blocks of the pre-activation (tanh applied on read)
   const unsigned long long* keys;  // [nbags][kMaxC]
   float* A;                 // packed [sumN,C]: receives the raw logits here
   float* recs;              // [total records][rec_floats(C,D)]
@@ -43,9 +42,9 @@ k_attend_b(const AttendArgs a) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int C = a.C, D = a.D;
   // which bag does this CTA belong to?
-  const int rec = a.rec0 + blockIdx.x;
-  int bag = a.bag0;
-  while (bag < a.bag0 + a.nb - 1 && rec >= a.bags[bag + 1].rec_off) ++bag;
+  const int rec = blockIdx.x;
+  int bag = 0;
+  while (bag < a.nb - 1 && rec >= a.bags[bag + 1].rec_off) ++bag;
   const BagDev bg = a.bags[bag];
   const int cta_in_bag = rec - bg.rec_off;
   const int ntiles = static_cast<int>((bg.N + kAttRows - 1) / kAttRows);
@@ -58,9 +57,8 @@ k_attend_b(const AttendArgs a) {
       v = a.qmax_ext[(static_cast<size_t>(bag) * C + k) * kQ + j];
     } else if (k < C) {
       const long long row = key_row(a.keys[static_cast<size_t>(bag) * kMaxC + k]);
-      v = a.q_blocked ? a.Q[static_cast<size_t>(bg.tile_off + row / kAttRows) * (kAttRows * kQ) + j * kAttRows + (row % kAttRows)]
+      v = a.q_blocked ? tanh_ex2(a.Q[static_cast<size_t>(bg.tile_off + row / kAttRows) * (kAttRows * kQ) + j * kAttRows + (row % kAttRows)])
                       : a.Q[(bg.row_off + row) * kQ + j];
-      if (a.q_blocked == 2) v = fast_tanh2(f2{v, 0.f}).x;
     }
     sq[k][j] = v;
   }
@@ -94,16 +92,15 @@ k_attend_b(const AttendArgs a) {
       for (int k = 0; k < CT; ++k) d[k] = 0.f;
 #pragma unroll 4
       for (int c = 0; c < 64; c += 4) {
-        float q0 = __ldg(qb + (c + 0) * kAttRows), q1 = __ldg(qb + (c + 1) * kAttRows);
-        float q2 = __ldg(qb + (c + 2) * kAttRows), q3 = __ldg(qb + (c + 3) * kAttRows);
-        if (a.q_blocked == 2) {                         // the tanh of dsmil.py:31, deferred from the phase-1 epilogue
-          const f2 ta = fast_tanh2(f2{q0, q1}), tb = fast_tanh2(f2{q2, q3});
-          q0 = ta.x; q1 = ta.y; q2 = tb.x; q3 = tb.y;
-        }
+        // one base pointer per step: the four loads issue together with immediate offsets
+        const float* qc = qb + c * kAttRows;
+        // the tanh of dsmil.py:31, deferred from the phase-1 epilogue
+        const f2 ta = fast_tanh2(f2{__ldg(qc), __ldg(qc + kAttRows)});
+        const f2 tb = fast_tanh2(f2{__ldg(qc + 2 * kAttRows), __ldg(qc + 3 * kAttRows)});
 #pragma unroll
         for (int k = 0; k < CT; ++k) {
           const float4 w = *reinterpret_cast<const float4*>(&sq[k][hf * 64 + c]);
-          d[k] = fmaf(q0, w.x, d[k]); d[k] = fmaf(q1, w.y, d[k]); d[k] = fmaf(q2, w.z, d[k]); d[k] = fmaf(q3, w.w, d[k]);
+          d[k] = fmaf(ta.x, w.x, d[k]); d[k] = fmaf(ta.y, w.y, d[k]); d[k] = fmaf(tb.x, w.z, d[k]); d[k] = fmaf(tb.y, w.w, d[k]);
         }
       }
       if (hf == 1) {
@@ -249,7 +246,6 @@ k_attend_b(const AttendArgs a) {
 
 struct FinalizeArgs {
   const BagDev* bags;
-  int bag0;
   int D, C;
   const float* recs;
   const unsigned long long* keys;
@@ -274,8 +270,9 @@ constexpr int kFinSlices = 32;
 // rows of A, combines its share of the B columns -- eight threads per column, each summing every eighth record with
 // all its loads in flight, partials added in a fixed order (deterministic) -- and contributes a partial Conv1d dot
 // product; the last CTA of the bag to finish adds the kFinSlices partials in slice order (dsmil.py:59-61) and writes
-// the critical indices.
-__global__ void __launch_bounds__(256)
+// the critical indices.  4 CTAs per SM (64 registers): left free, ptxas squeezes the kernel under 48 registers for a
+// fifth CTA and spills.
+__global__ void __launch_bounds__(256, 4)
 k_finalize_b(const FinalizeArgs a) {
   __shared__ float sw[kMaxRecPerBag][kMaxC];
   __shared__ float sM[kMaxC], sS[kMaxC];
@@ -284,7 +281,7 @@ k_finalize_b(const FinalizeArgs a) {
   __shared__ unsigned int s_last;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int C = a.C, D = a.D;
-  const int bag = a.bag0 + blockIdx.y;
+  const int bag = blockIdx.y;
   const BagDev bg = a.bags[bag];
   const size_t rstride = rec_floats(C, D);
   const bool ext = a.ext_P > 0;
@@ -394,7 +391,7 @@ k_finalize_b(const FinalizeArgs a) {
 // grid = (C, nb), 128 threads.  row_offsets[b] = global index of the bag's first local row.
 __global__ void __launch_bounds__(128)
 k_gather_cand_b(const BagDev* __restrict__ bags, const unsigned long long* __restrict__ keys,
-                const float* __restrict__ classes, const float* __restrict__ Q, int q_blocked,
+                const float* __restrict__ classes, const float* __restrict__ Q, bool q_blocked,
                 const long long* __restrict__ row_offsets, int C, float* __restrict__ cands) {
   const int k = blockIdx.x, bag = blockIdx.y;
   const BagDev bg = bags[bag];
@@ -413,37 +410,9 @@ k_gather_cand_b(const BagDev* __restrict__ bags, const unsigned long long* __res
     idx[k] = row + row_offsets[bag];
     score[k] = classes[(bg.row_off + row) * C + k];
   }
-  float qv = q_blocked
-      ? Q[static_cast<size_t>(bg.tile_off + row / kAttRows) * (kAttRows * kQ) + threadIdx.x * kAttRows + (row % kAttRows)]
+  qrow[threadIdx.x] = q_blocked
+      ? tanh_ex2(Q[static_cast<size_t>(bg.tile_off + row / kAttRows) * (kAttRows * kQ) + threadIdx.x * kAttRows + (row % kAttRows)])
       : Q[(bg.row_off + row) * kQ + threadIdx.x];
-  if (q_blocked == 2) qv = fast_tanh2(f2{qv, 0.f}).x;
-  qrow[threadIdx.x] = qv;
-}
-
-// Winner per (bag, class) over the G ranks' candidate records cands[g][bag]; grid = (C, nb), 128 threads.
-__global__ void __launch_bounds__(128)
-k_merge_cand_b(const float* __restrict__ cands, int G, int nb, int C, float* __restrict__ qmax,
-               long long* __restrict__ crit) {
-  const int k = blockIdx.x, bag = blockIdx.y;
-  const size_t stride = cand_floats(C);
-  int best_g = -1;
-  uint32_t best_key = 0;
-  long long best_idx = INT64_MAX;
-  for (int g = 0; g < G; ++g) {
-    const float* rec = cands + (static_cast<size_t>(g) * nb + bag) * stride;
-    const long long gi = reinterpret_cast<const long long*>(rec)[k];
-    if (gi == INT64_MAX) continue;
-    const uint32_t key = ordered_key(rec[2 * C + k]);
-    if (best_g < 0 || key > best_key || (key == best_key && gi < best_idx)) { best_g = g; best_key = key; best_idx = gi; }
-  }
-  float* out = qmax + (static_cast<size_t>(bag) * C + k) * kQ;
-  if (best_g < 0) {
-    if (threadIdx.x == 0) crit[static_cast<size_t>(bag) * C + k] = -1;
-    out[threadIdx.x] = 0.f;
-    return;
-  }
-  if (threadIdx.x == 0) crit[static_cast<size_t>(bag) * C + k] = best_idx;
-  out[threadIdx.x] = cands[(static_cast<size_t>(best_g) * nb + bag) * stride + 3 * C + static_cast<size_t>(k) * kQ + threadIdx.x];
 }
 
 inline bool batched_supported(const dsmil_params_t* p) {

@@ -153,17 +153,18 @@ k_gather_cand(const unsigned long long* __restrict__ keys, const float* __restri
   qrow[threadIdx.x] = Q[row * kQ + threadIdx.x];
 }
 
-// Winner per class over G candidate records: max score (NaN first), lowest global index on ties.
+// Winner per (bag, class) over the G candidate records cands[g][bag] of each of nb bags: max score (NaN first),
+// lowest global index on ties.  grid = (C, nb), 128 threads; q_max [nb][C][128], crit_idx [nb][C].
 __global__ void __launch_bounds__(128)
-k_merge_cand(const float* __restrict__ cands, int G, int C, float* __restrict__ q_max,
+k_merge_cand(const float* __restrict__ cands, int G, int nb, int C, float* __restrict__ q_max,
              int64_t* __restrict__ crit_idx) {
-  const int k = blockIdx.x;
+  const int k = blockIdx.x, bag = blockIdx.y;
   const size_t stride = cand_floats(C);
   int best_g = -1;
   uint32_t best_key = 0;
   int64_t best_idx = INT64_MAX;
   for (int g = 0; g < G; ++g) {
-    const float* rec = cands + g * stride;
+    const float* rec = cands + (static_cast<size_t>(g) * nb + bag) * stride;
     const int64_t gi = reinterpret_cast<const int64_t*>(rec)[k];
     if (gi == INT64_MAX) continue;
     const uint32_t key = ordered_key(rec[2 * C + k]);
@@ -171,13 +172,15 @@ k_merge_cand(const float* __restrict__ cands, int G, int C, float* __restrict__ 
       best_g = g; best_key = key; best_idx = gi;
     }
   }
+  float* out = q_max + (static_cast<size_t>(bag) * C + k) * kQ;
+  int64_t* crit = crit_idx + static_cast<size_t>(bag) * C;
   if (best_g < 0) {  // every shard empty
-    if (threadIdx.x == 0) crit_idx[k] = -1;
-    q_max[k * kQ + threadIdx.x] = 0.f;
+    if (threadIdx.x == 0) crit[k] = -1;
+    out[threadIdx.x] = 0.f;
     return;
   }
-  if (threadIdx.x == 0) crit_idx[k] = best_idx;
-  q_max[k * kQ + threadIdx.x] = cands[best_g * stride + 3 * C + static_cast<size_t>(k) * kQ + threadIdx.x];
+  if (threadIdx.x == 0) crit[k] = best_idx;
+  out[threadIdx.x] = cands[(static_cast<size_t>(best_g) * nb + bag) * stride + 3 * C + static_cast<size_t>(k) * kQ + threadIdx.x];
 }
 
 // ------------------------------------------------------------------------------------------

@@ -12,8 +12,8 @@
 //                          3 products per k step: hi*Whi + lo*Whi + hi*Wlo ("3xBF16", error at the fp32 noise floor --
 //                          SURVEY A.4, tests/test_oracle.py), fp32 accumulators in registers (m64n128k16).
 //                          Layer 2: H1 = relu(acc + b1), split the same way, is its A operand straight from the
-//                          accumulator registers; Q = tanh(acc2 + b2) -> global, in tile blocks (column-major) or
-//                          row-major when training keeps it
+//                          accumulator registers; Q -> global: row-major tanh(acc2 + b2) when training keeps it,
+//                          otherwise tile blocks (column-major) of the pre-activation, whose readers apply the tanh
 //        producer warpgroup  : gives most of its registers to the consumers (setmaxnreg); one thread streams the W1
 //                          chunks and, per tile, the two W2 chunks into a kWStages-deep smem ring (mbarrier full /
 //                          empty pairs; a stage is freed when both consumer warpgroups' MMAs on it have retired)
@@ -146,8 +146,7 @@ constexpr int kSmemBags = 96;
 
 struct QmlpArgs {
   const BagDev* bags;
-  int bag0, nb;           // bags [bag0, bag0+nb) are covered by this launch ...
-  int tile0, ntiles;      // ... which are tiles [tile0, tile0+ntiles)
+  int nb, ntiles;         // bags of the table and their 128-row tiles
   int D, C;
   const float* Wi;
   const float* bi;
@@ -159,15 +158,15 @@ struct QmlpArgs {
   unsigned long long* keys;  // [nbags][kMaxC]
   float* Q;               // packed row-major [sumN,128], or (q_blocked) per-tile column-major blocks [tile][128 col][128 row]
   float* H1;              // packed [sumN,128] or NULL
-  int q_blocked;          // 1: Q is written in tile blocks (inference path); 2: tile blocks of the PRE-activation
-                          // z2 = acc + b2 -- the tanh moves to the readers of Q (k_attend_b, k_gather_cand_b)
+  bool q_blocked;         // Q in tile blocks of the PRE-activation z2 = acc + b2 (inference path): the tanh moves to
+                          // the readers of Q (k_attend_b, k_gather_cand_b).  false: row-major tanh(z2)
 };
 
 // Walks the bag table as a role's tile index increases monotonically.
 struct TileCursor {
   const BagDev* bags;
   int bag, last;
-  __device__ TileCursor(const BagDev* b, int bag0, int nb) : bags(b), bag(bag0), last(bag0 + nb - 1) {}
+  __device__ TileCursor(const BagDev* b, int nb) : bags(b), bag(0), last(nb - 1) {}
   __device__ __forceinline__ void seek(int tile) {
     while (bag < last && tile >= bags[bag + 1].tile_off) ++bag;
   }
@@ -204,12 +203,11 @@ k_qmlp_sm90(const QmlpArgs a) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ __align__(8) uint64_t bars[2 * kWStages];
   __shared__ __align__(16) float s_b1[kQ], s_b2[kQ];
-  __shared__ BagDev s_bags[kSmemBags];           // the launch's slice of the bag table (tile-boundary lookups)
+  __shared__ BagDev s_bags[kSmemBags];           // the bag table (tile-boundary lookups)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int D = DT ? DT : a.D, C = a.C;
   const int nchunks = D / kChunkK;
-  const int tile_end = a.tile0 + a.ntiles;
   enum { W_FULL = 0, W_EMPTY = kWStages };
   auto bar = [&](int i) { return smem_u32(&bars[i]); };
 
@@ -220,9 +218,8 @@ k_qmlp_sm90(const QmlpArgs a) {
   if (tid < kQ) { s_b1[tid] = a.b1[tid]; s_b2[tid] = a.b2[tid]; }
   const bool tbl_in_smem = a.nb <= kSmemBags;
   if (tbl_in_smem)
-    for (int i = tid; i < a.nb; i += kThreads) s_bags[i] = a.bags[a.bag0 + i];
-  // cursors below index the table relative to bag0 when it is cached in shared memory
-  const BagDev* tbl = tbl_in_smem ? s_bags : a.bags + a.bag0;
+    for (int i = tid; i < a.nb; i += kThreads) s_bags[i] = a.bags[i];
+  const BagDev* tbl = tbl_in_smem ? s_bags : a.bags;
   if (tid == 0) {
     for (int s = 0; s < kWStages; ++s) { mbar_init(bar(W_FULL + s), 1); mbar_init(bar(W_EMPTY + s), kConsumerWGs); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -241,7 +238,7 @@ k_qmlp_sm90(const QmlpArgs a) {
         bulk_g2s(smem_u32(smem + kOffWRing + stage * kChunkBytes), src, kChunkBytes, bar(W_FULL + stage));
         if (++stage == kWStages) { stage = 0; phase ^= 1; }
       };
-      for (int tile = a.tile0 + blockIdx.x; tile < tile_end; tile += gridDim.x) {
+      for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
         for (int kc = 0; kc < nchunks; ++kc) push(a.w1img + static_cast<size_t>(kc) * kChunkBytes);
         push(a.w2img);
         push(a.w2img + kChunkBytes);
@@ -270,7 +267,7 @@ k_qmlp_sm90(const QmlpArgs a) {
     if (signaller) mbar_arrive(bar(W_EMPTY + s));
   };
 
-  TileCursor cur_bag(tbl, 0, a.nb);
+  TileCursor cur_bag(tbl, a.nb);
   // state of the tile whose chunks are being LOADED (may already be the next tile): 32-bit row numbers
   uint32_t ld_N = 0, ld_row = 0;               // rows in the bag, this thread's first row in the bag
   bool ld_full = false;                        // whole 128-row tile inside the bag: unpredicated loads
@@ -344,12 +341,12 @@ k_qmlp_sm90(const QmlpArgs a) {
     return st;
   };
 
-  int tile = a.tile0 + blockIdx.x;
+  int tile = blockIdx.x;
   float4 x[8];
-  if (tile < tile_end) { open_tile(tile); load_chunk(0, x); }
+  if (tile < a.ntiles) { open_tile(tile); load_chunk(0, x); }
   uint32_t ha[16], la[16], hb[16], lb[16];
-  while (tile < tile_end) {
-    const int my_bag = a.bag0 + cur_bag.bag;   // this tile's bag (the load state moves on below)
+  while (tile < a.ntiles) {
+    const int my_bag = cur_bag.bag;   // this tile's bag (the load state moves on below)
     const uint32_t t_N = ld_N, t_row = ld_row;
     const long long t_rowoff = ld_rowoff;
     const int next_tile = tile + gridDim.x;
@@ -368,7 +365,7 @@ k_qmlp_sm90(const QmlpArgs a) {
       const uint32_t s0 = mma_chunk(ha, la, kc);
       convert(x, kc + 1, hb, lb);
       if (kc + 2 < nchunks) load_chunk(kc + 2, x);
-      else if (next_tile < tile_end) { open_tile(next_tile); load_chunk(0, x); }
+      else if (next_tile < a.ntiles) { open_tile(next_tile); load_chunk(0, x); }
       wg_wait0();
       fence_acc(acc);
       w_release(s0);
@@ -445,22 +442,21 @@ k_qmlp_sm90(const QmlpArgs a) {
       w_release(w0);
       w_release(w1);
     }
-    // ---- Q = tanh(qa + b2) (or the pre-activation, q_blocked == 2) ----
+    // ---- the pre-activation qa + b2 (tile blocks) or Q = tanh(qa + b2) (row-major) ----
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       const int c = 8 * j + 2 * q;
       const float2 bb = *reinterpret_cast<const float2*>(&s_b2[c]);
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        float z0 = qa[4 * j + 2 * i] + bb.x, z1 = qa[4 * j + 2 * i + 1] + bb.y;
+        const float z0 = qa[4 * j + 2 * i] + bb.x, z1 = qa[4 * j + 2 * i + 1] + bb.y;
         if (a.q_blocked) {
           // tile-blocked, column-major: the 8 rows of a lane quad's column are one 32-byte sector
-          if (a.q_blocked == 1) { z0 = tanh_ex2(z0); z1 = tanh_ex2(z1); }
           float* dst = a.Q + static_cast<size_t>(tile) * (kTileM * kQ) + static_cast<size_t>(c) * kTileM + rloc + 8 * i;
           dst[0] = z0;
           dst[kTileM] = z1;
         } else if (t_row + 8 * i < t_N) {
-          // same tanh formulation as the tile-blocked (inference) store: train and eval give the same Q bits
+          // the same tanh_ex2 the readers of the tile blocks apply: train and eval give the same Q bits
           *reinterpret_cast<float2*>(a.Q + (t_rowoff + t_row + 8 * i) * kQ + c) = make_float2(tanh_ex2(z0), tanh_ex2(z1));
         }
       }
@@ -507,15 +503,14 @@ inline int launch_prep_wimg(const dsmil_params_t* p, uint8_t* wimg, cudaStream_t
   return 0;
 }
 
-// scores + arg-max keys + Q (+H1) for the tiles [tile0, tile0+ntiles) of bags [bag0, bag0+nb).
+// scores + arg-max keys + Q (+H1) for the ntiles 128-row tiles of the nb bags of the table.
 // wimg must already hold the images (launch_prep_wimg).
-inline int launch_qmlp(const dsmil_params_t* p, const BagDev* bags_dev, int bag0, int nb, int tile0, int ntiles,
-                       float* classes, unsigned long long* keys, float* Q, float* H1, const uint8_t* wimg,
-                       int num_sms, cudaStream_t st, int q_blocked = 0) {
+inline int launch_qmlp(const dsmil_params_t* p, const BagDev* bags_dev, int nb, int ntiles, float* classes,
+                       unsigned long long* keys, float* Q, float* H1, const uint8_t* wimg, int num_sms, cudaStream_t st,
+                       bool q_blocked) {
   const int D = p->D, C = p->C;
   const uint8_t* w2img = wimg + static_cast<size_t>(D / kChunkK) * kChunkBytes;
-  QmlpArgs a{bags_dev, bag0, nb, tile0, ntiles, D, C, p->Wi, p->bi, p->b1, p->b2, wimg, w2img, classes, keys, Q, H1,
-             q_blocked};
+  QmlpArgs a{bags_dev, nb, ntiles, D, C, p->Wi, p->bi, p->b1, p->b2, wimg, w2img, classes, keys, Q, H1, q_blocked};
   const size_t smem = qmlp_smem_bytes(C, D);
   const int grid = ntiles < num_sms ? ntiles : num_sms;
   auto go = [&](auto kern) -> int {

@@ -138,7 +138,8 @@ int dsmil_forward(const dsmil_params_t* p, const float* X, const float* x_for_v,
 /* A stream of bags in ONE call (throughput form of the same forward; slides/sec in BASELINE.json):
  * Xs[b] -> device features [Ns[b], D] (host arrays of nb entries).  Outputs are packed in bag order:
  * classes / A [sum N, C], pred [nb, C], B [nb, C, D], crit_idx [nb, C].  On the tensor-core path the
- * whole batch costs a handful of launches (bag table + L2-sized sub-batches); other shapes loop. */
+ * whole batch costs a handful of launches (one bag table); other shapes, and bags that are not
+ * 16-byte aligned, loop. */
 size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb);
 int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                        float* classes, float* pred, float* A, float* B, int64_t* crit_idx,

@@ -116,10 +116,7 @@ def test_size_arithmetic():
 
 def test_path_selector_is_pure_and_consistent():
     """dsmil_forward_path: which kernel family a shape takes (1 generic fp32 FFMA, 2 sm_90a wgmma)."""
-    import os
     lib = _lib.load()
-    if os.environ.get("DSMIL_B200_GENERIC") == "1":
-        pytest.skip("generic path forced by the environment")
     assert lib.dsmil_forward_path(C.byref(params()), 10000) == 2
     assert lib.dsmil_forward_path(C.byref(params(D=1024, C_=1)), 10000) == 2
     assert lib.dsmil_forward_path(C.byref(params(D=166, C_=1)), 10000) == 1          # D % 128 != 0
