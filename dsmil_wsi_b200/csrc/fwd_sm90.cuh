@@ -6,7 +6,8 @@
 //                   order in which the consumer threads hold X in their A fragments (see kLogicalK below).
 //   k_qmlp_sm90     persistent, one CTA per SM, 128-row tiles walked through a bag table (ragged batch of bags):
 //        consumer warpgroups x2 : 64 rows of the tile each.  A thread streams its two rows of X with 16-byte loads
-//                          straight into registers (one 64-float chunk ahead, across tile boundaries), adds them into
+//                          straight into registers (one 64-float chunk ahead, across tile boundaries; the chunk
+//                          kPrefetchChunks further on in the tile is requested into L2 with them), adds them into
 //                          the fp32 instance scores (+ packed arg-max key per bag), splits x = hi + lo (two bf16) and
 //                          hands both halves to wgmma as the register A operand -- X never goes through shared memory.
 //                          3 products per k step: hi*Whi + lo*Whi + hi*Wlo ("3xBF16", error at the fp32 noise floor --
@@ -32,6 +33,9 @@ constexpr int kChunkK = 64;            // k per smem operand chunk: 64 bf16 = 12
 constexpr int kTileBytes = kQ * kChunkK * 2;           // 16 KiB: one [128 features x 64 k] bf16 operand tile
 constexpr int kChunkBytes = 2 * kTileBytes;            // hi tile + lo tile
 constexpr int kWStages = 4;
+// X chunks a consumer thread requests into L2 ahead of its loads.  H100 80GB HBM3 at a 400 W limit, 16 bags x 10 000
+// x 512, C = 2, three interleaved runs each (DESIGN §4.1): none 0.210-0.211 ms, 2 0.204, 3 0.207-0.208, 4 0.214
+constexpr int kPrefetchChunks = 2;
 constexpr int kConsumerWGs = 2;
 constexpr int kWarpProd = 4 * kConsumerWGs;      // first warp of the producer warpgroup
 constexpr int kThreads = 128 * (kConsumerWGs + 1);
@@ -52,6 +56,7 @@ __device__ __forceinline__ float4 ldg_stream(const float4* p) {   // read-once d
                : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
   return v;
 }
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // ---- PTX wrappers -------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -282,8 +287,13 @@ k_qmlp_sm90(const QmlpArgs a) {
     ld_full = ld_row - rloc + kTileM <= ld_N;
     xrow = bp->X + static_cast<long long>(ld_row) * D + 4 * q;
   };
-  // x[2s + i]: row rloc + 8i, floats 64 kc + 16 s + 4q .. +3
+  // x[2s + i]: row rloc + 8i, floats 64 kc + 16 s + 4q .. +3.  With the loads of chunk kc, chunk kc + kPrefetchChunks
+  // of the same tile is requested into L2: a row's chunk is two 128-byte lines, and the four threads of a row pair
+  // (q = 0..3) take row rloc + 8 (q >> 1), line q & 1 -- one prefetch per thread, no registers held.  Not with 8
+  // class rows and a run-time D: that instantiation has no register to spare for the address and would spill.
   auto load_chunk = [&](int kc, float4 (&x)[8]) {
+    if ((CT <= 4 || DT != 0) && kc + kPrefetchChunks < nchunks && (ld_full || ld_row + 8 * (q >> 1) < ld_N))
+      prefetch_l2(xrow - 4 * q + static_cast<long long>(q >> 1) * (8ll * D) + (kc + kPrefetchChunks) * kChunkK + (q & 1) * 32);
 #pragma unroll
     for (int s = 0; s < 4; ++s)
 #pragma unroll
