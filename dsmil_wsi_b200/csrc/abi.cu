@@ -104,6 +104,13 @@ static int check_params(const dsmil_params_t* p, bool need_scores = false) {
   return 0;
 }
 
+// 0 when the caller passed a workspace and the carve fits in it; else DSMIL_ERR_WORKSPACE with the size it needs
+static int check_workspace(size_t need, bool ok, const void* ws, size_t cap) {
+  if (ws && ok) return 0;
+  set_error("workspace too small: need %zu bytes, got %zu", need, cap);
+  return DSMIL_ERR_WORKSPACE;
+}
+
 static inline int attend_ctas(int64_t N) {
   const int64_t tiles = (N + kAttendRows - 1) / kAttendRows;
   return static_cast<int>(tiles < kSplits ? (tiles < 1 ? 1 : tiles) : kSplits);
@@ -180,6 +187,11 @@ static bool stream_is_capturing(cudaStream_t st) {
   return cudaStreamIsCapturing(st, &cs) == cudaSuccess && cs != cudaStreamCaptureStatusNone;
 }
 
+// Whether a single-bag phase 1 runs on k_qmlp_sm90, which keeps H1 in registers; the generic path writes it out.
+static bool phase1_on_qmlp(const dsmil_params_t* p, const uint8_t* wimg, const float* X) {
+  return sm90::qmlp_supported(p) && wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
+}
+
 static int phase1_impl(const dsmil_params_t* p, const float* X, const float* xv, const float* classes_in,
                        int64_t N, int64_t row_offset, float* classes, float* Q, float* H1, float* V,
                        float* cand, unsigned long long* keys, uint8_t* wimg, cudaStream_t st) {
@@ -192,7 +204,7 @@ static int phase1_impl(const dsmil_params_t* p, const float* X, const float* xv,
     k_argmax<<<grid, 256, 0, st>>>(classes_in, N, C, keys);
     DSMIL_LAUNCH_OK("k_argmax");
   }
-  if (N > 0 && sm90::qmlp_supported(p) && wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0) {
+  if (N > 0 && phase1_on_qmlp(p, wimg, X)) {
     // tensor-core path: scores + arg-max + Q-MLP in one persistent kernel
     int rc;
     uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wimg) + 1023) & ~uintptr_t(1023));
@@ -304,10 +316,7 @@ static int forward_impl(const dsmil_params_t* p, const float* X, const float* xv
     return forward_bags_impl(p, &X, &N, 1, classes_in, classes, pred, A, B, crit_idx, save_Q, save_H1, ws, ws_bytes, st);
   bool ok;
   FwdWs w = carve_fwd(p, N, ws, ws_bytes, &ok);
-  if (!ws || !ok) {
-    set_error("workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
-    return DSMIL_ERR_WORKSPACE;
-  }
+  if ((rc = check_workspace(w.bytes, ok, ws, ws_bytes))) return rc;
   float* Q = save_Q ? save_Q : w.Q;
   float* H1 = p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr;
   float* V = p->passing_v ? (save_V ? save_V : w.V) : nullptr;
@@ -386,12 +395,10 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
   const int C = p->C, D = p->D;
   bool ok;
   BagsWs w = carve_bags(p, Ns, nb, save_Q == nullptr, ws, ws_bytes, &ok);
-  if (!ws || !ok) {
-    set_error("workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
-    return DSMIL_ERR_WORKSPACE;
-  }
+  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+  if (rc) return rc;
   std::vector<sm90::BagDev> tbl;
-  int tiles = 0, recs = 0, rc;
+  int tiles = 0, recs = 0;
   if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;
   DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
   DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
@@ -520,10 +527,9 @@ int dsmil_jpeg_decode_batch(const uint8_t* blob, int64_t blob_bytes, const void*
                 "headers must be 16-byte, workspace 256-byte, out_f32 16-byte, out_u8 4-byte aligned");
   size_t need = 0;
   JpegBatch a = carve_jpeg(workspace, static_cast<size_t>(workspace_bytes), n, H, W, blob_bytes, &need);
-  if (static_cast<int64_t>(need) > workspace_bytes) {
-    set_error("workspace too small: need %zu bytes, got %lld", need, static_cast<long long>(workspace_bytes));
-    return DSMIL_ERR_WORKSPACE;
-  }
+  const int rc = check_workspace(need, static_cast<int64_t>(need) <= workspace_bytes, workspace,
+                                 static_cast<size_t>(std::max<int64_t>(workspace_bytes, 0)));
+  if (rc) return rc;
   a.blob = blob;
   a.hdr = static_cast<const dsmil_jpeg_header*>(headers);
   a.out_u8 = out_u8;
@@ -593,13 +599,9 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
     DSMIL_REQUIRE(Xs[b], "bag %d: NULL features", b);
     aligned = aligned && (reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0;
   }
-  {   // one contract for both routes below: the size dsmil_forward_bags_workspace_bytes reports
-    const size_t need = dsmil_forward_bags_workspace_bytes(p, Ns, nb);
-    if (!workspace || workspace_bytes < need) {
-      set_error("workspace too small: need %zu bytes, got %zu", need, workspace ? workspace_bytes : size_t(0));
-      return DSMIL_ERR_WORKSPACE;
-    }
-  }
+  // one contract for both routes below: the size dsmil_forward_bags_workspace_bytes reports
+  const size_t need = dsmil_forward_bags_workspace_bytes(p, Ns, nb);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
   if (sm90::batched_supported(p) && aligned)
     return forward_bags_impl(p, Xs, Ns, nb, nullptr, classes, pred, A, B, crit_idx, nullptr, nullptr, workspace,
                              workspace_bytes, st);
@@ -657,13 +659,8 @@ int dsmil_shard_phase1(const dsmil_params_t* p, const float* X, const float* x_f
   DSMIL_REQUIRE(N_local == 0 || !p->passing_v || V, "passing_v needs a V buffer");
   bool ok;
   FwdWs w = carve_fwd(p, N_local, workspace, workspace_bytes, &ok);
-  if (!workspace || !ok) {
-    set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes);
-    return DSMIL_ERR_WORKSPACE;
-  }
-  // the tensor-core path keeps H1 in registers; the generic path (also taken for an unaligned X) needs a buffer
-  const bool tc = sm90::qmlp_supported(p) && w.wimg && (reinterpret_cast<uintptr_t>(X) & 15) == 0;
-  float* h1 = p->nonlinear ? (H1 ? H1 : (tc ? nullptr : w.H1)) : nullptr;
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+  float* h1 = p->nonlinear ? (H1 ? H1 : (phase1_on_qmlp(p, w.wimg, X) ? nullptr : w.H1)) : nullptr;
   return phase1_impl(p, X, x_for_v, classes_in, N_local, row_offset, classes, Q, h1, V, cand_rec, w.keys, w.wimg,
                      static_cast<cudaStream_t>(stream));
 }
@@ -684,10 +681,7 @@ int dsmil_shard_phase2(const dsmil_params_t* p, const float* Xv, const float* Q,
   DSMIL_REQUIRE(rec && q_max && (N_local == 0 || (Xv && Q && A_logits)), "NULL tensor pointer");
   bool ok;
   FwdWs w = carve_fwd(p, N_local, workspace, workspace_bytes, &ok);
-  if (!workspace || !ok) {
-    set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes);
-    return DSMIL_ERR_WORKSPACE;
-  }
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
   return phase2_impl(p, Xv, Q, N_local, q_max, A_logits, rec, w.recs, static_cast<cudaStream_t>(stream));
 }
 
@@ -743,6 +737,79 @@ size_t dsmil_backward_workspace_bytes(const dsmil_params_t* p, int64_t N, int ne
   return carve_bwd(p, N, need_gX, nullptr, 0, &ok).bytes;
 }
 
+// The backward in three phases, cut at its two cross-row sums (t and dq_max).  dsmil_backward runs them in a row;
+// the row-sharded backward runs one per call, with the caller's all-reduces in between.  A rank may hold no rows
+// (N == 0): the per-row launches are skipped and its weight-gradient shares come out zero.
+
+// Phase 1: dB, gWf/gbf, gWi/gbi, dA = Vv dB^T (+ d_A), and t's per-block partials sum_n A*dA in w.tpart (*gs of them).
+static int bwd_phase1_impl(const dsmil_params_t* p, const float* X, const float* Vv, int64_t N, const float* A,
+                           const float* B, const float* d_classes, const float* d_pred, const float* d_A,
+                           const float* d_B, const dsmil_grads_t* g, float* dA, const BwdWs& w, int* gs,
+                           cudaStream_t st) {
+  const int C = p->C, D = p->D;
+  int rc;
+  // bag classifier (dsmil.py:59-61) and B
+  k_bwd_bag<<<ceil_div(static_cast<int64_t>(C) * D, 256), 256, 0, st>>>(p->Wf, B, d_pred, d_B, C, D, w.dB, g->gWf,
+                                                                        g->gbf);
+  DSMIL_LAUNCH_OK("k_bwd_bag");
+  // instance classifier (dsmil.py:11): only rows with non-zero upstream grad contribute
+  if (g->gWi) {
+    if (d_classes && N > 0) { if ((rc = launch_gemm_tn(d_classes, C, X, D, N, w.tnpart, g->gWi, st))) return rc; }
+    else DSMIL_CUDA_OK(cudaMemsetAsync(g->gWi, 0, sizeof(float) * C * D, st));
+  }
+  if (g->gbi) {
+    if (d_classes && N > 0) { if ((rc = launch_colsum(d_classes, C, N, w.cspart, g->gbi, st))) return rc; }
+    else DSMIL_CUDA_OK(cudaMemsetAsync(g->gbi, 0, sizeof(float) * C, st));
+  }
+  *gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
+  if (N == 0) return 0;
+  // dA = V dB^T (+ upstream), softmax-over-instances backward (dsmil.py:56-57)
+  const size_t smem = sizeof(float) * C * D;
+  if (smem > 48 * 1024)
+    DSMIL_CUDA_OK(cudaFuncSetAttribute(k_rowdot, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 8), kSms * 8));
+  k_rowdot<<<grid, 256, smem, st>>>(Vv, N, D, w.dB, C, d_A, dA);
+  DSMIL_LAUNCH_OK("k_rowdot");
+  k_bwd_t_partial<<<*gs, 256, 0, st>>>(A, dA, N, C, w.tpart);
+  DSMIL_LAUNCH_OK("k_bwd_t_partial");
+  return 0;
+}
+
+// Phase 2: dL = A (dA - t) / sqrt(128) in place over dA, t the sum of the P partials in `part`; then
+// dq_max = dL^T Q (dsmil.py:55), zeros when N == 0.
+static int bwd_phase2_impl(const dsmil_params_t* p, int64_t N, const float* A, float* dA, const float* part, int P,
+                           const float* Q, float* dqm, const BwdWs& w, cudaStream_t st) {
+  if (N > 0) {
+    const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
+    k_bwd_dL<<<gs, 256, 0, st>>>(A, dA, N, p->C, part, P);
+    DSMIL_LAUNCH_OK("k_bwd_dL");
+  }
+  return launch_gemm_tn(dA, p->C, Q, kQ, N, w.tnpart, dqm, st);
+}
+
+// Phase 3: dQ rows (+ the critical rows' share, dsmil.py:53-54; k_bwd_dq reads qmax == NULL as "critical rows are
+// local"), back through the Q-MLP into gW2/gb2 and gW1/gb1.  *dz1 is the layer-1 gradient it leaves in w.
+static int bwd_phase3_impl(const dsmil_params_t* p, const float* X, int64_t N, int64_t row_offset, const float* Q,
+                           const float* H1, const float* dL, const float* dqm, const float* qmax, const int64_t* crit,
+                           const dsmil_grads_t* g, const BwdWs& w, const float** dz1, cudaStream_t st) {
+  int rc;
+  if (N > 0) {
+    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N * kQ, 256), kSms * 8));
+    k_bwd_dq<<<grid, 256, 0, st>>>(dL, Q, qmax, dqm, crit, N, row_offset, p->C, p->nonlinear, w.dz2);
+    DSMIL_LAUNCH_OK("k_bwd_dq");
+  }
+  *dz1 = w.dz2;
+  if (p->nonlinear) {
+    if (g->gW2 && (rc = launch_gemm_tn(w.dz2, kQ, H1, kQ, N, w.tnpart, g->gW2, st))) return rc;
+    if (g->gb2 && (rc = launch_colsum(w.dz2, kQ, N, w.cspart, g->gb2, st))) return rc;
+    if (N > 0 && (rc = launch_linear<ACT_MASK_POS, true>(w.dz2, N, kQ, p->W2, nullptr, kQ, w.dz1, H1, 0, st))) return rc;
+    *dz1 = w.dz1;
+  }
+  if (g->gW1 && (rc = launch_gemm_tn(*dz1, kQ, X, p->D, N, w.tnpart, g->gW1, st))) return rc;
+  if (g->gb1 && (rc = launch_colsum(*dz1, kQ, N, w.cspart, g->gb1, st))) return rc;
+  return 0;
+}
+
 int dsmil_backward(const dsmil_params_t* p, const float* X, const float* x_for_v, int64_t N, const float* Q,
                    const float* H1, const float* V, const float* A, const float* B, const int64_t* crit_idx,
                    const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
@@ -757,57 +824,15 @@ int dsmil_backward(const dsmil_params_t* p, const float* X, const float* x_for_v
   const int C = p->C, D = p->D;
   bool ok;
   BwdWs w = carve_bwd(p, N, g->gX != nullptr, workspace, workspace_bytes, &ok);
-  if (!workspace || !ok) {
-    set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes);
-    return DSMIL_ERR_WORKSPACE;
-  }
-  const float* Vv = p->passing_v ? V : X;
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
   const float* Xv = x_for_v ? x_for_v : X;
-  const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
-
-  // bag classifier (dsmil.py:59-61) and B
-  k_bwd_bag<<<ceil_div(static_cast<int64_t>(C) * D, 256), 256, 0, st>>>(p->Wf, B, d_pred, d_B, C, D, w.dB, g->gWf,
-                                                                        g->gbf);
-  DSMIL_LAUNCH_OK("k_bwd_bag");
-  // instance classifier (dsmil.py:11): only rows with non-zero upstream grad contribute
-  if (g->gWi) {
-    if (d_classes) { if ((rc = launch_gemm_tn(d_classes, C, X, D, N, w.tnpart, g->gWi, st))) return rc; }
-    else DSMIL_CUDA_OK(cudaMemsetAsync(g->gWi, 0, sizeof(float) * C * D, st));
-  }
-  if (g->gbi) {
-    if (d_classes) { if ((rc = launch_colsum(d_classes, C, N, w.cspart, g->gbi, st))) return rc; }
-    else DSMIL_CUDA_OK(cudaMemsetAsync(g->gbi, 0, sizeof(float) * C, st));
-  }
-  // dA = V dB^T (+ upstream), softmax-over-instances backward (dsmil.py:56-57)
-  {
-    const size_t smem = sizeof(float) * C * D;
-    if (smem > 48 * 1024)
-      DSMIL_CUDA_OK(cudaFuncSetAttribute(k_rowdot, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 8), kSms * 8));
-    k_rowdot<<<grid, 256, smem, st>>>(Vv, N, D, w.dB, C, d_A, w.dA);
-    DSMIL_LAUNCH_OK("k_rowdot");
-  }
-  k_bwd_t_partial<<<gs, 256, 0, st>>>(A, w.dA, N, C, w.tpart);
-  DSMIL_LAUNCH_OK("k_bwd_t_partial");
-  k_bwd_dL<<<gs, 256, 0, st>>>(A, w.dA, N, C, w.tpart, gs);
-  DSMIL_LAUNCH_OK("k_bwd_dL");
-  const float* dL = w.dA;
-  // dq_max = dL^T Q  (dsmil.py:55), then dQ rows (+ the critical rows' share, dsmil.py:53-54)
-  if ((rc = launch_gemm_tn(dL, C, Q, kQ, N, w.tnpart, w.dqm, st))) return rc;
-  {
-    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N * kQ, 256), kSms * 8));
-    k_bwd_dq<<<grid, 256, 0, st>>>(dL, Q, w.dqm, crit_idx, N, C, p->nonlinear, w.dz2);
-    DSMIL_LAUNCH_OK("k_bwd_dq");
-  }
-  const float* dz1 = w.dz2;
-  if (p->nonlinear) {
-    if (g->gW2 && (rc = launch_gemm_tn(w.dz2, kQ, H1, kQ, N, w.tnpart, g->gW2, st))) return rc;
-    if (g->gb2 && (rc = launch_colsum(w.dz2, kQ, N, w.cspart, g->gb2, st))) return rc;
-    if ((rc = launch_linear<ACT_MASK_POS, true>(w.dz2, N, kQ, p->W2, nullptr, kQ, w.dz1, H1, 0, st))) return rc;
-    dz1 = w.dz1;
-  }
-  if (g->gW1 && (rc = launch_gemm_tn(dz1, kQ, X, D, N, w.tnpart, g->gW1, st))) return rc;
-  if (g->gb1 && (rc = launch_colsum(dz1, kQ, N, w.cspart, g->gb1, st))) return rc;
+  // one rank: k_bwd_dL sums phase 1's partials of t itself (its summation order; no k_sum_partials launch)
+  int gs;
+  const float* dz1;
+  if ((rc = bwd_phase1_impl(p, X, p->passing_v ? V : X, N, A, B, d_classes, d_pred, d_A, d_B, g, w.dA, w, &gs, st)) ||
+      (rc = bwd_phase2_impl(p, N, A, w.dA, w.tpart, gs, Q, w.dqm, w, st)) ||
+      (rc = bwd_phase3_impl(p, X, N, 0, Q, H1, w.dA, w.dqm, nullptr, crit_idx, g, w, &dz1, st)))
+    return rc;
 
   const int ge = static_cast<int>(std::min<int64_t>(ceil_div(N * D, 256), kSms * 8));
   if (p->passing_v) {
@@ -829,17 +854,7 @@ int dsmil_backward(const dsmil_params_t* p, const float* X, const float* x_for_v
   return 0;
 }
 
-// ---- row-sharded backward: dsmil_backward cut at its two cross-row sums (+ the caller's grad all-reduce) ----
-static int shard_bwd_ws(const dsmil_params_t* p, int64_t N, void* ws, size_t cap, BwdWs* w) {
-  bool ok;
-  *w = carve_bwd(p, N, 0, ws, cap, &ok);
-  if (!ws || !ok) {
-    set_error("workspace too small: need %zu bytes, got %zu", w->bytes, cap);
-    return DSMIL_ERR_WORKSPACE;
-  }
-  return 0;
-}
-
+// ---- row-sharded backward: dsmil_backward's three phases, one per call (+ the caller's grad all-reduce) ----
 int dsmil_shard_backward_phase1(const dsmil_params_t* p, const float* X, int64_t N, const float* A, const float* B,
                                 const float* d_classes, const float* d_pred, float* dA, float* t_local, float* gWi,
                                 float* gbi, float* gWf, float* gbf, void* workspace, size_t workspace_bytes,
@@ -849,35 +864,18 @@ int dsmil_shard_backward_phase1(const dsmil_params_t* p, const float* X, int64_t
   DSMIL_REQUIRE(!p->passing_v, "sharded backward supports the identity v only");
   DSMIL_REQUIRE(N >= 0 && B && t_local && (N == 0 || (X && A && dA)), "NULL tensor pointer or N < 0");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int C = p->C, D = p->D;
-  BwdWs w;
-  if ((rc = shard_bwd_ws(p, N, workspace, workspace_bytes, &w))) return rc;
-  k_bwd_bag<<<ceil_div(static_cast<int64_t>(C) * D, 256), 256, 0, st>>>(p->Wf, B, d_pred, nullptr, C, D, w.dB, gWf, gbf);
-  DSMIL_LAUNCH_OK("k_bwd_bag");
-  if (gWi) {
-    if (d_classes && N > 0) { if ((rc = launch_gemm_tn(d_classes, C, X, D, N, w.tnpart, gWi, st))) return rc; }
-    else DSMIL_CUDA_OK(cudaMemsetAsync(gWi, 0, sizeof(float) * C * D, st));
-  }
-  if (gbi) {
-    if (d_classes && N > 0) { if ((rc = launch_colsum(d_classes, C, N, w.cspart, gbi, st))) return rc; }
-    else DSMIL_CUDA_OK(cudaMemsetAsync(gbi, 0, sizeof(float) * C, st));
-  }
+  bool ok;
+  BwdWs w = carve_bwd(p, N, 0, workspace, workspace_bytes, &ok);
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+  dsmil_grads_t g{};
+  g.gWi = gWi; g.gbi = gbi; g.gWf = gWf; g.gbf = gbf;
+  int gs;
+  if ((rc = bwd_phase1_impl(p, X, X, N, A, B, d_classes, d_pred, nullptr, nullptr, &g, dA, w, &gs, st))) return rc;
   if (N == 0) {
-    DSMIL_CUDA_OK(cudaMemsetAsync(t_local, 0, sizeof(float) * C, st));
+    DSMIL_CUDA_OK(cudaMemsetAsync(t_local, 0, sizeof(float) * p->C, st));
     return 0;
   }
-  const size_t smem = sizeof(float) * C * D;
-  if (smem > 48 * 1024)
-    DSMIL_CUDA_OK(cudaFuncSetAttribute(k_rowdot, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 8), kSms * 8));
-  k_rowdot<<<grid, 256, smem, st>>>(X, N, D, w.dB, C, nullptr, dA);
-  DSMIL_LAUNCH_OK("k_rowdot");
-  const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
-  k_bwd_t_partial<<<gs, 256, 0, st>>>(A, dA, N, C, w.tpart);
-  DSMIL_LAUNCH_OK("k_bwd_t_partial");
-  k_sum_partials<<<1, 256, 0, st>>>(w.tpart, gs, C, t_local);
-  DSMIL_LAUNCH_OK("k_sum_partials");
-  return 0;
+  return launch_sum_partials(w.tpart, gs, p->C, t_local, st);
 }
 
 int dsmil_shard_backward_phase2(const dsmil_params_t* p, int64_t N, const float* A, float* dA, const float* t_global,
@@ -886,16 +884,10 @@ int dsmil_shard_backward_phase2(const dsmil_params_t* p, int64_t N, const float*
   int rc = check_params(p);
   if (rc) return rc;
   DSMIL_REQUIRE(N >= 0 && t_global && dqm_local && (N == 0 || (A && dA && Q)), "NULL tensor pointer or N < 0");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int C = p->C;
-  BwdWs w;
-  if ((rc = shard_bwd_ws(p, N, workspace, workspace_bytes, &w))) return rc;
-  if (N > 0) {
-    const int gs = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
-    k_bwd_dL<<<gs, 256, 0, st>>>(A, dA, N, C, t_global, 1);
-    DSMIL_LAUNCH_OK("k_bwd_dL");
-  }
-  return launch_gemm_tn(dA, C, Q, kQ, N, w.tnpart, dqm_local, st);   // zeros when N == 0
+  bool ok;
+  BwdWs w = carve_bwd(p, N, 0, workspace, workspace_bytes, &ok);
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+  return bwd_phase2_impl(p, N, A, dA, t_global, 1, Q, dqm_local, w, static_cast<cudaStream_t>(stream));
 }
 
 int dsmil_shard_backward_phase3(const dsmil_params_t* p, const float* X, int64_t N, int64_t row_offset, const float* Q,
@@ -906,25 +898,14 @@ int dsmil_shard_backward_phase3(const dsmil_params_t* p, const float* X, int64_t
   if (rc) return rc;
   DSMIL_REQUIRE(N >= 0 && dqm_global && q_max && crit_idx && (N == 0 || (X && Q && dL)), "NULL tensor pointer or N < 0");
   DSMIL_REQUIRE(!p->nonlinear || N == 0 || H1, "nonlinear q backward needs saved H1");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int D = p->D, C = p->C;
-  BwdWs w;
-  if ((rc = shard_bwd_ws(p, N, workspace, workspace_bytes, &w))) return rc;
-  const float* dz1 = w.dz2;
-  if (N > 0) {
-    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N * kQ, 256), kSms * 8));
-    k_bwd_dq_shard<<<grid, 256, 0, st>>>(dL, Q, q_max, dqm_global, crit_idx, N, row_offset, C, p->nonlinear, w.dz2);
-    DSMIL_LAUNCH_OK("k_bwd_dq_shard");
-  }
-  if (p->nonlinear) {
-    if (gW2 && (rc = launch_gemm_tn(w.dz2, kQ, H1, kQ, N, w.tnpart, gW2, st))) return rc;
-    if (gb2 && (rc = launch_colsum(w.dz2, kQ, N, w.cspart, gb2, st))) return rc;
-    if (N > 0 && (rc = launch_linear<ACT_MASK_POS, true>(w.dz2, N, kQ, p->W2, nullptr, kQ, w.dz1, H1, 0, st))) return rc;
-    dz1 = w.dz1;
-  }
-  if (gW1 && (rc = launch_gemm_tn(dz1, kQ, X, D, N, w.tnpart, gW1, st))) return rc;
-  if (gb1 && (rc = launch_colsum(dz1, kQ, N, w.cspart, gb1, st))) return rc;
-  return 0;
+  bool ok;
+  BwdWs w = carve_bwd(p, N, 0, workspace, workspace_bytes, &ok);
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+  dsmil_grads_t g{};
+  g.gW1 = gW1; g.gb1 = gb1; g.gW2 = gW2; g.gb2 = gb2;
+  const float* dz1;
+  return bwd_phase3_impl(p, X, N, row_offset, Q, H1, dL, dqm_global, q_max, crit_idx, &g, w, &dz1,
+                         static_cast<cudaStream_t>(stream));
 }
 
 int dsmil_instance_scores_backward(const dsmil_params_t* p, const float* X, int64_t N, const float* d_classes,
@@ -937,11 +918,8 @@ int dsmil_instance_scores_backward(const dsmil_params_t* p, const float* X, int6
   Carver c(workspace, workspace_bytes);
   float* tnpart = c.take<float>(tn_partial_floats(C, D, N));
   float* cspart = c.take<float>(static_cast<size_t>(kSplits) * kMaxC);
-  if (!workspace || !c.ok()) {
-    set_error("workspace too small: need %zu bytes, got %zu", c.off, workspace_bytes);
-    return DSMIL_ERR_WORKSPACE;
-  }
-  int rc;
+  int rc = check_workspace(c.off, c.ok(), workspace, workspace_bytes);
+  if (rc) return rc;
   if (gWi && (rc = launch_gemm_tn(d_classes, C, X, D, N, tnpart, gWi, st))) return rc;
   if (gbi && (rc = launch_colsum(d_classes, C, N, cspart, gbi, st))) return rc;
   if (gX) {
@@ -971,7 +949,7 @@ int dsmil_shard_bags_phase1(const dsmil_params_t* p, const float* const* Xs, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
   ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
-  if (!workspace || !ok) { set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes); return DSMIL_ERR_WORKSPACE; }
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
   std::vector<sm90::BagDev> tbl;
   int tiles = 0, recs = 0;
   if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;
@@ -1001,7 +979,7 @@ int dsmil_shard_bags_phase2(const dsmil_params_t* p, const float* const* Xs, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
   ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
-  if (!workspace || !ok) { set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes); return DSMIL_ERR_WORKSPACE; }
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
   std::vector<sm90::BagDev> tbl;
   int tiles = 0, recs = 0;
   if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
@@ -1023,7 +1001,7 @@ int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
   ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
-  if (!workspace || !ok) { set_error("workspace too small: need %zu bytes, got %zu", w.bytes, workspace_bytes); return DSMIL_ERR_WORKSPACE; }
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
   sm90::FinalizeArgs fa{w.base.table, p->D, p->C, recs_all, w.base.keys, p->Wf, p->bf, A, B, pred, nullptr,
                          w.base.pred_part, w.base.counters, nullptr, G, nb};
   return sm90::launch_finalize_b(fa, nb, st);

@@ -98,50 +98,20 @@ k_bwd_dL(const float* __restrict__ A, float* __restrict__ dA, int64_t N, int C,
   }
 }
 
-// dz[n,j] = (sum_k dL[n,k]*Q[idx_k,j] + sum_k [n==idx_k] dqm[k,j]) * (tanh ? 1 - Q[n,j]^2 : 1)
+// dz[n,j] = (sum_k dL[n,k]*qmax[k,j] + sum_k [n==idx_k] dqm[k,j]) * (tanh ? 1 - Q[n,j]^2 : 1), idx_k = crit[k] -
+// row_offset: the dqm share goes to the row whose GLOBAL number n + row_offset is crit[k].  qmax is the forward's
+// exchanged q_max when the critical row may live on another rank; NULL reads it from the local rows, Q[idx_k].
 __global__ void __launch_bounds__(256)
-k_bwd_dq(const float* __restrict__ dL, const float* __restrict__ Q, const float* __restrict__ dqm,
-         const int64_t* __restrict__ crit, int64_t N, int C, int through_tanh, float* __restrict__ dz) {
+k_bwd_dq(const float* __restrict__ dL, const float* __restrict__ Q, const float* __restrict__ qmax,
+         const float* __restrict__ dqm, const int64_t* __restrict__ crit, int64_t N, int64_t row_offset, int C,
+         int through_tanh, float* __restrict__ dz) {
   __shared__ float sq[kMaxC][kQ];
   __shared__ float sd[kMaxC][kQ];
   __shared__ int64_t sidx[kMaxC];
   for (int i = threadIdx.x; i < C * kQ; i += blockDim.x) {
     const int k = i / kQ, j = i % kQ;
-    sq[k][j] = Q[crit[k] * kQ + j];
+    sq[k][j] = qmax ? qmax[i] : Q[(crit[k] - row_offset) * kQ + j];
     sd[k][j] = dqm[i];
-  }
-  if (threadIdx.x < C) sidx[threadIdx.x] = crit[threadIdx.x];
-  __syncthreads();
-  const int64_t total = N * kQ;
-  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
-  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
-    const int64_t n = i / kQ;
-    const int j = static_cast<int>(i % kQ);
-    float g = 0.f;
-    for (int k = 0; k < C; ++k) {
-      g = fmaf(dL[n * C + k], sq[k][j], g);
-      if (n == sidx[k]) g += sd[k][j];
-    }
-    if (through_tanh) {
-      const float q = Q[i];
-      g *= (1.f - q * q);
-    }
-    dz[i] = g;
-  }
-}
-
-// Row-sharded form of k_bwd_dq: q_max comes from the forward's exchange (the critical row may live on another
-// rank) and the dqm share is added where the GLOBAL row number n + row_offset equals crit[k].
-__global__ void __launch_bounds__(256)
-k_bwd_dq_shard(const float* __restrict__ dL, const float* __restrict__ Q, const float* __restrict__ qmax,
-               const float* __restrict__ dqm, const int64_t* __restrict__ crit, int64_t N, int64_t row_offset, int C,
-               int through_tanh, float* __restrict__ dz) {
-  __shared__ float sq[kMaxC][kQ];
-  __shared__ float sd[kMaxC][kQ];
-  __shared__ int64_t sidx[kMaxC];
-  for (int i = threadIdx.x; i < C * kQ; i += blockDim.x) {
-    sq[i / kQ][i % kQ] = qmax[i];
-    sd[i / kQ][i % kQ] = dqm[i];
   }
   if (threadIdx.x < C) sidx[threadIdx.x] = crit[threadIdx.x] - row_offset;
   __syncthreads();
