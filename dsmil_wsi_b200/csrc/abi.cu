@@ -116,18 +116,92 @@ static inline int attend_ctas(int64_t N) {
   return static_cast<int>(tiles < kSplits ? (tiles < 1 ? 1 : tiles) : kSplits);
 }
 
-struct FwdWs {
-  unsigned long long* keys;
+static int num_sms() {
+  static int cached[64] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kSms;
+  if (!cached[dev]) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kSms;
+    cached[dev] = n;
+  }
+  return cached[dev];
+}
+
+// ---- tensor-core phase 1 (k_qmlp_sm90) of nb bags: the single-bag, batched and sharded forwards share it ----------
+struct Phase1Ws {
+  sm90::BagDev* table;       // [nb]
+  unsigned long long* keys;  // [nb][kMaxC] arg-max keys, then nb finalize arrival counters: one memset zeroes both
+  unsigned int* counters;
+  uint8_t* wimg;             // bf16 weight images, 1024-byte aligned; NULL on shapes k_qmlp_sm90 does not take
+};
+static void carve_phase1(Carver& c, const dsmil_params_t* p, int nb, Phase1Ws& w) {
+  w.table = c.take<sm90::BagDev>(nb);
+  w.keys = c.take<unsigned long long>(static_cast<size_t>(nb) * (kMaxC + 1));
+  w.counters = reinterpret_cast<unsigned int*>(w.keys ? w.keys + static_cast<size_t>(nb) * kMaxC : nullptr);
+  w.wimg = nullptr;
+  if (sm90::qmlp_supported(p)) {
+    const uintptr_t img = reinterpret_cast<uintptr_t>(c.take<uint8_t>(sm90::wimg_bytes(p->D) + 1024));
+    w.wimg = reinterpret_cast<uint8_t*>((img + 1023) & ~uintptr_t(1023));
+  }
+}
+
+static inline int recs_for_bag(int64_t N) {
+  const int64_t t = (N + sm90::kAttRows - 1) / sm90::kAttRows;
+  return static_cast<int>(t < sm90::kMaxRecPerBag ? (t < 1 ? 1 : t) : sm90::kMaxRecPerBag);
+}
+// Host copy of the bag table: each bag's first row, 128-row tile and partial record, numbered across the batch.
+static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::vector<sm90::BagDev>& tbl, int* tiles,
+                       int* recs) {
+  long long row = 0;
+  int tile = 0, rec = 0;
+  tbl.resize(nb);
+  for (int b = 0; b < nb; ++b) {
+    DSMIL_REQUIRE(Ns[b] >= 1 && Ns[b] < 0xffffffffll && Xs[b], "bag %d: empty or NULL", b);
+    DSMIL_REQUIRE((reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0, "bag %d: features must be 16-byte aligned", b);
+    const int nrec = recs_for_bag(Ns[b]);
+    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
+    row += Ns[b];
+    tile += static_cast<int>((Ns[b] + sm90::kTileM - 1) / sm90::kTileM);
+    rec += nrec;
+  }
+  *tiles = tile;
+  *recs = rec;
+  return 0;
+}
+
+// Scores (or, single bag only, the arg-max of the given scores classes_in), arg-max keys and Q (+ H1 when non-NULL)
+// of the nb bags; *tiles and *recs return the batch's 128-row tiles and partial records.  upload == false leaves the
+// table and the weight images as an earlier call with the same arguments wrote them into the same workspace.
+static int bags_phase1_impl(const dsmil_params_t* p, const Phase1Ws& w, const float* const* Xs, const int64_t* Ns,
+                            int nb, const float* classes_in, float* classes, float* Q, float* H1, bool q_blocked,
+                            bool upload, int* tiles, int* recs, cudaStream_t st) {
+  std::vector<sm90::BagDev> tbl;
+  int rc;
+  if ((rc = build_table(Xs, Ns, nb, tbl, tiles, recs))) return rc;
+  if (upload)
+    DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
+  if (upload && (rc = sm90::launch_prep_wimg(p, w.wimg, st))) return rc;
+  if (classes_in) {
+    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(Ns[0], 256), kSplits));
+    k_argmax<<<grid, 256, 0, st>>>(classes_in, Ns[0], p->C, w.keys);
+    DSMIL_LAUNCH_OK("k_argmax");
+  }
+  return sm90::launch_qmlp(p, w.table, nb, *tiles, classes_in ? nullptr : classes, w.keys, Q, H1, w.wimg, num_sms(),
+                           st, q_blocked);
+}
+
+struct FwdWs : Phase1Ws {
   float *Q, *H1, *V, *cand, *qmax, *recs, *rec;
   int64_t* crit;
-  uint8_t* wimg;
   size_t bytes;
 };
 static FwdWs carve_fwd(const dsmil_params_t* p, int64_t N, void* ws, size_t cap, bool* ok) {
   Carver c(ws, cap);
   FwdWs w;
   const int64_t n = N > 0 ? N : 1;
-  w.keys = c.take<unsigned long long>(kMaxC);
+  carve_phase1(c, p, 1, w);
   w.Q = c.take<float>(n * kQ);
   w.H1 = p->nonlinear ? c.take<float>(n * kQ) : nullptr;
   w.V = p->passing_v ? c.take<float>(n * p->D) : nullptr;
@@ -136,7 +210,6 @@ static FwdWs carve_fwd(const dsmil_params_t* p, int64_t N, void* ws, size_t cap,
   w.crit = c.take<int64_t>(kMaxC);
   w.recs = c.take<float>(static_cast<size_t>(attend_ctas(N)) * rec_floats(p->C, p->D));
   w.rec = c.take<float>(rec_floats(p->C, p->D));
-  w.wimg = sm90::qmlp_supported(p) ? c.take<uint8_t>(sm90::wimg_bytes(p->D) + 1024 + 256) : nullptr;
   w.bytes = c.off;
   *ok = c.ok();
   return w;
@@ -167,18 +240,6 @@ static int launch_scores(const dsmil_params_t* p, const float* X, int64_t N, flo
   return 0;
 }
 
-static int num_sms() {
-  static int cached[64] = {0};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kSms;
-  if (!cached[dev]) {
-    int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kSms;
-    cached[dev] = n;
-  }
-  return cached[dev];
-}
-
 // Under stream capture (CUDA-graph serving loops) the pageable host->device copies of the bag table cannot be
 // recorded; the captured call then reuses the table that the preceding EAGER call with the same arguments wrote into
 // the same workspace (dsmil_wsi_b200.sharded.ShardedBagsGraph does exactly that: warm-up run, then capture).
@@ -194,48 +255,40 @@ static bool phase1_on_qmlp(const dsmil_params_t* p, const uint8_t* wimg, const f
 
 static int phase1_impl(const dsmil_params_t* p, const float* X, const float* xv, const float* classes_in,
                        int64_t N, int64_t row_offset, float* classes, float* Q, float* H1, float* V,
-                       float* cand, unsigned long long* keys, uint8_t* wimg, cudaStream_t st) {
+                       float* cand, const Phase1Ws& w, cudaStream_t st) {
   const int C = p->C, D = p->D;
-  DSMIL_CUDA_OK(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * kMaxC, st));
-  if (N > 0 && classes_in) {   // bag form: arg-max of the given scores
-    if (classes && classes != classes_in)
-      DSMIL_CUDA_OK(cudaMemcpyAsync(classes, classes_in, sizeof(float) * N * C, cudaMemcpyDeviceToDevice, st));
-    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
-    k_argmax<<<grid, 256, 0, st>>>(classes_in, N, C, keys);
-    DSMIL_LAUNCH_OK("k_argmax");
-  }
-  if (N > 0 && phase1_on_qmlp(p, wimg, X)) {
+  int rc;
+  if (N > 0 && classes_in && classes && classes != classes_in)
+    DSMIL_CUDA_OK(cudaMemcpyAsync(classes, classes_in, sizeof(float) * N * C, cudaMemcpyDeviceToDevice, st));
+  if (N > 0 && phase1_on_qmlp(p, w.wimg, X)) {
     // tensor-core path: scores + arg-max + Q-MLP in one persistent kernel
-    int rc;
-    uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wimg) + 1023) & ~uintptr_t(1023));
-    sm90::BagDev* tbl = reinterpret_cast<sm90::BagDev*>(img + sm90::wimg_bytes(D));
-    sm90::BagDev one{X, N, 0, 0, 0, 1, 0};
-    DSMIL_CUDA_OK(cudaMemcpyAsync(tbl, &one, sizeof(one), cudaMemcpyHostToDevice, st));
-    if ((rc = sm90::launch_prep_wimg(p, img, st))) return rc;
-    const int ntiles = static_cast<int>((N + sm90::kTileM - 1) / sm90::kTileM);
-    if ((rc = sm90::launch_qmlp(p, tbl, 1, ntiles, classes_in ? nullptr : classes, keys, Q, H1, img, num_sms(), st,
-                                false)))
-      return rc;
-    if (p->passing_v) {
-      if ((rc = launch_linear<ACT_RELU, false>(xv ? xv : X, N, D, p->Wv, p->bv, D, V, nullptr, 0, st))) return rc;
-    }
-  } else if (N > 0) {
-    int rc;
-    if (!classes_in && (rc = launch_scores(p, X, N, classes, keys, st))) return rc;
-    prof_begin(PROF_QMLP, st);
-    if (p->nonlinear) {
-      if ((rc = launch_linear<ACT_RELU, false>(X, N, D, p->W1, p->b1, kQ, H1, nullptr, 0, st))) return rc;
-      if ((rc = launch_linear<ACT_TANH, false>(H1, N, kQ, p->W2, p->b2, kQ, Q, nullptr, 0, st))) return rc;
-    } else {
-      if ((rc = launch_linear<ACT_NONE, false>(X, N, D, p->W1, p->b1, kQ, Q, nullptr, 0, st))) return rc;
-    }
-    prof_end(PROF_QMLP, st);
-    if (p->passing_v) {
-      if ((rc = launch_linear<ACT_RELU, false>(xv ? xv : X, N, D, p->Wv, p->bv, D, V, nullptr, 0, st))) return rc;
+    int tiles, recs;
+    if ((rc = bags_phase1_impl(p, w, &X, &N, 1, classes_in, classes, Q, H1, false, true, &tiles, &recs, st))) return rc;
+  } else {
+    DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * kMaxC, st));
+    if (N > 0) {
+      if (classes_in) {   // bag form: arg-max of the given scores
+        const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, 256), kSplits));
+        k_argmax<<<grid, 256, 0, st>>>(classes_in, N, C, w.keys);
+        DSMIL_LAUNCH_OK("k_argmax");
+      } else if ((rc = launch_scores(p, X, N, classes, w.keys, st))) {
+        return rc;
+      }
+      prof_begin(PROF_QMLP, st);
+      if (p->nonlinear) {
+        if ((rc = launch_linear<ACT_RELU, false>(X, N, D, p->W1, p->b1, kQ, H1, nullptr, 0, st))) return rc;
+        if ((rc = launch_linear<ACT_TANH, false>(H1, N, kQ, p->W2, p->b2, kQ, Q, nullptr, 0, st))) return rc;
+      } else {
+        if ((rc = launch_linear<ACT_NONE, false>(X, N, D, p->W1, p->b1, kQ, Q, nullptr, 0, st))) return rc;
+      }
+      prof_end(PROF_QMLP, st);
     }
   }
+  if (N > 0 && p->passing_v &&
+      (rc = launch_linear<ACT_RELU, false>(xv ? xv : X, N, D, p->Wv, p->bv, D, V, nullptr, 0, st)))
+    return rc;
   const float* cls = classes_in ? classes_in : classes;
-  k_gather_cand<<<C, kQ, 0, st>>>(keys, cls, Q, N, C, row_offset, cand);
+  k_gather_cand<<<C, kQ, 0, st>>>(w.keys, cls, Q, N, C, row_offset, cand);
   DSMIL_LAUNCH_OK("k_gather_cand");
   return 0;
 }
@@ -320,7 +373,7 @@ static int forward_impl(const dsmil_params_t* p, const float* X, const float* xv
   float* Q = save_Q ? save_Q : w.Q;
   float* H1 = p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr;
   float* V = p->passing_v ? (save_V ? save_V : w.V) : nullptr;
-  if ((rc = phase1_impl(p, X, xv, classes_in, N, 0, classes, Q, H1, V, w.cand, w.keys, w.wimg, st))) return rc;
+  if ((rc = phase1_impl(p, X, xv, classes_in, N, 0, classes, Q, H1, V, w.cand, w, st))) return rc;
   int64_t* crit = crit_idx ? crit_idx : w.crit;
   k_merge_cand<<<p->C, kQ, 0, st>>>(w.cand, 1, 1, p->C, w.qmax, crit);
   DSMIL_LAUNCH_OK("k_merge_cand");
@@ -331,61 +384,33 @@ static int forward_impl(const dsmil_params_t* p, const float* X, const float* xv
 
 
 // ---- batched forward: a stream of bags in a handful of launches (tensor-core path only) -----------
-struct BagsWs {
-  sm90::BagDev* table;
-  unsigned long long* keys;
+struct BagsWs : Phase1Ws {
   float* Q;
-  uint8_t* wimg;
   float* recs;
   float* pred_part;
-  unsigned int* counters;
+  long long* row_offsets;   // row-sharded batch only: [nb] device copy
+  float* qmax;              // row-sharded batch only: [nb][C][128]
   size_t bytes;
 };
-static inline int recs_for_bag(int64_t N) {
-  const int64_t t = (N + sm90::kAttRows - 1) / sm90::kAttRows;
-  return static_cast<int>(t < sm90::kMaxRecPerBag ? (t < 1 ? 1 : t) : sm90::kMaxRecPerBag);
-}
-static BagsWs carve_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, bool need_Q, void* ws, size_t cap,
-                         bool* ok) {
+static BagsWs carve_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, bool need_Q, bool sharded, void* ws,
+                         size_t cap, bool* ok) {
   Carver c(ws, cap);
   BagsWs w;
-  int64_t total = 0, nrec = 0;
-  for (int b = 0; b < nb; ++b) { total += Ns[b]; nrec += recs_for_bag(Ns[b]); }
-  w.table = c.take<sm90::BagDev>(nb);
-  // keys and the finalize arrival counters are zeroed together (one memset): keep them adjacent
-  w.keys = c.take<unsigned long long>(static_cast<size_t>(nb) * (kMaxC + 1));
-  w.counters = reinterpret_cast<unsigned int*>(w.keys ? w.keys + static_cast<size_t>(nb) * kMaxC : nullptr);
-  w.pred_part = c.take<float>(static_cast<size_t>(nb) * sm90::kFinSlices * kMaxC);
-  {   // tile-blocked Q: one 128x128 block per 128-row tile
-    int64_t tiles = 0;
-    for (int b = 0; b < nb; ++b) tiles += (Ns[b] + sm90::kTileM - 1) / sm90::kTileM;
-    w.Q = need_Q ? c.take<float>(static_cast<size_t>(tiles) * sm90::kTileM * kQ) : nullptr;
+  int64_t tiles = 0, nrec = 0;
+  for (int b = 0; b < nb; ++b) {
+    tiles += (Ns[b] + sm90::kTileM - 1) / sm90::kTileM;
+    nrec += recs_for_bag(Ns[b]);
   }
-  (void)total;
-  w.wimg = c.take<uint8_t>(sm90::wimg_bytes(p->D) + 1024);
+  carve_phase1(c, p, nb, w);
+  w.pred_part = c.take<float>(static_cast<size_t>(nb) * sm90::kFinSlices * kMaxC);
+  // tile-blocked Q: one 128x128 block per 128-row tile
+  w.Q = need_Q ? c.take<float>(static_cast<size_t>(tiles) * sm90::kTileM * kQ) : nullptr;
   w.recs = c.take<float>(static_cast<size_t>(nrec) * rec_floats(p->C, p->D));
+  w.row_offsets = sharded ? c.take<long long>(nb) : nullptr;
+  w.qmax = sharded ? c.take<float>(static_cast<size_t>(nb) * p->C * kQ) : nullptr;
   w.bytes = c.off;
   *ok = c.ok();
   return w;
-}
-// Host copy of the bag table: each bag's first row, 128-row tile and partial record, numbered across the batch.
-static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::vector<sm90::BagDev>& tbl, int* tiles,
-                       int* recs) {
-  long long row = 0;
-  int tile = 0, rec = 0;
-  tbl.resize(nb);
-  for (int b = 0; b < nb; ++b) {
-    DSMIL_REQUIRE(Ns[b] >= 1 && Ns[b] < 0xffffffffll && Xs[b], "bag %d: empty or NULL", b);
-    DSMIL_REQUIRE((reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0, "bag %d: features must be 16-byte aligned", b);
-    const int nrec = recs_for_bag(Ns[b]);
-    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
-    row += Ns[b];
-    tile += static_cast<int>((Ns[b] + sm90::kTileM - 1) / sm90::kTileM);
-    rec += nrec;
-  }
-  *tiles = tile;
-  *recs = rec;
-  return 0;
 }
 
 static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
@@ -394,51 +419,19 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
                              cudaStream_t st) {
   const int C = p->C, D = p->D;
   bool ok;
-  BagsWs w = carve_bags(p, Ns, nb, save_Q == nullptr, ws, ws_bytes, &ok);
+  BagsWs w = carve_bags(p, Ns, nb, save_Q == nullptr, false, ws, ws_bytes, &ok);
   int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
   if (rc) return rc;
-  std::vector<sm90::BagDev> tbl;
-  int tiles = 0, recs = 0;
-  if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
-  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
-  uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(w.wimg) + 1023) & ~uintptr_t(1023));
-  if ((rc = sm90::launch_prep_wimg(p, img, st))) return rc;
   float* Q = save_Q ? save_Q : w.Q;
-  if (classes_in) {   // bag form: arg-max of the given scores (single bag only)
-    const int grid = static_cast<int>(std::min<int64_t>(ceil_div(Ns[0], 256), kSplits));
-    k_argmax<<<grid, 256, 0, st>>>(classes_in, Ns[0], C, w.keys);
-    DSMIL_LAUNCH_OK("k_argmax");
-  }
   const bool q_blocked = save_Q == nullptr;   // training keeps Q (after tanh) row-major for the backward kernels
-  if ((rc = sm90::launch_qmlp(p, w.table, nb, tiles, classes_in ? nullptr : classes, w.keys, Q, save_H1, img, num_sms(),
-                              st, q_blocked)))
+  int tiles, recs;
+  if ((rc = bags_phase1_impl(p, w, Xs, Ns, nb, classes_in, classes, Q, save_H1, q_blocked, true, &tiles, &recs, st)))
     return rc;
   sm90::AttendArgs aa{w.table, nb, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr};
   if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
   sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, p->Wf, p->bf, A, B, pred, reinterpret_cast<long long*>(crit),
                          w.pred_part, w.counters, nullptr, 0, 0};
   return sm90::launch_finalize_b(fa, nb, st);
-}
-
-
-// ---- row-sharded BATCH of bags (one call per phase for all bags; two all-gathers per step) --------------
-struct ShardBagsWs {
-  BagsWs base;
-  long long* row_offsets;   // [nb] device copy
-  float* qmax;              // [nb][C][128]
-  size_t bytes;
-};
-static ShardBagsWs carve_shard_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, void* ws, size_t cap, bool* ok) {
-  ShardBagsWs s;
-  s.base = carve_bags(p, Ns, nb, true, ws, cap, ok);
-  Carver c(ws, cap);
-  c.off = s.base.bytes;
-  s.row_offsets = c.take<long long>(nb);
-  s.qmax = c.take<float>(static_cast<size_t>(nb) * p->C * kQ);
-  s.bytes = c.off;
-  *ok = c.ok();
-  return s;
 }
 
 }  // namespace dsmil
@@ -566,7 +559,7 @@ size_t dsmil_forward_workspace_bytes(const dsmil_params_t* p, int64_t N) {
   if (!p || p->C < 1 || p->C > DSMIL_MAX_C || p->D < 1 || p->D > DSMIL_MAX_D || N < 0) return 0;
   bool ok;
   size_t a = carve_fwd(p, N, nullptr, 0, &ok).bytes;
-  if (sm90::batched_supported(p) && N > 0) a = std::max(a, carve_bags(p, &N, 1, true, nullptr, 0, &ok).bytes);
+  if (sm90::batched_supported(p) && N > 0) a = std::max(a, carve_bags(p, &N, 1, true, false, nullptr, 0, &ok).bytes);
   return a;
 }
 
@@ -578,7 +571,7 @@ size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t
   int64_t mx = 0;
   for (int b = 0; b < nb; ++b) mx = std::max<int64_t>(mx, Ns[b]);
   size_t bytes = carve_fwd(p, mx, nullptr, 0, &ok).bytes;
-  if (sm90::batched_supported(p)) bytes = std::max(bytes, carve_bags(p, Ns, nb, true, nullptr, 0, &ok).bytes);
+  if (sm90::batched_supported(p)) bytes = std::max(bytes, carve_bags(p, Ns, nb, true, false, nullptr, 0, &ok).bytes);
   return bytes;
 }
 
@@ -661,7 +654,7 @@ int dsmil_shard_phase1(const dsmil_params_t* p, const float* X, const float* x_f
   FwdWs w = carve_fwd(p, N_local, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
   float* h1 = p->nonlinear ? (H1 ? H1 : (phase1_on_qmlp(p, w.wimg, X) ? nullptr : w.H1)) : nullptr;
-  return phase1_impl(p, X, x_for_v, classes_in, N_local, row_offset, classes, Q, h1, V, cand_rec, w.keys, w.wimg,
+  return phase1_impl(p, X, x_for_v, classes_in, N_local, row_offset, classes, Q, h1, V, cand_rec, w,
                      static_cast<cudaStream_t>(stream));
 }
 
@@ -937,7 +930,7 @@ int dsmil_shard_bags_supported(const dsmil_params_t* p) {
 size_t dsmil_shard_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
   if (!dsmil_shard_bags_supported(p) || !Ns || nb < 1) return 0;
   bool ok;
-  return carve_shard_bags(p, Ns, nb, nullptr, 0, &ok).bytes;
+  return carve_bags(p, Ns, nb, true, true, nullptr, 0, &ok).bytes;
 }
 int dsmil_shard_bags_phase1(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                             const int64_t* row_offsets, float* classes, float* cand_recs, void* workspace,
@@ -948,23 +941,17 @@ int dsmil_shard_bags_phase1(const dsmil_params_t* p, const float* const* Xs, con
   DSMIL_REQUIRE(Xs && Ns && nb >= 1 && row_offsets && classes && cand_recs, "NULL pointer or nb < 1");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
-  ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
+  BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
-  std::vector<sm90::BagDev> tbl;
-  int tiles = 0, recs = 0;
-  if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;
-  if (!stream_is_capturing(st)) {
-    DSMIL_CUDA_OK(cudaMemcpyAsync(w.base.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
-    DSMIL_CUDA_OK(cudaMemcpyAsync(w.row_offsets, row_offsets, sizeof(long long) * nb, cudaMemcpyHostToDevice, st));
-  }
-  DSMIL_CUDA_OK(cudaMemsetAsync(w.base.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
-  uint8_t* img = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(w.base.wimg) + 1023) & ~uintptr_t(1023));
-  // (a captured serving loop also reuses the weight images of the preceding eager call: re-capture after a weight update)
-  if (!stream_is_capturing(st) && (rc = sm90::launch_prep_wimg(p, img, st))) return rc;
-  if ((rc = sm90::launch_qmlp(p, w.base.table, nb, tiles, classes, w.base.keys, w.base.Q, nullptr, img, num_sms(), st,
-                              true)))
+  // a captured call reuses the table, row offsets and weight images of the preceding eager call: re-capture after a
+  // weight update
+  const bool upload = !stream_is_capturing(st);
+  int tiles, recs;
+  if ((rc = bags_phase1_impl(p, w, Xs, Ns, nb, nullptr, classes, w.Q, nullptr, true, upload, &tiles, &recs, st)))
     return rc;
-  sm90::k_gather_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(w.base.table, w.base.keys, classes, w.base.Q, true, w.row_offsets, p->C,
+  if (upload)
+    DSMIL_CUDA_OK(cudaMemcpyAsync(w.row_offsets, row_offsets, sizeof(long long) * nb, cudaMemcpyHostToDevice, st));
+  sm90::k_gather_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(w.table, w.keys, classes, w.Q, true, w.row_offsets, p->C,
                                                         cand_recs);
   DSMIL_LAUNCH_OK("k_gather_cand_b");
   return 0;
@@ -978,17 +965,17 @@ int dsmil_shard_bags_phase2(const dsmil_params_t* p, const float* const* Xs, con
                 "bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
-  ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
+  BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
   std::vector<sm90::BagDev> tbl;
   int tiles = 0, recs = 0;
   if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
   k_merge_cand<<<dim3(p->C, nb), kQ, 0, st>>>(cands_all, G, nb, p->C, w.qmax, crit_idx);
   DSMIL_LAUNCH_OK("k_merge_cand");
-  sm90::AttendArgs aa{w.base.table, nb, p->D, p->C, w.base.Q, true, w.base.keys, A, w.base.recs, w.qmax};
+  sm90::AttendArgs aa{w.table, nb, p->D, p->C, w.Q, true, w.keys, A, w.recs, w.qmax};
   if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
-  sm90::FinalizeArgs fa{w.base.table, p->D, p->C, w.base.recs, w.base.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
-                         w.base.pred_part, w.base.counters, recs_out, 0, 0};
+  sm90::FinalizeArgs fa{w.table, p->D, p->C, w.recs, w.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
+                         w.pred_part, w.counters, recs_out, 0, 0};
   return sm90::launch_finalize_b(fa, nb, st);
 }
 int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
@@ -1000,10 +987,10 @@ int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, con
                 "bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
-  ShardBagsWs w = carve_shard_bags(p, Ns, nb, workspace, workspace_bytes, &ok);
+  BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
-  sm90::FinalizeArgs fa{w.base.table, p->D, p->C, recs_all, w.base.keys, p->Wf, p->bf, A, B, pred, nullptr,
-                         w.base.pred_part, w.base.counters, nullptr, G, nb};
+  sm90::FinalizeArgs fa{w.table, p->D, p->C, recs_all, w.keys, p->Wf, p->bf, A, B, pred, nullptr,
+                         w.pred_part, w.counters, nullptr, G, nb};
   return sm90::launch_finalize_b(fa, nb, st);
 }
 

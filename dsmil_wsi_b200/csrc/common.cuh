@@ -79,16 +79,11 @@ __device__ __forceinline__ uint32_t ordered_key(float v) {
   if (v != v) u = 0x7fc00000u;  // canonical +NaN
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
-__device__ __forceinline__ float key_to_float(uint32_t k) {
-  uint32_t u = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
-  return __uint_as_float(u);
-}
 // (score, local row) -> 64-bit key whose max is "largest score, then LOWEST row".
 __device__ __forceinline__ unsigned long long pack_key(float v, uint32_t row) {
   return (static_cast<unsigned long long>(ordered_key(v)) << 32) | (0xffffffffu - row);
 }
 __device__ __forceinline__ uint32_t key_row(unsigned long long k) { return 0xffffffffu - static_cast<uint32_t>(k); }
-__device__ __forceinline__ float key_score(unsigned long long k) { return key_to_float(static_cast<uint32_t>(k >> 32)); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

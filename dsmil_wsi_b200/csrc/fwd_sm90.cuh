@@ -187,11 +187,6 @@ __device__ __forceinline__ float tanh_ex2(float x) {
   return __fmaf_rn(r, -2.f, 1.f);
 }
 __device__ __forceinline__ f2 fast_tanh2(f2 x) { return f2{tanh_ex2(x.x), tanh_ex2(x.y)}; }
-__device__ __forceinline__ float fast_tanh(float x) {
-  // tanh(x) = 1 - 2/(exp(2x)+1); ex2.approx + rcp.approx: |err| < ~3e-7 absolute, saturates correctly
-  const float e = __expf(2.f * x);
-  return 1.f - __fdividef(2.f, e + 1.f);
-}
 
 // dynamic smem carve (bytes, from a 1024-aligned base)
 constexpr int kOffWRing = 0;                                // kWStages x 32 KiB: W1 chunks AND the two W2 chunks stream here
