@@ -13,6 +13,7 @@
 #include "gemm_generic.cuh"
 #include "fwd_kernels.cuh"
 #include "bwd_kernels.cuh"
+#include "bwd_bags.cuh"
 #include "fwd_sm90.cuh"
 #include "fwd_batched.cuh"
 #include "embed_kernels.cuh"
@@ -109,6 +110,23 @@ static int check_workspace(size_t need, bool ok, const void* ws, size_t cap) {
   if (ws && ok) return 0;
   set_error("workspace too small: need %zu bytes, got %zu", need, cap);
   return DSMIL_ERR_WORKSPACE;
+}
+
+// Bags of the batch and their rows; DSMIL_ERR_EMPTY for an empty bag, as dsmil_forward_bags.
+static int check_bags(const float* const* Xs, const int64_t* Ns, int nb, int64_t* total, bool* aligned) {
+  *total = 0;
+  *aligned = true;
+  for (int b = 0; b < nb; ++b) {
+    DSMIL_REQUIRE(Ns[b] >= 0 && Ns[b] < 0xffffffffll, "bag %d: N=%lld out of range", b, (long long)Ns[b]);
+    if (Ns[b] == 0) {
+      set_error("bag %d: empty bag (N == 0): the reference raises IndexError at dsmil.py:53", b);
+      return DSMIL_ERR_EMPTY;
+    }
+    DSMIL_REQUIRE(Xs[b], "bag %d: NULL features", b);
+    *aligned = *aligned && (reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0;
+    *total += Ns[b];
+  }
+  return 0;
 }
 
 static inline int attend_ctas(int64_t N) {
@@ -582,16 +600,9 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
   if (rc) return rc;
   DSMIL_REQUIRE(Xs && Ns && nb >= 1 && classes && pred && A && B, "NULL pointer or nb < 1");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  bool aligned = true;
-  for (int b = 0; b < nb; ++b) {
-    DSMIL_REQUIRE(Ns[b] >= 0 && Ns[b] < 0xffffffffll, "bag %d: N=%lld out of range", b, (long long)Ns[b]);
-    if (Ns[b] == 0) {
-      set_error("bag %d: empty bag (N == 0): the reference raises IndexError at dsmil.py:53", b);
-      return DSMIL_ERR_EMPTY;
-    }
-    DSMIL_REQUIRE(Xs[b], "bag %d: NULL features", b);
-    aligned = aligned && (reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0;
-  }
+  int64_t total;
+  bool aligned;
+  if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
   // one contract for both routes below: the size dsmil_forward_bags_workspace_bytes reports
   const size_t need = dsmil_forward_bags_workspace_bytes(p, Ns, nb);
   if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
@@ -923,6 +934,129 @@ int dsmil_instance_scores_backward(const dsmil_params_t* p, const float* X, int6
   return 0;
 }
 
+// ---- batched training: forward that keeps Q/H1, and its backward over the bag table ------------------------------
+struct BwdBagsWs {
+  sm90::BagDev* table;
+  TnChunk *chi, *ch1;        // chunk tables of gWi = d_classes^T X and gW1 = dz1^T X
+  float *dB, *dA, *dL, *tpart, *dpart, *dqm, *dz2, *dz1, *tnpart, *cspart;
+  int G;                     // CTAs per bag of the per-row kernels (fixes their partial sums)
+  bool gemv_i;               // gWi on the streaming kernel
+  int nci, nc1;
+  int64_t rps_i, rps_1;
+  size_t bytes;
+};
+// `aligned`: every bag 16-byte aligned (the streaming gWi kernel needs it).  The carve reserves room for either gWi
+// form, so the reported size does not depend on alignment.
+static BwdBagsWs carve_bwd_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, bool aligned, void* ws,
+                                size_t cap, bool* ok) {
+  Carver c(ws, cap);
+  BwdBagsWs w;
+  const int C = p->C, D = p->D;
+  int64_t total = 0, mx = 1;
+  for (int b = 0; b < nb; ++b) {
+    total += Ns[b];
+    mx = std::max<int64_t>(mx, Ns[b]);
+  }
+  const int64_t n = std::max<int64_t>(total, 1);
+  w.G = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(kSms * 8, nb), ceil_div(mx, 64))));
+  const bool gemv_ok = tn_use_gemv(C, D);
+  w.gemv_i = gemv_ok && aligned;
+  const int64_t rps_gemv = rag_rows_per_chunk(C, D, total, true), rps_tile = rag_rows_per_chunk(C, D, total, false);
+  const int nci_gemv = gemv_ok ? rag_chunks(nullptr, Ns, nb, D, rps_gemv, nullptr) : 0;
+  const int nci_tile = rag_chunks(nullptr, Ns, nb, D, rps_tile, nullptr);
+  w.rps_i = w.gemv_i ? rps_gemv : rps_tile;
+  w.nci = w.gemv_i ? nci_gemv : nci_tile;
+  w.rps_1 = rag_rows_per_chunk(kQ, D, total, false);
+  w.nc1 = rag_chunks(nullptr, Ns, nb, D, w.rps_1, nullptr);
+  w.table = c.take<sm90::BagDev>(nb);
+  w.chi = c.take<TnChunk>(std::max(nci_gemv, nci_tile));
+  w.ch1 = c.take<TnChunk>(w.nc1);
+  w.dB = c.take<float>(static_cast<size_t>(nb) * C * D);
+  w.dA = c.take<float>(n * C);
+  w.dL = c.take<float>(n * C);
+  w.tpart = c.take<float>(static_cast<size_t>(nb) * w.G * C);
+  w.dpart = c.take<float>(static_cast<size_t>(nb) * w.G * C * kQ);
+  w.dqm = c.take<float>(static_cast<size_t>(nb) * C * kQ);
+  w.dz2 = c.take<float>(n * kQ);
+  w.dz1 = p->nonlinear ? c.take<float>(n * kQ) : nullptr;
+  size_t tn = static_cast<size_t>(std::max(nci_gemv, nci_tile)) * C * D;
+  tn = std::max(tn, static_cast<size_t>(w.nc1) * kQ * D);
+  tn = std::max(tn, tn_partial_floats(kQ, kQ, n));
+  w.tnpart = c.take<float>(tn);
+  w.cspart = c.take<float>(static_cast<size_t>(kSplits) * kQ);
+  w.bytes = c.off;
+  *ok = c.ok();
+  return w;
+}
+
+static int backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
+                              int64_t total, bool aligned, const float* Q, const float* H1, const float* A,
+                              const float* B, const int64_t* crit, const float* d_classes, const float* d_pred,
+                              const float* d_A, const float* d_B, const dsmil_grads_t* g, void* ws, size_t ws_bytes,
+                              cudaStream_t st) {
+  const int C = p->C, D = p->D;
+  bool ok;
+  BwdBagsWs w = carve_bwd_bags(p, Ns, nb, aligned, ws, ws_bytes, &ok);
+  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+  if (rc) return rc;
+  // the kernels read X, N and row_off of the table (not the forward's tile and record numbering), at any alignment
+  std::vector<sm90::BagDev> tbl(nb);
+  long long row = 0;
+  for (int b = 0; b < nb; ++b) {
+    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, 0, 0, 0, 0};
+    row += Ns[b];
+  }
+  std::vector<TnChunk> chi(w.nci), ch1(w.nc1);
+  rag_chunks(Xs, Ns, nb, D, w.rps_i, chi.data());
+  rag_chunks(Xs, Ns, nb, D, w.rps_1, ch1.data());
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.chi, chi.data(), sizeof(TnChunk) * w.nci, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.ch1, ch1.data(), sizeof(TnChunk) * w.nc1, cudaMemcpyHostToDevice, st));
+
+  // bag classifier (dsmil.py:59-61) and B, summed over the bags
+  k_bwd_bag_b<<<ceil_div(static_cast<int64_t>(C) * D, 256), 256, 0, st>>>(p->Wf, B, d_pred, d_B, nb, C, D, w.dB,
+                                                                          g->gWf, g->gbf);
+  DSMIL_LAUNCH_OK("k_bwd_bag_b");
+  // instance classifier (dsmil.py:11)
+  if (g->gWi) {
+    if (d_classes) { if ((rc = launch_gemm_tn_rag(d_classes, C, D, w.chi, w.nci, w.gemv_i, w.tnpart, g->gWi, st))) return rc; }
+    else DSMIL_CUDA_OK(cudaMemsetAsync(g->gWi, 0, sizeof(float) * C * D, st));
+  }
+  if (g->gbi) {
+    if (d_classes) { if ((rc = launch_colsum(d_classes, C, total, w.cspart, g->gbi, st))) return rc; }
+    else DSMIL_CUDA_OK(cudaMemsetAsync(g->gbi, 0, sizeof(float) * C, st));
+  }
+  // dA = X dB_b^T (+ d_A) and t_b's partials; dL and dq_max_b's partials; dq_max_b; dQ -> dz2
+  const dim3 grid(w.G, nb);
+  const size_t smem = sizeof(float) * C * D;
+  if (smem > 48 * 1024)
+    DSMIL_CUDA_OK(cudaFuncSetAttribute(k_bwd_rowdot_b, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_bwd_rowdot_b<<<grid, 256, smem, st>>>(w.table, D, w.dB, C, A, d_A, w.dA, w.tpart);
+  DSMIL_LAUNCH_OK("k_bwd_rowdot_b");
+  k_bwd_dL_b<<<grid, 256, 0, st>>>(w.table, C, A, w.dA, w.tpart, Q, w.dL, w.dpart);
+  DSMIL_LAUNCH_OK("k_bwd_dL_b");
+  k_sum_segments<<<dim3(ceil_div(C * kQ, 256), nb), 256, 0, st>>>(w.dpart, w.G, C * kQ, w.dqm);
+  DSMIL_LAUNCH_OK("k_sum_segments");
+  k_bwd_dq_b<<<grid, 256, 0, st>>>(w.table, C, w.dL, Q, w.dqm, crit, p->nonlinear, w.dz2);
+  DSMIL_LAUNCH_OK("k_bwd_dq_b");
+  // back through the Q-MLP: layer 2 over the packed rows, layer 1 against the bags' X
+  const float* dz1 = w.dz2;
+  if (p->nonlinear) {
+    if (g->gW2 && (rc = launch_gemm_tn(w.dz2, kQ, H1, kQ, total, w.tnpart, g->gW2, st))) return rc;
+    if (g->gb2 && (rc = launch_colsum(w.dz2, kQ, total, w.cspart, g->gb2, st))) return rc;
+    if ((rc = launch_linear<ACT_MASK_POS, true>(w.dz2, total, kQ, p->W2, nullptr, kQ, w.dz1, H1, 0, st))) return rc;
+    dz1 = w.dz1;
+  }
+  if (g->gW1 && (rc = launch_gemm_tn_rag(dz1, kQ, D, w.ch1, w.nc1, false, w.tnpart, g->gW1, st))) return rc;
+  if (g->gb1 && (rc = launch_colsum(dz1, kQ, total, w.cspart, g->gb1, st))) return rc;
+  if (g->gX) {
+    if ((rc = launch_linear<ACT_NONE, true>(dz1, total, kQ, p->W1, nullptr, D, g->gX, nullptr, 0, st))) return rc;
+    k_bwd_dx_extra_b<<<grid, 256, 0, st>>>(w.table, d_classes, p->Wi, A, w.dB, C, D, g->gX);
+    DSMIL_LAUNCH_OK("k_bwd_dx_extra_b");
+  }
+  return 0;
+}
+
 // ---- sharded batch ABI ---------------------------------------------------------------------------
 int dsmil_shard_bags_supported(const dsmil_params_t* p) {
   return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && sm90::batched_supported(p)) ? 1 : 0;
@@ -992,6 +1126,72 @@ int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, con
   sm90::FinalizeArgs fa{w.table, p->D, p->C, recs_all, w.keys, p->Wf, p->bf, A, B, pred, nullptr,
                          w.pred_part, w.counters, nullptr, G, nb};
   return sm90::launch_finalize_b(fa, nb, st);
+}
+
+
+// ---- batched training ------------------------------------------------------------------------------
+size_t dsmil_forward_bags_train_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
+  if (!p || p->passing_v) return 0;
+  return dsmil_forward_bags_workspace_bytes(p, Ns, nb);
+}
+
+int dsmil_forward_bags_train(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                             float* classes, float* pred, float* A, float* B, int64_t* crit_idx, float* save_Q,
+                             float* save_H1, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_params(p, true);
+  if (rc) return rc;
+  DSMIL_REQUIRE(!p->passing_v, "batched training supports the identity v only (passing_v: one bag per call)");
+  DSMIL_REQUIRE(Xs && Ns && nb >= 1 && classes && pred && A && B && crit_idx && save_Q && (!p->nonlinear || save_H1),
+                "NULL pointer or nb < 1");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int64_t total;
+  bool aligned;
+  if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
+  const size_t need = dsmil_forward_bags_train_workspace_bytes(p, Ns, nb);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  if (sm90::batched_supported(p) && aligned)
+    return forward_bags_impl(p, Xs, Ns, nb, nullptr, classes, pred, A, B, crit_idx, save_Q, save_H1, workspace,
+                             workspace_bytes, st);
+  // shapes or bags off the tensor-core batch: one bag at a time into the same packed buffers
+  int64_t row = 0;
+  for (int b = 0; b < nb; ++b) {
+    rc = forward_impl(p, Xs[b], nullptr, nullptr, Ns[b], classes + row * p->C, pred + static_cast<size_t>(b) * p->C,
+                      A + row * p->C, B + static_cast<size_t>(b) * p->C * p->D, crit_idx + static_cast<size_t>(b) * p->C,
+                      save_Q + row * kQ, save_H1 ? save_H1 + row * kQ : nullptr, nullptr, workspace, workspace_bytes,
+                      st);
+    if (rc) return rc;
+    row += Ns[b];
+  }
+  return 0;
+}
+
+size_t dsmil_backward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb, int need_gX) {
+  (void)need_gX;   // gX is the caller's buffer: the identity-v backward needs no scratch for it
+  if (!p || !Ns || nb < 1 || p->passing_v || p->C < 1 || p->C > DSMIL_MAX_C || p->D < 1 || p->D > DSMIL_MAX_D) return 0;
+  for (int b = 0; b < nb; ++b)
+    if (Ns[b] < 0) return 0;
+  bool ok;
+  return carve_bwd_bags(p, Ns, nb, true, nullptr, 0, &ok).bytes;
+}
+
+int dsmil_backward_bags(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                        const float* Q, const float* H1, const float* A, const float* B, const int64_t* crit_idx,
+                        const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                        const dsmil_grads_t* grads, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_params(p);
+  if (rc) return rc;
+  DSMIL_REQUIRE(!p->passing_v, "batched backward supports the identity v only (passing_v: dsmil_backward per bag)");
+  DSMIL_REQUIRE(Xs && Ns && nb >= 1 && nb <= 65535 && Q && A && B && crit_idx && grads,
+                "NULL pointer or nb outside [1, 65535]");
+  DSMIL_REQUIRE(!p->nonlinear || H1, "nonlinear q backward needs saved H1");
+  DSMIL_REQUIRE(!(grads->gX && d_classes) || p->Wi, "gX through d_classes needs Wi");
+  int64_t total;
+  bool aligned;
+  if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
+  const size_t need = dsmil_backward_bags_workspace_bytes(p, Ns, nb, grads->gX != nullptr);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  return backward_bags_impl(p, Xs, Ns, nb, total, aligned, Q, H1, A, B, crit_idx, d_classes, d_pred, d_A, d_B, grads,
+                            workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

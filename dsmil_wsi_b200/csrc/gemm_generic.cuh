@@ -116,16 +116,14 @@ inline int launch_linear(const float* X, int64_t N, int K, const float* W, const
 // 8 x 8 per thread: 64 FMAs per four 16-byte shared-memory loads, so the FMA pipe, not the LSU, is the limiter (the
 // former 64 x 64 / 4 x 4 tile was shared-memory-bound at half the FMA rate); the next k-tile is fetched into registers
 // while the current one is multiplied.
+// gemm_tn_tile: the CTA's tile (blockIdx.y, blockIdx.x) of out[M1,M2] = sum over rows [0, ne) of P[n,M1] * R[n,M2].
 constexpr int TBM = 128, TBK = 16;
-__global__ void __launch_bounds__(256, 2)
-k_gemm_tn(const float* __restrict__ P, int M1, const float* __restrict__ R, int M2, int64_t N,
-          int64_t rows_per_split, float* __restrict__ part) {
+__device__ __forceinline__ void gemm_tn_tile(const float* __restrict__ P, int M1, const float* __restrict__ R, int M2,
+                                             int64_t ne, float* __restrict__ out) {
   __shared__ __align__(16) float Ps[TBK][TBM + 4];
   __shared__ __align__(16) float Rs[TBK][TBM + 4];
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
   const int a0 = blockIdx.y * TBM, b0 = blockIdx.x * TBM;
-  const int64_t nb = static_cast<int64_t>(blockIdx.z) * rows_per_split;
-  const int64_t ne = min(N, nb + rows_per_split);
   float acc[8][8];
 #pragma unroll
   for (int i = 0; i < 8; ++i)
@@ -133,7 +131,9 @@ k_gemm_tn(const float* __restrict__ P, int M1, const float* __restrict__ R, int 
     for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
   // loader role: k-row (tid >> 4) of the tile, columns (tid & 15) * 4 .. + 3 and + 64
   const int ln = tid >> 4, lq = (tid & 15) * 4;
-  const bool pvec = (M1 & 3) == 0, rvec = (M2 & 3) == 0;
+  // float4 rows only when every row is 16-byte aligned (a bag may be a view at any float offset)
+  const bool pvec = (M1 & 3) == 0 && (reinterpret_cast<uintptr_t>(P) & 15) == 0;
+  const bool rvec = (M2 & 3) == 0 && (reinterpret_cast<uintptr_t>(R) & 15) == 0;
   float4 pf[2], rf[2];
   auto fetch = [&](int64_t n0) {
     const int64_t n = n0 + ln;
@@ -163,8 +163,8 @@ k_gemm_tn(const float* __restrict__ P, int M1, const float* __restrict__ R, int 
       rf[h] = rv;
     }
   };
-  if (nb < ne) fetch(nb);
-  for (int64_t n0 = nb; n0 < ne; n0 += TBK) {
+  if (ne > 0) fetch(0);
+  for (int64_t n0 = 0; n0 < ne; n0 += TBK) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       *reinterpret_cast<float4*>(&Ps[ln][lq + 64 * h]) = pf[h];
@@ -187,7 +187,6 @@ k_gemm_tn(const float* __restrict__ P, int M1, const float* __restrict__ R, int 
     }
     __syncthreads();
   }
-  float* out = part + static_cast<int64_t>(blockIdx.z) * M1 * M2;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int a = a0 + ty * 4 + (i & 3) + 64 * (i >> 2);
@@ -199,27 +198,32 @@ k_gemm_tn(const float* __restrict__ P, int M1, const float* __restrict__ R, int 
     }
   }
 }
+__global__ void __launch_bounds__(256, 2)
+k_gemm_tn(const float* __restrict__ P, int M1, const float* __restrict__ R, int M2, int64_t N,
+          int64_t rows_per_split, float* __restrict__ part) {
+  const int64_t nb = static_cast<int64_t>(blockIdx.z) * rows_per_split;
+  gemm_tn_tile(P + nb * M1, M1, R + nb * M2, M2, min(N, nb + rows_per_split) - nb,
+               part + static_cast<int64_t>(blockIdx.z) * M1 * M2);
+}
 
 // The same product for a handful of left columns (M1 <= 4: the per-class gradients gWi = d_classes^T X and
 // dq_max = dL^T Q): 2 * M1 FLOP per element of R, i.e. a pure stream over R.  Thread = one float4 column group of R,
 // 256 / (M2 / 4) rows in flight per CTA; partial per CTA, combined in a fixed order.
 constexpr int kGemvMaxM1 = 4;
+// gemv_tn_rows: out[M1,M2] = sum over rows [0, ne) of P[n,M1] * R[n,M2], by one CTA.
 template <int M1>
-__global__ void __launch_bounds__(256)
-k_gemv_tn(const float* __restrict__ P, const float* __restrict__ R, int M2, int64_t N, int64_t rows_per_split,
-          float* __restrict__ part) {
+__device__ __forceinline__ void gemv_tn_rows(const float* __restrict__ P, const float* __restrict__ R, int M2,
+                                             int64_t ne, float* __restrict__ out) {
   __shared__ float s_acc[256][4 * M1 + 1];
   const int G = M2 >> 2;                    // float4 groups per row (<= 256)
   const int rpi = 256 / G;                  // rows per iteration
   const int g = threadIdx.x % G, ro = threadIdx.x / G;
-  const int64_t nb = static_cast<int64_t>(blockIdx.x) * rows_per_split;
-  const int64_t ne = min(N, nb + rows_per_split);
   float acc[M1][4];
 #pragma unroll
   for (int c = 0; c < M1; ++c) acc[c][0] = acc[c][1] = acc[c][2] = acc[c][3] = 0.f;
   if (ro < rpi) {
 #pragma unroll 4
-    for (int64_t n = nb + ro; n < ne; n += rpi) {
+    for (int64_t n = ro; n < ne; n += rpi) {
       const float4 r = __ldg(reinterpret_cast<const float4*>(R + n * M2) + g);
 #pragma unroll
       for (int c = 0; c < M1; ++c) {
@@ -241,11 +245,18 @@ k_gemv_tn(const float* __restrict__ P, const float* __restrict__ R, int M2, int6
       for (int c = 0; c < M1; ++c)
 #pragma unroll
         for (int q = 0; q < 4; ++q) acc[c][q] += s_acc[r2 * G + g][4 * c + q];
-    float* out = part + static_cast<int64_t>(blockIdx.x) * M1 * M2;
 #pragma unroll
     for (int c = 0; c < M1; ++c)
       *reinterpret_cast<float4*>(out + static_cast<int64_t>(c) * M2 + 4 * g) = make_float4(acc[c][0], acc[c][1], acc[c][2], acc[c][3]);
   }
+}
+template <int M1>
+__global__ void __launch_bounds__(256)
+k_gemv_tn(const float* __restrict__ P, const float* __restrict__ R, int M2, int64_t N, int64_t rows_per_split,
+          float* __restrict__ part) {
+  const int64_t nb = static_cast<int64_t>(blockIdx.x) * rows_per_split;
+  gemv_tn_rows<M1>(P + nb * M1, R + nb * M2, M2, min(N, nb + rows_per_split) - nb,
+                   part + static_cast<int64_t>(blockIdx.x) * M1 * M2);
 }
 
 // part[z][M] = sum over the z-th row chunk of P[n, m]

@@ -90,11 +90,30 @@ class DeviceBagStore:
 
 
 def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_patch: float = 0.0,
-                order: Optional[Sequence[int]] = None, generator: Optional[torch.Generator] = None) -> float:
-    """One epoch of train_tcga.train() (train_tcga.py:55-76) over device-resident bags; one host sync per epoch."""
+                order: Optional[Sequence[int]] = None, generator: Optional[torch.Generator] = None,
+                bags_per_step: int = 1) -> float:
+    """One epoch of train_tcga.train() (train_tcga.py:55-76) over device-resident bags; one host sync per epoch.
+
+    bags_per_step = 1: the reference's loop, one forward, backward and optimizer step per bag.  k > 1: minibatches of
+    k consecutive bags of `order`; each is one `milnet.forward_bags(xs, grad=True)` call, one backward and one
+    optimizer step on the mean over the group of the per-bag 0.5 * criterion(bag) + 0.5 * criterion(max instance)
+    (criterion evaluated once on the group's [k, C] rows, which is that mean for an element-averaging criterion such
+    as the reference's BCEWithLogitsLoss).  Returns the mean loss per bag either way."""
     milnet.train()
     total = torch.zeros((), device=store.device)
     order = list(order) if order is not None else torch.randperm(len(store)).tolist()
+    if bags_per_step > 1:
+        for s in range(0, len(order), bags_per_step):
+            group = order[s:s + bags_per_step]
+            optimizer.zero_grad()
+            xs = [dropout_patches(store.bags[i][0], 1 - dropout_patch, generator) for i in group]
+            labels = torch.cat([store.bags[i][1].view(1, -1) for i in group])
+            bag_prediction, max_prediction = _group_predictions(milnet.forward_bags(xs, grad=True))
+            loss = 0.5 * criterion(bag_prediction, labels) + 0.5 * criterion(max_prediction, labels)
+            loss.backward()
+            optimizer.step()
+            total += loss.detach() * len(group)
+        return float(total.item()) / max(1, len(order))
     for i in order:
         feats, label = store.bags[i]
         optimizer.zero_grad()
@@ -107,6 +126,19 @@ def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_pat
         optimizer.step()
         total += loss.detach()
     return float(total.item()) / max(1, len(order))
+
+
+def _group_predictions(outs):
+    """(bag predictions [k, C], max-instance predictions [k, C]) of a group's forward_bags outputs.  The packed
+    outputs of the bag-table call carry each bag's critical rows, the per-class arg-max of its scores: gathering the
+    scores there is the per-bag max in one op (the gradient goes to that row, as torch.max's does when the max is
+    unique).  The per-bag fallback of forward_bags returns a plain list."""
+    if isinstance(outs, Fn.BagOutputs) and outs.crit is not None:
+        classes, pred = outs.packed[0], outs.packed[1]
+        first = torch.tensor([0] + outs.Ns[:-1], device=classes.device).cumsum(0)
+        return pred, classes.gather(0, outs.crit + first[:, None])
+    return (torch.cat([bag.view(1, -1) for _, bag, _, _ in outs]),
+            torch.stack([torch.max(ins, 0)[0] for ins, _, _, _ in outs]))
 
 
 def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, bags_per_launch: int = 16,
@@ -176,9 +208,11 @@ def compute_pos_weight(bags: Sequence[Tuple[int, object]]) -> float:
     return (len(bags) - pos) / pos
 
 
-def mil_epoch_train(milnet, store: DeviceBagStore, criterion, optimizer, order: Optional[Sequence[int]] = None) -> float:
-    """train_mil.epoch_train (train_mil.py:42-59): per bag, shuffle the instances, forward, 0.5/0.5 loss, step."""
-    return train_epoch(milnet, store, criterion, optimizer, dropout_patch=0.0, order=order)
+def mil_epoch_train(milnet, store: DeviceBagStore, criterion, optimizer, order: Optional[Sequence[int]] = None,
+                    bags_per_step: int = 1) -> float:
+    """train_mil.epoch_train (train_mil.py:42-59): per bag, shuffle the instances, forward, 0.5/0.5 loss, step
+    (bags_per_step > 1: one step per group of bags, as train_epoch)."""
+    return train_epoch(milnet, store, criterion, optimizer, dropout_patch=0.0, order=order, bags_per_step=bags_per_step)
 
 
 def mil_epoch_test(milnet, store: DeviceBagStore, criterion, bags_per_launch: int = 16):

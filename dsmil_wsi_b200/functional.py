@@ -224,9 +224,10 @@ class BagOutputs(collections.abc.Sequence):
     access: materialising 4 views per bag eagerly costs ~1.5 us each on the host -- as long as the GPU work of a
     16-bag step -- so the sequence hands them out lazily.  `.packed` exposes the packed tensors themselves."""
 
-    def __init__(self, classes, pred, A, B, Ns):
+    def __init__(self, classes, pred, A, B, Ns, crit=None):
         self.packed = (classes, pred, A, B)
         self.Ns = list(Ns)
+        self.crit = crit          # [nb, C] critical rows within each bag, when the caller kept them
         self._offsets = None
 
     def __len__(self):
@@ -248,10 +249,96 @@ class BagOutputs(collections.abc.Sequence):
         return classes[lo:hi], pred[b:b + 1], A[lo:hi], B[b:b + 1]
 
 
+def _bag_table(bags, P: ParamPack):
+    """Checked, contiguous bags and their host arrays (features pointers, row counts) for the bag-table calls."""
+    xs = [_check_feats(b, P.D) for b in bags]
+    Ns = [int(x.shape[0]) for x in xs]
+    if min(Ns) == 0:
+        raise IndexError("dsmil_b200: empty bag (N == 0) in the batch")
+    for x in xs:
+        if x.device != P.device:
+            raise RuntimeError(f"dsmil_b200: bag on {x.device} but parameters on {P.device}")
+    nb = len(xs)
+    return xs, Ns, (C.c_void_p * nb)(*[x.data_ptr() for x in xs]), (C.c_int64 * nb)(*Ns)
+
+
+class MILBagsFn(torch.autograd.Function):
+    """Packed (classes, pred, A, B, crit) of a batch of bags, differentiable: dsmil_forward_bags_train forward,
+    dsmil_backward_bags backward (one call each for the whole batch).  args: nb, the nb bags, then the ten parameter
+    tensors.  Parameter gradients are sums over the bags, as autograd gives for a loss over the packed outputs."""
+
+    @staticmethod
+    def forward(ctx, nb, *args):
+        lib = _lib.load()
+        ctx.set_materialize_grads(False)
+        P = ParamPack(*args[nb:])
+        if P.passing_v:
+            raise NotImplementedError("forward_bags(grad=True): passing_v models go through MILNet.forward per bag")
+        xs, Ns, c_X, c_N = _bag_table(args[:nb], P)
+        total, Cc, D, dev = sum(Ns), P.C, P.D, P.device
+        with torch.cuda.device(dev):
+            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+            classes, A = new(total, Cc), new(total, Cc)
+            pred, B = new(nb, Cc), new(nb, Cc, D)
+            crit = torch.empty(nb, Cc, dtype=torch.int64, device=dev)
+            sQ = new(total, Q_DIM)
+            sH = new(total, Q_DIM) if P.nonlinear else None
+            ws = _workspace(lib.dsmil_forward_bags_train_workspace_bytes(P.ref, c_N, nb), dev)
+            rc = lib.dsmil_forward_bags_train(P.ref, c_X, c_N, nb, _ptr(classes), _ptr(pred), _ptr(A), _ptr(B),
+                                              _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(ws), ws.numel(), _stream())
+            _lib.check(rc, "dsmil_forward_bags_train")
+        ctx.nb, ctx.Ns = nb, Ns
+        ctx.save_for_backward(*xs, sQ, sH, A, B, crit, *P.tensors)
+        ctx.mark_non_differentiable(crit)
+        return classes, pred, A, B, crit
+
+    @staticmethod
+    def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
+        lib = _lib.load()
+        nb, Ns = ctx.nb, ctx.Ns
+        saved = ctx.saved_tensors
+        xs, (sQ, sH, A, B, crit), params = saved[:nb], saved[nb:nb + 5], saved[nb + 5:]
+        P = ParamPack(*params)
+        need_bags, need_params = ctx.needs_input_grad[1:1 + nb], ctx.needs_input_grad[1 + nb:]
+        names = ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")
+        dev = P.device
+        c_X = (C.c_void_p * nb)(*[x.data_ptr() for x in xs])
+        c_N = (C.c_int64 * nb)(*Ns)
+        with torch.cuda.device(dev):
+            out = {nm: (torch.empty_like(t) if t is not None and need else None)
+                   for nm, t, need in zip(names, P.tensors, need_params)}
+            gX = torch.empty(sum(Ns), P.D, dtype=torch.float32, device=dev) if any(need_bags) else None
+            G = _lib.DsmilGrads(*[_ptr(out[n]) for n in names], _ptr(gX))
+            dc, dp, dA, dB = (_f32c(t) for t in (g_classes, g_pred, g_A, g_B))
+            ws = _workspace(lib.dsmil_backward_bags_workspace_bytes(P.ref, c_N, nb, int(gX is not None)), dev)
+            rc = lib.dsmil_backward_bags(P.ref, c_X, c_N, nb, _ptr(sQ), _ptr(sH), _ptr(A), _ptr(B), _ptr(crit),
+                                         _ptr(dc), _ptr(dp), _ptr(dA), _ptr(dB), C.byref(G), _ptr(ws), ws.numel(),
+                                         _stream())
+            _lib.check(rc, "dsmil_backward_bags")
+        gxs, lo = [], 0
+        for n, need in zip(Ns, need_bags):
+            gxs.append(gX[lo:lo + n] if need else None)
+            lo += n
+        return (None, *gxs, *[out[n] for n in names])
+
+
+def mil_forward_bags(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]], *, grad: bool = False):
+    """Forward of a STREAM of bags in one library call: returns a lazy sequence of (classes, prediction_bag, A, B)
+    per bag -- views into packed device buffers -- plus crit_idx [nb, C] (rows within each bag).
+
+    grad=False (default): inference, dsmil_forward_bags under no_grad.  grad=True with grad mode on: the packed
+    outputs carry autograd history (MILBagsFn), so a loss over them trains the whole batch with one backward call;
+    identity v only."""
+    if not (grad and torch.is_grad_enabled()):
+        return _mil_forward_bags_infer(bags, params)
+    if len(bags) == 0:
+        return [], None
+    classes, pred, A, B, crit = MILBagsFn.apply(len(bags), *bags, *params)
+    return BagOutputs(classes, pred, A, B, [int(b.shape[0]) for b in bags], crit), crit
+
+
 @torch.no_grad()
-def mil_forward_bags(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]]):
-    """Inference forward of a STREAM of bags in one library call (dsmil_forward_bags): returns a list of
-    (classes, prediction_bag, A, B) per bag -- views into packed device buffers -- plus crit_idx [nb, C]."""
+def _mil_forward_bags_infer(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]]):
     lib = _lib.load()
     P = ParamPack(*params)
     if P.passing_v:

@@ -130,11 +130,18 @@ class MILNet(nn.Module):
         prediction_bag, A, B = bc(feats, classes)
         return classes, prediction_bag, A, B
 
-    @torch.no_grad()
-    def forward_bags(self, bags):
+    def forward_bags(self, bags, *, grad=False):
         """Throughput form: a list of bags [N_i, D] -> sequence of (classes, prediction_bag, A, B), computed by ONE
         library call (bag table; see DESIGN.md).  The result is a lazy sequence of views over packed outputs
-        (`.packed`).  Inference only (no autograd)."""
+        (`.packed`).  grad=False (default): inference, no autograd.  grad=True with grad mode on: the packed outputs
+        carry autograd history and one backward call covers the whole batch (a minibatch training step).  Models
+        with passing_v or a foreign instance classifier run `self.forward` per bag, under autograd when asked."""
+        if not (grad and torch.is_grad_enabled()):
+            with torch.no_grad():
+                return self._forward_bags(bags, False)
+        return self._forward_bags(bags, True)
+
+    def _forward_bags(self, bags, grad):
         ic, bc = self.i_classifier, self.b_classifier
         if not (isinstance(bc, BClassifier) and isinstance(ic, (FCLayer, IClassifier))):
             return [self.forward(b) for b in bags]
@@ -145,7 +152,7 @@ class MILNet(nn.Module):
         if Wv is not None:
             return [self.forward(b) for b in bags]
         params = (lin.weight, lin.bias, W1, b1, W2, b2, None, None, bc.fcc.weight, bc.fcc.bias)
-        outs, _ = Fn.mil_forward_bags(feats, params)
+        outs, _ = Fn.mil_forward_bags(feats, params, grad=grad)
         return outs
 
     @torch.no_grad()

@@ -145,6 +145,25 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
                        float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
                        void* workspace, size_t workspace_bytes, void* stream);
 
+/* Training form of dsmil_forward_bags: the same packed outputs, plus save_Q [sum N,128] (after the tanh) and, for a
+ * nonlinear q, save_H1 [sum N,128], packed in bag order -- what dsmil_backward_bags needs.  crit_idx [nb,C] is
+ * required; its entries are rows within each bag.  Identity v only (passing_v: DSMIL_ERR_ARG).  Shapes or bags off
+ * the tensor-core batch loop per bag (as dsmil_forward_bags does) into the same packed buffers. */
+size_t dsmil_forward_bags_train_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb);
+int dsmil_forward_bags_train(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                             float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                             float* save_Q, float* save_H1, void* workspace, size_t workspace_bytes, void* stream);
+/* Reverse of dsmil_forward_bags_train for all nb bags in one call.  Upstream gradients are packed like the outputs:
+ * d_classes / d_A [sum N,C], d_pred [nb,C], d_B [nb,C,D]; each may be NULL == zero.  grads->g* are SUMS over the
+ * bags (overwritten; a loss that averages over bags carries its 1/nb itself); grads->gX, when non-NULL, is packed
+ * [sum N,D].  Any D and C of dsmil_backward and any alignment of the bags; identity v only.  Deterministic: no
+ * float atomics, fixed-order split sums. */
+size_t dsmil_backward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb, int need_gX);
+int dsmil_backward_bags(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                        const float* Q, const float* H1, const float* A, const float* B, const int64_t* crit_idx,
+                        const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                        const dsmil_grads_t* grads, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Call form (2)+(3) of the boundary (SURVEY §8b): the callers in attention_map.py:74,85 /
  * testing_tcga.py:72,83 run the instance classifier and the bag classifier separately.
  * dsmil_instance_scores == IClassifier.fc / FCLayer.fc (dsmil.py:11,24).
