@@ -106,6 +106,24 @@ SIGNATURES = {
     "dsmil_shard_bags_phase3": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(C.c_void_p), C.POINTER(c_i64), C.c_int32,
                                           C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_bags_phase1_train": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(C.c_void_p), C.POINTER(c_i64),
+                                                C.c_int32, C.POINTER(c_i64), C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_bags_phase2_train": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(C.c_void_p), C.POINTER(c_i64),
+                                                C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_backward_bags_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.POINTER(c_i64), C.c_int32]),
+    "dsmil_shard_backward_bags_phase1": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(C.c_void_p), C.POINTER(c_i64),
+                                                   C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_backward_bags_phase2": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(c_i64), C.c_int32, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_backward_bags_phase3": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(C.c_void_p), C.POINTER(c_i64),
+                                                   C.c_int32, C.POINTER(c_i64), C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -112,7 +112,8 @@ static int check_workspace(size_t need, bool ok, const void* ws, size_t cap) {
   return DSMIL_ERR_WORKSPACE;
 }
 
-// Bags of the batch and their rows; DSMIL_ERR_EMPTY for an empty bag, as dsmil_forward_bags.
+// Bags of the batch and their rows; DSMIL_ERR_EMPTY for an empty bag, as dsmil_forward_bags.  Xs == NULL checks the
+// row counts only (a phase that reads no features).
 static int check_bags(const float* const* Xs, const int64_t* Ns, int nb, int64_t* total, bool* aligned) {
   *total = 0;
   *aligned = true;
@@ -121,6 +122,10 @@ static int check_bags(const float* const* Xs, const int64_t* Ns, int nb, int64_t
     if (Ns[b] == 0) {
       set_error("bag %d: empty bag (N == 0): the reference raises IndexError at dsmil.py:53", b);
       return DSMIL_ERR_EMPTY;
+    }
+    if (!Xs) {
+      *total += Ns[b];
+      continue;
     }
     DSMIL_REQUIRE(Xs[b], "bag %d: NULL features", b);
     *aligned = *aligned && (reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0;
@@ -939,6 +944,7 @@ struct BwdBagsWs {
   sm90::BagDev* table;
   TnChunk *chi, *ch1;        // chunk tables of gWi = d_classes^T X and gW1 = dz1^T X
   float *dB, *dA, *dL, *tpart, *dpart, *dqm, *dz2, *dz1, *tnpart, *cspart;
+  long long* row_offsets;    // row-sharded batch only: [nb] device copy of each bag's first global row
   int G;                     // CTAs per bag of the per-row kernels (fixes their partial sums)
   bool gemv_i;               // gWi on the streaming kernel
   int nci, nc1;
@@ -946,9 +952,9 @@ struct BwdBagsWs {
   size_t bytes;
 };
 // `aligned`: every bag 16-byte aligned (the streaming gWi kernel needs it).  The carve reserves room for either gWi
-// form, so the reported size does not depend on alignment.
-static BwdBagsWs carve_bwd_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, bool aligned, void* ws,
-                                size_t cap, bool* ok) {
+// form, so the reported size does not depend on alignment.  `sharded` appends the row offsets of the row-sharded batch.
+static BwdBagsWs carve_bwd_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, bool aligned, bool sharded,
+                                void* ws, size_t cap, bool* ok) {
   Carver c(ws, cap);
   BwdBagsWs w;
   const int C = p->C, D = p->D;
@@ -984,21 +990,23 @@ static BwdBagsWs carve_bwd_bags(const dsmil_params_t* p, const int64_t* Ns, int 
   tn = std::max(tn, tn_partial_floats(kQ, kQ, n));
   w.tnpart = c.take<float>(tn);
   w.cspart = c.take<float>(static_cast<size_t>(kSplits) * kQ);
+  w.row_offsets = sharded ? c.take<long long>(nb) : nullptr;
   w.bytes = c.off;
   *ok = c.ok();
   return w;
 }
 
-static int backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
-                              int64_t total, bool aligned, const float* Q, const float* H1, const float* A,
-                              const float* B, const int64_t* crit, const float* d_classes, const float* d_pred,
-                              const float* d_A, const float* d_B, const dsmil_grads_t* g, void* ws, size_t ws_bytes,
-                              cudaStream_t st) {
+// The batched backward in three phases, cut at its two per-bag cross-row sums (t_b and dq_max_b), as bwd_phase1/2/3_impl
+// are for one bag.  dsmil_backward_bags runs them in a row; the row-sharded batch runs one per call, with the caller's
+// all-reduces in between.  Phase 1 uploads the bag and chunk tables into w; phases 2 and 3 read them from there.
+
+// Phase 1: dB, gWf/gbf, gWi/gbi, dA = X dB_b^T (+ d_A) into dA, and t_b's per-CTA partials in w.tpart (w.G per bag).
+static int bwd_bags_phase1_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
+                                int64_t total, const float* A, const float* B, const float* d_classes,
+                                const float* d_pred, const float* d_A, const float* d_B, const dsmil_grads_t* g,
+                                float* dA, const BwdBagsWs& w, cudaStream_t st) {
   const int C = p->C, D = p->D;
-  bool ok;
-  BwdBagsWs w = carve_bwd_bags(p, Ns, nb, aligned, ws, ws_bytes, &ok);
-  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
-  if (rc) return rc;
+  int rc;
   // the kernels read X, N and row_off of the table (not the forward's tile and record numbering), at any alignment
   std::vector<sm90::BagDev> tbl(nb);
   long long row = 0;
@@ -1026,32 +1034,69 @@ static int backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, c
     if (d_classes) { if ((rc = launch_colsum(d_classes, C, total, w.cspart, g->gbi, st))) return rc; }
     else DSMIL_CUDA_OK(cudaMemsetAsync(g->gbi, 0, sizeof(float) * C, st));
   }
-  // dA = X dB_b^T (+ d_A) and t_b's partials; dL and dq_max_b's partials; dq_max_b; dQ -> dz2
-  const dim3 grid(w.G, nb);
+  // dA = X dB_b^T (+ d_A) and t_b's partials
   const size_t smem = sizeof(float) * C * D;
   if (smem > 48 * 1024)
     DSMIL_CUDA_OK(cudaFuncSetAttribute(k_bwd_rowdot_b, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_bwd_rowdot_b<<<grid, 256, smem, st>>>(w.table, D, w.dB, C, A, d_A, w.dA, w.tpart);
+  k_bwd_rowdot_b<<<dim3(w.G, nb), 256, smem, st>>>(w.table, D, w.dB, C, A, d_A, dA, w.tpart);
   DSMIL_LAUNCH_OK("k_bwd_rowdot_b");
-  k_bwd_dL_b<<<grid, 256, 0, st>>>(w.table, C, A, w.dA, w.tpart, Q, w.dL, w.dpart);
+  return 0;
+}
+
+// Phase 2: dL = A (dA - t_b) / sqrt(128), t_b the sum of the P partials per bag in `tpart`; dqm[b] = dL_b^T Q_b,
+// summed over the CTAs' shares in a fixed order.
+static int bwd_bags_phase2_impl(const dsmil_params_t* p, int nb, const float* A, const float* dA, const float* tpart,
+                                int P, const float* Q, float* dL, float* dqm, const BwdBagsWs& w, cudaStream_t st) {
+  const int C = p->C;
+  k_bwd_dL_b<<<dim3(w.G, nb), 256, 0, st>>>(w.table, C, A, dA, tpart, P, Q, dL, w.dpart);
   DSMIL_LAUNCH_OK("k_bwd_dL_b");
-  k_sum_segments<<<dim3(ceil_div(C * kQ, 256), nb), 256, 0, st>>>(w.dpart, w.G, C * kQ, w.dqm);
+  k_sum_segments<<<dim3(ceil_div(C * kQ, 256), nb), 256, 0, st>>>(w.dpart, w.G, C * kQ, dqm);
   DSMIL_LAUNCH_OK("k_sum_segments");
-  k_bwd_dq_b<<<grid, 256, 0, st>>>(w.table, C, w.dL, Q, w.dqm, crit, p->nonlinear, w.dz2);
+  return 0;
+}
+
+// Phase 3: dQ -> dz2 (qmax / row_offsets as k_bwd_dq_b reads them: NULL when the critical rows are local), back through
+// the Q-MLP into gW2/gb2 and gW1/gb1.  *dz1 is the layer-1 gradient it leaves in w.
+static int bwd_bags_phase3_impl(const dsmil_params_t* p, int nb, int64_t total, const float* Q, const float* H1,
+                                const float* dL, const float* dqm, const float* qmax, const int64_t* crit,
+                                const long long* row_offsets, const dsmil_grads_t* g, const BwdBagsWs& w,
+                                const float** dz1, cudaStream_t st) {
+  const int D = p->D;
+  int rc;
+  k_bwd_dq_b<<<dim3(w.G, nb), 256, 0, st>>>(w.table, p->C, dL, Q, qmax, dqm, crit, row_offsets, p->nonlinear, w.dz2);
   DSMIL_LAUNCH_OK("k_bwd_dq_b");
   // back through the Q-MLP: layer 2 over the packed rows, layer 1 against the bags' X
-  const float* dz1 = w.dz2;
+  *dz1 = w.dz2;
   if (p->nonlinear) {
     if (g->gW2 && (rc = launch_gemm_tn(w.dz2, kQ, H1, kQ, total, w.tnpart, g->gW2, st))) return rc;
     if (g->gb2 && (rc = launch_colsum(w.dz2, kQ, total, w.cspart, g->gb2, st))) return rc;
     if ((rc = launch_linear<ACT_MASK_POS, true>(w.dz2, total, kQ, p->W2, nullptr, kQ, w.dz1, H1, 0, st))) return rc;
-    dz1 = w.dz1;
+    *dz1 = w.dz1;
   }
-  if (g->gW1 && (rc = launch_gemm_tn_rag(dz1, kQ, D, w.ch1, w.nc1, false, w.tnpart, g->gW1, st))) return rc;
-  if (g->gb1 && (rc = launch_colsum(dz1, kQ, total, w.cspart, g->gb1, st))) return rc;
+  if (g->gW1 && (rc = launch_gemm_tn_rag(*dz1, kQ, D, w.ch1, w.nc1, false, w.tnpart, g->gW1, st))) return rc;
+  if (g->gb1 && (rc = launch_colsum(*dz1, kQ, total, w.cspart, g->gb1, st))) return rc;
+  return 0;
+}
+
+static int backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
+                              int64_t total, bool aligned, const float* Q, const float* H1, const float* A,
+                              const float* B, const int64_t* crit, const float* d_classes, const float* d_pred,
+                              const float* d_A, const float* d_B, const dsmil_grads_t* g, void* ws, size_t ws_bytes,
+                              cudaStream_t st) {
+  const int C = p->C, D = p->D;
+  bool ok;
+  BwdBagsWs w = carve_bwd_bags(p, Ns, nb, aligned, false, ws, ws_bytes, &ok);
+  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+  if (rc) return rc;
+  // one device: k_bwd_dL_b sums phase 1's partials of t itself, and the critical rows are local
+  const float* dz1;
+  if ((rc = bwd_bags_phase1_impl(p, Xs, Ns, nb, total, A, B, d_classes, d_pred, d_A, d_B, g, w.dA, w, st)) ||
+      (rc = bwd_bags_phase2_impl(p, nb, A, w.dA, w.tpart, w.G, Q, w.dL, w.dqm, w, st)) ||
+      (rc = bwd_bags_phase3_impl(p, nb, total, Q, H1, w.dL, w.dqm, nullptr, crit, nullptr, g, w, &dz1, st)))
+    return rc;
   if (g->gX) {
     if ((rc = launch_linear<ACT_NONE, true>(dz1, total, kQ, p->W1, nullptr, D, g->gX, nullptr, 0, st))) return rc;
-    k_bwd_dx_extra_b<<<grid, 256, 0, st>>>(w.table, d_classes, p->Wi, A, w.dB, C, D, g->gX);
+    k_bwd_dx_extra_b<<<dim3(w.G, nb), 256, 0, st>>>(w.table, d_classes, p->Wi, A, w.dB, C, D, g->gX);
     DSMIL_LAUNCH_OK("k_bwd_dx_extra_b");
   }
   return 0;
@@ -1066,6 +1111,40 @@ size_t dsmil_shard_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* 
   bool ok;
   return carve_bags(p, Ns, nb, true, true, nullptr, 0, &ok).bytes;
 }
+// Phase 1 of the row-sharded batch: scores, arg-max keys and Q (+ H1 when non-NULL; Q tile-blocked when q_blocked),
+// then each bag's candidate record.  A captured call reuses the table, row offsets and weight images of the preceding
+// eager call: re-capture after a weight update.
+static int shard_bags_phase1_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
+                                  const int64_t* row_offsets, float* classes, float* Q, float* H1, bool q_blocked,
+                                  float* cand_recs, const BagsWs& w, cudaStream_t st) {
+  const bool upload = !stream_is_capturing(st);
+  int tiles, recs, rc;
+  if ((rc = bags_phase1_impl(p, w, Xs, Ns, nb, nullptr, classes, Q, H1, q_blocked, upload, &tiles, &recs, st)))
+    return rc;
+  if (upload)
+    DSMIL_CUDA_OK(cudaMemcpyAsync(w.row_offsets, row_offsets, sizeof(long long) * nb, cudaMemcpyHostToDevice, st));
+  sm90::k_gather_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(w.table, w.keys, classes, Q, q_blocked, w.row_offsets, p->C,
+                                                        cand_recs);
+  DSMIL_LAUNCH_OK("k_gather_cand_b");
+  return 0;
+}
+// Phase 2: merge the G ranks' candidates into q_max [nb,C,128] and crit_idx, attend on the local rows, and each bag's
+// partial record.
+static int shard_bags_phase2_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
+                                  const float* Q, bool q_blocked, const float* cands_all, int G, float* A,
+                                  int64_t* crit_idx, float* qmax, float* recs_out, const BagsWs& w, cudaStream_t st) {
+  std::vector<sm90::BagDev> tbl;
+  int tiles = 0, recs = 0, rc;
+  if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
+  k_merge_cand<<<dim3(p->C, nb), kQ, 0, st>>>(cands_all, G, nb, p->C, qmax, crit_idx);
+  DSMIL_LAUNCH_OK("k_merge_cand");
+  sm90::AttendArgs aa{w.table, nb, p->D, p->C, Q, q_blocked, w.keys, A, w.recs, qmax};
+  if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
+  sm90::FinalizeArgs fa{w.table, p->D, p->C, w.recs, w.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
+                         w.pred_part, w.counters, recs_out, 0, 0};
+  return sm90::launch_finalize_b(fa, nb, st);
+}
+
 int dsmil_shard_bags_phase1(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                             const int64_t* row_offsets, float* classes, float* cand_recs, void* workspace,
                             size_t workspace_bytes, void* stream) {
@@ -1073,22 +1152,11 @@ int dsmil_shard_bags_phase1(const dsmil_params_t* p, const float* const* Xs, con
   if (rc) return rc;
   DSMIL_REQUIRE(dsmil_shard_bags_supported(p), "shape not supported by the batched tensor-core path");
   DSMIL_REQUIRE(Xs && Ns && nb >= 1 && row_offsets && classes && cand_recs, "NULL pointer or nb < 1");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
   BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
-  // a captured call reuses the table, row offsets and weight images of the preceding eager call: re-capture after a
-  // weight update
-  const bool upload = !stream_is_capturing(st);
-  int tiles, recs;
-  if ((rc = bags_phase1_impl(p, w, Xs, Ns, nb, nullptr, classes, w.Q, nullptr, true, upload, &tiles, &recs, st)))
-    return rc;
-  if (upload)
-    DSMIL_CUDA_OK(cudaMemcpyAsync(w.row_offsets, row_offsets, sizeof(long long) * nb, cudaMemcpyHostToDevice, st));
-  sm90::k_gather_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(w.table, w.keys, classes, w.Q, true, w.row_offsets, p->C,
-                                                        cand_recs);
-  DSMIL_LAUNCH_OK("k_gather_cand_b");
-  return 0;
+  return shard_bags_phase1_impl(p, Xs, Ns, nb, row_offsets, classes, w.Q, nullptr, true, cand_recs, w,
+                                static_cast<cudaStream_t>(stream));
 }
 int dsmil_shard_bags_phase2(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                             const float* cands_all, int32_t G, float* A, int64_t* crit_idx, float* recs_out,
@@ -1097,20 +1165,11 @@ int dsmil_shard_bags_phase2(const dsmil_params_t* p, const float* const* Xs, con
   if (rc) return rc;
   DSMIL_REQUIRE(dsmil_shard_bags_supported(p) && Xs && Ns && nb >= 1 && cands_all && G >= 1 && A && crit_idx && recs_out,
                 "bad arguments");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
   BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
-  std::vector<sm90::BagDev> tbl;
-  int tiles = 0, recs = 0;
-  if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
-  k_merge_cand<<<dim3(p->C, nb), kQ, 0, st>>>(cands_all, G, nb, p->C, w.qmax, crit_idx);
-  DSMIL_LAUNCH_OK("k_merge_cand");
-  sm90::AttendArgs aa{w.table, nb, p->D, p->C, w.Q, true, w.keys, A, w.recs, w.qmax};
-  if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
-  sm90::FinalizeArgs fa{w.table, p->D, p->C, w.recs, w.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
-                         w.pred_part, w.counters, recs_out, 0, 0};
-  return sm90::launch_finalize_b(fa, nb, st);
+  return shard_bags_phase2_impl(p, Xs, Ns, nb, w.Q, true, cands_all, G, A, crit_idx, w.qmax, recs_out, w,
+                                static_cast<cudaStream_t>(stream));
 }
 int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                             const float* recs_all, int32_t G, float* A, float* B, float* pred, void* workspace,
@@ -1171,7 +1230,7 @@ size_t dsmil_backward_bags_workspace_bytes(const dsmil_params_t* p, const int64_
   for (int b = 0; b < nb; ++b)
     if (Ns[b] < 0) return 0;
   bool ok;
-  return carve_bwd_bags(p, Ns, nb, true, nullptr, 0, &ok).bytes;
+  return carve_bwd_bags(p, Ns, nb, true, false, nullptr, 0, &ok).bytes;
 }
 
 int dsmil_backward_bags(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
@@ -1192,6 +1251,123 @@ int dsmil_backward_bags(const dsmil_params_t* p, const float* const* Xs, const i
   if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
   return backward_bags_impl(p, Xs, Ns, nb, total, aligned, Q, H1, A, B, crit_idx, d_classes, d_pred, d_A, d_B, grads,
                             workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+
+// ---- row-sharded batch training: phases 1 and 2 that keep Q and H1 row-major, and the backward in three calls -------
+// What every call of it checks: the batched sharded shapes, identity v, 1 <= nb <= 65535, and at least one local row
+// in every bag (need_X == false: a phase that reads no features checks the row counts only).
+static int check_shard_bags_train(const dsmil_params_t* p, bool need_scores, const float* const* Xs, bool need_X,
+                                  const int64_t* Ns, int nb, int64_t* total, bool* aligned) {
+  int rc = check_params(p, need_scores);
+  if (rc) return rc;
+  DSMIL_REQUIRE(!p->passing_v, "row-sharded batched training supports the identity v only");
+  DSMIL_REQUIRE(dsmil_shard_bags_supported(p), "shape not supported by the batched tensor-core path");
+  DSMIL_REQUIRE(Ns && (Xs || !need_X) && nb >= 1 && nb <= 65535, "NULL pointer or nb outside [1, 65535]");
+  return check_bags(need_X ? Xs : nullptr, Ns, nb, total, aligned);
+}
+
+int dsmil_shard_bags_phase1_train(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                                  const int64_t* row_offsets, float* classes, float* save_Q, float* save_H1,
+                                  float* cand_recs, void* workspace, size_t workspace_bytes, void* stream) {
+  int64_t total;
+  bool aligned;
+  int rc = check_shard_bags_train(p, true, Xs, true, Ns, nb, &total, &aligned);
+  if (rc) return rc;
+  DSMIL_REQUIRE(row_offsets && classes && save_Q && save_H1 && cand_recs, "NULL pointer");
+  bool ok;
+  BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+  return shard_bags_phase1_impl(p, Xs, Ns, nb, row_offsets, classes, save_Q, save_H1, false, cand_recs, w,
+                                static_cast<cudaStream_t>(stream));
+}
+
+int dsmil_shard_bags_phase2_train(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                                  const float* Q, const float* cands_all, int32_t G, float* A, int64_t* crit_idx,
+                                  float* q_max, float* recs_out, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  int64_t total;
+  bool aligned;
+  int rc = check_shard_bags_train(p, true, Xs, true, Ns, nb, &total, &aligned);
+  if (rc) return rc;
+  DSMIL_REQUIRE(Q && cands_all && G >= 1 && A && crit_idx && q_max && recs_out, "NULL pointer or G < 1");
+  bool ok;
+  BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+  return shard_bags_phase2_impl(p, Xs, Ns, nb, Q, false, cands_all, G, A, crit_idx, q_max, recs_out, w,
+                                static_cast<cudaStream_t>(stream));
+}
+
+size_t dsmil_shard_backward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
+  if (!dsmil_shard_bags_supported(p) || !Ns || nb < 1) return 0;
+  for (int b = 0; b < nb; ++b)
+    if (Ns[b] < 0) return 0;
+  bool ok;
+  return carve_bwd_bags(p, Ns, nb, true, true, nullptr, 0, &ok).bytes;
+}
+
+int dsmil_shard_backward_bags_phase1(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                                     const float* A, const float* B, const float* d_classes_local,
+                                     const float* d_pred, float* dA_local, float* t_local, float* gWi, float* gbi,
+                                     float* gWf, float* gbf, void* workspace, size_t workspace_bytes, void* stream) {
+  int64_t total;
+  bool aligned;
+  int rc = check_shard_bags_train(p, false, Xs, true, Ns, nb, &total, &aligned);
+  if (rc) return rc;
+  DSMIL_REQUIRE(A && B && dA_local && t_local, "NULL tensor pointer");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  bool ok;
+  BwdBagsWs w = carve_bwd_bags(p, Ns, nb, aligned, true, workspace, workspace_bytes, &ok);
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+  dsmil_grads_t g{};
+  g.gWi = gWi; g.gbi = gbi; g.gWf = gWf; g.gbf = gbf;
+  if ((rc = bwd_bags_phase1_impl(p, Xs, Ns, nb, total, A, B, d_classes_local, d_pred, nullptr, nullptr, &g, dA_local,
+                                 w, st)))
+    return rc;
+  // t_local[b] = the per-CTA partials summed in a fixed order: with one rank, phase 2 then sees the t_b that
+  // dsmil_backward_bags's k_bwd_dL_b forms itself
+  k_sum_segments<<<dim3(ceil_div(p->C, 256), nb), 256, 0, st>>>(w.tpart, w.G, p->C, t_local);
+  DSMIL_LAUNCH_OK("k_sum_segments");
+  return 0;
+}
+
+int dsmil_shard_backward_bags_phase2(const dsmil_params_t* p, const int64_t* Ns, int32_t nb, const float* A,
+                                     float* dA_to_dL, const float* t_global, const float* Q, float* dqm_local,
+                                     void* workspace, size_t workspace_bytes, void* stream) {
+  int64_t total;
+  bool aligned;
+  int rc = check_shard_bags_train(p, false, nullptr, false, Ns, nb, &total, &aligned);
+  if (rc) return rc;
+  DSMIL_REQUIRE(A && dA_to_dL && t_global && Q && dqm_local, "NULL tensor pointer");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  bool ok;
+  BwdBagsWs w = carve_bwd_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+  // k_bwd_dL_b reads dA and writes dL from different threads: it reads a copy so that dL can replace dA
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.dA, dA_to_dL, sizeof(float) * total * p->C, cudaMemcpyDeviceToDevice, st));
+  return bwd_bags_phase2_impl(p, nb, A, w.dA, t_global, 1, Q, dA_to_dL, dqm_local, w, st);
+}
+
+int dsmil_shard_backward_bags_phase3(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                                     const int64_t* row_offsets, const float* Q, const float* H1, const float* dL_local,
+                                     const float* dqm_global, const float* q_max, const int64_t* crit_idx,
+                                     float* gW1, float* gb1, float* gW2, float* gb2, void* workspace,
+                                     size_t workspace_bytes, void* stream) {
+  int64_t total;
+  bool aligned;
+  int rc = check_shard_bags_train(p, false, Xs, true, Ns, nb, &total, &aligned);
+  if (rc) return rc;
+  DSMIL_REQUIRE(row_offsets && Q && H1 && dL_local && dqm_global && q_max && crit_idx, "NULL tensor pointer");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  bool ok;
+  BwdBagsWs w = carve_bwd_bags(p, Ns, nb, aligned, true, workspace, workspace_bytes, &ok);
+  if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.row_offsets, row_offsets, sizeof(long long) * nb, cudaMemcpyHostToDevice, st));
+  dsmil_grads_t g{};
+  g.gW1 = gW1; g.gb1 = gb1; g.gW2 = gW2; g.gb2 = gb2;
+  const float* dz1;
+  return bwd_bags_phase3_impl(p, nb, total, Q, H1, dL_local, dqm_global, q_max, crit_idx, w.row_offsets, &g, w, &dz1,
+                              st);
 }
 
 }  // extern "C"

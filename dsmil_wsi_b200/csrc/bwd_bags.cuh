@@ -2,7 +2,9 @@
 // v only.  Every kernel walks the forward's bag table (sm90::BagDev: X pointer, N, row_off); per-row buffers (classes,
 // A, Q, H1 and their gradients) are packed in bag order, [sum N, *].  Parameter gradients are sums over the bags.
 // Split sums go through partial buffers whose count depends on the shapes only (never on the SM count) and are added
-// in a fixed order: no float atomics, so two runs give the same bits on any H100.
+// in a fixed order: no float atomics, so two runs give the same bits on any H100.  The row-sharded batch
+// (dsmil_shard_backward_bags_phase1/2/3) runs the same kernels on each rank's rows, with the all-reduced t and
+// dq_max and the merged q_max passed in.
 #pragma once
 #include "common.cuh"
 #include "gemm_generic.cuh"
@@ -98,19 +100,21 @@ k_bwd_rowdot_b(const sm90::BagDev* __restrict__ bags, int D, const float* __rest
   }
 }
 
-// Softmax-over-instances backward (dsmil.py:55-57), segmented per bag.  CTA (x, b), t_b = sum_x' tpart[b][x']:
+// Softmax-over-instances backward (dsmil.py:55-57), segmented per bag.  CTA (x, b), t_b = sum_{x' < P} tpart[b][x']
+// (P partials per bag: the first pass's per-CTA shares, or P = 1 for a t that is already summed, e.g. all-reduced
+// over the ranks of a row-sharded batch):
 // dL[n,k] = A[n,k] (dA[n,k] - t_b[k]) / sqrt(128) for rows n = 2x + h, step 2*gridDim.x, of bag b, and the CTA's share
 // of dq_max_b = dL_b^T Q_b, [C,128], in dpart[b][x].
 __global__ void __launch_bounds__(256)
 k_bwd_dL_b(const sm90::BagDev* __restrict__ bags, int C, const float* __restrict__ A, const float* __restrict__ dA,
-           const float* __restrict__ tpart, const float* __restrict__ Q, float* __restrict__ dL,
+           const float* __restrict__ tpart, int P, const float* __restrict__ Q, float* __restrict__ dL,
            float* __restrict__ dpart) {
   __shared__ float t[kMaxC];
   __shared__ float red[kMaxC][kQ];
   const int b = blockIdx.y, G = gridDim.x;
   if (threadIdx.x < C) {
     float s = 0.f;
-    for (int x = 0; x < G; ++x) s += tpart[(static_cast<size_t>(b) * G + x) * C + threadIdx.x];
+    for (int x = 0; x < P; ++x) s += tpart[(static_cast<size_t>(b) * P + x) * C + threadIdx.x];
     t[threadIdx.x] = s;
   }
   __syncthreads();
@@ -152,22 +156,27 @@ k_sum_segments(const float* __restrict__ part, int P, int L, float* __restrict__
 }
 
 // dQ rows of bag b (dsmil.py:53-55), then tanh' when q is nonlinear:
-// dz[n,j] = (sum_k dL[n,k] q_max_b[k,j] + sum_k [n == crit[b,k]] dqm[b,k,j]) * (1 - Q[n,j]^2),
-// with q_max_b[k] = Q[row_off + crit[b,k]] (crit is the row within the bag).
+// dz[n,j] = (sum_k dL[n,k] q_max_b[k,j] + sum_k [n == idx_bk] dqm[b,k,j]) * (1 - Q[n,j]^2).
+// qmax == NULL, row_offsets == NULL: the critical rows are local, idx_bk = crit[b,k] (the row within the bag) and
+// q_max_b[k] = Q[row_off + idx_bk].  A row-sharded batch passes the merged qmax [nb,C,128] and each bag's first global
+// row row_offsets[b]: crit holds global rows, idx_bk = crit[b,k] - row_offsets[b] (no local row matches when the
+// critical row lives on another rank), and q_max_b comes from qmax.
 __global__ void __launch_bounds__(256)
 k_bwd_dq_b(const sm90::BagDev* __restrict__ bags, int C, const float* __restrict__ dL, const float* __restrict__ Q,
-           const float* __restrict__ dqm, const int64_t* __restrict__ crit, int through_tanh, float* __restrict__ dz) {
+           const float* __restrict__ qmax, const float* __restrict__ dqm, const int64_t* __restrict__ crit,
+           const long long* __restrict__ row_offsets, int through_tanh, float* __restrict__ dz) {
   __shared__ float sq[kMaxC][kQ];
   __shared__ float sd[kMaxC][kQ];
   __shared__ int64_t sidx[kMaxC];
   const int b = blockIdx.y;
   const sm90::BagDev bg = bags[b];
+  const int64_t off = row_offsets ? row_offsets[b] : 0;
   for (int i = threadIdx.x; i < C * kQ; i += blockDim.x) {
     const int k = i / kQ, j = i % kQ;
-    sq[k][j] = Q[(bg.row_off + crit[b * C + k]) * kQ + j];
+    sq[k][j] = qmax ? qmax[static_cast<size_t>(b) * C * kQ + i] : Q[(bg.row_off + crit[b * C + k]) * kQ + j];
     sd[k][j] = dqm[static_cast<size_t>(b) * C * kQ + i];
   }
-  if (threadIdx.x < C) sidx[threadIdx.x] = crit[b * C + threadIdx.x];
+  if (threadIdx.x < C) sidx[threadIdx.x] = crit[b * C + threadIdx.x] - off;
   __syncthreads();
   const int64_t total = bg.N * kQ;
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;

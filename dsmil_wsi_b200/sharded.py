@@ -12,6 +12,10 @@ sharded; prediction_bag, B and the critical indices are replicated.
 `ops` abstracts the five local steps so the exchange/merge logic can be exercised on CPU with
 gloo (tests/test_sharded_gloo.py injects an oracle-backed ops object; the product default is
 CudaShardOps, which has no fallback).
+
+A batch of such bags goes through CudaShardBagOps: three library calls and two all-gathers per forward step, and,
+for training (sharded_milnet_forward_bags + sharded_caller_loss_bags), three more calls and four more collectives
+(one all-reduce(max) in the loss, three all-reduce(sum) in the backward), whatever the number of bags.
 """
 from __future__ import annotations
 
@@ -203,6 +207,7 @@ class CudaShardBagOps:
             self._ws_key = key
         self.cand_f = int(self.lib.dsmil_cand_floats(P.C))
         self.rec_f = int(self.lib.dsmil_rec_floats(P.C, P.D))
+        return self.xs
 
     def new(self, *shape, dtype=torch.float32):
         return torch.empty(*shape, dtype=dtype, device=self.device)
@@ -241,6 +246,98 @@ class CudaShardBagOps:
             outs.append((self.classes[row:row + n], pred[b:b + 1], self.A[row:row + n], B[b:b + 1], self.crit[b]))
             row += n
         return outs
+
+    # ---- training: phases 1 and 2 that keep Q/H1 row-major and q_max, and the three backward phases ----------------
+    # (dsmil_shard_bags_phase1/2_train, dsmil_shard_backward_bags_phase1/2/3).  Outputs stay packed [sum N_local, *].
+    def phase1_train(self):
+        """After begin(): (classes, Q, H1, cand [nb, cand])."""
+        P = self.P
+        with torch.cuda.device(self.device):
+            classes = self.new(self.total, P.C)
+            Q, H1 = self.new(self.total, Fn.Q_DIM), self.new(self.total, Fn.Q_DIM)
+            cand = self.new(self.nb, self.cand_f)
+            rc = self.lib.dsmil_shard_bags_phase1_train(P.ref, self.c_X, self.c_N, self.nb, self.c_off, Fn._ptr(classes),
+                                                        Fn._ptr(Q), Fn._ptr(H1), Fn._ptr(cand), Fn._ptr(self.ws),
+                                                        self.ws.numel(), Fn._stream())
+            _lib.check(rc, "dsmil_shard_bags_phase1_train")
+        return classes, Q, H1, cand
+
+    def phase2_train(self, Q: torch.Tensor, cands_all: torch.Tensor, G: int):
+        """(A logits, crit [nb, C] global rows, q_max [nb, C, 128], recs [nb, rec])."""
+        P = self.P
+        with torch.cuda.device(self.device):
+            A = self.new(self.total, P.C)
+            crit = self.new(self.nb, P.C, dtype=torch.int64)
+            qmax = self.new(self.nb, P.C, Fn.Q_DIM)
+            recs = self.new(self.nb, self.rec_f)
+            rc = self.lib.dsmil_shard_bags_phase2_train(P.ref, self.c_X, self.c_N, self.nb, Fn._ptr(Q), Fn._ptr(cands_all),
+                                                        G, Fn._ptr(A), Fn._ptr(crit), Fn._ptr(qmax), Fn._ptr(recs),
+                                                        Fn._ptr(self.ws), self.ws.numel(), Fn._stream())
+            _lib.check(rc, "dsmil_shard_bags_phase2_train")
+        return A, crit, qmax, recs
+
+    def phase3_train(self, recs_all: torch.Tensor, G: int, A: torch.Tensor):
+        """dsmil_shard_bags_phase3 on phase2_train's logits: (A normalised in place, B [nb, C, D], pred [nb, C])."""
+        P = self.P
+        with torch.cuda.device(self.device):
+            B, pred = self.new(self.nb, P.C, P.D), self.new(self.nb, P.C)
+            rc = self.lib.dsmil_shard_bags_phase3(P.ref, self.c_X, self.c_N, self.nb, Fn._ptr(recs_all), G, Fn._ptr(A),
+                                                  Fn._ptr(B), Fn._ptr(pred), Fn._ptr(self.ws), self.ws.numel(), Fn._stream())
+            _lib.check(rc, "dsmil_shard_bags_phase3")
+        return A, B, pred
+
+    @staticmethod
+    def _table(xs):
+        nb = len(xs)
+        return (C.c_void_p * nb)(*[x.data_ptr() for x in xs]), (C.c_int64 * nb)(*[int(x.shape[0]) for x in xs]), nb
+
+    def bwd1(self, xs, A, B, d_classes, d_pred):
+        """(dA, t [nb, C], gWi, gbi, gWf, gbf).  Allocates the backward workspace that bwd2 and bwd3 of the same step
+        read the bag tables from."""
+        P = self.P
+        c_X, c_N, nb = self._table(xs)
+        total = sum(int(x.shape[0]) for x in xs)
+        with torch.cuda.device(self.device):
+            self.bws = Fn._workspace(self.lib.dsmil_shard_backward_bags_workspace_bytes(P.ref, c_N, nb), self.device)
+            dA, t = self.new(total, P.C), self.new(nb, P.C)
+            gWi, gbi = self.new(P.C, P.D), self.new(P.C)
+            gWf, gbf = self.new(P.C, P.C, P.D), self.new(P.C)
+            dc = None if d_classes is None else d_classes.to(torch.float32).contiguous()
+            dp = None if d_pred is None else d_pred.to(torch.float32).contiguous()
+            rc = self.lib.dsmil_shard_backward_bags_phase1(P.ref, c_X, c_N, nb, Fn._ptr(A), Fn._ptr(B.contiguous()),
+                                                           Fn._ptr(dc), Fn._ptr(dp), Fn._ptr(dA), Fn._ptr(t),
+                                                           Fn._ptr(gWi), Fn._ptr(gbi), Fn._ptr(gWf), Fn._ptr(gbf),
+                                                           Fn._ptr(self.bws), self.bws.numel(), Fn._stream())
+            _lib.check(rc, "dsmil_shard_backward_bags_phase1")
+        return dA, t, gWi, gbi, gWf, gbf
+
+    def bwd2(self, xs, A, dA, t, Q):
+        """(dL, dqm [nb, C, 128]); dL replaces dA in place."""
+        P = self.P
+        _, c_N, nb = self._table(xs)
+        with torch.cuda.device(self.device):
+            dqm = self.new(nb, P.C, Fn.Q_DIM)
+            rc = self.lib.dsmil_shard_backward_bags_phase2(P.ref, c_N, nb, Fn._ptr(A), Fn._ptr(dA), Fn._ptr(t.contiguous()),
+                                                           Fn._ptr(Q), Fn._ptr(dqm), Fn._ptr(self.bws), self.bws.numel(),
+                                                           Fn._stream())
+            _lib.check(rc, "dsmil_shard_backward_bags_phase2")
+        return dA, dqm
+
+    def bwd3(self, xs, row_offsets, Q, H1, dL, dqm, qmax, crit):
+        """(gW1, gb1, gW2, gb2), this rank's shares."""
+        P = self.P
+        c_X, c_N, nb = self._table(xs)
+        c_off = (C.c_int64 * nb)(*[int(o) for o in row_offsets])
+        with torch.cuda.device(self.device):
+            gW1, gb1 = self.new(Fn.Q_DIM, P.D), self.new(Fn.Q_DIM)
+            gW2, gb2 = self.new(Fn.Q_DIM, Fn.Q_DIM), self.new(Fn.Q_DIM)
+            rc = self.lib.dsmil_shard_backward_bags_phase3(P.ref, c_X, c_N, nb, c_off, Fn._ptr(Q), Fn._ptr(H1), Fn._ptr(dL),
+                                                           Fn._ptr(dqm.contiguous()), Fn._ptr(qmax.contiguous()),
+                                                           Fn._ptr(crit.contiguous()), Fn._ptr(gW1), Fn._ptr(gb1),
+                                                           Fn._ptr(gW2), Fn._ptr(gb2), Fn._ptr(self.bws), self.bws.numel(),
+                                                           Fn._stream())
+            _lib.check(rc, "dsmil_shard_backward_bags_phase3")
+        return gW1, gb1, gW2, gb2
 
 
 @torch.no_grad()
@@ -392,15 +489,22 @@ def sharded_backward(ops, saved: ShardSaved, d_classes_local: Optional[torch.Ten
     dL, dqm = ops.bwd2(saved.A, dA, t, saved.Q)
     dqm = reduce(dqm, group)                                                # reduce 2
     gW1, gb1, gW2, gb2 = ops.bwd3(saved.X, saved.row_offset, saved.Q, saved.H1, dL, dqm, saved.qmax, saved.crit)
-    parts = [g for g in (gWi, gbi, gW1, gb1, gW2, gb2) if g is not None]
-    flat = reduce(torch.cat([g.reshape(-1) for g in parts]), group)         # reduce 3
+    gWi, gbi, gW1, gb1, gW2, gb2 = _reduce_flat((gWi, gbi, gW1, gb1, gW2, gb2), group, reduce)   # reduce 3
+    return gWi, gbi, gW1, gb1, gW2, gb2, gWf, gbf                           # Wf/bf grads are replicated already
+
+
+def _reduce_flat(grads, group, reduce):
+    """One reduce over the non-None tensors of `grads`, packed into a flat buffer; returns views in the same order."""
+    parts = [g for g in grads if g is not None]
+    flat = reduce(torch.cat([g.reshape(-1) for g in parts]), group)
     out, off = [], 0
-    for g in parts:
+    for g in grads:
+        if g is None:
+            out.append(None)
+            continue
         out.append(flat[off:off + g.numel()].view_as(g))
         off += g.numel()
-    gWi, gbi, gW1, gb1 = out[:4]
-    gW2, gb2 = (out[4], out[5]) if len(out) == 6 else (None, None)
-    return gWi, gbi, gW1, gb1, gW2, gb2, gWf, gbf                           # Wf/bf grads are replicated already
+    return out
 
 
 class ShardedMILFn(torch.autograd.Function):
@@ -485,6 +589,176 @@ def virtual_sharded_train_step(ops, X: torch.Tensor, G: int, loss_grads):
     b2 = [ops.bwd2(o[0], b[0], t, l[1]) for l, o, b in zip(loc, outs, b1)]
     dqm = torch.stack([b[1] for b in b2]).sum(0)                         # reduce 2
     b3 = [ops.bwd3(l[3], lo, l[1], l[2], b[0], dqm, qmax, crit) for l, b, (lo, _) in zip(loc, b2, bounds)]
+    tot = lambda ts: None if ts[0] is None else torch.stack(list(ts)).sum(0)   # reduce 3
+    gWi, gbi = tot([b[2] for b in b1]), tot([b[3] for b in b1])
+    gW1, gb1, gW2, gb2 = (tot([b[i] for b in b3]) for i in range(4))
+    return (classes, pred, A, B, crit), (gWi, gbi, gW1, gb1, gW2, gb2, b1[0][4], b1[0][5])
+
+
+# ---- a minibatch of row-sharded bags: training step ---------------------------------------------------------------
+# Six collectives per step whatever the batch size: the forward's two all-gathers, one all-reduce(max) of nb*C floats
+# in the loss and three all-reduce(sum) in the reverse pass (t [nb,C], dq_max [nb,C,128], one flat buffer of parameter
+# gradients); 3 + 3 library calls.  `bops` is a CudaShardBagOps, or any object with its begin / phase*_train / phase3_train
+# / bwd1-3 methods (the host logic below calls nothing else, so it runs over gloo with a CPU stand-in).
+
+
+class ShardBagsSaved:
+    """What one rank keeps between the forward of a row-sharded batch and its reverse pass (per-row tensors packed in
+    bag order over the local rows)."""
+    __slots__ = ("xs", "row_offsets", "Q", "H1", "A", "B", "qmax", "crit")
+
+    def __init__(self, xs, row_offsets, Q, H1, A, B, qmax, crit):
+        self.xs, self.row_offsets, self.Q, self.H1 = list(xs), [int(o) for o in row_offsets], Q, H1
+        self.A, self.B, self.qmax, self.crit = A, B, qmax, crit
+
+
+@torch.no_grad()
+def sharded_forward_bags_train(bops, X_locals, row_offsets, group=None, gather=_all_gather):
+    """Forward of a batch of row-sharded bags that keeps what `sharded_backward_bags` needs.  Returns
+    ((classes_local [sum N_local, C], pred [nb, C], A_local [sum N_local, C], B [nb, C, D], crit [nb, C]), saved);
+    pred, B and crit (global rows: the row within the whole bag) are replicated."""
+    xs = bops.begin(X_locals, row_offsets)
+    classes, Q, H1, cand = bops.phase1_train()
+    cands_all, G = gather(cand.reshape(-1), group)                          # exchange 1: [G][nb][cand]
+    A, crit, qmax, recs = bops.phase2_train(Q, cands_all, G)
+    recs_all, G = gather(recs.reshape(-1), group)                           # exchange 2: [G][nb][rec]
+    A, B, pred = bops.phase3_train(recs_all, G, A)
+    return (classes, pred, A, B, crit), ShardBagsSaved(xs, row_offsets, Q, H1, A, B, qmax, crit)
+
+
+@torch.no_grad()
+def sharded_backward_bags(bops, saved: ShardBagsSaved, d_classes_local: Optional[torch.Tensor],
+                          d_pred: Optional[torch.Tensor], group=None, reduce=_all_reduce_sum):
+    """Reverse pass of `sharded_forward_bags_train`: exactly three all-reduce(sum) -- t [nb, C], dq_max [nb, C, 128] and
+    one flat buffer of the parameter gradients.  Returns (gWi, gbi, gW1, gb1, gW2, gb2, gWf, gbf), sums over the bags,
+    identical on every rank."""
+    dA, t, gWi, gbi, gWf, gbf = bops.bwd1(saved.xs, saved.A, saved.B, d_classes_local, d_pred)
+    t = reduce(t, group)                                                    # reduce 1
+    dL, dqm = bops.bwd2(saved.xs, saved.A, dA, t, saved.Q)
+    dqm = reduce(dqm, group)                                                # reduce 2
+    gW1, gb1, gW2, gb2 = bops.bwd3(saved.xs, saved.row_offsets, saved.Q, saved.H1, dL, dqm, saved.qmax, saved.crit)
+    gWi, gbi, gW1, gb1, gW2, gb2 = _reduce_flat((gWi, gbi, gW1, gb1, gW2, gb2), group, reduce)   # reduce 3
+    return gWi, gbi, gW1, gb1, gW2, gb2, gWf, gbf                           # Wf/bf grads are replicated already
+
+
+class ShardedMILBagsFn(torch.autograd.Function):
+    """autograd node of a batch of row-sharded bags: forward = sharded_forward_bags_train, backward =
+    sharded_backward_bags.  Every rank of the group must call it (and `.backward()`) in the same order.  args: bops,
+    row_offsets, group, nb, the nb local bags, then the ten parameter tensors in ABI order (Wv, bv must be None)."""
+
+    @staticmethod
+    def forward(ctx, bops, row_offsets, group, nb, *args):
+        ctx.set_materialize_grads(False)          # unused outputs (A, B) arrive as None, not as zero tensors
+        outs, saved = sharded_forward_bags_train(bops, args[:nb], row_offsets, group)
+        ctx.bops, ctx.saved, ctx.group, ctx.nb = bops, saved, group, nb
+        classes, pred, A, B, crit = outs
+        ctx.mark_non_differentiable(crit)
+        return classes, pred, A, B, crit
+
+    @staticmethod
+    def backward(ctx, d_classes, d_pred, d_A, d_B, _d_crit):
+        if d_A is not None or d_B is not None:
+            raise NotImplementedError("sharded backward: gradients through A / B are not supported "
+                                      "(the callers use classes and prediction_bag only, train_tcga.py:67-72)")
+        gWi, gbi, gW1, gb1, gW2, gb2, gWf, gbf = sharded_backward_bags(ctx.bops, ctx.saved, d_classes, d_pred, ctx.group)
+        return (None, None, None, None, *([None] * ctx.nb), gWi, gbi, gW1, gb1, gW2, gb2, None, None, gWf, gbf)
+
+
+def sharded_milnet_forward_bags(milnet, X_locals: Sequence[torch.Tensor], row_offsets: Sequence[int], group=None,
+                                ops=None):
+    """Packed `(classes_local, prediction_bag, A_local, B, crit_idx)` of a batch of bags whose rows live on several
+    ranks (bag b: this rank's rows [row_offsets[b], row_offsets[b] + len(X_locals[b])), at least one per bag), with
+    autograd: `loss.backward()` on every rank (loss from `sharded_caller_loss_bags`) leaves identical, fully reduced
+    `.grad`s on the parameters.  classes_local / A_local are [sum N_local, C] in bag order; prediction_bag [nb, C],
+    B [nb, C, D] and crit_idx [nb, C] (global rows) are replicated."""
+    params = milnet_params(milnet)
+    ops = ops or CudaShardBagOps(params)
+    return ShardedMILBagsFn.apply(ops, [int(o) for o in row_offsets], group, len(X_locals), *X_locals, *params)
+
+
+def sharded_max_prediction_bags(classes_local: torch.Tensor, crit: torch.Tensor, row_offsets: Sequence[int],
+                                Ns: Sequence[int], group=None):
+    """Per-bag `torch.max(ins_prediction, 0)[0]`, [nb, C], of bags whose rows are spread over ranks: one all-reduce(max)
+    of nb*C floats for the whole batch.  The value is the same on every rank; the gradient flows only into the row
+    that holds the maximum, on the rank that owns it.  classes_local is packed [sum Ns, C]; crit [nb, C] holds global
+    rows."""
+    import torch.distributed as dist
+    dev = classes_local.device
+    Cc = int(classes_local.shape[1])
+    n = torch.tensor([int(v) for v in Ns], dtype=torch.int64, device=dev)
+    first = torch.cumsum(n, 0) - n
+    loc = crit.to(dev) - torch.tensor([int(o) for o in row_offsets], dtype=torch.int64, device=dev)[:, None]
+    owned = (loc >= 0) & (loc < n[:, None])
+    total = int(classes_local.shape[0])
+    if total > 0:
+        # owned entries index their row; the others any valid row (their value is replaced, their gradient is zero)
+        mine = classes_local.gather(0, (first[:, None] + loc.clamp(min=0)).clamp(max=total - 1))
+    else:
+        mine = classes_local.new_zeros(len(Ns), Cc)
+    glob = torch.where(owned, mine.detach(), torch.full_like(mine, float("-inf")))
+    dist.all_reduce(glob, op=dist.ReduceOp.MAX, group=group)
+    return torch.where(owned, mine, glob)
+
+
+def sharded_caller_loss_bags(classes_local, prediction_bag, crit, row_offsets, labels, criterion, group=None, *, Ns):
+    """The minibatch loss of feed.train_epoch(bags_per_step=k), 0.5 * criterion(pred [k, C]) + 0.5 * criterion(max
+    instance [k, C]), for row-sharded bags: same value on every rank; `loss.backward()` on every rank gives the
+    single-device gradients.  Ns: this rank's row count of each bag (the packing of classes_local)."""
+    max_prediction = sharded_max_prediction_bags(classes_local, crit, row_offsets, Ns, group)
+    tgt = labels.reshape(prediction_bag.shape).to(prediction_bag.dtype)
+    return 0.5 * criterion(prediction_bag, tgt) + 0.5 * criterion(max_prediction, tgt)
+
+
+@torch.no_grad()
+def virtual_sharded_train_step_bags(make_ops, Xs: Sequence[torch.Tensor], G: int, loss_grads):
+    """A training step of a batch of bags with G logical shards each on ONE device: the all-gathers replaced by
+    concatenation and the all-reduces by local sums (same kernels, same record layouts).  `make_ops()` returns a fresh
+    ops object per logical rank (each holds its rank's workspaces).  `loss_grads(classes [sum N, C], pred [nb, C],
+    crit [nb, C]) -> (d_classes [sum N, C] | None, d_pred [nb, C] | None)`, with classes packed in bag order.  Returns
+    ((classes, pred, A, B, crit), grads) with classes / A packed in bag order and grads in the order of
+    `sharded_backward_bags`."""
+    bounds = [shard_bounds(int(x.shape[0]), G) for x in Xs]              # [bag][rank]
+    ranks = []
+    for r in range(G):
+        ops = make_ops()
+        xs = ops.begin([x[b[r][0]:b[r][1]] for x, b in zip(Xs, bounds)], [b[r][0] for b in bounds])
+        ranks.append(dict(ops=ops, xs=xs, offs=[b[r][0] for b in bounds], p1=ops.phase1_train()))
+    cands = torch.cat([R["p1"][3].reshape(-1) for R in ranks])
+    for R in ranks:
+        R["p2"] = R["ops"].phase2_train(R["p1"][1], cands, G)             # A, crit, qmax, recs
+    recs = torch.cat([R["p2"][3].reshape(-1) for R in ranks])
+    for R in ranks:
+        R["p3"] = R["ops"].phase3_train(recs, G, R["p2"][0])              # A, B, pred
+    B, pred, crit = ranks[0]["p3"][1], ranks[0]["p3"][2], ranks[0]["p2"][1]
+
+    def rank_rows(r):                                                    # this rank's packed rows, per bag
+        out, lo = [], 0
+        for b in bounds:
+            n = b[r][1] - b[r][0]
+            out.append((lo, lo + n))
+            lo += n
+        return out
+    rows = [rank_rows(r) for r in range(G)]
+
+    def to_bag_order(per_rank):                                          # [rank][sum N_r, *] -> [sum N, *]
+        return torch.cat([per_rank[r][slice(*rows[r][b])] for b in range(len(Xs)) for r in range(G)])
+
+    classes = to_bag_order([R["p1"][0] for R in ranks])
+    A = to_bag_order([R["p3"][0] for R in ranks])
+    d_classes, d_pred = loss_grads(classes, pred, crit)
+    if d_classes is not None:                                            # bag order -> each rank's packing
+        start = [0]
+        for x in Xs:
+            start.append(start[-1] + int(x.shape[0]))
+        d_loc = [torch.cat([d_classes[start[b] + bounds[b][r][0]:start[b] + bounds[b][r][1]] for b in range(len(Xs))])
+                 for r in range(G)]
+    b1 = [R["ops"].bwd1(R["xs"], R["p3"][0], B, None if d_classes is None else d_loc[r], d_pred)
+          for r, R in enumerate(ranks)]                                  # dA, t, gWi, gbi, gWf, gbf
+    t = torch.stack([b[1] for b in b1]).sum(0)                           # reduce 1
+    b2 = [R["ops"].bwd2(R["xs"], R["p3"][0], b[0], t, R["p1"][1]) for R, b in zip(ranks, b1)]
+    dqm = torch.stack([b[1] for b in b2]).sum(0)                         # reduce 2
+    b3 = [R["ops"].bwd3(R["xs"], R["offs"], R["p1"][1], R["p1"][2], b[0], dqm, R["p2"][2], R["p2"][1])
+          for R, b in zip(ranks, b2)]
     tot = lambda ts: None if ts[0] is None else torch.stack(list(ts)).sum(0)   # reduce 3
     gWi, gbi = tot([b[2] for b in b1]), tot([b[3] for b in b1])
     gW1, gb1, gW2, gb2 = (tot([b[i] for b in b3]) for i in range(4))

@@ -264,6 +264,51 @@ int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, con
                             const float* recs_all, int32_t G, float* A, float* B, float* pred,
                             void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- row-sharded batch training (identity v; dsmil_shard_bags_supported shapes) -------------------------------------
+ * A minibatch of row-sharded bags in 3 + 3 library calls and 6 collectives per step, whatever nb: 2 all-gathers in the
+ * forward, all-reduce(max) of nb*C floats in the callers' loss, 3 all-reduce(sum) in the backward.
+ *
+ * Forward: dsmil_shard_bags_phase1_train, then dsmil_shard_bags_phase2_train, then the inference dsmil_shard_bags_phase3
+ * unchanged.  The training phases carve the workspace (dsmil_shard_bags_workspace_bytes) exactly as the inference
+ * phases do, so phase 3 finishes the step from it.  The differences:
+ *   phase1_train keeps Q (after the tanh) and H1 row-major in the caller's save_Q / save_H1, packed [sum N_local, 128]
+ *   phase2_train attends on that Q and also returns the merged q_max [nb][C][128]; crit_idx [nb][C] holds GLOBAL rows
+ *   (row within the whole bag), as dsmil_shard_bags_phase2.
+ * Every bag must hold at least one local row on every rank (else DSMIL_ERR_EMPTY); 1 <= nb <= 65535.
+ *
+ * Backward: three phases with the caller's all-reduce(sum) between them.  One workspace of
+ * dsmil_shard_backward_bags_workspace_bytes for all three calls of a step (phase 1 leaves the bag and chunk tables in
+ * it for phases 2 and 3).  Per-row buffers are packed [sum N_local, *] in bag order, as dsmil_backward_bags; parameter
+ * gradients are sums over the bags, overwritten.
+ *   phase1: dA_local [sum N,C]; t_local [nb][C] (per-bag sum_n A.dA over the local rows, in a fixed order); gWf/gbf
+ *           replicated (no reduction); local partial gWi/gbi (d_classes_local may be NULL; any gradient buffer may be
+ *           NULL == not wanted)                                       -> all-reduce t (nb*C floats)
+ *   phase2: dA becomes dL in place with the global t; dqm_local [nb][C][128] -> all-reduce dqm
+ *   phase3: Q-MLP backward over the local rows; the dq_max share goes to the rank that holds row crit_idx[b][k]
+ *           (global) - row_offsets[b]; q_max is phase2_train's; local partial gW1/gb1/gW2/gb2
+ *                                                                     -> all-reduce the parameter gradients
+ * With one rank (identity reductions) the three phases give dsmil_backward_bags's bits.  No gX and no upstream d_A/d_B. */
+int dsmil_shard_bags_phase1_train(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                                  const int64_t* row_offsets, float* classes, float* save_Q, float* save_H1,
+                                  float* cand_recs, void* workspace, size_t workspace_bytes, void* stream);
+int dsmil_shard_bags_phase2_train(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                                  const float* Q, const float* cands_all, int32_t G, float* A, int64_t* crit_idx,
+                                  float* q_max, float* recs_out, void* workspace, size_t workspace_bytes,
+                                  void* stream);
+size_t dsmil_shard_backward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb);
+int dsmil_shard_backward_bags_phase1(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                                     const float* A, const float* B, const float* d_classes_local,
+                                     const float* d_pred, float* dA_local, float* t_local, float* gWi, float* gbi,
+                                     float* gWf, float* gbf, void* workspace, size_t workspace_bytes, void* stream);
+int dsmil_shard_backward_bags_phase2(const dsmil_params_t* p, const int64_t* Ns, int32_t nb, const float* A,
+                                     float* dA_to_dL, const float* t_global, const float* Q, float* dqm_local,
+                                     void* workspace, size_t workspace_bytes, void* stream);
+int dsmil_shard_backward_bags_phase3(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
+                                     const int64_t* row_offsets, const float* Q, const float* H1, const float* dL_local,
+                                     const float* dqm_global, const float* q_max, const int64_t* crit_idx,
+                                     float* gW1, float* gb1, float* gW2, float* gb2, void* workspace,
+                                     size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
