@@ -96,6 +96,16 @@ SIGNATURES = {
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(DsmilGrads), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_forward_bags_train_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
+    "dsmil_forward_bags_train_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_int32, c_i64,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                               C.c_void_p]),
+    "dsmil_backward_bags_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
+    "dsmil_backward_bags_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_int32, c_i64,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.POINTER(DsmilGrads), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dsmil_shard_bags_supported": (C.c_int, [C.POINTER(DsmilParams)]),
     "dsmil_shard_bags_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.POINTER(c_i64), C.c_int32]),
     "dsmil_shard_bags_phase1": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(C.c_void_p), C.POINTER(c_i64), C.c_int32,

@@ -8,6 +8,7 @@
 #include <cstdlib>
 #include <vector>
 #include <algorithm>
+#include <climits>
 
 #include "common.cuh"
 #include "gemm_generic.cuh"
@@ -16,6 +17,7 @@
 #include "bwd_bags.cuh"
 #include "fwd_sm90.cuh"
 #include "fwd_batched.cuh"
+#include "bag_plan.cuh"
 #include "embed_kernels.cuh"
 #include "jpeg_kernels.cuh"
 
@@ -169,11 +171,8 @@ static void carve_phase1(Carver& c, const dsmil_params_t* p, int nb, Phase1Ws& w
   }
 }
 
-static inline int recs_for_bag(int64_t N) {
-  const int64_t t = (N + sm90::kAttRows - 1) / sm90::kAttRows;
-  return static_cast<int>(t < sm90::kMaxRecPerBag ? (t < 1 ? 1 : t) : sm90::kMaxRecPerBag);
-}
-// Host copy of the bag table: each bag's first row, 128-row tile and partial record, numbered across the batch.
+// Host copy of the bag table: each bag's first row, 128-row tile and partial record, numbered across the batch
+// (bag_entry, as the dev calls' planner numbers it).
 static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::vector<sm90::BagDev>& tbl, int* tiles,
                        int* recs) {
   long long row = 0;
@@ -182,11 +181,7 @@ static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::v
   for (int b = 0; b < nb; ++b) {
     DSMIL_REQUIRE(Ns[b] >= 1 && Ns[b] < 0xffffffffll && Xs[b], "bag %d: empty or NULL", b);
     DSMIL_REQUIRE((reinterpret_cast<uintptr_t>(Xs[b]) & 15) == 0, "bag %d: features must be 16-byte aligned", b);
-    const int nrec = recs_for_bag(Ns[b]);
-    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, tile, rec, nrec, 0};
-    row += Ns[b];
-    tile += static_cast<int>((Ns[b] + sm90::kTileM - 1) / sm90::kTileM);
-    rec += nrec;
+    tbl[b] = bag_entry(Xs[b], Ns[b], row, tile, rec);
   }
   *tiles = tile;
   *recs = rec;
@@ -421,7 +416,7 @@ static BagsWs carve_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, boo
   BagsWs w;
   int64_t tiles = 0, nrec = 0;
   for (int b = 0; b < nb; ++b) {
-    tiles += (Ns[b] + sm90::kTileM - 1) / sm90::kTileM;
+    tiles += tiles_for_bag(Ns[b]);
     nrec += recs_for_bag(Ns[b]);
   }
   carve_phase1(c, p, nb, w);
@@ -436,11 +431,24 @@ static BagsWs carve_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, boo
   return w;
 }
 
+// Phases 2 and 3 of the batched forward: attend (one CTA per partial record: `recs` of them, or, with recs_dev, the
+// first *recs_dev of a capacity grid of `recs`), then each bag's A, B, logits and critical rows.
+static int bags_attend_finalize(const dsmil_params_t* p, const BagsWs& w, int nb, const float* Q, bool q_blocked,
+                                float* pred, float* A, float* B, int64_t* crit, int recs, const int* recs_dev,
+                                cudaStream_t st) {
+  const int C = p->C, D = p->D;
+  int rc;
+  sm90::AttendArgs aa{w.table, nb, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr, recs_dev};
+  if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
+  sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, p->Wf, p->bf, A, B, pred, reinterpret_cast<long long*>(crit),
+                         w.pred_part, w.counters, nullptr, 0, 0};
+  return sm90::launch_finalize_b(fa, nb, st);
+}
+
 static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
                              const float* classes_in, float* classes, float* pred, float* A, float* B,
                              int64_t* crit, float* save_Q, float* save_H1, void* ws, size_t ws_bytes,
                              cudaStream_t st) {
-  const int C = p->C, D = p->D;
   bool ok;
   BagsWs w = carve_bags(p, Ns, nb, save_Q == nullptr, false, ws, ws_bytes, &ok);
   int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
@@ -450,11 +458,7 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
   int tiles, recs;
   if ((rc = bags_phase1_impl(p, w, Xs, Ns, nb, classes_in, classes, Q, save_H1, q_blocked, true, &tiles, &recs, st)))
     return rc;
-  sm90::AttendArgs aa{w.table, nb, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr};
-  if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
-  sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, p->Wf, p->bf, A, B, pred, reinterpret_cast<long long*>(crit),
-                         w.pred_part, w.counters, nullptr, 0, 0};
-  return sm90::launch_finalize_b(fa, nb, st);
+  return bags_attend_finalize(p, w, nb, Q, q_blocked, pred, A, B, crit, recs, nullptr, st);
 }
 
 }  // namespace dsmil
@@ -941,6 +945,8 @@ int dsmil_instance_scores_backward(const dsmil_params_t* p, const float* X, int6
 
 // ---- batched training: forward that keeps Q/H1, and its backward over the bag table ------------------------------
 struct BwdBagsWs {
+  BagsPlan* plan;            // dev calls: the planner's live counts (G, nci, nc1 are then capacities); NULL: eager
+  float* zero_row;           // dev calls: the stand-in bag row of a refused batch
   sm90::BagDev* table;
   TnChunk *chi, *ch1;        // chunk tables of gWi = d_classes^T X and gW1 = dz1^T X
   float *dB, *dA, *dL, *tpart, *dpart, *dqm, *dz2, *dz1, *tnpart, *cspart;
@@ -953,6 +959,28 @@ struct BwdBagsWs {
 };
 // `aligned`: every bag 16-byte aligned (the streaming gWi kernel needs it).  The carve reserves room for either gWi
 // form, so the reported size does not depend on alignment.  `sharded` appends the row offsets of the row-sharded batch.
+// The carve of w for nb bags, n packed rows and room for nchi gWi chunks, w.G / w.nc1 already set.
+static void layout_bwd_bags(Carver& c, const dsmil_params_t* p, int nb, int64_t n, int nchi, bool sharded,
+                            BwdBagsWs& w) {
+  const int C = p->C, D = p->D;
+  w.table = c.take<sm90::BagDev>(nb);
+  w.chi = c.take<TnChunk>(nchi);
+  w.ch1 = c.take<TnChunk>(w.nc1);
+  w.dB = c.take<float>(static_cast<size_t>(nb) * C * D);
+  w.dA = c.take<float>(n * C);
+  w.dL = c.take<float>(n * C);
+  w.tpart = c.take<float>(static_cast<size_t>(nb) * w.G * C);
+  w.dpart = c.take<float>(static_cast<size_t>(nb) * w.G * C * kQ);
+  w.dqm = c.take<float>(static_cast<size_t>(nb) * C * kQ);
+  w.dz2 = c.take<float>(n * kQ);
+  w.dz1 = p->nonlinear ? c.take<float>(n * kQ) : nullptr;
+  size_t tn = static_cast<size_t>(nchi) * C * D;
+  tn = std::max(tn, static_cast<size_t>(w.nc1) * kQ * D);
+  tn = std::max(tn, tn_partial_floats(kQ, kQ, n));
+  w.tnpart = c.take<float>(tn);
+  w.cspart = c.take<float>(static_cast<size_t>(kSplits) * kQ);
+  w.row_offsets = sharded ? c.take<long long>(nb) : nullptr;
+}
 static BwdBagsWs carve_bwd_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, bool aligned, bool sharded,
                                 void* ws, size_t cap, bool* ok) {
   Carver c(ws, cap);
@@ -963,8 +991,9 @@ static BwdBagsWs carve_bwd_bags(const dsmil_params_t* p, const int64_t* Ns, int 
     total += Ns[b];
     mx = std::max<int64_t>(mx, Ns[b]);
   }
-  const int64_t n = std::max<int64_t>(total, 1);
-  w.G = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(ceil_div(kSms * 8, nb), ceil_div(mx, 64))));
+  w.plan = nullptr;
+  w.zero_row = nullptr;
+  w.G = bwd_bags_ctas(nb, mx);
   const bool gemv_ok = tn_use_gemv(C, D);
   w.gemv_i = gemv_ok && aligned;
   const int64_t rps_gemv = rag_rows_per_chunk(C, D, total, true), rps_tile = rag_rows_per_chunk(C, D, total, false);
@@ -974,23 +1003,26 @@ static BwdBagsWs carve_bwd_bags(const dsmil_params_t* p, const int64_t* Ns, int 
   w.nci = w.gemv_i ? nci_gemv : nci_tile;
   w.rps_1 = rag_rows_per_chunk(kQ, D, total, false);
   w.nc1 = rag_chunks(nullptr, Ns, nb, D, w.rps_1, nullptr);
-  w.table = c.take<sm90::BagDev>(nb);
-  w.chi = c.take<TnChunk>(std::max(nci_gemv, nci_tile));
-  w.ch1 = c.take<TnChunk>(w.nc1);
-  w.dB = c.take<float>(static_cast<size_t>(nb) * C * D);
-  w.dA = c.take<float>(n * C);
-  w.dL = c.take<float>(n * C);
-  w.tpart = c.take<float>(static_cast<size_t>(nb) * w.G * C);
-  w.dpart = c.take<float>(static_cast<size_t>(nb) * w.G * C * kQ);
-  w.dqm = c.take<float>(static_cast<size_t>(nb) * C * kQ);
-  w.dz2 = c.take<float>(n * kQ);
-  w.dz1 = p->nonlinear ? c.take<float>(n * kQ) : nullptr;
-  size_t tn = static_cast<size_t>(std::max(nci_gemv, nci_tile)) * C * D;
-  tn = std::max(tn, static_cast<size_t>(w.nc1) * kQ * D);
-  tn = std::max(tn, tn_partial_floats(kQ, kQ, n));
-  w.tnpart = c.take<float>(tn);
-  w.cspart = c.take<float>(static_cast<size_t>(kSplits) * kQ);
-  w.row_offsets = sharded ? c.take<long long>(nb) : nullptr;
+  layout_bwd_bags(c, p, nb, std::max<int64_t>(total, 1), std::max(nci_gemv, nci_tile), sharded, w);
+  w.bytes = c.off;
+  *ok = c.ok();
+  return w;
+}
+// A dev call's carve: every count at its capacity for nb bags of up to max_rows rows (bag_plan.cuh bounds the
+// chunks), the bags 16-byte aligned, and the planner's BagsPlan at the end.
+static BwdBagsWs carve_bwd_bags_dev(const dsmil_params_t* p, int nb, int64_t max_rows, void* ws, size_t cap,
+                                    bool* ok) {
+  Carver c(ws, cap);
+  BwdBagsWs w;
+  const int C = p->C, D = p->D;
+  w.G = bwd_bags_ctas(nb, max_rows);
+  w.gemv_i = tn_use_gemv(C, D);
+  w.nci = rag_chunks_cap(C, D, w.gemv_i, nb);
+  w.nc1 = rag_chunks_cap(kQ, D, false, nb);
+  w.rps_i = w.rps_1 = 0;
+  layout_bwd_bags(c, p, nb, static_cast<int64_t>(nb) * max_rows, w.nci, false, w);
+  w.plan = c.take<BagsPlan>(1);
+  w.zero_row = c.take<float>(D);
   w.bytes = c.off;
   *ok = c.ok();
   return w;
@@ -998,7 +1030,9 @@ static BwdBagsWs carve_bwd_bags(const dsmil_params_t* p, const int64_t* Ns, int 
 
 // The batched backward in three phases, cut at its two per-bag cross-row sums (t_b and dq_max_b), as bwd_phase1/2/3_impl
 // are for one bag.  dsmil_backward_bags runs them in a row; the row-sharded batch runs one per call, with the caller's
-// all-reduces in between.  Phase 1 uploads the bag and chunk tables into w; phases 2 and 3 read them from there.
+// all-reduces in between.  Phase 1 uploads the bag and chunk tables into w; phases 2 and 3 read them from there.  In a
+// dev call (w.plan != NULL) the planner has written the tables, `total` is the row capacity, and every launch that
+// depends on the live rows reads its count from w.plan.
 
 // Phase 1: dB, gWf/gbf, gWi/gbi, dA = X dB_b^T (+ d_A) into dA, and t_b's per-CTA partials in w.tpart (w.G per bag).
 static int bwd_bags_phase1_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
@@ -1006,20 +1040,23 @@ static int bwd_bags_phase1_impl(const dsmil_params_t* p, const float* const* Xs,
                                 const float* d_pred, const float* d_A, const float* d_B, const dsmil_grads_t* g,
                                 float* dA, const BwdBagsWs& w, cudaStream_t st) {
   const int C = p->C, D = p->D;
+  const BagsPlan* pl = w.plan;
   int rc;
-  // the kernels read X, N and row_off of the table (not the forward's tile and record numbering), at any alignment
-  std::vector<sm90::BagDev> tbl(nb);
-  long long row = 0;
-  for (int b = 0; b < nb; ++b) {
-    tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, 0, 0, 0, 0};
-    row += Ns[b];
+  if (!pl) {
+    // the kernels read X, N and row_off of the table (not the forward's tile and record numbering), at any alignment
+    std::vector<sm90::BagDev> tbl(nb);
+    long long row = 0;
+    for (int b = 0; b < nb; ++b) {
+      tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, 0, 0, 0, 0};
+      row += Ns[b];
+    }
+    std::vector<TnChunk> chi(w.nci), ch1(w.nc1);
+    rag_chunks(Xs, Ns, nb, D, w.rps_i, chi.data());
+    rag_chunks(Xs, Ns, nb, D, w.rps_1, ch1.data());
+    DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
+    DSMIL_CUDA_OK(cudaMemcpyAsync(w.chi, chi.data(), sizeof(TnChunk) * w.nci, cudaMemcpyHostToDevice, st));
+    DSMIL_CUDA_OK(cudaMemcpyAsync(w.ch1, ch1.data(), sizeof(TnChunk) * w.nc1, cudaMemcpyHostToDevice, st));
   }
-  std::vector<TnChunk> chi(w.nci), ch1(w.nc1);
-  rag_chunks(Xs, Ns, nb, D, w.rps_i, chi.data());
-  rag_chunks(Xs, Ns, nb, D, w.rps_1, ch1.data());
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.chi, chi.data(), sizeof(TnChunk) * w.nci, cudaMemcpyHostToDevice, st));
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.ch1, ch1.data(), sizeof(TnChunk) * w.nc1, cudaMemcpyHostToDevice, st));
 
   // bag classifier (dsmil.py:59-61) and B, summed over the bags
   k_bwd_bag_b<<<ceil_div(static_cast<int64_t>(C) * D, 256), 256, 0, st>>>(p->Wf, B, d_pred, d_B, nb, C, D, w.dB,
@@ -1027,30 +1064,34 @@ static int bwd_bags_phase1_impl(const dsmil_params_t* p, const float* const* Xs,
   DSMIL_LAUNCH_OK("k_bwd_bag_b");
   // instance classifier (dsmil.py:11)
   if (g->gWi) {
-    if (d_classes) { if ((rc = launch_gemm_tn_rag(d_classes, C, D, w.chi, w.nci, w.gemv_i, w.tnpart, g->gWi, st))) return rc; }
+    if (d_classes) {
+      if ((rc = launch_gemm_tn_rag(d_classes, C, D, w.chi, w.nci, w.gemv_i, w.tnpart, g->gWi, st, pl ? &pl->nci : nullptr)))
+        return rc;
+    }
     else DSMIL_CUDA_OK(cudaMemsetAsync(g->gWi, 0, sizeof(float) * C * D, st));
   }
   if (g->gbi) {
-    if (d_classes) { if ((rc = launch_colsum(d_classes, C, total, w.cspart, g->gbi, st))) return rc; }
+    if (d_classes) { if ((rc = launch_colsum(d_classes, C, total, w.cspart, g->gbi, st, pl ? &pl->cs : nullptr))) return rc; }
     else DSMIL_CUDA_OK(cudaMemsetAsync(g->gbi, 0, sizeof(float) * C, st));
   }
   // dA = X dB_b^T (+ d_A) and t_b's partials
   const size_t smem = sizeof(float) * C * D;
   if (smem > 48 * 1024)
     DSMIL_CUDA_OK(cudaFuncSetAttribute(k_bwd_rowdot_b, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_bwd_rowdot_b<<<dim3(w.G, nb), 256, smem, st>>>(w.table, D, w.dB, C, A, d_A, dA, w.tpart);
+  k_bwd_rowdot_b<<<dim3(w.G, nb), 256, smem, st>>>(w.table, D, w.dB, C, A, d_A, dA, w.tpart, pl ? &pl->G : nullptr);
   DSMIL_LAUNCH_OK("k_bwd_rowdot_b");
   return 0;
 }
 
-// Phase 2: dL = A (dA - t_b) / sqrt(128), t_b the sum of the P partials per bag in `tpart`; dqm[b] = dL_b^T Q_b,
-// summed over the CTAs' shares in a fixed order.
+// Phase 2: dL = A (dA - t_b) / sqrt(128), t_b the sum of the P partials per bag in `tpart` (a dev call: phase 1's
+// live G of them); dqm[b] = dL_b^T Q_b, summed over the CTAs' shares in a fixed order.
 static int bwd_bags_phase2_impl(const dsmil_params_t* p, int nb, const float* A, const float* dA, const float* tpart,
                                 int P, const float* Q, float* dL, float* dqm, const BwdBagsWs& w, cudaStream_t st) {
   const int C = p->C;
-  k_bwd_dL_b<<<dim3(w.G, nb), 256, 0, st>>>(w.table, C, A, dA, tpart, P, Q, dL, w.dpart);
+  const int* G_dev = w.plan ? &w.plan->G : nullptr;
+  k_bwd_dL_b<<<dim3(w.G, nb), 256, 0, st>>>(w.table, C, A, dA, tpart, P, Q, dL, w.dpart, G_dev);
   DSMIL_LAUNCH_OK("k_bwd_dL_b");
-  k_sum_segments<<<dim3(ceil_div(C * kQ, 256), nb), 256, 0, st>>>(w.dpart, w.G, C * kQ, dqm);
+  k_sum_segments<<<dim3(ceil_div(C * kQ, 256), nb), 256, 0, st>>>(w.dpart, w.G, C * kQ, dqm, G_dev);
   DSMIL_LAUNCH_OK("k_sum_segments");
   return 0;
 }
@@ -1062,33 +1103,36 @@ static int bwd_bags_phase3_impl(const dsmil_params_t* p, int nb, int64_t total, 
                                 const long long* row_offsets, const dsmil_grads_t* g, const BwdBagsWs& w,
                                 const float** dz1, cudaStream_t st) {
   const int D = p->D;
+  const BagsPlan* pl = w.plan;
   int rc;
   k_bwd_dq_b<<<dim3(w.G, nb), 256, 0, st>>>(w.table, p->C, dL, Q, qmax, dqm, crit, row_offsets, p->nonlinear, w.dz2);
   DSMIL_LAUNCH_OK("k_bwd_dq_b");
   // back through the Q-MLP: layer 2 over the packed rows, layer 1 against the bags' X
   *dz1 = w.dz2;
   if (p->nonlinear) {
-    if (g->gW2 && (rc = launch_gemm_tn(w.dz2, kQ, H1, kQ, total, w.tnpart, g->gW2, st))) return rc;
-    if (g->gb2 && (rc = launch_colsum(w.dz2, kQ, total, w.cspart, g->gb2, st))) return rc;
-    if ((rc = launch_linear<ACT_MASK_POS, true>(w.dz2, total, kQ, p->W2, nullptr, kQ, w.dz1, H1, 0, st))) return rc;
+    if (g->gW2 && (rc = launch_gemm_tn(w.dz2, kQ, H1, kQ, total, w.tnpart, g->gW2, st, pl ? &pl->tn2 : nullptr)))
+      return rc;
+    if (g->gb2 && (rc = launch_colsum(w.dz2, kQ, total, w.cspart, g->gb2, st, pl ? &pl->cs : nullptr))) return rc;
+    if ((rc = launch_linear<ACT_MASK_POS, true>(w.dz2, total, kQ, p->W2, nullptr, kQ, w.dz1, H1, 0, st,
+                                                pl ? &pl->total : nullptr)))
+      return rc;
     *dz1 = w.dz1;
   }
-  if (g->gW1 && (rc = launch_gemm_tn_rag(*dz1, kQ, D, w.ch1, w.nc1, false, w.tnpart, g->gW1, st))) return rc;
-  if (g->gb1 && (rc = launch_colsum(*dz1, kQ, total, w.cspart, g->gb1, st))) return rc;
+  if (g->gW1 &&
+      (rc = launch_gemm_tn_rag(*dz1, kQ, D, w.ch1, w.nc1, false, w.tnpart, g->gW1, st, pl ? &pl->nc1 : nullptr)))
+    return rc;
+  if (g->gb1 && (rc = launch_colsum(*dz1, kQ, total, w.cspart, g->gb1, st, pl ? &pl->cs : nullptr))) return rc;
   return 0;
 }
 
-static int backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
-                              int64_t total, bool aligned, const float* Q, const float* H1, const float* A,
-                              const float* B, const int64_t* crit, const float* d_classes, const float* d_pred,
-                              const float* d_A, const float* d_B, const dsmil_grads_t* g, void* ws, size_t ws_bytes,
-                              cudaStream_t st) {
+// The single-device batched backward over a carved w: the three phases in a row (+ gX).  One device: k_bwd_dL_b sums
+// phase 1's partials of t itself, and the critical rows are local.
+static int backward_bags_run(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb, int64_t total,
+                             const float* Q, const float* H1, const float* A, const float* B, const int64_t* crit,
+                             const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                             const dsmil_grads_t* g, const BwdBagsWs& w, cudaStream_t st) {
   const int C = p->C, D = p->D;
-  bool ok;
-  BwdBagsWs w = carve_bwd_bags(p, Ns, nb, aligned, false, ws, ws_bytes, &ok);
-  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
-  if (rc) return rc;
-  // one device: k_bwd_dL_b sums phase 1's partials of t itself, and the critical rows are local
+  int rc;
   const float* dz1;
   if ((rc = bwd_bags_phase1_impl(p, Xs, Ns, nb, total, A, B, d_classes, d_pred, d_A, d_B, g, w.dA, w, st)) ||
       (rc = bwd_bags_phase2_impl(p, nb, A, w.dA, w.tpart, w.G, Q, w.dL, w.dqm, w, st)) ||
@@ -1100,6 +1144,18 @@ static int backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, c
     DSMIL_LAUNCH_OK("k_bwd_dx_extra_b");
   }
   return 0;
+}
+
+static int backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
+                              int64_t total, bool aligned, const float* Q, const float* H1, const float* A,
+                              const float* B, const int64_t* crit, const float* d_classes, const float* d_pred,
+                              const float* d_A, const float* d_B, const dsmil_grads_t* g, void* ws, size_t ws_bytes,
+                              cudaStream_t st) {
+  bool ok;
+  BwdBagsWs w = carve_bwd_bags(p, Ns, nb, aligned, false, ws, ws_bytes, &ok);
+  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+  if (rc) return rc;
+  return backward_bags_run(p, Xs, Ns, nb, total, Q, H1, A, B, crit, d_classes, d_pred, d_A, d_B, g, w, st);
 }
 
 // ---- sharded batch ABI ---------------------------------------------------------------------------
@@ -1138,7 +1194,7 @@ static int shard_bags_phase2_impl(const dsmil_params_t* p, const float* const* X
   if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
   k_merge_cand<<<dim3(p->C, nb), kQ, 0, st>>>(cands_all, G, nb, p->C, qmax, crit_idx);
   DSMIL_LAUNCH_OK("k_merge_cand");
-  sm90::AttendArgs aa{w.table, nb, p->D, p->C, Q, q_blocked, w.keys, A, w.recs, qmax};
+  sm90::AttendArgs aa{w.table, nb, p->D, p->C, Q, q_blocked, w.keys, A, w.recs, qmax, nullptr};
   if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
   sm90::FinalizeArgs fa{w.table, p->D, p->C, w.recs, w.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
                          w.pred_part, w.counters, recs_out, 0, 0};
@@ -1326,7 +1382,7 @@ int dsmil_shard_backward_bags_phase1(const dsmil_params_t* p, const float* const
     return rc;
   // t_local[b] = the per-CTA partials summed in a fixed order: with one rank, phase 2 then sees the t_b that
   // dsmil_backward_bags's k_bwd_dL_b forms itself
-  k_sum_segments<<<dim3(ceil_div(p->C, 256), nb), 256, 0, st>>>(w.tpart, w.G, p->C, t_local);
+  k_sum_segments<<<dim3(ceil_div(p->C, 256), nb), 256, 0, st>>>(w.tpart, w.G, p->C, t_local, nullptr);
   DSMIL_LAUNCH_OK("k_sum_segments");
   return 0;
 }
@@ -1368,6 +1424,107 @@ int dsmil_shard_backward_bags_phase3(const dsmil_params_t* p, const float* const
   const float* dz1;
   return bwd_bags_phase3_impl(p, nb, total, Q, H1, dL_local, dqm_global, q_max, crit_idx, w.row_offsets, &g, w, &dz1,
                               st);
+}
+
+
+// ---- capture-safe batched training: the bag list in device memory, every launch sized for a capacity -------------
+// What both dev calls check: the batched tensor-core shapes, the bag list, 1 <= nb <= 65535 and a row capacity whose
+// 128-row tiles the kernels can number (an int).
+static int check_bags_dev(const dsmil_params_t* p, bool need_scores, const float* const* Xs, const int64_t* Ns, int nb,
+                          int64_t max_rows, const int32_t* status) {
+  int rc = check_params(p, need_scores);
+  if (rc) return rc;
+  DSMIL_REQUIRE(dsmil_shard_bags_supported(p),
+                "shape not supported by the batched tensor-core path (D=%d, C=%d, nonlinear=%d, passing_v=%d)", p->D,
+                p->C, p->nonlinear, p->passing_v);
+  DSMIL_REQUIRE(Xs && Ns && status, "NULL bag list or status");
+  DSMIL_REQUIRE(nb >= 1 && nb <= 65535, "nb=%d outside [1, 65535]", nb);
+  DSMIL_REQUIRE(max_rows >= 1 && max_rows < 0xffffffffll &&
+                static_cast<int64_t>(nb) * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) <= INT_MAX,
+                "max_rows=%lld out of range for nb=%d", (long long)max_rows, nb);
+  return 0;
+}
+
+// The forward's carve for nb bags of max_rows rows (Q and H1 are the caller's), then the planner's BagsPlan and the
+// zero row of a refused batch.
+static BagsWs carve_bags_dev(const dsmil_params_t* p, int nb, int64_t max_rows, void* ws, size_t cap, bool* ok,
+                             BagsPlan** plan, float** zero_row) {
+  const std::vector<int64_t> Ns(nb, max_rows);
+  BagsWs w = carve_bags(p, Ns.data(), nb, false, false, ws, cap, ok);
+  Carver c(ws, cap);
+  c.off = w.bytes;
+  *plan = c.take<BagsPlan>(1);
+  *zero_row = c.take<float>(p->D);
+  w.bytes = c.off;
+  *ok = c.ok();
+  return w;
+}
+
+size_t dsmil_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
+  bool ok;
+  BagsPlan* plan;
+  float* zero_row;
+  const size_t dev = carve_bags_dev(p, nb, max_rows, nullptr, 0, &ok, &plan, &zero_row).bytes;
+  // never below the eager call's size for the same capacity: one buffer serves both forms
+  const std::vector<int64_t> Ns(nb, max_rows);
+  return std::max(dev, dsmil_forward_bags_train_workspace_bytes(p, Ns.data(), nb));
+}
+
+int dsmil_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                 int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
+                                 int64_t* crit_idx, float* save_Q, float* save_H1, int32_t* status, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+  int rc = check_bags_dev(p, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && save_H1, "NULL output pointer");
+  const size_t need = dsmil_forward_bags_train_dev_workspace_bytes(p, nb, max_rows);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  bool ok;
+  BagsPlan* plan;
+  float* zero_row;
+  BagsWs w = carve_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok, &plan, &zero_row);
+  k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, zero_row, w.table, nullptr, nullptr, plan,
+                                status);
+  DSMIL_LAUNCH_OK("k_plan_bags");
+  // bags_phase1_impl's launches, on the planner's table and with the weight images rebuilt on every call (a replayed
+  // graph sees the weights of the last optimizer step)
+  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
+  if ((rc = sm90::launch_prep_wimg(p, w.wimg, st))) return rc;
+  if ((rc = sm90::launch_qmlp(p, w.table, nb, nb * tiles_for_bag(max_rows), classes, w.keys, save_Q, save_H1, w.wimg,
+                              num_sms(), st, false, &plan->tiles)))
+    return rc;
+  return bags_attend_finalize(p, w, nb, save_Q, false, pred, A, B, crit_idx, nb * recs_for_bag(max_rows), &plan->recs,
+                              st);
+}
+
+size_t dsmil_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
+  bool ok;
+  return carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
+}
+
+int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev, int32_t nb,
+                            int64_t max_rows, const float* Q, const float* H1, const float* A, const float* B,
+                            const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
+                            const float* d_B, const dsmil_grads_t* grads, int32_t* status, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  int rc = check_bags_dev(p, false, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(Q && H1 && A && B && crit_idx && grads, "NULL pointer");
+  DSMIL_REQUIRE(!d_A && !d_B && !grads->gX,
+                "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
+  const size_t need = dsmil_backward_bags_dev_workspace_bytes(p, nb, max_rows);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  bool ok;
+  BwdBagsWs w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
+  k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, w.zero_row, w.table, w.chi, w.ch1, w.plan,
+                                status);
+  DSMIL_LAUNCH_OK("k_plan_bags");
+  return backward_bags_run(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, A, B, crit_idx,
+                           d_classes, d_pred, nullptr, nullptr, grads, w, st);
 }
 
 }  // extern "C"

@@ -9,16 +9,12 @@
 #include "common.cuh"
 #include "gemm_generic.cuh"
 #include "fwd_sm90.cuh"
+#include "bag_plan.cuh"
 
 namespace dsmil {
 
-// One row range of the ragged TN GEMMs: rows [prow, prow + rows) of the packed left operand against the bag rows
-// starting at R.  A chunk never straddles two bags.
-struct TnChunk {
-  const float* R;
-  long long prow;
-  long long rows;
-};
+// The dev calls launch the per-bag kernels on a capacity grid: G_dev points at the live CTAs per bag (the planner's),
+// and the CTAs past it return at once.  With G_dev == NULL, G is gridDim.x.
 
 // Bag classifier for all bags (dsmil.py:59-61):  dB[b] = Wf^T dp[b] (+ dB_up[b]);  gWf[k] = sum_b dp[b,k] B[b];
 // gbf = sum_b dp[b].  The sums over b run in bag order.
@@ -56,9 +52,11 @@ k_bwd_bag_b(const float* __restrict__ Wf, const float* __restrict__ B, const flo
 __global__ void __launch_bounds__(256)
 k_bwd_rowdot_b(const sm90::BagDev* __restrict__ bags, int D, const float* __restrict__ dB, int C,
                const float* __restrict__ A, const float* __restrict__ add, float* __restrict__ dA,
-               float* __restrict__ tpart) {
+               float* __restrict__ tpart, const int* __restrict__ G_dev) {
   extern __shared__ __align__(16) float sW[];  // [C*D]: dB of this CTA's bag
   __shared__ float red[8][kMaxC];
+  const int G = G_dev ? *G_dev : static_cast<int>(gridDim.x);
+  if (static_cast<int>(blockIdx.x) >= G) return;
   const int b = blockIdx.y;
   const sm90::BagDev bg = bags[b];
   const float* W = dB + static_cast<size_t>(b) * C * D;
@@ -68,7 +66,7 @@ k_bwd_rowdot_b(const sm90::BagDev* __restrict__ bags, int D, const float* __rest
   float tacc[kMaxC];
 #pragma unroll
   for (int k = 0; k < kMaxC; ++k) tacc[k] = 0.f;
-  const int64_t stride = static_cast<int64_t>(gridDim.x) * 8;
+  const int64_t stride = static_cast<int64_t>(G) * 8;
   for (int64_t n = static_cast<int64_t>(blockIdx.x) * 8 + warp; n < bg.N; n += stride) {
     float acc[kMaxC];
 #pragma unroll
@@ -96,7 +94,7 @@ k_bwd_rowdot_b(const sm90::BagDev* __restrict__ bags, int D, const float* __rest
   if (threadIdx.x < C) {
     float s = 0.f;
     for (int w = 0; w < 8; ++w) s += red[w][threadIdx.x];
-    tpart[(static_cast<size_t>(b) * gridDim.x + blockIdx.x) * C + threadIdx.x] = s;
+    tpart[(static_cast<size_t>(b) * G + blockIdx.x) * C + threadIdx.x] = s;
   }
 }
 
@@ -104,14 +102,17 @@ k_bwd_rowdot_b(const sm90::BagDev* __restrict__ bags, int D, const float* __rest
 // (P partials per bag: the first pass's per-CTA shares, or P = 1 for a t that is already summed, e.g. all-reduced
 // over the ranks of a row-sharded batch):
 // dL[n,k] = A[n,k] (dA[n,k] - t_b[k]) / sqrt(128) for rows n = 2x + h, step 2*gridDim.x, of bag b, and the CTA's share
-// of dq_max_b = dL_b^T Q_b, [C,128], in dpart[b][x].
+// of dq_max_b = dL_b^T Q_b, [C,128], in dpart[b][x].  G_dev != NULL (one device, first-pass partials): G and P are
+// both *G_dev.
 __global__ void __launch_bounds__(256)
 k_bwd_dL_b(const sm90::BagDev* __restrict__ bags, int C, const float* __restrict__ A, const float* __restrict__ dA,
            const float* __restrict__ tpart, int P, const float* __restrict__ Q, float* __restrict__ dL,
-           float* __restrict__ dpart) {
+           float* __restrict__ dpart, const int* __restrict__ G_dev) {
   __shared__ float t[kMaxC];
   __shared__ float red[kMaxC][kQ];
-  const int b = blockIdx.y, G = gridDim.x;
+  const int b = blockIdx.y, G = G_dev ? *G_dev : static_cast<int>(gridDim.x);
+  if (static_cast<int>(blockIdx.x) >= G) return;
+  if (G_dev) P = G;
   if (threadIdx.x < C) {
     float s = 0.f;
     for (int x = 0; x < P; ++x) s += tpart[(static_cast<size_t>(b) * P + x) * C + threadIdx.x];
@@ -145,11 +146,12 @@ k_bwd_dL_b(const sm90::BagDev* __restrict__ bags, int C, const float* __restrict
       if (k < C) dpart[((static_cast<size_t>(b) * G + blockIdx.x) * C + k) * kQ + j] = acc[k] + red[k][j];
 }
 
-// dqm[b][i] = sum_{x < P} dpart[b][x][i], i < L (in x order)
+// dqm[b][i] = sum_{x < P} dpart[b][x][i], i < L (in x order); P = *P_dev when P_dev != NULL
 __global__ void __launch_bounds__(256)
-k_sum_segments(const float* __restrict__ part, int P, int L, float* __restrict__ out) {
+k_sum_segments(const float* __restrict__ part, int P, int L, float* __restrict__ out, const int* __restrict__ P_dev) {
   const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= L) return;
+  if (P_dev) P = *P_dev;
   float s = 0.f;
   for (int x = 0; x < P; ++x) s += part[(static_cast<size_t>(b) * P + x) * L + i];
   out[static_cast<size_t>(b) * L + i] = s;
@@ -218,58 +220,42 @@ k_bwd_dx_extra_b(const sm90::BagDev* __restrict__ bags, const float* __restrict_
   }
 }
 
-// Ragged out = P^T X: chunk z of the table is one row range of one bag; its partial goes to part[z].
+// Ragged out = P^T X: chunk z of the table is one row range of one bag; its partial goes to part[z].  nz_dev != NULL:
+// the live chunk count of a capacity grid.
 __global__ void __launch_bounds__(256, 2)
 k_gemm_tn_rag(const float* __restrict__ P, int M1, int M2, const TnChunk* __restrict__ chunks,
-              float* __restrict__ part) {
+              float* __restrict__ part, const int* __restrict__ nz_dev) {
+  if (nz_dev && static_cast<int>(blockIdx.z) >= *nz_dev) return;
   const TnChunk c = chunks[blockIdx.z];
   gemm_tn_tile(P + c.prow * M1, M1, c.R, M2, c.rows, part + static_cast<int64_t>(blockIdx.z) * M1 * M2);
 }
 template <int M1>
 __global__ void __launch_bounds__(256)
-k_gemv_tn_rag(const float* __restrict__ P, int M2, const TnChunk* __restrict__ chunks, float* __restrict__ part) {
+k_gemv_tn_rag(const float* __restrict__ P, int M2, const TnChunk* __restrict__ chunks, float* __restrict__ part,
+              const int* __restrict__ nz_dev) {
+  if (nz_dev && static_cast<int>(blockIdx.x) >= *nz_dev) return;
   const TnChunk c = chunks[blockIdx.x];
   gemv_tn_rows<M1>(P + c.prow * M1, c.R, M2, c.rows, part + static_cast<int64_t>(blockIdx.x) * M1 * M2);
 }
 
-// Host plan of a ragged TN GEMM over the bags: rows per chunk, from the shapes alone.  The streaming form (M1 <= 4,
-// float4 rows) takes chunks of >= 64 rows, at most about kSplits of them; the 128 x 128 tile form keeps the tiles x
-// chunks CTAs near kSplits, as launch_gemm_tn does.
-inline int64_t rag_rows_per_chunk(int M1, int M2, int64_t total, bool gemv) {
-  if (gemv) return std::max<int64_t>(64, (total + kSplits - 1) / kSplits);
-  const int tiles = ceil_div(M1, TBM) * ceil_div(M2, TBM);
-  const int64_t s = std::max(1, kSplits / tiles);
-  return std::max<int64_t>(128, ((total + s - 1) / s + TBK - 1) / TBK * TBK);
-}
-// Chunks of `rps` rows over the bags (the last chunk of a bag may be shorter); returns how many.  Xs == NULL: count
-// only.
-inline int rag_chunks(const float* const* Xs, const int64_t* Ns, int nb, int M2, int64_t rps, TnChunk* out) {
-  int z = 0;
-  long long row = 0;
-  for (int b = 0; b < nb; ++b) {
-    for (int64_t r0 = 0; r0 < Ns[b]; r0 += rps, ++z)
-      if (Xs) out[z] = TnChunk{Xs[b] + r0 * M2, row + r0, std::min<int64_t>(rps, Ns[b] - r0)};
-    row += Ns[b];
-  }
-  return z;
-}
-// out[M1,M2] = P^T X over nz chunks (device table `chunks`); `part` holds nz * M1 * M2 floats.
+// out[M1,M2] = P^T X over nz chunks (device table `chunks`); `part` holds nz * M1 * M2 floats.  nz_dev != NULL: nz is
+// the chunk capacity and *nz_dev the live count.
 inline int launch_gemm_tn_rag(const float* P, int M1, int M2, const TnChunk* chunks, int nz, bool gemv, float* part,
-                              float* out, cudaStream_t st) {
+                              float* out, cudaStream_t st, const int* nz_dev = nullptr) {
   if (gemv) {
     switch (M1) {
-      case 1: k_gemv_tn_rag<1><<<nz, 256, 0, st>>>(P, M2, chunks, part); break;
-      case 2: k_gemv_tn_rag<2><<<nz, 256, 0, st>>>(P, M2, chunks, part); break;
-      case 3: k_gemv_tn_rag<3><<<nz, 256, 0, st>>>(P, M2, chunks, part); break;
-      default: k_gemv_tn_rag<4><<<nz, 256, 0, st>>>(P, M2, chunks, part); break;
+      case 1: k_gemv_tn_rag<1><<<nz, 256, 0, st>>>(P, M2, chunks, part, nz_dev); break;
+      case 2: k_gemv_tn_rag<2><<<nz, 256, 0, st>>>(P, M2, chunks, part, nz_dev); break;
+      case 3: k_gemv_tn_rag<3><<<nz, 256, 0, st>>>(P, M2, chunks, part, nz_dev); break;
+      default: k_gemv_tn_rag<4><<<nz, 256, 0, st>>>(P, M2, chunks, part, nz_dev); break;
     }
     DSMIL_LAUNCH_OK("k_gemv_tn_rag");
   } else {
     dim3 grid(ceil_div(M2, TBM), ceil_div(M1, TBM), nz);
-    k_gemm_tn_rag<<<grid, 256, 0, st>>>(P, M1, M2, chunks, part);
+    k_gemm_tn_rag<<<grid, 256, 0, st>>>(P, M1, M2, chunks, part, nz_dev);
     DSMIL_LAUNCH_OK("k_gemm_tn_rag");
   }
-  return launch_sum_partials(part, nz, static_cast<int64_t>(M1) * M2, out, st);
+  return launch_sum_partials(part, nz, static_cast<int64_t>(M1) * M2, out, st, nz_dev);
 }
 
 }  // namespace dsmil

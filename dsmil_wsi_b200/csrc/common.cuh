@@ -104,6 +104,6 @@ __device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v)
   return v;
 }
 
-inline int ceil_div(int64_t a, int64_t b) { return static_cast<int>((a + b - 1) / b); }
+__host__ __device__ inline int ceil_div(int64_t a, int64_t b) { return static_cast<int>((a + b - 1) / b); }
 
 }  // namespace dsmil

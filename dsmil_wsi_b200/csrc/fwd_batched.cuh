@@ -25,6 +25,7 @@ struct AttendArgs {
   float* A;                 // packed [sumN,C]: receives the raw logits here
   float* recs;              // [total records][rec_floats(C,D)]
   const float* qmax_ext;    // sharded: [nbags][C][128] merged critical queries (NULL: gather from Q via keys)
+  const int* nrec_dev;      // dev calls: the live record count of a capacity grid (NULL: one CTA per record)
 };
 
 // CT = classes rounded up to 1,2,4; NJ = float4 column groups per thread (D <= 512*NJ)
@@ -41,6 +42,7 @@ k_attend_b(const AttendArgs a) {
   __shared__ float s_red[8][CT];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int C = a.C, D = a.D;
+  if (a.nrec_dev != nullptr && static_cast<int>(blockIdx.x) >= *a.nrec_dev) return;
   // which bag does this CTA belong to?
   const int rec = blockIdx.x;
   int bag = 0;

@@ -165,6 +165,7 @@ struct QmlpArgs {
   float* H1;              // packed [sumN,128] or NULL
   bool q_blocked;         // Q in tile blocks of the PRE-activation z2 = acc + b2 (inference path): the tanh moves to
                           // the readers of Q (k_attend_b, k_gather_cand_b).  false: row-major tanh(z2)
+  const int* ntiles_dev;  // dev calls: the live tile count (ntiles is then the capacity); NULL: ntiles
 };
 
 // Walks the bag table as a role's tile index increases monotonically.
@@ -194,8 +195,9 @@ constexpr int kOffWi = kOffWRing + kWStages * kChunkBytes;  // CT*D floats
 constexpr int kSmemFixed = kOffWi;
 
 // CT: classes rounded up to 1/2/4/8.  DT: compile-time feature size (512 = every shipped configuration:
-// the chunk loops unroll and the load offsets become immediates) or 0 = run-time D.
-template <int CT, int DT>
+// the chunk loops unroll and the load offsets become immediates) or 0 = run-time D.  DEV: the dev calls' form, whose
+// live tile count is read on the device (a.ntiles_dev); the eager form's code does not carry that test.
+template <int CT, int DT, bool DEV = false>
 __global__ void __launch_bounds__(kThreads, 1)
 k_qmlp_sm90(const QmlpArgs a) {
   extern __shared__ uint8_t smem_raw[];
@@ -208,6 +210,9 @@ k_qmlp_sm90(const QmlpArgs a) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int D = DT ? DT : a.D, C = a.C;
   const int nchunks = D / kChunkK;
+  // a tile is live when below the launch's count and, in a dev call, the planner's; the device count is read at each
+  // test, not held: the C = 4 run-time-D instantiation has no register to spare for it
+  auto live = [&](int t) { return t < a.ntiles && (!DEV || t < *a.ntiles_dev); };
   enum { W_FULL = 0, W_EMPTY = kWStages };
   auto bar = [&](int i) { return smem_u32(&bars[i]); };
 
@@ -238,7 +243,7 @@ k_qmlp_sm90(const QmlpArgs a) {
         bulk_g2s(smem_u32(smem + kOffWRing + stage * kChunkBytes), src, kChunkBytes, bar(W_FULL + stage));
         if (++stage == kWStages) { stage = 0; phase ^= 1; }
       };
-      for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
+      for (int tile = blockIdx.x; live(tile); tile += gridDim.x) {
         for (int kc = 0; kc < nchunks; ++kc) push(a.w1img + static_cast<size_t>(kc) * kChunkBytes);
         push(a.w2img);
         push(a.w2img + kChunkBytes);
@@ -348,9 +353,9 @@ k_qmlp_sm90(const QmlpArgs a) {
 
   int tile = blockIdx.x;
   float4 x[8];
-  if (tile < a.ntiles) { open_tile(tile); load_chunk(0, x); }
+  if (live(tile)) { open_tile(tile); load_chunk(0, x); }
   uint32_t ha[16], la[16], hb[16], lb[16];
-  while (tile < a.ntiles) {
+  while (live(tile)) {
     const int my_bag = cur_bag.bag;   // this tile's bag (the load state moves on below)
     const uint32_t t_N = ld_N, t_row = ld_row;
     const long long t_rowoff = ld_rowoff;
@@ -370,7 +375,7 @@ k_qmlp_sm90(const QmlpArgs a) {
       const uint32_t s0 = mma_chunk(ha, la, kc);
       convert(x, kc + 1, hb, lb);
       if (kc + 2 < nchunks) load_chunk(kc + 2, x);
-      else if (next_tile < a.ntiles) { open_tile(next_tile); load_chunk(0, x); }
+      else if (live(next_tile)) { open_tile(next_tile); load_chunk(0, x); }
       wg_wait0();
       fence_acc(acc);
       w_release(s0);
@@ -509,13 +514,19 @@ inline int launch_prep_wimg(const dsmil_params_t* p, uint8_t* wimg, cudaStream_t
 }
 
 // scores + arg-max keys + Q (+H1) for the ntiles 128-row tiles of the nb bags of the table.
-// wimg must already hold the images (launch_prep_wimg).
+// wimg must already hold the images (launch_prep_wimg).  ntiles_dev != NULL: ntiles is the capacity, *ntiles_dev the
+// live count.
 inline int launch_qmlp(const dsmil_params_t* p, const BagDev* bags_dev, int nb, int ntiles, float* classes,
                        unsigned long long* keys, float* Q, float* H1, const uint8_t* wimg, int num_sms, cudaStream_t st,
-                       bool q_blocked) {
+                       bool q_blocked, const int* ntiles_dev = nullptr) {
   const int D = p->D, C = p->C;
+  if (ntiles_dev != nullptr && C > 4) {
+    set_error("launch_qmlp: a device tile count needs C <= 4");
+    return DSMIL_ERR_ARG;
+  }
   const uint8_t* w2img = wimg + static_cast<size_t>(D / kChunkK) * kChunkBytes;
-  QmlpArgs a{bags_dev, nb, ntiles, D, C, p->Wi, p->bi, p->b1, p->b2, wimg, w2img, classes, keys, Q, H1, q_blocked};
+  QmlpArgs a{bags_dev, nb, ntiles, D, C, p->Wi, p->bi, p->b1, p->b2, wimg, w2img, classes, keys, Q, H1, q_blocked,
+             ntiles_dev};
   const size_t smem = qmlp_smem_bytes(C, D);
   const int grid = ntiles < num_sms ? ntiles : num_sms;
   auto go = [&](auto kern) -> int {
@@ -528,6 +539,16 @@ inline int launch_qmlp(const dsmil_params_t* p, const BagDev* bags_dev, int nb, 
     DSMIL_LAUNCH_OK("k_qmlp_sm90");
     return 0;
   };
+  if (ntiles_dev != nullptr) {   // the dev calls' shapes: C <= 4
+    if (D == 512) {
+      if (C == 1) return go(k_qmlp_sm90<1, 512, true>);
+      if (C == 2) return go(k_qmlp_sm90<2, 512, true>);
+      return go(k_qmlp_sm90<4, 512, true>);
+    }
+    if (C == 1) return go(k_qmlp_sm90<1, 0, true>);
+    if (C == 2) return go(k_qmlp_sm90<2, 0, true>);
+    return go(k_qmlp_sm90<4, 0, true>);
+  }
   if (D == 512) {
     if (C == 1) return go(k_qmlp_sm90<1, 512>);
     if (C == 2) return go(k_qmlp_sm90<2, 512>);

@@ -18,12 +18,16 @@ template <int ACT, bool WT>
 __global__ void __launch_bounds__(256)
 k_linear(const float* __restrict__ X, int64_t N, int K, const float* __restrict__ W,
          const float* __restrict__ b, int M, float* __restrict__ Y, const float* __restrict__ aux,
-         int accumulate) {
+         int accumulate, const long long* __restrict__ N_dev) {
   __shared__ __align__(16) float As[LBK][LBM + 4];
   __shared__ __align__(16) float Bs[LBK][LBN + 4];
   const int tid = threadIdx.x;
   const int ty = tid >> 4, tx = tid & 15;
   const int64_t n0 = static_cast<int64_t>(blockIdx.x) * LBM;
+  if (N_dev) {               // the live row count of a capacity grid
+    N = *N_dev;
+    if (n0 >= N) return;
+  }
   const int m0 = blockIdx.y * LBN;
   float acc[4][8];
 #pragma unroll
@@ -101,12 +105,13 @@ k_linear(const float* __restrict__ X, int64_t N, int K, const float* __restrict_
   }
 }
 
+// N_dev != NULL: N is the row capacity (the grid), *N_dev the live row count, read on the device.
 template <int ACT, bool WT>
 inline int launch_linear(const float* X, int64_t N, int K, const float* W, const float* b, int M, float* Y,
-                         const float* aux, int accumulate, cudaStream_t st) {
+                         const float* aux, int accumulate, cudaStream_t st, const long long* N_dev = nullptr) {
   if (N <= 0) return 0;
   dim3 grid(ceil_div(N, LBM), ceil_div(M, LBN));
-  k_linear<ACT, WT><<<grid, 256, 0, st>>>(X, N, K, W, b, M, Y, aux, accumulate);
+  k_linear<ACT, WT><<<grid, 256, 0, st>>>(X, N, K, W, b, M, Y, aux, accumulate, N_dev);
   DSMIL_LAUNCH_OK("k_linear");
   return 0;
 }
@@ -198,9 +203,22 @@ __device__ __forceinline__ void gemm_tn_tile(const float* __restrict__ P, int M1
     }
   }
 }
+// A row split decided on the device (capacity grids, bag_plan.cuh): the live rows N, rows per split and splits S.
+struct RowSplit {
+  long long N;
+  long long rps;
+  int S;
+  int pad_;
+};
+
 __global__ void __launch_bounds__(256, 2)
 k_gemm_tn(const float* __restrict__ P, int M1, const float* __restrict__ R, int M2, int64_t N,
-          int64_t rows_per_split, float* __restrict__ part) {
+          int64_t rows_per_split, float* __restrict__ part, const RowSplit* __restrict__ dyn) {
+  if (dyn) {
+    if (static_cast<int>(blockIdx.z) >= dyn->S) return;
+    N = dyn->N;
+    rows_per_split = dyn->rps;
+  }
   const int64_t nb = static_cast<int64_t>(blockIdx.z) * rows_per_split;
   gemm_tn_tile(P + nb * M1, M1, R + nb * M2, M2, min(N, nb + rows_per_split) - nb,
                part + static_cast<int64_t>(blockIdx.z) * M1 * M2);
@@ -261,7 +279,13 @@ k_gemv_tn(const float* __restrict__ P, const float* __restrict__ R, int M2, int6
 
 // part[z][M] = sum over the z-th row chunk of P[n, m]
 __global__ void __launch_bounds__(256)
-k_colsum(const float* __restrict__ P, int M, int64_t N, int64_t rows_per_split, float* __restrict__ part) {
+k_colsum(const float* __restrict__ P, int M, int64_t N, int64_t rows_per_split, float* __restrict__ part,
+         const RowSplit* __restrict__ dyn) {
+  if (dyn) {
+    if (static_cast<int>(blockIdx.x) >= dyn->S) return;
+    N = dyn->N;
+    rows_per_split = dyn->rps;
+  }
   const int64_t nb = static_cast<int64_t>(blockIdx.x) * rows_per_split;
   const int64_t ne = min(N, nb + rows_per_split);
   for (int m = threadIdx.x; m < M; m += blockDim.x) {
@@ -275,8 +299,9 @@ k_colsum(const float* __restrict__ P, int M, int64_t N, int64_t rows_per_split, 
 // the eight warp sums are then added in warp order).  32 outputs per CTA, so a short vector (a bias gradient: 128
 // values from 235 partials) is no longer one CTA walking 235 dependent steps.
 __global__ void __launch_bounds__(256)
-k_sum_partials(const float* __restrict__ part, int S, int64_t L, float* __restrict__ out) {
+k_sum_partials(const float* __restrict__ part, int S, int64_t L, float* __restrict__ out, const int* __restrict__ S_dev) {
   __shared__ float s_w[8][32];
+  if (S_dev) S = *S_dev;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t i = static_cast<int64_t>(blockIdx.x) * 32 + lane;
   float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -296,14 +321,15 @@ k_sum_partials(const float* __restrict__ part, int S, int64_t L, float* __restri
     out[i] = ((s_w[0][lane] + s_w[1][lane]) + (s_w[2][lane] + s_w[3][lane])) +
              ((s_w[4][lane] + s_w[5][lane]) + (s_w[6][lane] + s_w[7][lane]));
 }
-inline int launch_sum_partials(const float* part, int S, int64_t L, float* out, cudaStream_t st) {
-  k_sum_partials<<<static_cast<unsigned>(ceil_div(L, 32)), 256, 0, st>>>(part, S, L, out);
+inline int launch_sum_partials(const float* part, int S, int64_t L, float* out, cudaStream_t st,
+                               const int* S_dev = nullptr) {
+  k_sum_partials<<<static_cast<unsigned>(ceil_div(L, 32)), 256, 0, st>>>(part, S, L, out, S_dev);
   DSMIL_LAUNCH_OK("k_sum_partials");
   return 0;
 }
 
-inline bool tn_use_gemv(int M1, int M2) { return M1 <= kGemvMaxM1 && (M2 & 3) == 0 && (M2 >> 2) <= 256; }
-inline int tn_splits(int M1, int M2, int64_t N) {
+__host__ __device__ inline bool tn_use_gemv(int M1, int M2) { return M1 <= kGemvMaxM1 && (M2 & 3) == 0 && (M2 >> 2) <= 256; }
+__host__ __device__ inline int tn_splits(int M1, int M2, int64_t N) {
   int s, maxs;
   if (tn_use_gemv(M1, M2)) {
     s = kSplits;
@@ -320,9 +346,20 @@ inline int tn_splits(int M1, int M2, int64_t N) {
 inline size_t tn_partial_floats(int M1, int M2, int64_t N) {
   return static_cast<size_t>(tn_splits(M1, M2, N)) * M1 * M2;
 }
-// out[M1,M2] = P^T R, via partials in `part` (>= tn_partial_floats floats).
+// out[M1,M2] = P^T R, via partials in `part` (>= tn_partial_floats floats).  dyn != NULL: N is the row capacity and
+// the split is the device's (the tile form only: M1 > kGemvMaxM1).
 inline int launch_gemm_tn(const float* P, int M1, const float* R, int M2, int64_t N, float* part, float* out,
-                          cudaStream_t st) {
+                          cudaStream_t st, const RowSplit* dyn = nullptr) {
+  if (dyn) {
+    if (tn_use_gemv(M1, M2)) {
+      set_error("launch_gemm_tn: a device-side split needs the tile form");
+      return DSMIL_ERR_ARG;
+    }
+    const int S = tn_splits(M1, M2, N);
+    k_gemm_tn<<<dim3(ceil_div(M2, TBM), ceil_div(M1, TBM), S), 256, 0, st>>>(P, M1, R, M2, N, 0, part, dyn);
+    DSMIL_LAUNCH_OK("k_gemm_tn");
+    return launch_sum_partials(part, S, static_cast<int64_t>(M1) * M2, out, st, &dyn->S);
+  }
   if (N <= 0) {
     DSMIL_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float) * M1 * M2, st));
     return 0;
@@ -348,22 +385,30 @@ inline int launch_gemm_tn(const float* P, int M1, const float* R, int M2, int64_
   int64_t rps = (N + Sg - 1) / Sg;
   rps = (rps + TBK - 1) / TBK * TBK;
   dim3 grid(ceil_div(M2, TBM), ceil_div(M1, TBM), Sg);
-  k_gemm_tn<<<grid, 256, 0, st>>>(P, M1, R, M2, N, rps, part);
+  k_gemm_tn<<<grid, 256, 0, st>>>(P, M1, R, M2, N, rps, part, nullptr);
   DSMIL_LAUNCH_OK("k_gemm_tn");
   return launch_sum_partials(part, Sg, L, out, st);
 }
-inline int colsum_splits(int64_t N) {
+__host__ __device__ inline int colsum_splits(int64_t N) {
   int s = ceil_div(N, 64);
   return s > kSplits ? kSplits : (s < 1 ? 1 : s);
 }
-inline int launch_colsum(const float* P, int M, int64_t N, float* part, float* out, cudaStream_t st) {
+// dyn != NULL: N is the row capacity and the split is the device's.
+inline int launch_colsum(const float* P, int M, int64_t N, float* part, float* out, cudaStream_t st,
+                         const RowSplit* dyn = nullptr) {
+  if (dyn) {
+    const int S = colsum_splits(N);
+    k_colsum<<<S, 256, 0, st>>>(P, M, N, 0, part, dyn);
+    DSMIL_LAUNCH_OK("k_colsum");
+    return launch_sum_partials(part, S, M, out, st, &dyn->S);
+  }
   if (N <= 0) {
     DSMIL_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float) * M, st));
     return 0;
   }
   const int S = colsum_splits(N);
   const int64_t rps = (N + S - 1) / S;
-  k_colsum<<<S, 256, 0, st>>>(P, M, N, rps, part);
+  k_colsum<<<S, 256, 0, st>>>(P, M, N, rps, part, nullptr);
   DSMIL_LAUNCH_OK("k_colsum");
   return launch_sum_partials(part, S, M, out, st);
 }

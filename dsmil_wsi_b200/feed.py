@@ -17,26 +17,34 @@ from . import _lib
 from . import functional as Fn
 
 
-def gather_rows(feats: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
-    """out[m] = feats[idx[m]] on the device (== `feats[idx]` of train_tcga.py:82)."""
+def gather_rows(feats: torch.Tensor, idx: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[m] = feats[idx[m]] on the device (== `feats[idx]` of train_tcga.py:82).  `out`: a contiguous float32
+    [len(idx), D] tensor on the same device to write into (e.g. a slot of a recorded training step)."""
     Fn.require_cuda(feats, "feats")
     feats = Fn._f32c(feats)
     idx = idx.to(device=feats.device, dtype=torch.int64).contiguous()
     M, D = int(idx.numel()), int(feats.shape[1])
+    if out is not None and (tuple(out.shape) != (M, D) or out.dtype != torch.float32 or not out.is_contiguous()
+                            or out.device != feats.device):
+        raise ValueError(f"out must be a contiguous float32 [{M}, {D}] tensor on {feats.device}, got "
+                         f"{out.dtype} {tuple(out.shape)} on {out.device}")
     with torch.cuda.device(feats.device):
-        out = torch.empty(M, D, dtype=torch.float32, device=feats.device)
+        if out is None:
+            out = torch.empty(M, D, dtype=torch.float32, device=feats.device)
         _lib.check(_lib.load().dsmil_gather_rows(feats.data_ptr(), int(feats.shape[0]), D, idx.data_ptr(), M,
                                                  out.data_ptr(), Fn._stream()), "dsmil_gather_rows")
     return out
 
 
-def dropout_patches(feats: torch.Tensor, p: float, generator: Optional[torch.Generator] = None) -> torch.Tensor:
+def dropout_patches(feats: torch.Tensor, p: float, generator: Optional[torch.Generator] = None,
+                    out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """train_tcga.py:78-83 with the arguments of the call site (`dropout_patches(bag_feats, 1 - dropout_patch)`):
-    keep int(N * p) rows in random order (p = 1 -> a full random permutation), everything on the device."""
+    keep int(N * p) rows in random order (p = 1 -> a full random permutation), everything on the device.  `out`: a
+    buffer of at least that many rows; the kept rows go to its first rows, which are returned."""
     n = int(feats.shape[0])
     keep = int(n * p)
     perm = torch.randperm(n, device=feats.device, generator=generator)[:keep]
-    return gather_rows(feats, perm)
+    return gather_rows(feats, perm, None if out is None else out[:keep])
 
 
 class DeviceBagStore:
@@ -91,17 +99,29 @@ class DeviceBagStore:
 
 def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_patch: float = 0.0,
                 order: Optional[Sequence[int]] = None, generator: Optional[torch.Generator] = None,
-                bags_per_step: int = 1) -> float:
+                bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None) -> float:
     """One epoch of train_tcga.train() (train_tcga.py:55-76) over device-resident bags; one host sync per epoch.
 
     bags_per_step = 1: the reference's loop, one forward, backward and optimizer step per bag.  k > 1: minibatches of
     k consecutive bags of `order`; each is one `milnet.forward_bags(xs, grad=True)` call, one backward and one
     optimizer step on the mean over the group of the per-bag 0.5 * criterion(bag) + 0.5 * criterion(max instance)
     (criterion evaluated once on the group's [k, C] rows, which is that mean for an element-averaging criterion such
-    as the reference's BCEWithLogitsLoss).  Returns the mean loss per bag either way."""
+    as the reference's BCEWithLogitsLoss).  Returns the mean loss per bag either way.
+
+    graph=True: the minibatch step (for any k >= 1, k = 1 included) is recorded once as a CUDA graph
+    (train_graph.TrainStepGraph) and replayed for every group; the bags go through the same dropout_patches, straight
+    into the graph's slots, and the results are the k-bag step's bits.  max_rows is the per-bag row capacity of the
+    graph (default: the largest bag of the store); a bag over it raises ValueError before any step.  Each call records
+    its graphs afresh (one warm-up step, one capture, new [k, max_rows, D] slots and a graph memory pool per group size,
+    freed when the call returns), so a graph holds the optimizer's hyperparameters of its call, e.g. a learning rate
+    that a scheduler changes between epochs.  Needs the batched tensor-core shapes and a capture-safe optimizer
+    (SGD, or Adam / AdamW with capturable=True)."""
     milnet.train()
     total = torch.zeros((), device=store.device)
     order = list(order) if order is not None else torch.randperm(len(store)).tolist()
+    if graph:
+        return _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator,
+                                  max(1, bags_per_step), max_rows)
     if bags_per_step > 1:
         for s in range(0, len(order), bags_per_step):
             group = order[s:s + bags_per_step]
@@ -109,7 +129,7 @@ def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_pat
             xs = [dropout_patches(store.bags[i][0], 1 - dropout_patch, generator) for i in group]
             labels = torch.cat([store.bags[i][1].view(1, -1) for i in group])
             bag_prediction, max_prediction = _group_predictions(milnet.forward_bags(xs, grad=True))
-            loss = 0.5 * criterion(bag_prediction, labels) + 0.5 * criterion(max_prediction, labels)
+            loss = minibatch_loss(criterion, bag_prediction, max_prediction, labels)
             loss.backward()
             optimizer.step()
             total += loss.detach() * len(group)
@@ -126,6 +146,42 @@ def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_pat
         optimizer.step()
         total += loss.detach()
     return float(total.item()) / max(1, len(order))
+
+
+def minibatch_loss(criterion, bag_prediction, max_prediction, labels):
+    """The minibatch step's loss over a group's [k, C] predictions and labels."""
+    return 0.5 * criterion(bag_prediction, labels) + 0.5 * criterion(max_prediction, labels)
+
+
+def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator, k, max_rows):
+    from .train_graph import TrainStepGraph, step_shape
+    step_shape(milnet)                                         # a shape off the batched path raises here
+    p = 1 - dropout_patch
+    keep = [int(int(store.bags[i][0].shape[0]) * p) for i in order]   # dropout_patches' row counts
+    cap = int(max_rows) if max_rows is not None else max([int(f.shape[0]) for f, _ in store.bags], default=1)
+    for i, n in zip(order, keep):
+        if n > cap:
+            raise ValueError(f"bag {i}: {n} rows exceed the training graph's max_rows={cap}")
+        if n < 1:
+            raise IndexError(f"dsmil_b200: bag {i} is empty after patch dropout (N == 0)")
+    graphs = {}
+    total = torch.zeros((), device=store.device)
+    for s in range(0, len(order), k):
+        group = order[s:s + k]
+        g = graphs.get(len(group))
+        if g is None:                                          # the first full group, and a short last one
+            g = graphs[len(group)] = TrainStepGraph(milnet, criterion, optimizer, len(group), cap)
+        for b, i in enumerate(group):
+            dropout_patches(store.bags[i][0], p, generator, out=g.slots[b])
+            g.Ns[b].fill_(keep[s + b])
+        torch.cat([store.bags[i][1].view(1, -1) for i in group], out=g.labels)
+        total += g.step() * len(group)
+    # the epoch's one host sync, which also reads the planners' status words
+    status = sum((g.status for g in graphs.values()), torch.zeros(1, dtype=torch.int32, device=store.device))
+    loss, bad = torch.stack([total.double(), status[0].double()]).tolist()
+    if bad:
+        raise RuntimeError(f"training graph: a batch held a bag outside [1, {cap}] rows (planner status {int(bad)})")
+    return loss / max(1, len(order))
 
 
 def _group_predictions(outs):

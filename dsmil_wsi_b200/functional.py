@@ -322,6 +322,68 @@ class MILBagsFn(torch.autograd.Function):
         return (None, *gxs, *[out[n] for n in names])
 
 
+class MILBagsDevFn(torch.autograd.Function):
+    """MILBagsFn over the capture-safe entry points (dsmil_forward_bags_train_dev / dsmil_backward_bags_dev): the bag
+    list lives on the device, so one recorded call serves every batch of nb bags of 1..max_rows rows.
+
+    args: slots [nb, max_rows, D] (bag b is slots[b, :Ns[b]]), Ns [nb] int64 and status [1] int32 on the device, then
+    the ten parameter tensors.  The packed per-row outputs (classes, A) have nb * max_rows rows; the live ones are
+    packed at the prefix sums of Ns, as MILBagsFn packs them.  Parameter gradients only (no gradient to the slots)."""
+
+    @staticmethod
+    def forward(ctx, slots, Ns, status, *params):
+        lib = _lib.load()
+        ctx.set_materialize_grads(False)
+        P = ParamPack(*params)
+        if not lib.dsmil_shard_bags_supported(P.ref):
+            raise ValueError(f"graph-captured training runs on the batched tensor-core path only; D={P.D}, C={P.C}, "
+                             f"nonlinear={P.nonlinear}, passing_v={P.passing_v} is not on it")
+        if slots.dim() != 3 or slots.shape[2] != P.D or slots.dtype != torch.float32 or not slots.is_contiguous():
+            raise ValueError(f"slots must be contiguous float32 [nb, max_rows, {P.D}], got {tuple(slots.shape)}")
+        nb, max_rows = int(slots.shape[0]), int(slots.shape[1])
+        dev = P.device
+        with torch.cuda.device(dev):
+            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+            rows = nb * max_rows
+            classes, A = new(rows, P.C), new(rows, P.C)
+            pred, B = new(nb, P.C), new(nb, P.C, P.D)
+            crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
+            sQ, sH = new(rows, Q_DIM), new(rows, Q_DIM)
+            xs = slots.data_ptr() + 4 * max_rows * P.D * torch.arange(nb, dtype=torch.int64, device=dev)
+            ws = _workspace(lib.dsmil_forward_bags_train_dev_workspace_bytes(P.ref, nb, max_rows), dev)
+            rc = lib.dsmil_forward_bags_train_dev(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred),
+                                                  _ptr(A), _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(status),
+                                                  _ptr(ws), ws.numel(), _stream())
+            _lib.check(rc, "dsmil_forward_bags_train_dev")
+        ctx.save_for_backward(xs, Ns, status, sQ, sH, A, B, crit, *P.tensors)
+        ctx.shape = (nb, max_rows)
+        ctx.mark_non_differentiable(crit)
+        return classes, pred, A, B, crit
+
+    @staticmethod
+    def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
+        if ctx.needs_input_grad[0] or g_A is not None or g_B is not None:
+            raise NotImplementedError("the graph-captured training step takes gradients through the instance scores "
+                                      "and the bag prediction only (no gradient to A, B or the features)")
+        lib = _lib.load()
+        xs, Ns, status, sQ, sH, A, B, crit, *params = ctx.saved_tensors
+        P = ParamPack(*params)
+        nb, max_rows = ctx.shape
+        names = ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")
+        dev = P.device
+        with torch.cuda.device(dev):
+            out = {nm: (torch.empty_like(t) if t is not None and need else None)
+                   for nm, t, need in zip(names, P.tensors, ctx.needs_input_grad[3:])}
+            G = _lib.DsmilGrads(*[_ptr(out[n]) for n in names], None)
+            dc, dp = _f32c(g_classes), _f32c(g_pred)
+            ws = _workspace(lib.dsmil_backward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
+            rc = lib.dsmil_backward_bags_dev(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(sQ), _ptr(sH), _ptr(A),
+                                             _ptr(B), _ptr(crit), _ptr(dc), _ptr(dp), None, None, C.byref(G),
+                                             _ptr(status), _ptr(ws), ws.numel(), _stream())
+            _lib.check(rc, "dsmil_backward_bags_dev")
+        return (None, None, None, *[out[n] for n in names])
+
+
 def mil_forward_bags(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]], *, grad: bool = False):
     """Forward of a STREAM of bags in one library call: returns a lazy sequence of (classes, prediction_bag, A, B)
     per bag -- views into packed device buffers -- plus crit_idx [nb, C] (rows within each bag).

@@ -164,6 +164,35 @@ int dsmil_backward_bags(const dsmil_params_t* p, const float* const* Xs, const i
                         const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
                         const dsmil_grads_t* grads, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Capture-safe forms of dsmil_forward_bags_train / dsmil_backward_bags, for a training step recorded once as a CUDA
+ * graph and replayed over batches of different bag sizes.  The bag list is in DEVICE memory: Xs_dev [nb] feature
+ * pointers, Ns_dev [nb] row counts.  max_rows is the per-bag row capacity: classes, A, save_Q and save_H1 (and
+ * d_classes) are sized for nb * max_rows rows, and hold the live rows packed in bag order at the live prefix sums, as
+ * the eager calls pack them.  Each call only enqueues work on `stream` (no host<->device copy, allocation or
+ * synchronisation, nothing read from Ns on the host): one recorded call serves every batch of nb bags with
+ * 1 <= Ns[b] <= max_rows.  A small planner kernel at the start of each call reads the bag list and writes the bag
+ * table and the live counts into the workspace.  A bag with N outside [1, max_rows], or features that are NULL or not
+ * 16-byte aligned, sets *status (device int32) to 1 + the first such bag's index, and the call then computes a stand-in
+ * batch in which every bag is one row of zeros: every output is finite and every index in range (crit_idx 0, pred =
+ * bf, B 0, row b of the packed outputs is bag b's), but none is the batch's, and a caller must discard what it derives
+ * from them.  A status is never cleared by the library: the caller zeroes it and reads it when it synchronises.  The forward builds
+ * the W1/W2 weight images on every call, so a replay after an optimizer step uses the current weights.
+ * Shapes: those of dsmil_shard_bags_supported (identity v).  Gradients through classes and pred only: d_A, d_B and
+ * grads->gX must be NULL (DSMIL_ERR_ARG).  On the same bags the results are the eager calls' bits.
+ * 1 <= nb <= 65535, max_rows >= 1; a short workspace is DSMIL_ERR_WORKSPACE.  The workspace sizes depend on
+ * (nb, max_rows) only and are never below the eager calls' for nb bags of max_rows rows. */
+size_t dsmil_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                 int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
+                                 int64_t* crit_idx, float* save_Q, float* save_H1, int32_t* status, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+size_t dsmil_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev, int32_t nb,
+                            int64_t max_rows, const float* Q, const float* H1, const float* A, const float* B,
+                            const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
+                            const float* d_B, const dsmil_grads_t* grads, int32_t* status, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 /* Call form (2)+(3) of the boundary (SURVEY §8b): the callers in attention_map.py:74,85 /
  * testing_tcga.py:72,83 run the instance classifier and the bag classifier separately.
  * dsmil_instance_scores == IClassifier.fc / FCLayer.fc (dsmil.py:11,24).
