@@ -9,17 +9,20 @@ there are exactly two data-path collectives, both all-gathers of a few KB:
 Everything else is local: phase1/2/3 of the C ABI (include/dsmil_b200.h).  classes and A stay
 sharded; prediction_bag, B and the critical indices are replicated.
 
-`ops` abstracts the five local steps so the exchange/merge logic can be exercised on CPU with
-gloo (tests/test_sharded_gloo.py injects an oracle-backed ops object; the product default is
-CudaShardOps, which has no fallback).
-
-A batch of such bags goes through CudaShardBagOps: three library calls and two all-gathers per forward step, and,
-for training (sharded_milnet_forward_bags + sharded_caller_loss_bags), three more calls and four more collectives
+The host logic is written once, for a batch of bags, over an ops object with the interface of CudaShardBagOps.
+CudaShardBagOps runs the batched ABI (dsmil_shard_bags_*): three library calls and two all-gathers per forward step,
+and, for training (sharded_milnet_forward_bags + sharded_caller_loss_bags), three more calls and four more collectives
 (one all-reduce(max) in the loss, three all-reduce(sum) in the backward), whatever the number of bags.
+PerBagShardOps gives that interface to a one-bag ops object (CudaShardOps: the one-bag ABI, dsmil_shard_phase1/2/3,
+which also serves the shapes the batched ABI refuses) by running it one bag at a time.  The one-bag entry points
+(sharded_forward, sharded_milnet_forward, sharded_caller_loss) are the batch step with nb = 1 over the one-bag ABI.
+The ops object is what the CPU tests replace: they run the same exchange/merge logic over gloo with an oracle-backed
+stand-in (the product default, CudaShardOps, has no fallback).
 """
 from __future__ import annotations
 
 import ctypes as C
+from itertools import accumulate
 from typing import List, Optional, Sequence, Tuple
 
 import torch
@@ -60,19 +63,28 @@ class CudaShardOps:
     def _ws(self, N):
         return Fn._workspace(self.lib.dsmil_shard_workspace_bytes(self.P.ref, N), self.device)
 
-    def phase1(self, X: torch.Tensor, row_offset: int):
+    def _phase1(self, X: torch.Tensor, row_offset: int, train: bool):
+        """dsmil_shard_phase1: (classes, Q, H1, V or X, cand).  `train` keeps H1 for the reverse pass (identity v
+        only); otherwise a passing_v model gets its V."""
         P, N = self.P, int(X.shape[0])
+        if train and P.passing_v:
+            raise NotImplementedError("sharded training: identity v only")
         X = Fn._check_feats(X, P.D) if N > 0 else X
         with torch.cuda.device(self.device):
             classes, Q = self.new(N, P.C), self.new(N, Fn.Q_DIM)
+            H1 = self.new(N, Fn.Q_DIM) if train and P.nonlinear else None
             V = self.new(N, P.D) if P.passing_v else None
             cand = self.new(self.cand_floats())
             ws = self._ws(N)
             rc = self.lib.dsmil_shard_phase1(P.ref, Fn._ptr(X), None, None, N, int(row_offset), Fn._ptr(classes),
-                                             Fn._ptr(Q), None, Fn._ptr(V), Fn._ptr(cand), Fn._ptr(ws), ws.numel(),
-                                             Fn._stream())
+                                             Fn._ptr(Q), Fn._ptr(H1), Fn._ptr(V), Fn._ptr(cand), Fn._ptr(ws),
+                                             ws.numel(), Fn._stream())
             _lib.check(rc, "dsmil_shard_phase1")
-        return classes, Q, (V if P.passing_v else X), cand
+        return classes, Q, H1, (X if V is None else V), cand
+
+    def phase1(self, X: torch.Tensor, row_offset: int):
+        classes, Q, _, Vv, cand = self._phase1(X, row_offset, train=False)
+        return classes, Q, Vv, cand
 
     def merge_candidates(self, cands: torch.Tensor, G: int):
         with torch.cuda.device(self.device):
@@ -113,21 +125,8 @@ class CudaShardOps:
 
     # ---- training: phase 1 that keeps H1, and the three backward phases (dsmil_shard_backward_*) ----
     def phase1_train(self, X: torch.Tensor, row_offset: int):
-        """phase1 with Q and H1 kept row-major for the reverse pass (identity v only)."""
-        P, N = self.P, int(X.shape[0])
-        if P.passing_v:
-            raise NotImplementedError("sharded training: identity v only")
-        X = Fn._check_feats(X, P.D) if N > 0 else X
-        with torch.cuda.device(self.device):
-            classes, Q = self.new(N, P.C), self.new(N, Fn.Q_DIM)
-            H1 = self.new(N, Fn.Q_DIM) if P.nonlinear else None
-            cand = self.new(self.cand_floats())
-            ws = self._ws(N)
-            rc = self.lib.dsmil_shard_phase1(P.ref, Fn._ptr(X), None, None, N, int(row_offset), Fn._ptr(classes),
-                                             Fn._ptr(Q), Fn._ptr(H1), None, Fn._ptr(cand), Fn._ptr(ws), ws.numel(),
-                                             Fn._stream())
-            _lib.check(rc, "dsmil_shard_phase1")
-        return classes, Q, H1, X, cand
+        """phase1 with Q and H1 kept row-major for the reverse pass (identity v only): (classes, Q, H1, X, cand)."""
+        return self._phase1(X, row_offset, train=True)
 
     def _bws(self, N):
         return Fn._workspace(self.lib.dsmil_backward_workspace_bytes(self.P.ref, N, 0), self.device)
@@ -340,9 +339,110 @@ class CudaShardBagOps:
         return gW1, gb1, gW2, gb2
 
 
+# One bag's own tensor passes through these unchanged, so a batch of one does the device work of the one-bag phases.
+def _cat(ts):
+    """Per-bag tensors packed in bag order along dim 0 (None for a tensor the model lacks: H1 of a linear q)."""
+    return ts[0] if len(ts) == 1 or ts[0] is None else torch.cat(ts)
+
+
+def _stack(ts):
+    """Per-bag records as [nb, *]."""
+    return ts[0][None] if len(ts) == 1 else torch.stack(ts)
+
+
+def _sum(ts):
+    """Sum over the bags of per-bag gradient shares (None for gW2 / gb2 of a linear q)."""
+    return ts[0] if len(ts) == 1 or ts[0] is None else torch.stack(ts).sum(0)
+
+
+def _gathered(recs_all, G, nb):
+    """The all-gathered records [G][nb][*] of the batch as one contiguous [G][*] block per bag."""
+    return [recs_all] if nb == 1 else [r.contiguous() for r in recs_all.view(G, nb, -1).unbind(1)]
+
+
+def _bags(t, nb):
+    """Per-bag [1, *] slices (views) of a tensor with a bag axis."""
+    return [t] * nb if t is None or nb == 1 else list(t.split(1))
+
+
+def _rows(t, xs):
+    """Per-bag row blocks (views) of a tensor packed [sum N_local, *] in the order of the bags xs."""
+    if t is None or len(xs) == 1:
+        return [t] * len(xs)
+    return list(t.split([int(x.shape[0]) for x in xs]))
+
+
+class PerBagShardOps:
+    """The interface of CudaShardBagOps over a one-bag ops object (CudaShardOps, or a stand-in with its methods), run
+    one bag at a time: per-bag library calls, but the batch's collectives.  This is the sharded path of the shapes the
+    batched ABI refuses (linear q, passing_v, D not a multiple of 128, more than 4 classes, D above 2048), and a bag may
+    hold no local rows.  For one bag, it returns the one-bag ops' own tensors (viewed as [1, *] where the batch
+    interface has a bag axis)."""
+
+    def __init__(self, one):
+        self.one = one
+
+    def begin(self, X_locals: Sequence[torch.Tensor], row_offsets: Sequence[int]):
+        """Returns the list of bags that phase1_train then fills with each bag's features as the one-bag phase 1
+        returned them; phase2_train and the reverse pass (which is handed that list back) read those."""
+        self.xs, self.offs = list(X_locals), [int(o) for o in row_offsets]
+        return self.xs
+
+    def phase1(self):
+        self.p1 = list(map(self.one.phase1, self.xs, self.offs))                   # classes, Q, V (or X), cand
+        return _stack([r[3] for r in self.p1])
+
+    def phase2(self, cands_all: torch.Tensor, G: int):
+        self.p2 = []
+        for (_, Q, Vv, _), cands in zip(self.p1, _gathered(cands_all, G, len(self.xs))):
+            qmax, crit = self.one.merge_candidates(cands, G)
+            self.p2.append((*self.one.phase2(Vv, Q, qmax), crit))                   # A, rec, crit
+        return _stack([r[1] for r in self.p2])
+
+    def phase3(self, recs_all: torch.Tensor, G: int):
+        outs = []
+        for (classes, *_), (A, _, crit), recs in zip(self.p1, self.p2, _gathered(recs_all, G, len(self.xs))):
+            A, B, pred = self.one.phase3(self.one.merge_partials(recs, G), A)
+            outs.append((classes, pred, A, B, crit))
+        return outs
+
+    def phase1_train(self):
+        classes, Q, H1, feats, cand = zip(*map(self.one.phase1_train, self.xs, self.offs))
+        self.xs[:] = feats
+        return _cat(classes), _cat(Q), _cat(H1), _stack(cand)
+
+    def phase2_train(self, Q: torch.Tensor, cands_all: torch.Tensor, G: int):
+        out = []
+        for x, q, cands in zip(self.xs, _rows(Q, self.xs), _gathered(cands_all, G, len(self.xs))):
+            qmax, crit = self.one.merge_candidates(cands, G)
+            out.append((*self.one.phase2(x, q, qmax), crit, qmax))
+        A, recs, crit, qmax = zip(*out)
+        return _cat(A), _stack(crit), _stack(qmax), _stack(recs)
+
+    def phase3_train(self, recs_all: torch.Tensor, G: int, A: torch.Tensor):
+        A, B, pred = zip(*[self.one.phase3(self.one.merge_partials(recs, G), a)
+                           for a, recs in zip(_rows(A, self.xs), _gathered(recs_all, G, len(self.xs)))])
+        return _cat(A), _cat(B), _cat(pred)
+
+    def bwd1(self, xs, A, B, d_classes, d_pred):
+        dA, t, *grads = zip(*map(self.one.bwd1, xs, _rows(A, xs), _bags(B, len(xs)), _rows(d_classes, xs),
+                                 _bags(d_pred, len(xs))))
+        return (_cat(dA), _stack(t), *map(_sum, grads))                             # grads: gWi, gbi, gWf, gbf
+
+    def bwd2(self, xs, A, dA, t, Q):
+        dL, dqm = zip(*map(self.one.bwd2, _rows(A, xs), _rows(dA, xs), t.unbind(), _rows(Q, xs)))
+        return _cat(dL), _stack(dqm)
+
+    def bwd3(self, xs, row_offsets, Q, H1, dL, dqm, qmax, crit):
+        return tuple(map(_sum, zip(*map(self.one.bwd3, xs, row_offsets, _rows(Q, xs), _rows(H1, xs), _rows(dL, xs),
+                                        dqm.unbind(), qmax.unbind(), crit.unbind()))))
+
+
 @torch.no_grad()
-def sharded_forward_bags_batched(bops: "CudaShardBagOps", X_locals, row_offsets, group=None):
-    """sharded_forward_bags on the batched ABI: 3 library calls + 2 all-gathers per step, whatever the batch."""
+def sharded_forward_bags_batched(bops, X_locals, row_offsets, group=None):
+    """The forward of a batch of row-sharded bags: 2 all-gathers per step, whatever the batch.  `bops` is a
+    CudaShardBagOps (3 library calls per step) or a PerBagShardOps.  Returns one (classes_local [N_r, C],
+    prediction_bag [1, C], A_local [N_r, C], B [1, C, D], crit_idx [C]) per bag."""
     bops.begin(X_locals, row_offsets)
     cand = bops.phase1()
     cands_all, G = _all_gather(cand.view(-1), group)        # exchange 1: [G][nb][cand]
@@ -387,18 +487,10 @@ def _all_gather(rec: torch.Tensor, group) -> Tuple[torch.Tensor, int]:
     return out, G
 
 
-@torch.no_grad()
 def sharded_forward(ops, X_local: torch.Tensor, row_offset: int, group=None):
-    """Forward of one bag whose rows are spread over the ranks of `group`.
+    """Forward of one bag whose rows are spread over the ranks of `group`: `sharded_forward_bags` of a batch of one.
     Returns (classes_local[N_r,C], prediction_bag[1,C], A_local[N_r,C], B[1,C,D], crit_idx[C])."""
-    classes, Q, Vv, cand = ops.phase1(X_local, row_offset)
-    cands, G = _all_gather(cand, group)                     # exchange 1
-    qmax, crit = ops.merge_candidates(cands, G)
-    A, rec = ops.phase2(Vv, Q, qmax)
-    recs, G = _all_gather(rec, group)                       # exchange 2
-    rec_g = ops.merge_partials(recs, G)
-    A, B, pred = ops.phase3(rec_g, A)
-    return classes, pred, A, B, crit
+    return sharded_forward_bags(ops, [X_local], [row_offset], group)[0]
 
 
 @torch.no_grad()
@@ -424,73 +516,25 @@ def milnet_params(milnet) -> Tuple[Optional[torch.Tensor], ...]:
     return (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
 
 
-@torch.no_grad()
 def sharded_forward_bags(ops, X_locals: Sequence[torch.Tensor], row_offsets: Sequence[int], group=None):
-    """A batch of giant bags, each row-sharded over the group: the per-bag records are packed so the
-    whole batch costs TWO collectives (not two per bag) -- at a few KB per record the exchange is
-    latency-bound, so batching is what keeps NVLink out of the critical path."""
-    nb = len(X_locals)
-    p1 = [ops.phase1(x, off) for x, off in zip(X_locals, row_offsets)]
-    cand_all, G = _all_gather(torch.cat([t[3] for t in p1]), group)          # exchange 1 (all bags)
-    cand_all = cand_all.view(G, nb, -1)
-    outs_mid = []
-    for b in range(nb):
-        qmax, crit = ops.merge_candidates(cand_all[:, b].contiguous(), G)
-        A, rec = ops.phase2(p1[b][2], p1[b][1], qmax)
-        outs_mid.append((A, rec, crit))
-    rec_all, G = _all_gather(torch.cat([t[1] for t in outs_mid]), group)      # exchange 2 (all bags)
-    rec_all = rec_all.view(G, nb, -1)
-    outs = []
-    for b in range(nb):
-        rec_g = ops.merge_partials(rec_all[:, b].contiguous(), G)
-        A, B, pred = ops.phase3(rec_g, outs_mid[b][0])
-        outs.append((p1[b][0], pred, A, B, outs_mid[b][2]))
-    return outs
+    """A batch of giant bags, each row-sharded over the group, through the one-bag ops `ops` (CudaShardOps) a bag at a
+    time: the per-bag records are packed so the whole batch costs TWO collectives (not two per bag) -- at a few KB per
+    record the exchange is latency-bound, so batching is what keeps NVLink out of the critical path."""
+    return sharded_forward_bags_batched(PerBagShardOps(ops), X_locals, row_offsets, group)
 
 
-# ---- row-sharded training step (SURVEY §8e "Backward"; oracle: backward_sharded) ---------------------------------
+# ---- row-sharded training step of a minibatch of bags (SURVEY §8e "Backward"; oracle: backward_sharded) ----------
+# Six collectives per step whatever the batch size: the forward's two all-gathers, one all-reduce(max) of nb*C floats
+# in the loss and three all-reduce(sum) in the reverse pass (t [nb,C], dq_max [nb,C,128], one flat buffer of parameter
+# gradients).  `bops` is a CudaShardBagOps (3 + 3 library calls per step), a PerBagShardOps (the one-bag calls per bag;
+# one bag is the one-bag training step), or any object with their begin / phase*_train / bwd1-3 methods (the host
+# logic below calls nothing else, so it runs over gloo with a CPU stand-in).
 
 
 def _all_reduce_sum(t: torch.Tensor, group) -> torch.Tensor:
     import torch.distributed as dist
     dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
     return t
-
-
-class ShardSaved:
-    """What one rank keeps between the sharded forward and its reverse pass."""
-    __slots__ = ("X", "row_offset", "Q", "H1", "A", "B", "qmax", "crit")
-
-    def __init__(self, X, row_offset, Q, H1, A, B, qmax, crit):
-        self.X, self.row_offset, self.Q, self.H1, self.A, self.B, self.qmax, self.crit = X, row_offset, Q, H1, A, B, qmax, crit
-
-
-@torch.no_grad()
-def sharded_forward_train(ops, X_local: torch.Tensor, row_offset: int, group=None, gather=_all_gather):
-    """`sharded_forward` that also returns the per-rank state `sharded_backward` needs (Q and H1 row-major)."""
-    classes, Q, H1, Xc, cand = ops.phase1_train(X_local, row_offset)
-    cands, G = gather(cand, group)                          # exchange 1
-    qmax, crit = ops.merge_candidates(cands, G)
-    A, rec = ops.phase2(Xc, Q, qmax)
-    recs, G = gather(rec, group)                            # exchange 2
-    rec_g = ops.merge_partials(recs, G)
-    A, B, pred = ops.phase3(rec_g, A)
-    return (classes, pred, A, B, crit), ShardSaved(Xc, row_offset, Q, H1, A, B, qmax, crit)
-
-
-@torch.no_grad()
-def sharded_backward(ops, saved: ShardSaved, d_classes_local: Optional[torch.Tensor], d_pred: Optional[torch.Tensor],
-                     group=None, reduce=_all_reduce_sum):
-    """Reverse pass of the sharded forward: three all-reduce(sum) steps -- t (C floats), dq_max (C x 128) and the
-    parameter gradients (one flat buffer, 341 KB at D=512, C=2).  Returns the gradients in ABI order
-    (gWi, gbi, gW1, gb1, gW2, gb2, gWf, gbf), identical on every rank; gW2/gb2 are None for the linear q."""
-    dA, t, gWi, gbi, gWf, gbf = ops.bwd1(saved.X, saved.A, saved.B, d_classes_local, d_pred)
-    t = reduce(t, group)                                                    # reduce 1
-    dL, dqm = ops.bwd2(saved.A, dA, t, saved.Q)
-    dqm = reduce(dqm, group)                                                # reduce 2
-    gW1, gb1, gW2, gb2 = ops.bwd3(saved.X, saved.row_offset, saved.Q, saved.H1, dL, dqm, saved.qmax, saved.crit)
-    gWi, gbi, gW1, gb1, gW2, gb2 = _reduce_flat((gWi, gbi, gW1, gb1, gW2, gb2), group, reduce)   # reduce 3
-    return gWi, gbi, gW1, gb1, gW2, gb2, gWf, gbf                           # Wf/bf grads are replicated already
 
 
 def _reduce_flat(grads, group, reduce):
@@ -505,101 +549,6 @@ def _reduce_flat(grads, group, reduce):
         out.append(flat[off:off + g.numel()].view_as(g))
         off += g.numel()
     return out
-
-
-class ShardedMILFn(torch.autograd.Function):
-    """autograd node of one row-sharded bag: forward = sharded_forward_train, backward = sharded_backward.
-    Every rank of the group must call it (and `.backward()`) in the same order: both directions contain
-    collectives.  Inputs after `group`: the ten parameter tensors in ABI order (Wv, bv must be None)."""
-
-    @staticmethod
-    def forward(ctx, ops, X_local, row_offset, group, *params):
-        ctx.set_materialize_grads(False)          # unused outputs (A, B) arrive as None, not as zero tensors
-        outs, saved = sharded_forward_train(ops, X_local, row_offset, group)
-        ctx.ops, ctx.saved, ctx.group = ops, saved, group
-        ctx.nonlinear = params[4] is not None
-        classes, pred, A, B, crit = outs
-        ctx.mark_non_differentiable(crit)
-        return classes, pred, A, B, crit
-
-    @staticmethod
-    def backward(ctx, d_classes, d_pred, d_A, d_B, _d_crit):
-        if d_A is not None or d_B is not None:
-            raise NotImplementedError("sharded backward: gradients through A / B are not supported "
-                                      "(the callers use classes and prediction_bag only, train_tcga.py:67-72)")
-        gWi, gbi, gW1, gb1, gW2, gb2, gWf, gbf = sharded_backward(ctx.ops, ctx.saved, d_classes, d_pred, ctx.group)
-        return (None, None, None, None, gWi, gbi, gW1, gb1, gW2, gb2, None, None, gWf, gbf)
-
-
-def sharded_milnet_forward(milnet, X_local: torch.Tensor, row_offset: int, group=None, ops=None):
-    """`classes_local, prediction_bag, A_local, B (, crit_idx) = milnet(X)` for a bag whose rows live on several
-    ranks, with autograd: `loss.backward()` on every rank (loss from `sharded_caller_loss`) leaves identical, fully
-    reduced `.grad`s on the parameters."""
-    params = milnet_params(milnet)
-    ops = ops or CudaShardOps(params)
-    classes, pred, A, B, crit = ShardedMILFn.apply(ops, X_local, int(row_offset), group, *params)
-    return classes, pred, A, B, crit
-
-
-def sharded_max_prediction(classes_local: torch.Tensor, crit: torch.Tensor, row_offset: int, group=None):
-    """`torch.max(ins_prediction, 0)[0]` of the callers' loss (train_tcga.py:68, train_mil.py:51) when the rows of
-    `ins_prediction` are spread over ranks: the value is the same on every rank (one all-reduce(max) of C
-    floats), the gradient flows only into the row that holds the maximum, on the rank that owns it.  `crit` is
-    the forward's critical-instance index (== that arg-max, lowest index on ties)."""
-    import torch.distributed as dist
-    n, C = int(classes_local.shape[0]), int(classes_local.shape[1])
-    loc = crit.to(classes_local.device) - int(row_offset)
-    owned = (loc >= 0) & (loc < n)
-    if n > 0:
-        mine = classes_local[loc.clamp(0, n - 1), torch.arange(C, device=classes_local.device)]
-    else:
-        mine = classes_local.new_zeros(C)
-    glob = torch.where(owned, mine.detach(), torch.full_like(mine, float("-inf")))
-    dist.all_reduce(glob, op=dist.ReduceOp.MAX, group=group)
-    return torch.where(owned, mine, glob)
-
-
-def sharded_caller_loss(classes_local, prediction_bag, crit, row_offset, label, criterion, group=None):
-    """0.5 * criterion(bag) + 0.5 * criterion(max instance) (train_tcga.py:67-71) for a row-sharded bag: same
-    value on every rank; `loss.backward()` on every rank gives the single-device gradients."""
-    max_prediction = sharded_max_prediction(classes_local, crit, row_offset, group)
-    tgt = label.view(1, -1).to(prediction_bag.dtype)
-    return 0.5 * criterion(prediction_bag.view(1, -1), tgt) + 0.5 * criterion(max_prediction.view(1, -1), tgt)
-
-
-@torch.no_grad()
-def virtual_sharded_train_step(ops, X: torch.Tensor, G: int, loss_grads):
-    """Forward + reverse pass with G logical shards on ONE device, the two all-gathers replaced by concatenation
-    and the three all-reduces by local sums (same kernels, same record layouts) -- validates the sharded
-    training algebra without G GPUs.  `loss_grads(classes[N,C], pred[1,C]) -> (d_classes[N,C] | None,
-    d_pred[1,C] | None)` supplies the callers' loss gradient.  Returns ((classes, pred, A, B, crit), grads) with
-    grads in the order of `sharded_backward`."""
-    bounds = shard_bounds(int(X.shape[0]), G)
-    loc = [ops.phase1_train(X[lo:hi], lo) for lo, hi in bounds]          # classes, Q, H1, X, cand
-    qmax, crit = ops.merge_candidates(torch.cat([l[4] for l in loc]), G)
-    part = [ops.phase2(l[3], l[1], qmax) for l in loc]
-    rec_g = ops.merge_partials(torch.cat([p[1] for p in part]), G)
-    outs = [ops.phase3(rec_g, p[0]) for p in part]                       # A, B, pred
-    classes, A = torch.cat([l[0] for l in loc]), torch.cat([o[0] for o in outs])
-    B, pred = outs[0][1], outs[0][2]
-    d_classes, d_pred = loss_grads(classes, pred)
-    b1 = [ops.bwd1(l[3], o[0], B, None if d_classes is None else d_classes[lo:hi], d_pred)
-          for l, o, (lo, hi) in zip(loc, outs, bounds)]                  # dA, t, gWi, gbi, gWf, gbf
-    t = torch.stack([b[1] for b in b1]).sum(0)                           # reduce 1
-    b2 = [ops.bwd2(o[0], b[0], t, l[1]) for l, o, b in zip(loc, outs, b1)]
-    dqm = torch.stack([b[1] for b in b2]).sum(0)                         # reduce 2
-    b3 = [ops.bwd3(l[3], lo, l[1], l[2], b[0], dqm, qmax, crit) for l, b, (lo, _) in zip(loc, b2, bounds)]
-    tot = lambda ts: None if ts[0] is None else torch.stack(list(ts)).sum(0)   # reduce 3
-    gWi, gbi = tot([b[2] for b in b1]), tot([b[3] for b in b1])
-    gW1, gb1, gW2, gb2 = (tot([b[i] for b in b3]) for i in range(4))
-    return (classes, pred, A, B, crit), (gWi, gbi, gW1, gb1, gW2, gb2, b1[0][4], b1[0][5])
-
-
-# ---- a minibatch of row-sharded bags: training step ---------------------------------------------------------------
-# Six collectives per step whatever the batch size: the forward's two all-gathers, one all-reduce(max) of nb*C floats
-# in the loss and three all-reduce(sum) in the reverse pass (t [nb,C], dq_max [nb,C,128], one flat buffer of parameter
-# gradients); 3 + 3 library calls.  `bops` is a CudaShardBagOps, or any object with its begin / phase*_train / phase3_train
-# / bwd1-3 methods (the host logic below calls nothing else, so it runs over gloo with a CPU stand-in).
 
 
 class ShardBagsSaved:
@@ -667,7 +616,8 @@ class ShardedMILBagsFn(torch.autograd.Function):
 def sharded_milnet_forward_bags(milnet, X_locals: Sequence[torch.Tensor], row_offsets: Sequence[int], group=None,
                                 ops=None):
     """Packed `(classes_local, prediction_bag, A_local, B, crit_idx)` of a batch of bags whose rows live on several
-    ranks (bag b: this rank's rows [row_offsets[b], row_offsets[b] + len(X_locals[b])), at least one per bag), with
+    ranks (bag b: this rank's rows [row_offsets[b], row_offsets[b] + len(X_locals[b])); CudaShardBagOps needs at
+    least one per bag), with
     autograd: `loss.backward()` on every rank (loss from `sharded_caller_loss_bags`) leaves identical, fully reduced
     `.grad`s on the parameters.  classes_local / A_local are [sum N_local, C] in bag order; prediction_bag [nb, C],
     B [nb, C, D] and crit_idx [nb, C] (global rows) are replicated."""
@@ -685,14 +635,21 @@ def sharded_max_prediction_bags(classes_local: torch.Tensor, crit: torch.Tensor,
     import torch.distributed as dist
     dev = classes_local.device
     Cc = int(classes_local.shape[1])
-    n = torch.tensor([int(v) for v in Ns], dtype=torch.int64, device=dev)
-    first = torch.cumsum(n, 0) - n
-    loc = crit.to(dev) - torch.tensor([int(o) for o in row_offsets], dtype=torch.int64, device=dev)[:, None]
-    owned = (loc >= 0) & (loc < n[:, None])
+    Ns = [int(v) for v in Ns]
+    # per bag: row offset, local rows, first packed row.  One bag passes them as kernel arguments; a batch copies them
+    # from pinned memory, which does not block the host (a pageable copy would synchronise with the stream).
+    if len(Ns) == 1:
+        off, n, first = int(row_offsets[0]), Ns[0], 0
+    else:
+        host = torch.tensor([[int(o) for o in row_offsets], Ns, list(accumulate([0] + Ns[:-1]))], dtype=torch.int64,
+                            pin_memory=dev.type == "cuda")
+        off, n, first = host.to(dev, non_blocking=True)[:, :, None]
+    loc = crit.to(dev) - off
+    owned = (loc >= 0) & (loc < n)
     total = int(classes_local.shape[0])
     if total > 0:
         # owned entries index their row; the others any valid row (their value is replaced, their gradient is zero)
-        mine = classes_local.gather(0, (first[:, None] + loc.clamp(min=0)).clamp(max=total - 1))
+        mine = classes_local.gather(0, (first + loc.clamp(min=0)).clamp(max=total - 1))
     else:
         mine = classes_local.new_zeros(len(Ns), Cc)
     glob = torch.where(owned, mine.detach(), torch.full_like(mine, float("-inf")))
@@ -707,6 +664,23 @@ def sharded_caller_loss_bags(classes_local, prediction_bag, crit, row_offsets, l
     max_prediction = sharded_max_prediction_bags(classes_local, crit, row_offsets, Ns, group)
     tgt = labels.reshape(prediction_bag.shape).to(prediction_bag.dtype)
     return 0.5 * criterion(prediction_bag, tgt) + 0.5 * criterion(max_prediction, tgt)
+
+
+def sharded_milnet_forward(milnet, X_local: torch.Tensor, row_offset: int, group=None, ops=None):
+    """`classes_local, prediction_bag, A_local, B (, crit_idx) = milnet(X)` for a bag whose rows live on several
+    ranks, with autograd: `loss.backward()` on every rank (loss from `sharded_caller_loss`) leaves identical, fully
+    reduced `.grad`s on the parameters.  A batch of one through `sharded_milnet_forward_bags` over the one-bag ops
+    `ops` (default: CudaShardOps, the one-bag ABI, which takes every shape and a rank with no rows of the bag)."""
+    ops = PerBagShardOps(ops or CudaShardOps(milnet_params(milnet)))
+    classes, pred, A, B, crit = sharded_milnet_forward_bags(milnet, [X_local], [row_offset], group, ops)
+    return classes, pred, A, B, crit[0]
+
+
+def sharded_caller_loss(classes_local, prediction_bag, crit, row_offset, label, criterion, group=None):
+    """0.5 * criterion(bag) + 0.5 * criterion(max instance) (train_tcga.py:67-71) for a row-sharded bag: same
+    value on every rank; `loss.backward()` on every rank gives the single-device gradients."""
+    return sharded_caller_loss_bags(classes_local, prediction_bag.view(1, -1), crit.view(1, -1), [row_offset], label,
+                                    criterion, group, Ns=[len(classes_local)])
 
 
 @torch.no_grad()

@@ -1,7 +1,7 @@
 """Training on a minibatch of row-sharded bags, without a GPU: argument validation and workspace sizes of the new entry
 points (calls that return before any CUDA work), and the host logic of the step -- sharded_forward_bags_train,
-sharded_caller_loss_bags, sharded_backward_bags through ShardedMILBagsFn -- over gloo with 2 and 3 ranks and with an
-oracle-backed stand-in for the batched ops, plus the single-process virtual-rank helper."""
+sharded_caller_loss_bags, sharded_backward_bags through ShardedMILBagsFn -- over gloo with 2 and 3 ranks and with the
+fp64 oracle's one-bag ops run per bag through PerBagShardOps, plus the single-process virtual-rank helper."""
 import ctypes as C
 import os
 
@@ -132,66 +132,7 @@ def test_workspace_sizes_grow_with_rows(D, C_):
     assert lib.dsmil_shard_backward_bags_workspace_bytes(C.byref(p), n, 0) == 0
 
 
-# ---- the host logic over gloo, with the batched ops restated per bag on the fp64 oracle --------------------------
-class OracleBagOps:
-    """The methods of CudaShardBagOps that the training step calls, per bag on OracleTrainOps, with the packed
-    layouts of the library ([sum N_local, *] in bag order).  A bag may hold no local rows here."""
-
-    def __init__(self, p: orc.Params):
-        self.one = OracleTrainOps(p)
-
-    @staticmethod
-    def _split(t, xs):
-        out, lo = [], 0
-        for x in xs:
-            out.append(t[lo:lo + x.shape[0]])
-            lo += x.shape[0]
-        return out
-
-    def begin(self, X_locals, row_offsets):
-        self.xs, self.offs = list(X_locals), [int(o) for o in row_offsets]
-        return self.xs
-
-    def phase1_train(self):
-        r = [self.one.phase1_train(x, o) for x, o in zip(self.xs, self.offs)]     # classes, Q, H1, x, cand
-        return (torch.cat([t[0] for t in r]), torch.cat([t[1] for t in r]), torch.cat([t[2] for t in r]),
-                torch.stack([t[4] for t in r]))
-
-    def phase2_train(self, Q, cands_all, G):
-        nb = len(self.xs)
-        cands = cands_all.view(G, nb, -1)
-        A, crit, qmax, recs = [], [], [], []
-        for b, (x, q) in enumerate(zip(self.xs, self._split(Q, self.xs))):
-            qm, cr = self.one.merge_candidates(cands[:, b].reshape(-1).contiguous(), G)
-            a, rec = self.one.phase2(x.double(), q, qm)
-            A.append(a), crit.append(cr), qmax.append(qm), recs.append(rec)
-        return torch.cat(A), torch.stack(crit), torch.stack(qmax), torch.stack(recs)
-
-    def phase3_train(self, recs_all, G, A):
-        nb = len(self.xs)
-        recs = recs_all.view(G, nb, -1)
-        out = [self.one.phase3(self.one.merge_partials(recs[:, b].reshape(-1).contiguous(), G), a)
-               for b, a in enumerate(self._split(A, self.xs))]
-        return torch.cat([o[0] for o in out]), torch.cat([o[1] for o in out]), torch.cat([o[2] for o in out])
-
-    def bwd1(self, xs, A, B, d_classes, d_pred):
-        dcs = [None] * len(xs) if d_classes is None else self._split(d_classes, xs)
-        r = [self.one.bwd1(x.double(), a, B[b:b + 1], dc, None if d_pred is None else d_pred[b])
-             for b, (x, a, dc) in enumerate(zip(xs, self._split(A, xs), dcs))]
-        tot = lambda i: torch.stack([t[i] for t in r]).sum(0)
-        return torch.cat([t[0] for t in r]), torch.stack([t[1] for t in r]), tot(2), tot(3), tot(4), tot(5)
-
-    def bwd2(self, xs, A, dA, t, Q):
-        r = [self.one.bwd2(a, d, t[b], q) for b, (a, d, q) in
-             enumerate(zip(self._split(A, xs), self._split(dA, xs), self._split(Q, xs)))]
-        return torch.cat([v[0] for v in r]), torch.stack([v[1] for v in r])
-
-    def bwd3(self, xs, row_offsets, Q, H1, dL, dqm, qmax, crit):
-        r = [self.one.bwd3(x.double(), int(o), q, h, d, dqm[b], qmax[b], crit[b]) for b, (x, o, q, h, d) in
-             enumerate(zip(xs, row_offsets, self._split(Q, xs), self._split(H1, xs), self._split(dL, xs)))]
-        return tuple(torch.stack([v[i] for v in r]).sum(0) for i in range(4))
-
-
+# ---- the host logic over gloo, with the one-bag fp64 oracle run per bag through PerBagShardOps ----------------
 def _problem(sizes, D=48, C_=2):
     p = orc.random_params(D, C_, seed=31, scale=1.5)
     Xs = [orc.synthetic_bag(n, D, 500 + i, "normal") for i, n in enumerate(sizes)]
@@ -216,7 +157,8 @@ def _bags_train_worker(rank, world, port, sizes, ret):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
         from helpers import build_net
-        from dsmil_wsi_b200.sharded import shard_bounds, sharded_caller_loss_bags, sharded_milnet_forward_bags
+        from dsmil_wsi_b200.sharded import (PerBagShardOps, shard_bounds, sharded_caller_loss_bags,
+                                            sharded_milnet_forward_bags)
         p, Xs, y = _problem(sizes)
         net = build_net(p, device="cpu")
         xs, offs = [], []
@@ -235,7 +177,7 @@ def _bags_train_worker(rank, world, port, sizes, ret):
             counts["max" if op == dist.ReduceOp.MAX else "sum"] += 1
             return real_reduce(t, op=op, **k)
         dist.all_gather_into_tensor, dist.all_reduce = gather, reduce
-        classes, pred, A, B, crit = sharded_milnet_forward_bags(net, xs, offs, ops=OracleBagOps(p))
+        classes, pred, A, B, crit = sharded_milnet_forward_bags(net, xs, offs, ops=PerBagShardOps(OracleTrainOps(p)))
         loss = sharded_caller_loss_bags(classes, pred, crit, offs, torch.from_numpy(y), torch.nn.BCEWithLogitsLoss(),
                                         Ns=[x.shape[0] for x in xs])
         loss.backward()
@@ -285,12 +227,13 @@ def _loss_grads(y):
 
 @pytest.mark.parametrize("G,sizes", [(1, [37, 5]), (2, [37, 5, 120, 1]), (3, [2, 64, 9, 3]), (8, [40, 17, 8])])
 def test_virtual_sharded_train_step_bags_host_logic(G, sizes):
-    from dsmil_wsi_b200.sharded import virtual_sharded_train_step_bags
+    from dsmil_wsi_b200.sharded import PerBagShardOps, virtual_sharded_train_step_bags
     p, Xs, y = _problem(sizes)
     loss, want = _oracle_batch(p, Xs, y)
     lg = _loss_grads(y)
     lg.Ns = sizes
-    outs, grads = virtual_sharded_train_step_bags(lambda: OracleBagOps(p), [torch.from_numpy(X) for X in Xs], G, lg)
+    outs, grads = virtual_sharded_train_step_bags(lambda: PerBagShardOps(OracleTrainOps(p)),
+                                                  [torch.from_numpy(X) for X in Xs], G, lg)
     classes, pred, A, B, crit = outs
     ones = [orc.forward(X, p) for X in Xs]
     assert np.array_equal(crit.numpy(), np.stack([o.idx for o in ones]))

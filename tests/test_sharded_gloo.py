@@ -208,11 +208,22 @@ def _train_worker(rank, world, port, name, N_override, ret):
         lo, hi = shard_bounds(X.shape[0], world)[rank]
         net = build_net(p, device="cpu")
         y = torch.from_numpy(np.asarray(g["y"], np.float32).reshape(-1))
+        counts = {"all_gather": 0, "sum": 0, "max": 0}
+        real_gather, real_reduce = dist.all_gather_into_tensor, dist.all_reduce
+
+        def gather(*a, **k):
+            counts["all_gather"] += 1
+            return real_gather(*a, **k)
+
+        def reduce(t, op=dist.ReduceOp.SUM, **k):
+            counts["max" if op == dist.ReduceOp.MAX else "sum"] += 1
+            return real_reduce(t, op=op, **k)
+        dist.all_gather_into_tensor, dist.all_reduce = gather, reduce
         classes, pred, A, B, crit = sharded_milnet_forward(net, torch.from_numpy(X[lo:hi]), lo, ops=OracleTrainOps(p))
         loss = sharded_caller_loss(classes, pred, crit, lo, y, torch.nn.BCEWithLogitsLoss())
         loss.backward()
-        ret[rank] = dict(loss=float(loss.detach()), grads={k: v.grad.numpy().copy() for k, v in net.named_parameters()
-                                                  if v.grad is not None})
+        ret[rank] = dict(loss=float(loss.detach()), counts=counts,
+                         grads={k: v.grad.numpy().copy() for k, v in net.named_parameters() if v.grad is not None})
     finally:
         dist.destroy_process_group()
 
@@ -221,7 +232,8 @@ def _train_worker(rank, world, port, name, N_override, ret):
                                                    (2, "musk_d166_n7", None), (2, "musk_d166_n7", 1)])
 def test_sharded_training_step_over_gloo(world, name, N_override):
     """Every rank ends with the single-device gradients of the callers' loss (train_tcga.py:67-72), and the same
-    loss value: three all-reduces in the reverse pass, one all-reduce(max) in the loss."""
+    loss value: two all-gathers in the forward, three all-reduces in the reverse pass, one all-reduce(max) in the
+    loss."""
     from helpers import grad_name
     port = _free_port()
     ret = mp.Manager().dict()
@@ -234,6 +246,7 @@ def test_sharded_training_step_over_gloo(world, name, N_override):
     loss, d_cls, d_pred = orc.caller_loss_grads(one, y)
     ref = orc.backward(X, p, one, d_cls, d_pred)
     for r in range(world):
+        assert ret[r]["counts"] == {"all_gather": 2, "sum": 3, "max": 1}, ret[r]["counts"]
         assert abs(ret[r]["loss"] - loss) < 2e-6
         grads = ret[r]["grads"]
         for short, want in ref.items():
@@ -249,18 +262,19 @@ def test_sharded_training_step_over_gloo(world, name, N_override):
 
 
 @pytest.mark.parametrize("name,G", [("shipped_tcga", 3), ("lin_d512_c3", 4), ("musk_d166_n7", 8), ("musk_d166_n1", 2)])
-def test_virtual_sharded_train_step_host_logic(name, G):
+def test_virtual_sharded_train_step_bags_one_bag_host_logic(name, G):
     """The single-device validation helper (reductions as local sums) with the oracle-backed ops: same indexing
     and record plumbing the GPU test (tests/test_zz_shard_backward_gpu.py) relies on."""
-    from dsmil_wsi_b200.sharded import virtual_sharded_train_step
+    from dsmil_wsi_b200.sharded import PerBagShardOps, virtual_sharded_train_step_bags
     g, p, X = load_golden(name)
     one = orc.forward(X, p)
     y = np.asarray(g["y"], np.float64).reshape(-1)
     _, d_cls, d_pred = orc.caller_loss_grads(one, y)
     ref = orc.backward(X, p, one, d_cls, d_pred)
-    grads_of = lambda classes, pred: (torch.from_numpy(d_cls), torch.from_numpy(d_pred))
-    outs, grads = virtual_sharded_train_step(OracleTrainOps(p), torch.from_numpy(X), G, grads_of)
-    assert np.array_equal(outs[4].numpy(), one.idx) and rel_to_max(outs[2].numpy(), one.A) < 2e-6
+    grads_of = lambda classes, pred, crit: (torch.from_numpy(d_cls), torch.from_numpy(d_pred))
+    outs, grads = virtual_sharded_train_step_bags(lambda: PerBagShardOps(OracleTrainOps(p)), [torch.from_numpy(X)], G,
+                                                  grads_of)
+    assert np.array_equal(outs[4][0].numpy(), one.idx) and rel_to_max(outs[2].numpy(), one.A) < 2e-6
     for short, got in zip(["Wi", "bi", "W1", "b1", "W2", "b2", "Wf", "bf"], grads):
         if got is None:
             assert not p.nonlinear and short in ("W2", "b2")

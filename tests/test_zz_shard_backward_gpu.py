@@ -19,7 +19,7 @@ ORDER = ["Wi", "bi", "W1", "b1", "W2", "b2", "Wf", "bf"]
 
 
 def _loss_grads(y):
-    def fn(classes, pred):
+    def fn(classes, pred, crit):
         with torch.enable_grad():
             c, p = classes.detach().clone().requires_grad_(True), pred.detach().clone().requires_grad_(True)
             caller_loss(c, p, y).backward()
@@ -29,8 +29,8 @@ def _loss_grads(y):
 
 @pytest.mark.parametrize("name,G", [("shipped_tcga", 1), ("shipped_tcga", 3), ("shipped_c16", 2), ("musk_d166_n7", 8),
                                     ("lin_d512_c3", 4), ("tree_d1024_c2", 7), ("musk_d166_n1", 2)])
-def test_virtual_shards_give_single_device_gradients(name, G):
-    from dsmil_wsi_b200.sharded import CudaShardOps, milnet_params, virtual_sharded_train_step
+def test_virtual_shards_of_one_bag_give_single_device_gradients(name, G):
+    from dsmil_wsi_b200.sharded import CudaShardOps, PerBagShardOps, milnet_params, virtual_sharded_train_step_bags
     g, p, X = load_golden(name)
     net = build_net(p).train()
     x = torch.from_numpy(X).cuda()
@@ -40,8 +40,9 @@ def test_virtual_shards_give_single_device_gradients(name, G):
     caller_loss(c1, p1, y).backward()
     single = {k: v.grad.detach().cpu().numpy() for k, v in net.named_parameters()}
     ops = CudaShardOps(milnet_params(net))
-    (classes, pred, A, B, crit), grads = virtual_sharded_train_step(ops, x, G, _loss_grads(y))
-    assert torch.equal(classes, c1.detach()) and np.array_equal(crit.cpu().numpy(), g["idx"])
+    (classes, pred, A, B, crit), grads = virtual_sharded_train_step_bags(lambda: PerBagShardOps(ops), [x], G,
+                                                                         _loss_grads(y))
+    assert torch.equal(classes, c1.detach()) and np.array_equal(crit[0].cpu().numpy(), g["idx"])
     one = orc.forward(X, p)
     _, d_cls, d_pred = orc.caller_loss_grads(one, np.asarray(g["y"], np.float64).reshape(-1))
     ref = orc.backward(X, p, one, d_cls, d_pred)

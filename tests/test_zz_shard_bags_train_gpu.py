@@ -1,6 +1,6 @@
 """Training on a minibatch of row-sharded bags, on the device: the three batched sharded backward phases at one rank
 against dsmil_backward_bags bit for bit; G virtual ranks on one GPU against forward_bags(grad=True) and the fp64
-oracle; determinism; an SGD step through ShardedMILBagsFn + sharded_caller_loss_bags over two processes against
+oracle; determinism; a loss that never waits for the stream; an SGD step through ShardedMILBagsFn + sharded_caller_loss_bags over two processes against
 feed.train_epoch(bags_per_step=k); and the same step over NCCL on two GPUs when the box has them."""
 import copy
 import ctypes as C
@@ -165,6 +165,48 @@ def test_virtual_step_is_deterministic():
     runs = [virtual_sharded_train_step_bags(lambda: CudaShardBagOps(params), xs, 3, lg) for _ in range(2)]
     for a, b in zip(runs[0][0] + runs[0][1], runs[1][0] + runs[1][1]):
         assert torch.equal(a, b)
+
+
+def test_caller_loss_does_not_sync_the_host(monkeypatch):
+    """The sharded loss of one bag and of three, forward and backward, only enqueues device work: no call waits for
+    the stream.  The all-reduce(max) is stubbed as the identity of one rank, so this rank owns every critical row."""
+    import torch.distributed as dist
+    from dsmil_wsi_b200.sharded import sharded_caller_loss, sharded_caller_loss_bags
+    monkeypatch.setattr(dist, "all_reduce", lambda tensor, op=None, group=None, async_op=False: None)
+    Ns, offs, C_ = [37, 1, 200], [0, 5, 1000], 2
+    g = torch.Generator(device="cuda").manual_seed(11)
+    classes = torch.randn(sum(Ns), C_, device="cuda", generator=g)
+    pred = torch.randn(len(Ns), C_, device="cuda", generator=g)
+    y = (torch.rand(len(Ns), C_, device="cuda", generator=g) > 0.5).float()
+    first = [0] + list(np.cumsum(Ns)[:-1])
+    local = torch.stack([classes[f:f + n].argmax(0) for f, n in zip(first, Ns)])          # [nb, C] local rows
+    crit = local + torch.tensor(offs, device="cuda")[:, None]
+    bce = torch.nn.BCEWithLogitsLoss()
+
+    def leaves(nb):
+        n = sum(Ns[:nb])
+        return classes[:n].clone().requires_grad_(True), pred[:nb].clone().requires_grad_(True)
+
+    def check(loss, c, p, nb):
+        """Against the single-device loss of the same bags (its max instance: each bag's critical row)."""
+        cr, pr = leaves(nb)
+        rows = local[:nb] + torch.tensor(first[:nb], device="cuda")[:, None]
+        ref = 0.5 * bce(pr, y[:nb]) + 0.5 * bce(cr.gather(0, rows), y[:nb])
+        ref.backward()
+        assert torch.equal(loss, ref) and torch.equal(c.grad, cr.grad) and torch.equal(p.grad, pr.grad), nb
+
+    (c1, p1), (c3, p3) = leaves(1), leaves(3)
+    torch.cuda.synchronize()
+    torch.cuda.set_sync_debug_mode("error")
+    try:
+        one = sharded_caller_loss(c1, p1, crit[0], offs[0], y[0], bce)
+        one.backward()
+        many = sharded_caller_loss_bags(c3, p3, crit, offs, y, bce, Ns=Ns)
+        many.backward()
+    finally:
+        torch.cuda.set_sync_debug_mode(0)
+    check(one, c1, p1, 1)
+    check(many, c3, p3, 3)
 
 
 # ---- an SGD step through the autograd node, two ranks (two processes) ----------------------------------------------
