@@ -134,6 +134,27 @@ SIGNATURES = {
                                                    C.c_int32, C.POINTER(c_i64), C.c_void_p, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_bags_train_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
+    "dsmil_shard_bags_phase1_train_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_int32, c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_bags_phase2_train_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_int32, c_i64, C.c_void_p, C.c_void_p,
+                                                    C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_bags_phase3_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_int32, c_i64, C.c_void_p, C.c_int32,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_backward_bags_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
+    "dsmil_shard_backward_bags_phase1_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_int32,
+                                                       c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_backward_bags_phase2_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_int32, c_i64, C.c_void_p,
+                                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_shard_backward_bags_phase3_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_int32, c_i64, C.c_void_p,
+                                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -1083,8 +1083,8 @@ static int bwd_bags_phase1_impl(const dsmil_params_t* p, const float* const* Xs,
   return 0;
 }
 
-// Phase 2: dL = A (dA - t_b) / sqrt(128), t_b the sum of the P partials per bag in `tpart` (a dev call: phase 1's
-// live G of them); dqm[b] = dL_b^T Q_b, summed over the CTAs' shares in a fixed order.
+// Phase 2: dL = A (dA - t_b) / sqrt(128), t_b the sum of the P partials per bag in `tpart` (P == 0 in a dev call:
+// phase 1's live G of them); dqm[b] = dL_b^T Q_b, summed over the CTAs' shares in a fixed order.
 static int bwd_bags_phase2_impl(const dsmil_params_t* p, int nb, const float* A, const float* dA, const float* tpart,
                                 int P, const float* Q, float* dL, float* dqm, const BwdBagsWs& w, cudaStream_t st) {
   const int C = p->C;
@@ -1135,7 +1135,7 @@ static int backward_bags_run(const dsmil_params_t* p, const float* const* Xs, co
   int rc;
   const float* dz1;
   if ((rc = bwd_bags_phase1_impl(p, Xs, Ns, nb, total, A, B, d_classes, d_pred, d_A, d_B, g, w.dA, w, st)) ||
-      (rc = bwd_bags_phase2_impl(p, nb, A, w.dA, w.tpart, w.G, Q, w.dL, w.dqm, w, st)) ||
+      (rc = bwd_bags_phase2_impl(p, nb, A, w.dA, w.tpart, w.plan ? 0 : w.G, Q, w.dL, w.dqm, w, st)) ||
       (rc = bwd_bags_phase3_impl(p, nb, total, Q, H1, w.dL, w.dqm, nullptr, crit, nullptr, g, w, &dz1, st)))
     return rc;
   if (g->gX) {
@@ -1185,16 +1185,15 @@ static int shard_bags_phase1_impl(const dsmil_params_t* p, const float* const* X
   return 0;
 }
 // Phase 2: merge the G ranks' candidates into q_max [nb,C,128] and crit_idx, attend on the local rows, and each bag's
-// partial record.
-static int shard_bags_phase2_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
-                                  const float* Q, bool q_blocked, const float* cands_all, int G, float* A,
-                                  int64_t* crit_idx, float* qmax, float* recs_out, const BagsWs& w, cudaStream_t st) {
-  std::vector<sm90::BagDev> tbl;
-  int tiles = 0, recs = 0, rc;
-  if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
+// partial record.  Attend runs one CTA per partial record: `recs` of them, or, with recs_dev, the first *recs_dev of a
+// capacity grid of `recs`.
+static int shard_bags_phase2_impl(const dsmil_params_t* p, int nb, const float* Q, bool q_blocked,
+                                  const float* cands_all, int G, float* A, int64_t* crit_idx, float* qmax,
+                                  float* recs_out, const BagsWs& w, int recs, const int* recs_dev, cudaStream_t st) {
+  int rc;
   k_merge_cand<<<dim3(p->C, nb), kQ, 0, st>>>(cands_all, G, nb, p->C, qmax, crit_idx);
   DSMIL_LAUNCH_OK("k_merge_cand");
-  sm90::AttendArgs aa{w.table, nb, p->D, p->C, Q, q_blocked, w.keys, A, w.recs, qmax, nullptr};
+  sm90::AttendArgs aa{w.table, nb, p->D, p->C, Q, q_blocked, w.keys, A, w.recs, qmax, recs_dev};
   if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
   sm90::FinalizeArgs fa{w.table, p->D, p->C, w.recs, w.keys, p->Wf, p->bf, A, nullptr, nullptr, nullptr,
                          w.pred_part, w.counters, recs_out, 0, 0};
@@ -1224,7 +1223,10 @@ int dsmil_shard_bags_phase2(const dsmil_params_t* p, const float* const* Xs, con
   bool ok;
   BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
-  return shard_bags_phase2_impl(p, Xs, Ns, nb, w.Q, true, cands_all, G, A, crit_idx, w.qmax, recs_out, w,
+  std::vector<sm90::BagDev> tbl;
+  int tiles, recs;
+  if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
+  return shard_bags_phase2_impl(p, nb, w.Q, true, cands_all, G, A, crit_idx, w.qmax, recs_out, w, recs, nullptr,
                                 static_cast<cudaStream_t>(stream));
 }
 int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
@@ -1350,7 +1352,10 @@ int dsmil_shard_bags_phase2_train(const dsmil_params_t* p, const float* const* X
   bool ok;
   BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
-  return shard_bags_phase2_impl(p, Xs, Ns, nb, Q, false, cands_all, G, A, crit_idx, q_max, recs_out, w,
+  std::vector<sm90::BagDev> tbl;
+  int tiles, recs;
+  if ((rc = build_table(Xs, Ns, nb, tbl, &tiles, &recs))) return rc;   // the device table was written by phase 1
+  return shard_bags_phase2_impl(p, nb, Q, false, cands_all, G, A, crit_idx, q_max, recs_out, w, recs, nullptr,
                                 static_cast<cudaStream_t>(stream));
 }
 
@@ -1428,16 +1433,16 @@ int dsmil_shard_backward_bags_phase3(const dsmil_params_t* p, const float* const
 
 
 // ---- capture-safe batched training: the bag list in device memory, every launch sized for a capacity -------------
-// What both dev calls check: the batched tensor-core shapes, the bag list, 1 <= nb <= 65535 and a row capacity whose
-// 128-row tiles the kernels can number (an int).
-static int check_bags_dev(const dsmil_params_t* p, bool need_scores, const float* const* Xs, const int64_t* Ns, int nb,
-                          int64_t max_rows, const int32_t* status) {
+// What every dev call checks: the batched tensor-core shapes, the bag list and status (need_list: the calls that run
+// the planner), 1 <= nb <= 65535 and a row capacity whose 128-row tiles the kernels can number (an int).
+static int check_bags_dev(const dsmil_params_t* p, bool need_scores, bool need_list, const float* const* Xs,
+                          const int64_t* Ns, int nb, int64_t max_rows, const int32_t* status) {
   int rc = check_params(p, need_scores);
   if (rc) return rc;
   DSMIL_REQUIRE(dsmil_shard_bags_supported(p),
                 "shape not supported by the batched tensor-core path (D=%d, C=%d, nonlinear=%d, passing_v=%d)", p->D,
                 p->C, p->nonlinear, p->passing_v);
-  DSMIL_REQUIRE(Xs && Ns && status, "NULL bag list or status");
+  DSMIL_REQUIRE(!need_list || (Xs && Ns && status), "NULL bag list or status");
   DSMIL_REQUIRE(nb >= 1 && nb <= 65535, "nb=%d outside [1, 65535]", nb);
   DSMIL_REQUIRE(max_rows >= 1 && max_rows < 0xffffffffll &&
                 static_cast<int64_t>(nb) * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) <= INT_MAX,
@@ -1445,12 +1450,12 @@ static int check_bags_dev(const dsmil_params_t* p, bool need_scores, const float
   return 0;
 }
 
-// The forward's carve for nb bags of max_rows rows (Q and H1 are the caller's), then the planner's BagsPlan and the
-// zero row of a refused batch.
-static BagsWs carve_bags_dev(const dsmil_params_t* p, int nb, int64_t max_rows, void* ws, size_t cap, bool* ok,
-                             BagsPlan** plan, float** zero_row) {
+// The forward's carve for nb bags of max_rows rows (Q and H1 are the caller's; `sharded` adds the row offsets and
+// q_max of the row-sharded batch), then the planner's BagsPlan and the zero row of a refused batch.
+static BagsWs carve_bags_dev(const dsmil_params_t* p, int nb, int64_t max_rows, bool sharded, void* ws, size_t cap,
+                             bool* ok, BagsPlan** plan, float** zero_row) {
   const std::vector<int64_t> Ns(nb, max_rows);
-  BagsWs w = carve_bags(p, Ns.data(), nb, false, false, ws, cap, ok);
+  BagsWs w = carve_bags(p, Ns.data(), nb, false, sharded, ws, cap, ok);
   Carver c(ws, cap);
   c.off = w.bytes;
   *plan = c.take<BagsPlan>(1);
@@ -1460,12 +1465,23 @@ static BagsWs carve_bags_dev(const dsmil_params_t* p, int nb, int64_t max_rows, 
   return w;
 }
 
+// bags_phase1_impl's launches in a dev call, on the planner's table (k_qmlp_sm90 on the capacity grid of 128-row
+// tiles), with the weight images rebuilt on every call: a replayed graph sees the weights of the last optimizer step.
+static int bags_phase1_dev(const dsmil_params_t* p, const BagsWs& w, const BagsPlan* plan, int nb, int64_t max_rows,
+                           float* classes, float* Q, float* H1, cudaStream_t st) {
+  int rc;
+  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
+  if ((rc = sm90::launch_prep_wimg(p, w.wimg, st))) return rc;
+  return sm90::launch_qmlp(p, w.table, nb, nb * tiles_for_bag(max_rows), classes, w.keys, Q, H1, w.wimg, num_sms(), st,
+                           false, &plan->tiles);
+}
+
 size_t dsmil_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
   if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
   bool ok;
   BagsPlan* plan;
   float* zero_row;
-  const size_t dev = carve_bags_dev(p, nb, max_rows, nullptr, 0, &ok, &plan, &zero_row).bytes;
+  const size_t dev = carve_bags_dev(p, nb, max_rows, false, nullptr, 0, &ok, &plan, &zero_row).bytes;
   // never below the eager call's size for the same capacity: one buffer serves both forms
   const std::vector<int64_t> Ns(nb, max_rows);
   return std::max(dev, dsmil_forward_bags_train_workspace_bytes(p, Ns.data(), nb));
@@ -1475,7 +1491,7 @@ int dsmil_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs
                                  int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
                                  int64_t* crit_idx, float* save_Q, float* save_H1, int32_t* status, void* workspace,
                                  size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  int rc = check_bags_dev(p, true, true, Xs_dev, Ns_dev, nb, max_rows, status);
   if (rc) return rc;
   DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && save_H1, "NULL output pointer");
   const size_t need = dsmil_forward_bags_train_dev_workspace_bytes(p, nb, max_rows);
@@ -1484,17 +1500,11 @@ int dsmil_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs
   bool ok;
   BagsPlan* plan;
   float* zero_row;
-  BagsWs w = carve_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok, &plan, &zero_row);
+  BagsWs w = carve_bags_dev(p, nb, max_rows, false, workspace, workspace_bytes, &ok, &plan, &zero_row);
   k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, zero_row, w.table, nullptr, nullptr, plan,
-                                status);
+                                status, nullptr, nullptr);
   DSMIL_LAUNCH_OK("k_plan_bags");
-  // bags_phase1_impl's launches, on the planner's table and with the weight images rebuilt on every call (a replayed
-  // graph sees the weights of the last optimizer step)
-  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
-  if ((rc = sm90::launch_prep_wimg(p, w.wimg, st))) return rc;
-  if ((rc = sm90::launch_qmlp(p, w.table, nb, nb * tiles_for_bag(max_rows), classes, w.keys, save_Q, save_H1, w.wimg,
-                              num_sms(), st, false, &plan->tiles)))
-    return rc;
+  if ((rc = bags_phase1_dev(p, w, plan, nb, max_rows, classes, save_Q, save_H1, st))) return rc;
   return bags_attend_finalize(p, w, nb, save_Q, false, pred, A, B, crit_idx, nb * recs_for_bag(max_rows), &plan->recs,
                               st);
 }
@@ -1510,7 +1520,7 @@ int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev,
                             const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
                             const float* d_B, const dsmil_grads_t* grads, int32_t* status, void* workspace,
                             size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, false, Xs_dev, Ns_dev, nb, max_rows, status);
+  int rc = check_bags_dev(p, false, true, Xs_dev, Ns_dev, nb, max_rows, status);
   if (rc) return rc;
   DSMIL_REQUIRE(Q && H1 && A && B && crit_idx && grads, "NULL pointer");
   DSMIL_REQUIRE(!d_A && !d_B && !grads->gX,
@@ -1521,10 +1531,162 @@ int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev,
   bool ok;
   BwdBagsWs w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
   k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, w.zero_row, w.table, w.chi, w.ch1, w.plan,
-                                status);
+                                status, nullptr, nullptr);
   DSMIL_LAUNCH_OK("k_plan_bags");
   return backward_bags_run(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, A, B, crit_idx,
                            d_classes, d_pred, nullptr, nullptr, grads, w, st);
+}
+
+// ---- capture-safe row-sharded batch training: the six calls of the sharded step in dev form -----------------------
+// As the dev pair above: the bag list (and the row offsets) in device memory, launches on capacity grids whose live
+// counts the planner writes, no host<->device traffic.  Forward phases 2 and 3 read phase 1's table and counts from the
+// forward workspace, backward phases 2 and 3 read backward phase 1's from the backward workspace.
+size_t dsmil_shard_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
+  bool ok;
+  BagsPlan* plan;
+  float* zero_row;
+  const size_t dev = carve_bags_dev(p, nb, max_rows, true, nullptr, 0, &ok, &plan, &zero_row).bytes;
+  const std::vector<int64_t> Ns(nb, max_rows);
+  return std::max(dev, dsmil_shard_bags_workspace_bytes(p, Ns.data(), nb));
+}
+
+// The forward workspace of a sharded dev call, after its checks.
+static int shard_bags_dev_ws(const dsmil_params_t* p, int nb, int64_t max_rows, void* workspace,
+                             size_t workspace_bytes, BagsWs* w, BagsPlan** plan, float** zero_row) {
+  const size_t need = dsmil_shard_bags_train_dev_workspace_bytes(p, nb, max_rows);
+  int rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0);
+  if (rc) return rc;
+  bool ok;
+  *w = carve_bags_dev(p, nb, max_rows, true, workspace, workspace_bytes, &ok, plan, zero_row);
+  return 0;
+}
+
+int dsmil_shard_bags_phase1_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                      const int64_t* row_offsets_dev, int32_t nb, int64_t max_rows, float* classes,
+                                      float* save_Q, float* save_H1, float* cand_recs, int32_t* status,
+                                      void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_bags_dev(p, true, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(row_offsets_dev && classes && save_Q && save_H1 && cand_recs, "NULL pointer");
+  BagsWs w;
+  BagsPlan* plan;
+  float* zero_row;
+  if ((rc = shard_bags_dev_ws(p, nb, max_rows, workspace, workspace_bytes, &w, &plan, &zero_row))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, zero_row, w.table, nullptr, nullptr, plan,
+                                status, row_offsets_dev, w.row_offsets);
+  DSMIL_LAUNCH_OK("k_plan_bags");
+  if ((rc = bags_phase1_dev(p, w, plan, nb, max_rows, classes, save_Q, save_H1, st))) return rc;
+  sm90::k_gather_cand_b<<<dim3(p->C, nb), kQ, 0, st>>>(w.table, w.keys, classes, save_Q, false, w.row_offsets, p->C,
+                                                        cand_recs);
+  DSMIL_LAUNCH_OK("k_gather_cand_b");
+  return 0;
+}
+
+int dsmil_shard_bags_phase2_train_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows, const float* Q,
+                                      const float* cands_all, int32_t G, float* A, int64_t* crit_idx, float* q_max,
+                                      float* recs_out, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_bags_dev(p, true, false, nullptr, nullptr, nb, max_rows, nullptr);
+  if (rc) return rc;
+  DSMIL_REQUIRE(Q && cands_all && G >= 1 && A && crit_idx && q_max && recs_out, "NULL pointer or G < 1");
+  BagsWs w;
+  BagsPlan* plan;
+  float* zero_row;
+  if ((rc = shard_bags_dev_ws(p, nb, max_rows, workspace, workspace_bytes, &w, &plan, &zero_row))) return rc;
+  return shard_bags_phase2_impl(p, nb, Q, false, cands_all, G, A, crit_idx, q_max, recs_out, w,
+                                nb * recs_for_bag(max_rows), &plan->recs, static_cast<cudaStream_t>(stream));
+}
+
+int dsmil_shard_bags_phase3_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows, const float* recs_all,
+                                int32_t G, float* A, float* B, float* pred, void* workspace, size_t workspace_bytes,
+                                void* stream) {
+  int rc = check_bags_dev(p, true, false, nullptr, nullptr, nb, max_rows, nullptr);
+  if (rc) return rc;
+  DSMIL_REQUIRE(recs_all && G >= 1 && G <= sm90::kMaxRecPerBag && A && B && pred, "NULL pointer or G out of range");
+  BagsWs w;
+  BagsPlan* plan;
+  float* zero_row;
+  if ((rc = shard_bags_dev_ws(p, nb, max_rows, workspace, workspace_bytes, &w, &plan, &zero_row))) return rc;
+  sm90::FinalizeArgs fa{w.table, p->D, p->C, recs_all, w.keys, p->Wf, p->bf, A, B, pred, nullptr,
+                         w.pred_part, w.counters, nullptr, G, nb};
+  return sm90::launch_finalize_b(fa, nb, static_cast<cudaStream_t>(stream));
+}
+
+size_t dsmil_shard_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
+  bool ok;
+  const size_t dev = carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
+  const std::vector<int64_t> Ns(nb, max_rows);
+  return std::max(dev, dsmil_shard_backward_bags_workspace_bytes(p, Ns.data(), nb));
+}
+
+// The backward workspace of a sharded dev call, after its checks.
+static int shard_bwd_bags_dev_ws(const dsmil_params_t* p, int nb, int64_t max_rows, void* workspace,
+                                 size_t workspace_bytes, BwdBagsWs* w) {
+  const size_t need = dsmil_shard_backward_bags_dev_workspace_bytes(p, nb, max_rows);
+  int rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0);
+  if (rc) return rc;
+  bool ok;
+  *w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
+  return 0;
+}
+
+int dsmil_shard_backward_bags_phase1_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                         int32_t nb, int64_t max_rows, const float* A, const float* B,
+                                         const float* d_classes_local, const float* d_pred, float* dA_local,
+                                         float* t_local, float* gWi, float* gbi, float* gWf, float* gbf,
+                                         int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_bags_dev(p, false, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(A && B && dA_local && t_local, "NULL tensor pointer");
+  BwdBagsWs w;
+  if ((rc = shard_bwd_bags_dev_ws(p, nb, max_rows, workspace, workspace_bytes, &w))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, w.zero_row, w.table, w.chi, w.ch1, w.plan,
+                                status, nullptr, nullptr);
+  DSMIL_LAUNCH_OK("k_plan_bags");
+  dsmil_grads_t g{};
+  g.gWi = gWi; g.gbi = gbi; g.gWf = gWf; g.gbf = gbf;
+  if ((rc = bwd_bags_phase1_impl(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, A, B, d_classes_local,
+                                 d_pred, nullptr, nullptr, &g, dA_local, w, st)))
+    return rc;
+  // t_local[b]: the live partials summed in the eager call's order
+  k_sum_segments<<<dim3(ceil_div(p->C, 256), nb), 256, 0, st>>>(w.tpart, w.G, p->C, t_local, &w.plan->G);
+  DSMIL_LAUNCH_OK("k_sum_segments");
+  return 0;
+}
+
+int dsmil_shard_backward_bags_phase2_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows, const float* A,
+                                         float* dA_to_dL, const float* t_global, const float* Q, float* dqm_local,
+                                         void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_bags_dev(p, false, false, nullptr, nullptr, nb, max_rows, nullptr);
+  if (rc) return rc;
+  DSMIL_REQUIRE(A && dA_to_dL && t_global && Q && dqm_local, "NULL tensor pointer");
+  BwdBagsWs w;
+  if ((rc = shard_bwd_bags_dev_ws(p, nb, max_rows, workspace, workspace_bytes, &w))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // the copy that lets dL replace dA (as the eager call), over the capacity rows: the live total is on the device
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.dA, dA_to_dL, sizeof(float) * nb * max_rows * p->C, cudaMemcpyDeviceToDevice, st));
+  return bwd_bags_phase2_impl(p, nb, A, w.dA, t_global, 1, Q, dA_to_dL, dqm_local, w, st);
+}
+
+int dsmil_shard_backward_bags_phase3_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows,
+                                         const int64_t* row_offsets_dev, const float* Q, const float* H1,
+                                         const float* dL_local, const float* dqm_global, const float* q_max,
+                                         const int64_t* crit_idx, float* gW1, float* gb1, float* gW2, float* gb2,
+                                         void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_bags_dev(p, false, false, nullptr, nullptr, nb, max_rows, nullptr);
+  if (rc) return rc;
+  DSMIL_REQUIRE(row_offsets_dev && Q && H1 && dL_local && dqm_global && q_max && crit_idx, "NULL tensor pointer");
+  BwdBagsWs w;
+  if ((rc = shard_bwd_bags_dev_ws(p, nb, max_rows, workspace, workspace_bytes, &w))) return rc;
+  dsmil_grads_t g{};
+  g.gW1 = gW1; g.gb1 = gb1; g.gW2 = gW2; g.gb2 = gb2;
+  const float* dz1;
+  return bwd_bags_phase3_impl(p, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, dL_local, dqm_global, q_max, crit_idx,
+                              reinterpret_cast<const long long*>(row_offsets_dev), &g, w, &dz1,
+                              static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -1,8 +1,8 @@
 // The integer plan of a batch of bags: the bag table's numbering, the batched backward's CTAs per bag and the chunking
 // of its ragged GEMMs.  The eager calls evaluate these formulas on the host from host arrays; the capture-safe calls
-// (dsmil_forward_bags_train_dev / dsmil_backward_bags_dev) evaluate the same functions on the device, in k_plan_bags,
-// from the bag list in device memory.  One definition for both, so the two cannot drift: a dev call gives the eager
-// call's bits.
+// (dsmil_forward_bags_train_dev / dsmil_backward_bags_dev and the dsmil_shard_*_dev calls) evaluate the same functions
+// on the device, in k_plan_bags, from the bag list in device memory.  One definition for both, so the two cannot drift:
+// a dev call gives the eager call's bits.
 #pragma once
 #include "common.cuh"
 #include "gemm_generic.cuh"
@@ -105,17 +105,22 @@ struct BagsPlan {
 // features that are NULL or not 16-byte aligned sets *status to 1 + its index (the first such bag; a set status is
 // never cleared here), and the call then runs on a stand-in batch instead: every bag becomes one row of zeros
 // (zero_row, D floats of the workspace).  Every output of a refused call is then finite and every index in range
-// (crit_idx 0, pred = bf, B = 0), and nothing reads the caller's bag list.
+// (crit_idx 0, pred = bf, B = 0), and nothing reads the caller's bag list.  A row-sharded batch also passes each bag's
+// first global row (offs_in, device memory): the planner copies it to offs_out, a negative offset is refused like a
+// bad bag, and a refused batch's offsets are 0.
 __global__ void __launch_bounds__(32)
 k_plan_bags(const float* const* __restrict__ Xs, const int64_t* __restrict__ Ns, int nb, long long max_rows, int C,
             int D, float* __restrict__ zero_row, sm90::BagDev* __restrict__ table, TnChunk* __restrict__ chi,
-            TnChunk* __restrict__ ch1, BagsPlan* __restrict__ plan, int* __restrict__ status) {
+            TnChunk* __restrict__ ch1, BagsPlan* __restrict__ plan, int* __restrict__ status,
+            const int64_t* __restrict__ offs_in, long long* __restrict__ offs_out) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   int bad = 0;
   long long mx = 0;
   for (int b = 0; b < nb && !bad; ++b) {
     const int64_t N = Ns[b];
-    if (N < 1 || N > max_rows || Xs[b] == nullptr || (reinterpret_cast<uintptr_t>(Xs[b]) & 15) != 0) bad = b + 1;
+    if (N < 1 || N > max_rows || Xs[b] == nullptr || (reinterpret_cast<uintptr_t>(Xs[b]) & 15) != 0 ||
+        (offs_in && offs_in[b] < 0))
+      bad = b + 1;
     mx = N > mx ? N : mx;
   }
   if (bad) {
@@ -127,6 +132,8 @@ k_plan_bags(const float* const* __restrict__ Xs, const int64_t* __restrict__ Ns,
   long long row = 0;
   int tile = 0, rec = 0;
   for (int b = 0; b < nb; ++b) table[b] = bad ? bag_entry(zero_row, 1, row, tile, rec) : bag_entry(Xs[b], Ns[b], row, tile, rec);
+  if (offs_out)
+    for (int b = 0; b < nb; ++b) offs_out[b] = bad ? 0 : offs_in[b];
   pl.total = row;
   pl.tiles = tile;
   pl.recs = rec;

@@ -102,8 +102,8 @@ k_bwd_rowdot_b(const sm90::BagDev* __restrict__ bags, int D, const float* __rest
 // (P partials per bag: the first pass's per-CTA shares, or P = 1 for a t that is already summed, e.g. all-reduced
 // over the ranks of a row-sharded batch):
 // dL[n,k] = A[n,k] (dA[n,k] - t_b[k]) / sqrt(128) for rows n = 2x + h, step 2*gridDim.x, of bag b, and the CTA's share
-// of dq_max_b = dL_b^T Q_b, [C,128], in dpart[b][x].  G_dev != NULL (one device, first-pass partials): G and P are
-// both *G_dev.
+// of dq_max_b = dL_b^T Q_b, [C,128], in dpart[b][x].  P == 0 (a dev call on one device, first-pass partials): P is
+// the live G.
 __global__ void __launch_bounds__(256)
 k_bwd_dL_b(const sm90::BagDev* __restrict__ bags, int C, const float* __restrict__ A, const float* __restrict__ dA,
            const float* __restrict__ tpart, int P, const float* __restrict__ Q, float* __restrict__ dL,
@@ -112,7 +112,7 @@ k_bwd_dL_b(const sm90::BagDev* __restrict__ bags, int C, const float* __restrict
   __shared__ float red[kMaxC][kQ];
   const int b = blockIdx.y, G = G_dev ? *G_dev : static_cast<int>(gridDim.x);
   if (static_cast<int>(blockIdx.x) >= G) return;
-  if (G_dev) P = G;
+  if (P == 0) P = G;
   if (threadIdx.x < C) {
     float s = 0.f;
     for (int x = 0; x < P; ++x) s += tpart[(static_cast<size_t>(b) * P + x) * C + threadIdx.x];

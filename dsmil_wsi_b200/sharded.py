@@ -14,7 +14,9 @@ CudaShardBagOps runs the batched ABI (dsmil_shard_bags_*): three library calls a
 and, for training (sharded_milnet_forward_bags + sharded_caller_loss_bags), three more calls and four more collectives
 (one all-reduce(max) in the loss, three all-reduce(sum) in the backward), whatever the number of bags.
 PerBagShardOps gives that interface to a one-bag ops object (CudaShardOps: the one-bag ABI, dsmil_shard_phase1/2/3,
-which also serves the shapes the batched ABI refuses) by running it one bag at a time.  The one-bag entry points
+which also serves the shapes the batched ABI refuses) by running it one bag at a time.  CudaShardBagDevOps gives the
+training interface to the capture-safe calls (dsmil_shard_*_dev), so train_graph.ShardedTrainStepGraph records the same
+host logic, collectives included, as one CUDA graph.  The one-bag entry points
 (sharded_forward, sharded_milnet_forward, sharded_caller_loss) are the batch step with nb = 1 over the one-bag ABI.
 The ops object is what the CPU tests replace: they run the same exchange/merge logic over gloo with an oracle-backed
 stand-in (the product default, CudaShardOps, has no fallback).
@@ -438,6 +440,124 @@ class PerBagShardOps:
                                         dqm.unbind(), qmax.unbind(), crit.unbind()))))
 
 
+class CudaShardBagDevOps:
+    """The training interface of CudaShardBagOps (begin, phase1-3_train, bwd1-3) over the capture-safe calls
+    (dsmil_shard_bags_*_dev, dsmil_shard_backward_bags_*_dev): every call only enqueues device work, so the sharded step
+    and its collectives can be recorded once in a CUDA graph and replayed over batches of new local sizes.
+
+    The batch is static: begin() takes [slots] (slots [nb, max_rows, D]: bag b's local rows are slots[b, :Ns[b]]) and
+    the row offsets [nb] int64 on the device; Ns [nb] int64 and status [1] int32 are device tensors given here.  The
+    packed per-row outputs have nb * max_rows rows, the live ones at the prefix sums of Ns.  A bag the planner refuses
+    sets status, and the step runs on the library's stand-in batch (see include/dsmil_b200.h)."""
+
+    def __init__(self, params: Sequence[Optional[torch.Tensor]], Ns: torch.Tensor, status: torch.Tensor):
+        self.lib = _lib.load()
+        self.P = Fn.ParamPack(*params)
+        self.device = self.P.device
+        if not self.lib.dsmil_shard_bags_supported(self.P.ref):
+            raise ValueError(f"the capture-safe sharded step runs on the batched tensor-core path only; D={self.P.D}, "
+                             f"C={self.P.C}, nonlinear={self.P.nonlinear}, passing_v={self.P.passing_v} is not on it")
+        self.Ns, self.status = Ns, status
+
+    def new(self, *shape, dtype=torch.float32):
+        return torch.empty(*shape, dtype=dtype, device=self.device)
+
+    def begin(self, X_locals: Sequence[torch.Tensor], row_offsets: torch.Tensor):
+        (slots,) = X_locals
+        P = self.P
+        if slots.dim() != 3 or slots.shape[2] != P.D or slots.dtype != torch.float32 or not slots.is_contiguous():
+            raise ValueError(f"slots must be contiguous float32 [nb, max_rows, {P.D}], got {tuple(slots.shape)}")
+        self.nb, self.max_rows = int(slots.shape[0]), int(slots.shape[1])
+        self.rows, self.offs = self.nb * self.max_rows, row_offsets
+        with torch.cuda.device(self.device):
+            self.xs = slots.data_ptr() + 4 * self.max_rows * P.D * torch.arange(self.nb, dtype=torch.int64,
+                                                                                 device=self.device)
+            self.ws = Fn._workspace(self.lib.dsmil_shard_bags_train_dev_workspace_bytes(P.ref, self.nb, self.max_rows),
+                                    self.device)
+        self.cand_f = int(self.lib.dsmil_cand_floats(P.C))
+        self.rec_f = int(self.lib.dsmil_rec_floats(P.C, P.D))
+        return [slots]
+
+    def phase1_train(self):
+        """(classes, Q, H1 [nb * max_rows, *], cand [nb, cand])."""
+        P = self.P
+        with torch.cuda.device(self.device):
+            classes, Q, H1 = self.new(self.rows, P.C), self.new(self.rows, Fn.Q_DIM), self.new(self.rows, Fn.Q_DIM)
+            cand = self.new(self.nb, self.cand_f)
+            rc = self.lib.dsmil_shard_bags_phase1_train_dev(P.ref, Fn._ptr(self.xs), Fn._ptr(self.Ns), Fn._ptr(self.offs),
+                                                            self.nb, self.max_rows, Fn._ptr(classes), Fn._ptr(Q),
+                                                            Fn._ptr(H1), Fn._ptr(cand), Fn._ptr(self.status),
+                                                            Fn._ptr(self.ws), self.ws.numel(), Fn._stream())
+            _lib.check(rc, "dsmil_shard_bags_phase1_train_dev")
+        return classes, Q, H1, cand
+
+    def phase2_train(self, Q: torch.Tensor, cands_all: torch.Tensor, G: int):
+        P = self.P
+        with torch.cuda.device(self.device):
+            A = self.new(self.rows, P.C)
+            crit = self.new(self.nb, P.C, dtype=torch.int64)
+            qmax = self.new(self.nb, P.C, Fn.Q_DIM)
+            recs = self.new(self.nb, self.rec_f)
+            rc = self.lib.dsmil_shard_bags_phase2_train_dev(P.ref, self.nb, self.max_rows, Fn._ptr(Q), Fn._ptr(cands_all),
+                                                            G, Fn._ptr(A), Fn._ptr(crit), Fn._ptr(qmax), Fn._ptr(recs),
+                                                            Fn._ptr(self.ws), self.ws.numel(), Fn._stream())
+            _lib.check(rc, "dsmil_shard_bags_phase2_train_dev")
+        return A, crit, qmax, recs
+
+    def phase3_train(self, recs_all: torch.Tensor, G: int, A: torch.Tensor):
+        P = self.P
+        with torch.cuda.device(self.device):
+            B, pred = self.new(self.nb, P.C, P.D), self.new(self.nb, P.C)
+            rc = self.lib.dsmil_shard_bags_phase3_dev(P.ref, self.nb, self.max_rows, Fn._ptr(recs_all), G, Fn._ptr(A),
+                                                      Fn._ptr(B), Fn._ptr(pred), Fn._ptr(self.ws), self.ws.numel(),
+                                                      Fn._stream())
+            _lib.check(rc, "dsmil_shard_bags_phase3_dev")
+        return A, B, pred
+
+    def bwd1(self, xs, A, B, d_classes, d_pred):
+        P = self.P
+        with torch.cuda.device(self.device):
+            self.bws = Fn._workspace(self.lib.dsmil_shard_backward_bags_dev_workspace_bytes(P.ref, self.nb, self.max_rows),
+                                     self.device)
+            dA, t = self.new(self.rows, P.C), self.new(self.nb, P.C)
+            gWi, gbi = self.new(P.C, P.D), self.new(P.C)
+            gWf, gbf = self.new(P.C, P.C, P.D), self.new(P.C)
+            dc = None if d_classes is None else d_classes.to(torch.float32).contiguous()
+            dp = None if d_pred is None else d_pred.to(torch.float32).contiguous()
+            rc = self.lib.dsmil_shard_backward_bags_phase1_dev(P.ref, Fn._ptr(self.xs), Fn._ptr(self.Ns), self.nb,
+                                                               self.max_rows, Fn._ptr(A), Fn._ptr(B.contiguous()),
+                                                               Fn._ptr(dc), Fn._ptr(dp), Fn._ptr(dA), Fn._ptr(t),
+                                                               Fn._ptr(gWi), Fn._ptr(gbi), Fn._ptr(gWf), Fn._ptr(gbf),
+                                                               Fn._ptr(self.status), Fn._ptr(self.bws), self.bws.numel(),
+                                                               Fn._stream())
+            _lib.check(rc, "dsmil_shard_backward_bags_phase1_dev")
+        return dA, t, gWi, gbi, gWf, gbf
+
+    def bwd2(self, xs, A, dA, t, Q):
+        P = self.P
+        with torch.cuda.device(self.device):
+            dqm = self.new(self.nb, P.C, Fn.Q_DIM)
+            rc = self.lib.dsmil_shard_backward_bags_phase2_dev(P.ref, self.nb, self.max_rows, Fn._ptr(A), Fn._ptr(dA),
+                                                               Fn._ptr(t.contiguous()), Fn._ptr(Q), Fn._ptr(dqm),
+                                                               Fn._ptr(self.bws), self.bws.numel(), Fn._stream())
+            _lib.check(rc, "dsmil_shard_backward_bags_phase2_dev")
+        return dA, dqm
+
+    def bwd3(self, xs, row_offsets, Q, H1, dL, dqm, qmax, crit):
+        P = self.P
+        with torch.cuda.device(self.device):
+            gW1, gb1 = self.new(Fn.Q_DIM, P.D), self.new(Fn.Q_DIM)
+            gW2, gb2 = self.new(Fn.Q_DIM, Fn.Q_DIM), self.new(Fn.Q_DIM)
+            rc = self.lib.dsmil_shard_backward_bags_phase3_dev(P.ref, self.nb, self.max_rows, Fn._ptr(row_offsets),
+                                                               Fn._ptr(Q), Fn._ptr(H1), Fn._ptr(dL),
+                                                               Fn._ptr(dqm.contiguous()), Fn._ptr(qmax.contiguous()),
+                                                               Fn._ptr(crit.contiguous()), Fn._ptr(gW1), Fn._ptr(gb1),
+                                                               Fn._ptr(gW2), Fn._ptr(gb2), Fn._ptr(self.bws),
+                                                               self.bws.numel(), Fn._stream())
+            _lib.check(rc, "dsmil_shard_backward_bags_phase3_dev")
+        return gW1, gb1, gW2, gb2
+
+
 @torch.no_grad()
 def sharded_forward_bags_batched(bops, X_locals, row_offsets, group=None):
     """The forward of a batch of row-sharded bags: 2 all-gathers per step, whatever the batch.  `bops` is a
@@ -557,7 +677,9 @@ class ShardBagsSaved:
     __slots__ = ("xs", "row_offsets", "Q", "H1", "A", "B", "qmax", "crit")
 
     def __init__(self, xs, row_offsets, Q, H1, A, B, qmax, crit):
-        self.xs, self.row_offsets, self.Q, self.H1 = list(xs), [int(o) for o in row_offsets], Q, H1
+        # a device tensor of offsets (CudaShardBagDevOps) stays on the device
+        offs = row_offsets if torch.is_tensor(row_offsets) else [int(o) for o in row_offsets]
+        self.xs, self.row_offsets, self.Q, self.H1 = list(xs), offs, Q, H1
         self.A, self.B, self.qmax, self.crit = A, B, qmax, crit
 
 
@@ -655,6 +777,26 @@ def sharded_max_prediction_bags(classes_local: torch.Tensor, crit: torch.Tensor,
     glob = torch.where(owned, mine.detach(), torch.full_like(mine, float("-inf")))
     dist.all_reduce(glob, op=dist.ReduceOp.MAX, group=group)
     return torch.where(owned, mine, glob)
+
+
+def sharded_max_prediction_bags_dev(classes_local: torch.Tensor, crit: torch.Tensor, row_offsets: torch.Tensor,
+                                    Ns: torch.Tensor, refused: torch.Tensor, group=None):
+    """sharded_max_prediction_bags with the local sizes Ns [nb] and the row offsets [nb] in device tensors (each bag's
+    first packed row is the prefix sum of Ns), for a step recorded in a CUDA graph.  `refused` (a device bool scalar:
+    this rank refused the batch) rides in the same all-reduce(max) as one extra float, so a step still makes one
+    collective here.  Returns (max_prediction [nb, C], refused on any rank: a device bool scalar); the values and
+    gradients are those of sharded_max_prediction_bags."""
+    import torch.distributed as dist
+    Ns = Ns.to(crit.device)
+    first = torch.cumsum(Ns, 0) - Ns
+    loc = crit - row_offsets[:, None]
+    owned = (loc >= 0) & (loc < Ns[:, None])
+    total = int(classes_local.shape[0])
+    mine = classes_local.gather(0, (first[:, None] + loc.clamp(min=0)).clamp(max=total - 1))
+    glob = torch.where(owned, mine.detach(), torch.full_like(mine, float("-inf")))
+    buf = torch.cat([glob.reshape(-1), refused.reshape(1).to(glob.dtype)])
+    dist.all_reduce(buf, op=dist.ReduceOp.MAX, group=group)
+    return torch.where(owned, mine, buf[:-1].view_as(mine)), buf[-1] > 0
 
 
 def sharded_caller_loss_bags(classes_local, prediction_bag, crit, row_offsets, labels, criterion, group=None, *, Ns):

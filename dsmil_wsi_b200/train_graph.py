@@ -1,4 +1,5 @@
-"""The minibatch training step recorded once as a CUDA graph and replayed over batches of ragged bags.
+"""The minibatch training step recorded once as a CUDA graph and replayed over batches of ragged bags, on one device
+(TrainStepGraph) or row-sharded over the ranks of a process group (ShardedTrainStepGraph).
 
 A k-bag step of feed.train_epoch(bags_per_step=k) costs a few milliseconds of host work: Python autograd, ctypes,
 workspace allocation, host-built bag tables and their uploads, the loss ops and the optimizer's launches.  Here the
@@ -84,6 +85,7 @@ class TrainStepGraph:
         self.labels = torch.zeros(nb, C, device=dev)
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
         self._step_status = torch.zeros(1, dtype=torch.int32, device=dev)   # this replay's planners
+        self._buffers(dev)
         snap = self._snapshot()
         side = torch.cuda.Stream(dev)
         side.wait_stream(torch.cuda.current_stream(dev))
@@ -102,18 +104,27 @@ class TrainStepGraph:
             self.loss = self._step(guard=True)
         self.status.zero_()
 
-    def _step(self, guard=False):
+    def _buffers(self, dev):
+        """Static buffers of a subclass's step beyond the slots, sizes, labels and status."""
+
+    def _params(self):
         ic, bc = self.milnet.i_classifier, self.milnet.b_classifier
         lin = ic._linear()
         W1, b1, W2, b2 = bc._q_params()
-        params = (lin.weight, lin.bias, W1, b1, W2, b2, None, None, bc.fcc.weight, bc.fcc.bias)
-        self._step_status.zero_()
-        classes, pred, _, _, crit = Fn.MILBagsDevFn.apply(self.slots, self.Ns, self._step_status, *params)
+        return (lin.weight, lin.bias, W1, b1, W2, b2, None, None, bc.fcc.weight, bc.fcc.bias)
+
+    def _loss(self):
+        """The recorded forward and minibatch loss: (loss, ok), ok a device bool that is false for a refused batch."""
+        classes, pred, _, _, crit = Fn.MILBagsDevFn.apply(self.slots, self.Ns, self._step_status, *self._params())
         ok = self._step_status[0] == 0
         n = self.Ns.clamp(0, self.max_rows)               # the live sizes (a refused batch's stay in range)
         first = torch.cumsum(n, 0) - n                    # each bag's first packed row
         mx = classes.gather(0, crit + first[:, None])     # the per-bag max instance, as feed._group_predictions
-        loss = feed.minibatch_loss(self.criterion, pred, mx, self.labels)
+        return feed.minibatch_loss(self.criterion, pred, mx, self.labels), ok
+
+    def _step(self, guard=False):
+        self._step_status.zero_()
+        loss, ok = self._loss()
         # a refused batch: NaN loss and no gradient (where's backward sends none to the unselected side)
         loss = torch.where(ok, loss, torch.full_like(loss, float("nan")))
         loss.backward()
@@ -157,3 +168,35 @@ class TrainStepGraph:
                         v.copy_(old[k]) if k in old else v.zero_()
                     elif k in old:
                         cur[k] = old[k]
+
+
+class ShardedTrainStepGraph(TrainStepGraph):
+    """TrainStepGraph for a minibatch of row-sharded bags: one recorded step per rank of `group` (default: the world),
+    replayed over batches of new local sizes.  The step is CudaShardBagDevOps under ShardedMILBagsFn (two all-gathers),
+    the minibatch loss with its all-reduce(max) (sharded_max_prediction_bags_dev), the backward (three all-reduce(sum))
+    and optimizer.step(): 6 collectives, as the eager sharded step.  Every rank builds the graph and replays it
+    collectively, in the same order.
+
+    Fill `slots[b, :n_b]` with this rank's rows of bag b, `Ns[b]` with n_b, `row_offsets[b]` with the global index of
+    its first row and `labels` [nb, C], then `step()`.  A local n_b outside 1..max_rows (or a negative offset) refuses
+    the batch on EVERY rank: this rank's flag rides in the loss's all-reduce(max), every rank's loss is NaN, and every
+    rank keeps its parameters and optimizer state, so the replicas stay equal.  `status` holds this rank's own first
+    refusal (1 + bag index), as in TrainStepGraph."""
+
+    def __init__(self, milnet, criterion, optimizer, nb: int, max_rows: int, group=None, warmup: int = 1):
+        self.group = group
+        super().__init__(milnet, criterion, optimizer, nb, max_rows, warmup)
+
+    def _buffers(self, dev):
+        self.row_offsets = torch.zeros(self.nb, dtype=torch.int64, device=dev)
+
+    def _loss(self):
+        from . import sharded
+        params = self._params()
+        ops = sharded.CudaShardBagDevOps(params, self.Ns, self._step_status)
+        classes, pred, _, _, crit = sharded.ShardedMILBagsFn.apply(ops, self.row_offsets, self.group, 1, self.slots,
+                                                                   *params)
+        mx, refused = sharded.sharded_max_prediction_bags_dev(classes, crit, self.row_offsets,
+                                                              self.Ns.clamp(0, self.max_rows),
+                                                              self._step_status[0] != 0, self.group)
+        return feed.minibatch_loss(self.criterion, pred, mx, self.labels), ~refused

@@ -338,6 +338,49 @@ int dsmil_shard_backward_bags_phase3(const dsmil_params_t* p, const float* const
                                      float* gW1, float* gb1, float* gW2, float* gb2, void* workspace,
                                      size_t workspace_bytes, void* stream);
 
+/* Capture-safe forms of the six row-sharded batch training calls above, for a sharded step recorded once as a CUDA
+ * graph (with its collectives) and replayed over batches of different local bag sizes.  The rules of
+ * dsmil_forward_bags_train_dev / dsmil_backward_bags_dev hold: the bag list (Xs_dev, Ns_dev: this rank's local rows)
+ * and the row offsets are in DEVICE memory; max_rows is the per-bag capacity of this rank's local rows, and the packed
+ * per-row buffers (classes, save_Q, save_H1, A, dA_local / dL_local, d_classes_local) are sized for nb * max_rows rows
+ * with the live rows at the live prefix sums; each call only enqueues work on `stream`.  The planner runs in forward
+ * phase 1 and backward phase 1: a bag with a local N outside [1, max_rows], features that are NULL or not 16-byte
+ * aligned, or a negative row offset sets *status to 1 + the first such bag's index, and the step then runs on the
+ * stand-in batch of one-row zero bags (offsets 0).  The other rank(s) see nothing of it: a caller that must refuse the
+ * batch everywhere reduces the flag itself (dsmil_wsi_b200.sharded folds it into the loss's all-reduce(max)).
+ *   forward:  dsmil_shard_bags_phase1_train_dev -> phase2_train_dev -> phase3_dev, one workspace of
+ *             dsmil_shard_bags_train_dev_workspace_bytes for the three (phases 2 and 3 read phase 1's table from it)
+ *   backward: dsmil_shard_backward_bags_phase1_dev -> phase2_dev -> phase3_dev, one workspace of
+ *             dsmil_shard_backward_bags_dev_workspace_bytes; phase 3 reads the row offsets from row_offsets_dev
+ * Exchanged buffers have the eager calls' fixed sizes for a given nb.  On the same bags each call gives the eager
+ * call's bits.  1 <= nb <= 65535; a short workspace is DSMIL_ERR_WORKSPACE.  The workspace sizes depend on
+ * (nb, max_rows) only and are never below the eager calls' for nb bags of max_rows rows. */
+size_t dsmil_shard_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_shard_bags_phase1_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                      const int64_t* row_offsets_dev, int32_t nb, int64_t max_rows, float* classes,
+                                      float* save_Q, float* save_H1, float* cand_recs, int32_t* status,
+                                      void* workspace, size_t workspace_bytes, void* stream);
+int dsmil_shard_bags_phase2_train_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows, const float* Q,
+                                      const float* cands_all, int32_t G, float* A, int64_t* crit_idx, float* q_max,
+                                      float* recs_out, void* workspace, size_t workspace_bytes, void* stream);
+int dsmil_shard_bags_phase3_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows, const float* recs_all,
+                                int32_t G, float* A, float* B, float* pred, void* workspace, size_t workspace_bytes,
+                                void* stream);
+size_t dsmil_shard_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_shard_backward_bags_phase1_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                         int32_t nb, int64_t max_rows, const float* A, const float* B,
+                                         const float* d_classes_local, const float* d_pred, float* dA_local,
+                                         float* t_local, float* gWi, float* gbi, float* gWf, float* gbf,
+                                         int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+int dsmil_shard_backward_bags_phase2_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows, const float* A,
+                                         float* dA_to_dL, const float* t_global, const float* Q, float* dqm_local,
+                                         void* workspace, size_t workspace_bytes, void* stream);
+int dsmil_shard_backward_bags_phase3_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows,
+                                         const int64_t* row_offsets_dev, const float* Q, const float* H1,
+                                         const float* dL_local, const float* dqm_global, const float* q_max,
+                                         const int64_t* crit_idx, float* gW1, float* gb1, float* gW2, float* gb2,
+                                         void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
