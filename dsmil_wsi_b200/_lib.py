@@ -54,6 +54,7 @@ SIGNATURES = {
     "dsmil_forward_bags": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(C.c_void_p), C.POINTER(c_i64), C.c_int32,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_forward_bags_phase1_ctas": (C.c_int32, [c_i64]),
     "dsmil_instance_scores": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, c_i64, C.c_void_p, C.c_void_p]),
     "dsmil_instance_scores_backward": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, c_i64, C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,

@@ -37,24 +37,35 @@ def _digest():
     return h.hexdigest()
 
 
+def _compile(out, verbose=False, defines=()):
+    cmd = [_nvcc(), "-O3", "-std=c++17", "-lineinfo", *ARCH, "-shared", "-Xcompiler", "-fPIC,-O3",
+           "-Xptxas", "-v" if verbose else "-O3", *[f"-D{d}" for d in defines],
+           "-I", os.path.join(HERE, "..", "include"), "-o", out] + [os.path.join(CSRC, s) for s in SOURCES]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(r.stdout + r.stderr)
+        raise RuntimeError(f"nvcc failed building {out}")
+    if verbose:
+        sys.stderr.write(r.stdout + r.stderr)
+    return out
+
+
 def build_library(force=False, verbose=False):
     os.makedirs(LIBDIR, exist_ok=True)
     stamp = os.path.join(LIBDIR, ".build_digest")
     dig = _digest()
     if not force and os.path.exists(LIB) and os.path.exists(stamp) and open(stamp).read() == dig:
         return LIB
-    cmd = [_nvcc(), "-O3", "-std=c++17", "-lineinfo", *ARCH, "-shared", "-Xcompiler", "-fPIC,-O3",
-           "-Xptxas", "-v" if verbose else "-O3",
-           "-I", os.path.join(HERE, "..", "include"), "-o", LIB] + [os.path.join(CSRC, s) for s in SOURCES]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(r.stdout + r.stderr)
-        raise RuntimeError("nvcc failed building libdsmil_b200.so")
-    if verbose:
-        sys.stderr.write(r.stdout + r.stderr)
+    _compile(LIB, verbose)
     with open(stamp, "w") as f:
         f.write(dig)
     return LIB
+
+
+def build_variant(out, defines):
+    """A build of the same sources with extra preprocessor definitions at `out` (tuning sweeps in tools/; load it
+    through DSMIL_B200_LIBPATH).  The in-tree library is left as it is."""
+    return _compile(out, defines=defines)
 
 
 def _host_digest():

@@ -156,14 +156,16 @@ static int num_sms() {
 // ---- tensor-core phase 1 (k_qmlp_sm90) of nb bags: the single-bag, batched and sharded forwards share it ----------
 struct Phase1Ws {
   sm90::BagDev* table;       // [nb]
-  unsigned long long* keys;  // [nb][kMaxC] arg-max keys, then nb finalize arrival counters: one memset zeroes both
-  unsigned int* counters;
+  unsigned long long* keys;  // [nb][kMaxC] arg-max keys, then the nb finalize arrival counters and the nb phase-1
+  unsigned int* counters;    // tile counts (one 8-byte slot per bag holds both): one memset per call zeroes all three
+  unsigned int* done;
   uint8_t* wimg;             // bf16 weight images, 1024-byte aligned; NULL on shapes k_qmlp_sm90 does not take
 };
 static void carve_phase1(Carver& c, const dsmil_params_t* p, int nb, Phase1Ws& w) {
   w.table = c.take<sm90::BagDev>(nb);
   w.keys = c.take<unsigned long long>(static_cast<size_t>(nb) * (kMaxC + 1));
   w.counters = reinterpret_cast<unsigned int*>(w.keys ? w.keys + static_cast<size_t>(nb) * kMaxC : nullptr);
+  w.done = w.counters ? w.counters + nb : nullptr;
   w.wimg = nullptr;
   if (sm90::qmlp_supported(p)) {
     const uintptr_t img = reinterpret_cast<uintptr_t>(c.take<uint8_t>(sm90::wimg_bytes(p->D) + 1024));
@@ -188,12 +190,27 @@ static int build_table(const float* const* Xs, const int64_t* Ns, int nb, std::v
   return 0;
 }
 
+// SMs the overlapped phase 1 leaves to the attend pass (forward_bags_impl).  H100 80GB HBM3 at a 700 W limit, 16 bags
+// x 10 000 x 512, C = 2, best of three ms per step: 0 -> 0.335, 8 -> 0.329, 16 -> 0.326, 24 -> 0.322, 32 -> 0.310,
+// 40 -> 0.301, 48 -> 0.315; the plain launch 0.365 (DESIGN §4.2, profiles/h100_fwd_overlap_1gpu.json).  A macro so
+// that tools/bench_fwd_overlap.py can build the sweep's variants; the library is built with the default.
+#ifndef DSMIL_PHASE1_RESERVE
+#define DSMIL_PHASE1_RESERVE 40
+#endif
+constexpr int kPhase1Reserve = DSMIL_PHASE1_RESERVE;
+static int overlap_phase1_ctas(int64_t tiles) {
+  const int ctas = std::max(num_sms() - kPhase1Reserve, 1);
+  return static_cast<int>(std::min<int64_t>(tiles, ctas));
+}
+
 // Scores (or, single bag only, the arg-max of the given scores classes_in), arg-max keys and Q (+ H1 when non-NULL)
 // of the nb bags; *tiles and *recs return the batch's 128-row tiles and partial records.  upload == false leaves the
 // table and the weight images as an earlier call with the same arguments wrote them into the same workspace.
+// overlap: phase 1 runs on overlap_phase1_ctas CTAs and counts each bag's finished tiles into w.done, for a
+// k_attend_b launched right after it with the same counters.
 static int bags_phase1_impl(const dsmil_params_t* p, const Phase1Ws& w, const float* const* Xs, const int64_t* Ns,
                             int nb, const float* classes_in, float* classes, float* Q, float* H1, bool q_blocked,
-                            bool upload, int* tiles, int* recs, cudaStream_t st) {
+                            bool upload, int* tiles, int* recs, cudaStream_t st, bool overlap = false) {
   std::vector<sm90::BagDev> tbl;
   int rc;
   if ((rc = build_table(Xs, Ns, nb, tbl, tiles, recs))) return rc;
@@ -206,8 +223,9 @@ static int bags_phase1_impl(const dsmil_params_t* p, const Phase1Ws& w, const fl
     k_argmax<<<grid, 256, 0, st>>>(classes_in, Ns[0], p->C, w.keys);
     DSMIL_LAUNCH_OK("k_argmax");
   }
-  return sm90::launch_qmlp(p, w.table, nb, *tiles, classes_in ? nullptr : classes, w.keys, Q, H1, w.wimg, num_sms(),
-                           st, q_blocked);
+  return sm90::launch_qmlp(p, w.table, nb, *tiles, classes_in ? nullptr : classes, w.keys, Q, H1, w.wimg,
+                           overlap ? overlap_phase1_ctas(*tiles) : num_sms(), st, q_blocked, nullptr,
+                           overlap ? w.done : nullptr);
 }
 
 struct FwdWs : Phase1Ws {
@@ -432,13 +450,15 @@ static BagsWs carve_bags(const dsmil_params_t* p, const int64_t* Ns, int nb, boo
 }
 
 // Phases 2 and 3 of the batched forward: attend (one CTA per partial record: `recs` of them, or, with recs_dev, the
-// first *recs_dev of a capacity grid of `recs`), then each bag's A, B, logits and critical rows.
+// first *recs_dev of a capacity grid of `recs`), then each bag's A, B, logits and critical rows.  overlap: the
+// attend pass is a programmatic dependent of the phase 1 that bags_phase1_impl(overlap) has just launched.
 static int bags_attend_finalize(const dsmil_params_t* p, const BagsWs& w, int nb, const float* Q, bool q_blocked,
                                 float* pred, float* A, float* B, int64_t* crit, int recs, const int* recs_dev,
-                                cudaStream_t st) {
+                                cudaStream_t st, bool overlap = false) {
   const int C = p->C, D = p->D;
   int rc;
-  sm90::AttendArgs aa{w.table, nb, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr, recs_dev};
+  sm90::AttendArgs aa{w.table, nb, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr, recs_dev,
+                      overlap ? w.done : nullptr};
   if ((rc = sm90::launch_attend_b(aa, recs, st))) return rc;
   sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, p->Wf, p->bf, A, B, pred, reinterpret_cast<long long*>(crit),
                          w.pred_part, w.counters, nullptr, 0, 0};
@@ -455,10 +475,15 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
   if (rc) return rc;
   float* Q = save_Q ? save_Q : w.Q;
   const bool q_blocked = save_Q == nullptr;   // training keeps Q (after tanh) row-major for the backward kernels
+  // The attend pass starts on each bag as soon as phase 1 has finished it, while the bag is still in L2 (DESIGN §4.2).
+  // Same bits either way.  Not under stream capture, and not while kernels are being timed: the event between the two
+  // launches would break the programmatic edge.
+  const bool overlap = !g_prof_on && !stream_is_capturing(st);
   int tiles, recs;
-  if ((rc = bags_phase1_impl(p, w, Xs, Ns, nb, classes_in, classes, Q, save_H1, q_blocked, true, &tiles, &recs, st)))
+  if ((rc = bags_phase1_impl(p, w, Xs, Ns, nb, classes_in, classes, Q, save_H1, q_blocked, true, &tiles, &recs, st,
+                             overlap)))
     return rc;
-  return bags_attend_finalize(p, w, nb, Q, q_blocked, pred, A, B, crit, recs, nullptr, st);
+  return bags_attend_finalize(p, w, nb, Q, q_blocked, pred, A, B, crit, recs, nullptr, st, overlap);
 }
 
 }  // namespace dsmil
@@ -630,6 +655,8 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
   }
   return 0;
 }
+int32_t dsmil_forward_bags_phase1_ctas(int64_t tiles) { return tiles < 1 ? 0 : overlap_phase1_ctas(tiles); }
+
 size_t dsmil_shard_workspace_bytes(const dsmil_params_t* p, int64_t N_local) {
   return dsmil_forward_workspace_bytes(p, N_local);
 }

@@ -26,7 +26,14 @@ struct AttendArgs {
   float* recs;              // [total records][rec_floats(C,D)]
   const float* qmax_ext;    // sharded: [nbags][C][128] merged critical queries (NULL: gather from Q via keys)
   const int* nrec_dev;      // dev calls: the live record count of a capacity grid (NULL: one CTA per record)
+  const unsigned int* done; // overlapped launch: [nbags] phase-1 tile releases (QmlpArgs::done); NULL: phase 1 is complete
 };
+
+__device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* p) {
+  unsigned int v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
 
 // CT = classes rounded up to 1,2,4; NJ = float4 column groups per thread (D <= 512*NJ)
 // Occupancy: the D <= 512, C <= 2 instantiations fit 48 registers without spills, i.e. 5 CTAs per SM instead of 4.
@@ -51,6 +58,23 @@ k_attend_b(const AttendArgs a) {
   const int cta_in_bag = rec - bg.rec_off;
   const int ntiles = static_cast<int>((bg.N + kAttRows - 1) / kAttRows);
 
+  // Overlapped with phase 1: wait until both consumer warpgroups have released every tile of this bag.  The phase-1
+  // CTAs are all resident before this grid is scheduled (they trigger at their start), and their tiles wait on
+  // nothing, so the count always gets there.  Q and the keys are then read with coherent (L2) loads: they were
+  // written by a grid that may still be running, which the read-only path does not cover.
+  if (a.done != nullptr) {
+    if (tid == 0) {
+      const unsigned int target = 2u * static_cast<unsigned int>(ntiles);
+      unsigned int ns = 64, spins = 0;
+      while (ld_acquire_gpu(a.done + bag) < target) {
+        __nanosleep(ns);
+        if (ns < 1024) ns *= 2;
+        if (++spins > (1u << 24)) __trap();   // seconds: a protocol bug must not hang the GPU
+      }
+    }
+    __syncthreads();
+  }
+
   // q_max rows (dsmil.py:53-54: the critical instances' queries; here gathered from Q, same bits)
   for (int i = tid; i < CT * kQ; i += 256) {
     const int k = i / kQ, j = i % kQ;
@@ -58,9 +82,9 @@ k_attend_b(const AttendArgs a) {
     if (k < C && a.qmax_ext != nullptr) {
       v = a.qmax_ext[(static_cast<size_t>(bag) * C + k) * kQ + j];
     } else if (k < C) {
-      const long long row = key_row(a.keys[static_cast<size_t>(bag) * kMaxC + k]);
-      v = a.q_blocked ? tanh_ex2(a.Q[static_cast<size_t>(bg.tile_off + row / kAttRows) * (kAttRows * kQ) + j * kAttRows + (row % kAttRows)])
-                      : a.Q[(bg.row_off + row) * kQ + j];
+      const long long row = key_row(__ldcg(a.keys + static_cast<size_t>(bag) * kMaxC + k));
+      v = a.q_blocked ? tanh_ex2(__ldcg(a.Q + static_cast<size_t>(bg.tile_off + row / kAttRows) * (kAttRows * kQ) + j * kAttRows + (row % kAttRows)))
+                      : __ldcg(a.Q + (bg.row_off + row) * kQ + j);
     }
     sq[k][j] = v;
   }
@@ -97,8 +121,8 @@ k_attend_b(const AttendArgs a) {
         // one base pointer per step: the four loads issue together with immediate offsets
         const float* qc = qb + c * kAttRows;
         // the tanh of dsmil.py:31, deferred from the phase-1 epilogue
-        const f2 ta = fast_tanh2(f2{__ldg(qc), __ldg(qc + kAttRows)});
-        const f2 tb = fast_tanh2(f2{__ldg(qc + 2 * kAttRows), __ldg(qc + 3 * kAttRows)});
+        const f2 ta = fast_tanh2(f2{__ldcg(qc), __ldcg(qc + kAttRows)});
+        const f2 tb = fast_tanh2(f2{__ldcg(qc + 2 * kAttRows), __ldcg(qc + 3 * kAttRows)});
 #pragma unroll
         for (int k = 0; k < CT; ++k) {
           const float4 w = *reinterpret_cast<const float4*>(&sq[k][hf * 64 + c]);
@@ -123,7 +147,7 @@ k_attend_b(const AttendArgs a) {
       for (int rr = 0; rr < 16; ++rr) {
         const int r = warp * 16 + rr;
         if (r < rows) {
-          const float4 q = __ldg(reinterpret_cast<const float4*>(a.Q + (bg.row_off + r0 + r) * kQ) + lane);
+          const float4 q = __ldcg(reinterpret_cast<const float4*>(a.Q + (bg.row_off + r0 + r) * kQ) + lane);
 #pragma unroll
           for (int k = 0; k < CT; ++k) {
             const float4 w = *reinterpret_cast<const float4*>(&sq[k][lane * 4]);
@@ -244,6 +268,9 @@ k_attend_b(const AttendArgs a) {
     for (int k = 0; k < CT; ++k)
       if (k < C) { recp[k] = run_m[k]; recp[C + k] = run_s[k]; }
   }
+  // Overlapped: the last bag's CTAs end only once the phase-1 grid has completed, so this grid's completion -- what
+  // k_finalize_b and later work on the stream are ordered after -- implies phase 1's.  They run last: the wait is short.
+  if (a.done != nullptr && bag == a.nb - 1) asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
 struct FinalizeArgs {
@@ -422,6 +449,8 @@ inline bool batched_supported(const dsmil_params_t* p) {
          ((p->C <= 2) || p->D <= 1024);
 }
 
+// a.done != NULL: launched as a programmatic dependent of the phase-1 kernel just before it on the stream (which must
+// have been given the same counters), so that it can start on the bags phase 1 has finished.
 inline int launch_attend_b(const AttendArgs& a, int nrecs, cudaStream_t st) {
   const int C = a.C, D = a.D;
   const size_t smem = sizeof(float) * C * D;
@@ -430,7 +459,21 @@ inline int launch_attend_b(const AttendArgs& a, int nrecs, cudaStream_t st) {
     if (smem > 48 * 1024)
       DSMIL_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     prof_begin(PROF_ATTEND, st);
-    kern<<<nrecs, 256, smem, st>>>(a);
+    if (a.done != nullptr) {
+      cudaLaunchConfig_t cfg = {};
+      cfg.gridDim = dim3(nrecs);
+      cfg.blockDim = dim3(256);
+      cfg.dynamicSmemBytes = smem;
+      cfg.stream = st;
+      cudaLaunchAttribute attr[1];
+      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+      attr[0].val.programmaticStreamSerializationAllowed = 1;
+      cfg.attrs = attr;
+      cfg.numAttrs = 1;
+      DSMIL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, a));
+    } else {
+      kern<<<nrecs, 256, smem, st>>>(a);
+    }
     prof_end(PROF_ATTEND, st);
     DSMIL_LAUNCH_OK("k_attend_b");
     return 0;

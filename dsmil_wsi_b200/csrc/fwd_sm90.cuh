@@ -166,6 +166,8 @@ struct QmlpArgs {
   bool q_blocked;         // Q in tile blocks of the PRE-activation z2 = acc + b2 (inference path): the tanh moves to
                           // the readers of Q (k_attend_b, k_gather_cand_b).  false: row-major tanh(z2)
   const int* ntiles_dev;  // dev calls: the live tile count (ntiles is then the capacity); NULL: ntiles
+  unsigned int* done;     // [nb] or NULL: each consumer warpgroup adds 1 to its bag's count once its half of a tile
+                          // (scores, key, Q, H1) is in global memory -- k_attend_b waits for 2 x tiles of the bag
 };
 
 // Walks the bag table as a role's tile index increases monotonically.
@@ -206,6 +208,8 @@ k_qmlp_sm90(const QmlpArgs a) {
   __shared__ __align__(8) uint64_t bars[2 * kWStages];
   __shared__ __align__(16) float s_b1[kQ], s_b2[kQ];
   __shared__ BagDev s_bags[kSmemBags];           // the bag table (tile-boundary lookups)
+  // a dependent attend grid may be scheduled as soon as every CTA of this grid is resident: it waits per bag on a.done
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int D = DT ? DT : a.D, C = a.C;
@@ -471,6 +475,15 @@ k_qmlp_sm90(const QmlpArgs a) {
         }
       }
     }
+    // release this warpgroup's half of the tile: all 128 threads' writes above, then one gpu-scope fence + count
+    if (!DEV && a.done != nullptr) {
+      if (warp < 4) asm volatile("bar.sync 1, 128;" ::: "memory");   // named barriers 1 and 2: one per warpgroup
+      else asm volatile("bar.sync 2, 128;" ::: "memory");
+      if (signaller) {
+        __threadfence();
+        atomicAdd(a.done + my_bag, 1u);
+      }
+    }
     tile = next_tile;
   }
 }
@@ -513,22 +526,22 @@ inline int launch_prep_wimg(const dsmil_params_t* p, uint8_t* wimg, cudaStream_t
   return 0;
 }
 
-// scores + arg-max keys + Q (+H1) for the ntiles 128-row tiles of the nb bags of the table.
+// scores + arg-max keys + Q (+H1) for the ntiles 128-row tiles of the nb bags of the table, on at most max_ctas CTAs.
 // wimg must already hold the images (launch_prep_wimg).  ntiles_dev != NULL: ntiles is the capacity, *ntiles_dev the
-// live count.
+// live count.  done != NULL (eager form only): per-bag tile releases for an overlapped k_attend_b.
 inline int launch_qmlp(const dsmil_params_t* p, const BagDev* bags_dev, int nb, int ntiles, float* classes,
-                       unsigned long long* keys, float* Q, float* H1, const uint8_t* wimg, int num_sms, cudaStream_t st,
-                       bool q_blocked, const int* ntiles_dev = nullptr) {
+                       unsigned long long* keys, float* Q, float* H1, const uint8_t* wimg, int max_ctas, cudaStream_t st,
+                       bool q_blocked, const int* ntiles_dev = nullptr, unsigned int* done = nullptr) {
   const int D = p->D, C = p->C;
-  if (ntiles_dev != nullptr && C > 4) {
-    set_error("launch_qmlp: a device tile count needs C <= 4");
+  if (ntiles_dev != nullptr && (C > 4 || done != nullptr)) {
+    set_error("launch_qmlp: a device tile count needs C <= 4 and no tile releases");
     return DSMIL_ERR_ARG;
   }
   const uint8_t* w2img = wimg + static_cast<size_t>(D / kChunkK) * kChunkBytes;
   QmlpArgs a{bags_dev, nb, ntiles, D, C, p->Wi, p->bi, p->b1, p->b2, wimg, w2img, classes, keys, Q, H1, q_blocked,
-             ntiles_dev};
+             ntiles_dev, done};
   const size_t smem = qmlp_smem_bytes(C, D);
-  const int grid = ntiles < num_sms ? ntiles : num_sms;
+  const int grid = ntiles < max_ctas ? ntiles : max_ctas;
   auto go = [&](auto kern) -> int {
     // (set on every launch: the instantiations share one function-pointer TYPE, so a cached flag here would be
     //  shared between them -- found by the D=1024 / C=1 shape tests; the call costs ~1 us of host time)

@@ -144,6 +144,10 @@ size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t
 int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                        float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
                        void* workspace, size_t workspace_bytes, void* stream);
+/* CTAs of the tensor-core phase 1 of dsmil_forward_bags (and of the _train form) for a batch of `tiles` 128-row tiles
+ * on the current device, when its attend pass is overlapped with it: the SMs it leaves free start on the bags phase 1
+ * has finished.  The grid changes no result; tests use it to place batches at its edges.  0 for tiles < 1. */
+int32_t dsmil_forward_bags_phase1_ctas(int64_t tiles);
 
 /* Training form of dsmil_forward_bags: the same packed outputs, plus save_Q [sum N,128] (after the tanh) and, for a
  * nonlinear q, save_H1 [sum N,128], packed in bag order -- what dsmil_backward_bags needs.  crit_idx [nb,C] is
