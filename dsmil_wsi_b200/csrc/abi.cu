@@ -1477,12 +1477,13 @@ static int check_bags_dev(const dsmil_params_t* p, bool need_scores, bool need_l
   return 0;
 }
 
-// The forward's carve for nb bags of max_rows rows (Q and H1 are the caller's; `sharded` adds the row offsets and
-// q_max of the row-sharded batch), then the planner's BagsPlan and the zero row of a refused batch.
-static BagsWs carve_bags_dev(const dsmil_params_t* p, int nb, int64_t max_rows, bool sharded, void* ws, size_t cap,
-                             bool* ok, BagsPlan** plan, float** zero_row) {
+// The forward's carve for nb bags of max_rows rows (need_Q: the tile blocks of Q for the capacity tiles, as inference
+// keeps them; otherwise Q and H1 are the caller's; `sharded` adds the row offsets and q_max of the row-sharded batch),
+// then the planner's BagsPlan and the zero row of a refused batch.
+static BagsWs carve_bags_dev(const dsmil_params_t* p, int nb, int64_t max_rows, bool need_Q, bool sharded, void* ws,
+                             size_t cap, bool* ok, BagsPlan** plan, float** zero_row) {
   const std::vector<int64_t> Ns(nb, max_rows);
-  BagsWs w = carve_bags(p, Ns.data(), nb, false, sharded, ws, cap, ok);
+  BagsWs w = carve_bags(p, Ns.data(), nb, need_Q, sharded, ws, cap, ok);
   Carver c(ws, cap);
   c.off = w.bytes;
   *plan = c.take<BagsPlan>(1);
@@ -1494,13 +1495,17 @@ static BagsWs carve_bags_dev(const dsmil_params_t* p, int nb, int64_t max_rows, 
 
 // bags_phase1_impl's launches in a dev call, on the planner's table (k_qmlp_sm90 on the capacity grid of 128-row
 // tiles), with the weight images rebuilt on every call: a replayed graph sees the weights of the last optimizer step.
+// q_blocked: Q in tile blocks (inference).  overlap: as bags_phase1_impl's, on the grid it gives the capacity tiles.
 static int bags_phase1_dev(const dsmil_params_t* p, const BagsWs& w, const BagsPlan* plan, int nb, int64_t max_rows,
-                           float* classes, float* Q, float* H1, cudaStream_t st) {
+                           float* classes, float* Q, float* H1, cudaStream_t st, bool q_blocked = false,
+                           bool overlap = false) {
   int rc;
   DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * nb, st));
   if ((rc = sm90::launch_prep_wimg(p, w.wimg, st))) return rc;
-  return sm90::launch_qmlp(p, w.table, nb, nb * tiles_for_bag(max_rows), classes, w.keys, Q, H1, w.wimg, num_sms(), st,
-                           false, &plan->tiles);
+  const int tiles = nb * tiles_for_bag(max_rows);
+  return sm90::launch_qmlp(p, w.table, nb, tiles, classes, w.keys, Q, H1, w.wimg,
+                           overlap ? overlap_phase1_ctas(tiles) : num_sms(), st, q_blocked, &plan->tiles,
+                           overlap ? w.done : nullptr);
 }
 
 size_t dsmil_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
@@ -1508,7 +1513,7 @@ size_t dsmil_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int
   bool ok;
   BagsPlan* plan;
   float* zero_row;
-  const size_t dev = carve_bags_dev(p, nb, max_rows, false, nullptr, 0, &ok, &plan, &zero_row).bytes;
+  const size_t dev = carve_bags_dev(p, nb, max_rows, false, false, nullptr, 0, &ok, &plan, &zero_row).bytes;
   // never below the eager call's size for the same capacity: one buffer serves both forms
   const std::vector<int64_t> Ns(nb, max_rows);
   return std::max(dev, dsmil_forward_bags_train_workspace_bytes(p, Ns.data(), nb));
@@ -1527,13 +1532,48 @@ int dsmil_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs
   bool ok;
   BagsPlan* plan;
   float* zero_row;
-  BagsWs w = carve_bags_dev(p, nb, max_rows, false, workspace, workspace_bytes, &ok, &plan, &zero_row);
+  BagsWs w = carve_bags_dev(p, nb, max_rows, false, false, workspace, workspace_bytes, &ok, &plan, &zero_row);
   k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, zero_row, w.table, nullptr, nullptr, plan,
                                 status, nullptr, nullptr);
   DSMIL_LAUNCH_OK("k_plan_bags");
   if ((rc = bags_phase1_dev(p, w, plan, nb, max_rows, classes, save_Q, save_H1, st))) return rc;
   return bags_attend_finalize(p, w, nb, save_Q, false, pred, A, B, crit_idx, nb * recs_for_bag(max_rows), &plan->recs,
                               st);
+}
+
+size_t dsmil_forward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
+  bool ok;
+  BagsPlan* plan;
+  float* zero_row;
+  const size_t dev = carve_bags_dev(p, nb, max_rows, true, false, nullptr, 0, &ok, &plan, &zero_row).bytes;
+  const std::vector<int64_t> Ns(nb, max_rows);
+  return std::max(dev, dsmil_forward_bags_workspace_bytes(p, Ns.data(), nb));
+}
+
+// The inference twin of dsmil_forward_bags_train_dev: Q stays in the workspace as tile blocks, and the attend pass is
+// a programmatic dependent of phase 1 as in dsmil_forward_bags -- under stream capture too, where the launch attribute
+// becomes a programmatic edge of the graph (DESIGN §4.3).  Only kernel timing keeps the plain launch.
+int dsmil_forward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev, int32_t nb,
+                           int64_t max_rows, float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                           int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_bags_dev(p, true, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(classes && pred && A && B, "NULL output pointer");
+  const size_t need = dsmil_forward_bags_dev_workspace_bytes(p, nb, max_rows);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  bool ok;
+  BagsPlan* plan;
+  float* zero_row;
+  BagsWs w = carve_bags_dev(p, nb, max_rows, true, false, workspace, workspace_bytes, &ok, &plan, &zero_row);
+  k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, zero_row, w.table, nullptr, nullptr, plan,
+                                status, nullptr, nullptr);
+  DSMIL_LAUNCH_OK("k_plan_bags");
+  const bool overlap = !g_prof_on;
+  if ((rc = bags_phase1_dev(p, w, plan, nb, max_rows, classes, w.Q, nullptr, st, true, overlap))) return rc;
+  return bags_attend_finalize(p, w, nb, w.Q, true, pred, A, B, crit_idx, nb * recs_for_bag(max_rows), &plan->recs, st,
+                              overlap);
 }
 
 size_t dsmil_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
@@ -1573,7 +1613,7 @@ size_t dsmil_shard_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32
   bool ok;
   BagsPlan* plan;
   float* zero_row;
-  const size_t dev = carve_bags_dev(p, nb, max_rows, true, nullptr, 0, &ok, &plan, &zero_row).bytes;
+  const size_t dev = carve_bags_dev(p, nb, max_rows, false, true, nullptr, 0, &ok, &plan, &zero_row).bytes;
   const std::vector<int64_t> Ns(nb, max_rows);
   return std::max(dev, dsmil_shard_bags_workspace_bytes(p, Ns.data(), nb));
 }
@@ -1585,7 +1625,7 @@ static int shard_bags_dev_ws(const dsmil_params_t* p, int nb, int64_t max_rows, 
   int rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0);
   if (rc) return rc;
   bool ok;
-  *w = carve_bags_dev(p, nb, max_rows, true, workspace, workspace_bytes, &ok, plan, zero_row);
+  *w = carve_bags_dev(p, nb, max_rows, false, true, workspace, workspace_bytes, &ok, plan, zero_row);
   return 0;
 }
 

@@ -108,17 +108,28 @@ struct BagsPlan {
 // (crit_idx 0, pred = bf, B = 0), and nothing reads the caller's bag list.  A row-sharded batch also passes each bag's
 // first global row (offs_in, device memory): the planner copies it to offs_out, a negative offset is refused like a
 // bad bag, and a refused batch's offsets are 0.
+// The walk is one thread's; the warp first stages the list of the first kPlanStaged bags into shared memory with its
+// loads in flight together, so the walk does not wait on one global load per bag.
+constexpr int kPlanStaged = 256;
 __global__ void __launch_bounds__(32)
 k_plan_bags(const float* const* __restrict__ Xs, const int64_t* __restrict__ Ns, int nb, long long max_rows, int C,
             int D, float* __restrict__ zero_row, sm90::BagDev* __restrict__ table, TnChunk* __restrict__ chi,
             TnChunk* __restrict__ ch1, BagsPlan* __restrict__ plan, int* __restrict__ status,
             const int64_t* __restrict__ offs_in, long long* __restrict__ offs_out) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  __shared__ const float* sX[kPlanStaged];
+  __shared__ int64_t sN[kPlanStaged];
+  if (blockIdx.x != 0) return;
+  for (int b = threadIdx.x; b < nb && b < kPlanStaged; b += 32) { sX[b] = Xs[b]; sN[b] = Ns[b]; }
+  __syncwarp();
+  if (threadIdx.x != 0) return;
+  auto X_of = [&](int b) { return b < kPlanStaged ? sX[b] : Xs[b]; };
+  auto N_of = [&](int b) { return b < kPlanStaged ? sN[b] : Ns[b]; };
   int bad = 0;
   long long mx = 0;
   for (int b = 0; b < nb && !bad; ++b) {
-    const int64_t N = Ns[b];
-    if (N < 1 || N > max_rows || Xs[b] == nullptr || (reinterpret_cast<uintptr_t>(Xs[b]) & 15) != 0 ||
+    const int64_t N = N_of(b);
+    const float* X = X_of(b);
+    if (N < 1 || N > max_rows || X == nullptr || (reinterpret_cast<uintptr_t>(X) & 15) != 0 ||
         (offs_in && offs_in[b] < 0))
       bad = b + 1;
     mx = N > mx ? N : mx;
@@ -131,7 +142,7 @@ k_plan_bags(const float* const* __restrict__ Xs, const int64_t* __restrict__ Ns,
   BagsPlan pl{};
   long long row = 0;
   int tile = 0, rec = 0;
-  for (int b = 0; b < nb; ++b) table[b] = bad ? bag_entry(zero_row, 1, row, tile, rec) : bag_entry(Xs[b], Ns[b], row, tile, rec);
+  for (int b = 0; b < nb; ++b) table[b] = bad ? bag_entry(zero_row, 1, row, tile, rec) : bag_entry(X_of(b), N_of(b), row, tile, rec);
   if (offs_out)
     for (int b = 0; b < nb; ++b) offs_out[b] = bad ? 0 : offs_in[b];
   pl.total = row;

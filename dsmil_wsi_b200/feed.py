@@ -9,8 +9,10 @@ on the device until the epoch ends.
 """
 from __future__ import annotations
 
+import weakref
 from typing import Iterable, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -198,7 +200,8 @@ def _group_predictions(outs):
 
 
 def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, bags_per_launch: int = 16,
-               dropout_patch: float = 0.0, generator: Optional[torch.Generator] = None):
+               dropout_patch: float = 0.0, generator: Optional[torch.Generator] = None, graph: bool = False,
+               max_rows: Optional[int] = None):
     """The measuring half of train_tcga.test() (train_tcga.py:85-107): mean loss, labels [n_bags, C] and
     sigmoid predictions [n_bags, C] (`average=True`: sigmoid(max) + sigmoid(bag), as `args.average`).  The ROC /
     threshold logic that follows in the reference (:108-132) is the caller's and works on these arrays.
@@ -208,11 +211,22 @@ def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, 
     device and there is one host sync per epoch instead of two `.item()` per bag.  The reference also routes test
     bags through `dropout_patches` (a row permutation when dropout_patch == 0); a permutation does not change
     any output of the operator except the order of the per-instance rows, so it is skipped unless rows are
-    actually dropped."""
+    actually dropped.
+
+    graph=True: each group of bags_per_launch bags (and a short last group) replays a recorded graph
+    (infer_graph.EvalBagsGraph) of the forward, the per-bag losses and the predictions; the bags are read in place and
+    the results are the eager epoch's bits.  max_rows is the per-bag row capacity of the graphs (default: the largest
+    bag of the store); a bag over it raises ValueError before any launch.  The graphs stay cached with the model (held
+    weakly) and later calls with the same group sizes, capacity, `average` and criterion object replay them: the first
+    call pays the recording, and a model whose parameter tensors were replaced gets new graphs.  Needs the batched
+    tensor-core shapes."""
     milnet.eval()
     n = len(store)
     if n == 0:
         raise ValueError("eval_epoch over an empty store")
+    if graph:
+        return _eval_epoch_graph(milnet, store, criterion, average, max(1, bags_per_launch), dropout_patch, generator,
+                                 max_rows)
     losses, labels, preds = [], [], []
     batched = hasattr(milnet, "forward_bags") and bags_per_launch > 1
     with torch.no_grad():
@@ -229,6 +243,58 @@ def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, 
                 preds.append(torch.sigmoid(max_prediction).view(-1) + p if average else p)
     loss = float(torch.stack([l.reshape(()) for l in losses]).mean().item())
     return loss, torch.stack(labels).cpu().numpy().astype(int), torch.stack(preds).cpu().numpy()
+
+
+# model -> {(bags per graph, max_rows, average): EvalBagsGraph}: later epochs replay the graphs of earlier ones (the
+# graphs read the parameters in place, so training between epochs is seen); kept off the model itself, as
+# embed._GRAPHS, so that deepcopy / pickling of the caller's model never meets a CUDA graph
+_EVAL_GRAPHS = weakref.WeakKeyDictionary()
+
+
+def _eval_epoch_graph(milnet, store, criterion, average, k, dropout_patch, generator, max_rows):
+    from .infer_graph import EvalBagsGraph
+    from .train_graph import step_shape
+    step_shape(milnet)                                         # a shape off the batched path raises here
+    p = 1 - dropout_patch
+    keep = [int(int(f.shape[0]) * p) if dropout_patch > 0 else int(f.shape[0]) for f, _ in store.bags]
+    cap = int(max_rows) if max_rows is not None else max(int(f.shape[0]) for f, _ in store.bags)
+    for i, m in enumerate(keep):
+        if m > cap:
+            raise ValueError(f"bag {i}: {m} rows exceed the inference graph's max_rows={cap}")
+        if m < 1:
+            raise IndexError(f"dsmil_b200: bag {i} is empty after patch dropout (N == 0)")
+    n, C = len(store), int(store.bags[0][1].numel())
+    cached = _EVAL_GRAPHS.setdefault(milnet, {})
+    graphs = {}
+    losses = torch.empty(n, device=store.device)
+    preds = torch.empty(n, C, device=store.device)
+    labels = torch.stack([label.view(-1) for _, label in store.bags])
+    for s in range(0, n, k):
+        group = store.bags[s:s + k]
+        g = graphs.get(len(group))
+        if g is None:                                          # the first full group, and a short last one
+            key = (len(group), cap, bool(average))
+            g = cached.get(key)
+            if g is None or g.criterion is not criterion or not g.current():
+                g = cached[key] = EvalBagsGraph(milnet, criterion, len(group), cap, average)
+            graphs[len(group)] = g
+        xs = [dropout_patches(f, p, generator) if dropout_patch > 0 else f for f, _ in group]
+        g.labels.copy_(labels[s:s + len(group)])
+        g.run(xs)
+        losses[s:s + len(group)] = g.loss
+        preds[s:s + len(group)] = g.pred
+    # the epoch's one host sync: the mean loss, the planners' status words, the labels and the predictions (float32
+    # and the integer labels are exact in float64)
+    status = sum((g.status for g in graphs.values()), torch.zeros(1, dtype=torch.int32, device=store.device))
+    host = torch.cat([losses.mean().double().view(1), status.double(), labels.double().view(-1),
+                      preds.double().view(-1)]).cpu().numpy()
+    for g in graphs.values():
+        g.status.zero_()
+        g.release()
+    if host[1]:
+        raise RuntimeError(f"inference graph: a batch held a bag the library refused (planner status {int(host[1])})")
+    return (float(host[0]), host[2:2 + n * C].reshape(n, C).astype(int),
+            host[2 + n * C:].reshape(n, C).astype(np.float32))
 
 
 # ---- classic-MIL drivers (train_mil.py) ---------------------------------------------------------------------

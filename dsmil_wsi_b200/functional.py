@@ -400,6 +400,33 @@ def mil_forward_bags(bags: Sequence[torch.Tensor], params: Sequence[Optional[tor
 
 
 @torch.no_grad()
+def mil_forward_bags_dev(xs: torch.Tensor, Ns: torch.Tensor, status: torch.Tensor, max_rows: int,
+                         params: Sequence[Optional[torch.Tensor]]):
+    """Inference over a bag list held on the device (dsmil_forward_bags_dev), with no host work that depends on the
+    bags: one call can be recorded into a CUDA graph and replayed over every batch of nb bags of 1..max_rows rows.
+
+    xs [nb] int64 (the bags' feature addresses: contiguous float32 [N_b, D]), Ns [nb] int64 and status [1] int32 on
+    the device.  Returns the packed (classes, pred, A, B, crit): classes and A have nb * max_rows rows, the live ones
+    packed at the prefix sums of Ns, as dsmil_forward_bags packs them.  A refused batch sets status (see the header)."""
+    lib = _lib.load()
+    P = ParamPack(*params)
+    if not lib.dsmil_shard_bags_supported(P.ref):
+        raise ValueError(f"the device bag list runs on the batched tensor-core path only; D={P.D}, C={P.C}, "
+                         f"nonlinear={P.nonlinear}, passing_v={P.passing_v} is not on it")
+    nb, dev = int(xs.numel()), P.device
+    with torch.cuda.device(dev):
+        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        classes, A = new(nb * max_rows, P.C), new(nb * max_rows, P.C)
+        pred, B = new(nb, P.C), new(nb, P.C, P.D)
+        crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
+        ws = _workspace(lib.dsmil_forward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
+        rc = lib.dsmil_forward_bags_dev(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred), _ptr(A),
+                                        _ptr(B), _ptr(crit), _ptr(status), _ptr(ws), ws.numel(), _stream())
+        _lib.check(rc, "dsmil_forward_bags_dev")
+    return classes, pred, A, B, crit
+
+
+@torch.no_grad()
 def _mil_forward_bags_infer(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]]):
     lib = _lib.load()
     P = ParamPack(*params)

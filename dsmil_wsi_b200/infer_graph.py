@@ -1,0 +1,153 @@
+"""Inference over batches of ragged bags recorded once as a CUDA graph and replayed (ForwardBagsGraph), for serving
+loops and the evaluation epoch.
+
+An eager `milnet(x)` or `milnet.forward_bags(xs)` pays its host cost on every call: ParamPack, workspace allocation,
+the host-built bag table and its upload, ctypes.  For one slide per call that host work is most of the call.  Here one
+dsmil_forward_bags_dev call is captured over static buffers -- the bags' feature addresses, their row counts and a
+status word on the device -- and every batch of nb bags of 1..max_rows rows replays it.  The bags are read where they
+are: `run` writes their addresses, not their rows.  The attend pass stays a programmatic dependent of phase 1 inside
+the graph, so a replay keeps the eager call's overlap, and its outputs are the eager call's bits.
+"""
+from __future__ import annotations
+
+import weakref
+from typing import Sequence
+
+import torch
+
+from . import functional as Fn
+from .sharded import milnet_params
+from .train_graph import step_shape
+
+
+class ForwardBagsGraph:
+    """One recorded inference call over nb bags of up to max_rows rows (nb = 1: one slide per call).
+
+    `run(bags)` takes nb contiguous float32 [N_b, D] CUDA tensors with 1 <= N_b <= max_rows, replays the graph on the
+    current stream and returns Fn.BagOutputs over the graph's packed outputs: per-bag (classes, prediction_bag, A, B)
+    views, `.packed` and `.crit`.  They are overwritten by the next `run`; clone what must outlive it.  The object keeps
+    the last call's bags alive until the next call, since the replay reads them in place.
+
+    The graph reads the parameters in place: in-place updates (an optimizer step, `load_state_dict`) are seen by the
+    next replay.  A parameter replaced by another tensor is not, and `run` raises RuntimeError; build a new graph.  A
+    bag the library refuses (features not 16-byte aligned) sets `status` to 1 + its index (never cleared here) and the
+    batch's outputs are a finite stand-in; read `status` when you synchronise."""
+
+    def __init__(self, milnet, nb: int, max_rows: int, warmup: int = 1):
+        self.D, self.C = step_shape(milnet)
+        nb, max_rows = int(nb), int(max_rows)
+        if not 1 <= nb <= 65535 or max_rows < 1:
+            raise ValueError(f"ForwardBagsGraph: nb={nb} outside [1, 65535] or max_rows={max_rows} < 1")
+        self._milnet = weakref.ref(milnet)      # a graph cached on the model must not keep it alive
+        self.nb, self.max_rows = nb, max_rows
+        self.params = milnet_params(milnet)
+        Fn.require_cuda(self.params[-2], "the model")
+        dev = self.device = self.params[-2].device
+        self._addrs = _param_addrs(milnet)
+        self.bag_list = torch.zeros(2, nb, dtype=torch.int64, device=dev)    # feature addresses; row counts
+        self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        # pinned staging of the bag list, two buffers: the host fills one while the copy from the other may be queued
+        self._stage = [torch.zeros(2, nb, dtype=torch.int64, pin_memory=True) for _ in range(2)]
+        self._stage_np = [s.numpy() for s in self._stage]
+        self._copied = [torch.cuda.Event() for _ in range(2)]
+        self._turn = 0
+        self._bags: Sequence[torch.Tensor] = ()
+        self._buffers(dev)
+        # warm-up and capture on a batch of one-row bags of zeros
+        self._scratch = torch.zeros(nb, self.D, device=dev)
+        self.bag_list[0] = self._scratch.data_ptr() + 4 * self.D * torch.arange(nb, device=dev)
+        self.bag_list[1] = 1
+        side = torch.cuda.Stream(dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(max(1, warmup)):
+                self._record()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self._record()
+        self.status.zero_()
+
+    def _buffers(self, dev):
+        """Static buffers of a subclass's recorded work beyond the bag list and status."""
+
+    def _record(self):
+        self.out = Fn.mil_forward_bags_dev(self.bag_list[0], self.bag_list[1], self.status, self.max_rows, self.params)
+        self._after(*self.out)
+
+    def _after(self, classes, pred, A, B, crit):
+        """Work a subclass records after the forward, in the same graph."""
+
+    def current(self) -> bool:
+        """Whether the model is alive and holds the parameter tensors the graph was recorded on."""
+        milnet = self._milnet()
+        return milnet is not None and _param_addrs(milnet) == self._addrs
+
+    def _load(self, bags):
+        """Checks the bags and queues the upload of their addresses and row counts into the bag list."""
+        if not self.current():
+            raise RuntimeError("ForwardBagsGraph: the model is gone, or a parameter tensor of it was replaced since "
+                               "the capture (the graph reads the old one); update parameters in place, or build a new "
+                               "graph")
+        if len(bags) != self.nb:
+            raise ValueError(f"ForwardBagsGraph: {len(bags)} bags for a graph of nb={self.nb}")
+        Ns = []
+        for b, x in enumerate(bags):
+            if (not x.is_cuda or x.device != self.device or x.dtype != torch.float32 or x.dim() != 2
+                    or x.shape[1] != self.D or not x.is_contiguous()):
+                raise ValueError(f"bag {b}: need a contiguous float32 [N, {self.D}] tensor on {self.device}, got "
+                                 f"{x.dtype} {tuple(x.shape)} on {x.device}")
+            n = int(x.shape[0])
+            if n < 1:
+                raise IndexError(f"dsmil_b200: bag {b} is empty (N == 0)")
+            if n > self.max_rows:
+                raise ValueError(f"bag {b}: {n} rows exceed the inference graph's max_rows={self.max_rows}")
+            Ns.append(n)
+        i = self._turn
+        self._turn ^= 1
+        self._copied[i].synchronize()            # the copy that last read this staging buffer has run
+        self._stage_np[i][0] = [x.data_ptr() for x in bags]
+        self._stage_np[i][1] = Ns
+        self.bag_list.copy_(self._stage[i], non_blocking=True)
+        self._copied[i].record()
+        self._bags = list(bags)
+        return Ns
+
+    def release(self):
+        """Drops the references to the last call's bags (call it once the stream has run the replay)."""
+        self._bags = ()
+
+    def run(self, bags: Sequence[torch.Tensor]) -> Fn.BagOutputs:
+        Ns = self._load(bags)
+        self.graph.replay()
+        classes, pred, A, B, crit = self.out
+        total = sum(Ns)
+        return Fn.BagOutputs(classes[:total], pred, A[:total], B, Ns, crit)
+
+
+def _param_addrs(milnet):
+    return tuple(None if t is None else t.data_ptr() for t in milnet_params(milnet))
+
+
+class EvalBagsGraph(ForwardBagsGraph):
+    """ForwardBagsGraph with the evaluation epoch's per-bag work recorded after the forward: each bag's max-instance
+    prediction (the scores at its critical rows), its loss 0.5 * criterion(bag) + 0.5 * criterion(max instance) on
+    [1, C] rows as feed.eval_epoch computes it, and the sigmoid predictions (average: sigmoid(max) + sigmoid(bag)).
+    Fill `labels` [nb, C], then `run(bags)`; `loss` [nb] and `pred` [nb, C] hold the batch's results."""
+
+    def __init__(self, milnet, criterion, nb: int, max_rows: int, average: bool = False):
+        self.criterion, self.average = criterion, bool(average)
+        super().__init__(milnet, nb, max_rows)
+
+    def _buffers(self, dev):
+        self.labels = torch.zeros(self.nb, self.C, device=dev)
+
+    def _after(self, classes, pred, A, B, crit):
+        n = self.bag_list[1].clamp(0, self.max_rows)          # the live sizes (a refused batch's stay in range)
+        first = torch.cumsum(n, 0) - n                         # each bag's first packed row
+        mx = classes.gather(0, crit + first[:, None])
+        y = self.labels
+        self.loss = torch.stack([(0.5 * self.criterion(pred[b:b + 1], y[b:b + 1]) +
+                                  0.5 * self.criterion(mx[b:b + 1], y[b:b + 1])).reshape(()) for b in range(self.nb)])
+        p = torch.sigmoid(pred)
+        self.pred = torch.sigmoid(mx) + p if self.average else p

@@ -196,6 +196,19 @@ int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev,
                             const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
                             const float* d_B, const dsmil_grads_t* grads, int32_t* status, void* workspace,
                             size_t workspace_bytes, void* stream);
+/* Capture-safe form of dsmil_forward_bags (inference), under the rules of dsmil_forward_bags_train_dev above: the bag
+ * list in device memory, classes and A sized for nb * max_rows rows with the live rows packed at the live prefix sums,
+ * no host<->device copy, allocation or synchronisation, the same refusal through *status and the same stand-in batch,
+ * the W1/W2 images rebuilt on every call.  crit_idx [nb,C] may be NULL, as in dsmil_forward_bags.  As in
+ * dsmil_forward_bags, the attend pass is a programmatic dependent of phase 1, also when the call is recorded into a
+ * CUDA graph (the graph holds a programmatic edge between the two kernel nodes); only dsmil_profile_enable(1) keeps the
+ * plain launch.  On the same bags every output is dsmil_forward_bags's, bit for bit.  The workspace size depends on
+ * (nb, max_rows) only and is never below dsmil_forward_bags_workspace_bytes for nb bags of max_rows rows; 0 for
+ * shapes off dsmil_shard_bags_supported. */
+size_t dsmil_forward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_forward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev, int32_t nb,
+                           int64_t max_rows, float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                           int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Call form (2)+(3) of the boundary (SURVEY §8b): the callers in attention_map.py:74,85 /
  * testing_tcga.py:72,83 run the instance classifier and the bag classifier separately.
