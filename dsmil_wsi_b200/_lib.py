@@ -55,6 +55,12 @@ SIGNATURES = {
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_size_t, C.c_void_p]),
     "dsmil_forward_bags_phase1_ctas": (C.c_int32, [c_i64]),
+    "dsmil_models_supported": (C.c_int, [C.POINTER(DsmilParams), C.c_int32]),
+    "dsmil_forward_bags_models_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, C.POINTER(c_i64),
+                                                               C.c_int32]),
+    "dsmil_forward_bags_models": (C.c_int, [C.POINTER(DsmilParams), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(c_i64),
+                                            C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_size_t, C.c_void_p]),
     "dsmil_instance_scores": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, c_i64, C.c_void_p, C.c_void_p]),
     "dsmil_instance_scores_backward": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, c_i64, C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,

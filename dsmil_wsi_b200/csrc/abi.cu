@@ -657,6 +657,152 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
 }
 int32_t dsmil_forward_bags_phase1_ctas(int64_t tiles) { return tiles < 1 ? 0 : overlap_phase1_ctas(tiles); }
 
+// ---- ensemble forward: M models over one batch of bags ---------------------------------------------------------------
+// The fused form's table has one entry per (bag, model), model-major inside each bag (entry b * M + m), so the M passes
+// over a bag follow each other on the persistent grid and the later ones find its features in L2 (DESIGN §4.2e).
+// Entry (b, m)'s rows sit at m * sum N + (first row of b) in the packed outputs, which makes classes and A model-major;
+// keys, counters, Q tile blocks and records keep the per-entry numbering of the one-model batch.
+static int check_models(const dsmil_params_t* ps, int M) {
+  DSMIL_REQUIRE(ps != nullptr, "params is NULL");
+  DSMIL_REQUIRE(M >= 1 && M <= sm90::kMaxModels, "models: M=%d outside [1,%d]", M, sm90::kMaxModels);
+  for (int m = 0; m < M; ++m) {
+    const int rc = check_params(&ps[m], true);
+    if (rc) return rc;
+    DSMIL_REQUIRE(ps[m].D == ps[0].D && ps[m].C == ps[0].C && ps[m].nonlinear == ps[0].nonlinear &&
+                      ps[m].passing_v == ps[0].passing_v,
+                  "model %d: (D=%d, C=%d, nonlinear=%d, passing_v=%d) differs from model 0's (%d, %d, %d, %d)", m,
+                  ps[m].D, ps[m].C, ps[m].nonlinear, ps[m].passing_v, ps[0].D, ps[0].C, ps[0].nonlinear,
+                  ps[0].passing_v);
+  }
+  return 0;
+}
+static bool models_batched(const dsmil_params_t* ps, int M) {
+  for (int m = 0; m < M; ++m)
+    if (!dsmil_shard_bags_supported(&ps[m])) return false;
+  return true;
+}
+
+struct ModelsWs : BagsWs {
+  sm90::ModelDev* models;   // [M]
+};
+static ModelsWs carve_models(const dsmil_params_t* p, int M, const int64_t* Ns, int nb, void* ws, size_t cap,
+                             bool* ok) {
+  Carver c(ws, cap);
+  ModelsWs w;
+  int64_t tiles = 0, nrec = 0;
+  for (int b = 0; b < nb; ++b) {
+    tiles += tiles_for_bag(Ns[b]);
+    nrec += recs_for_bag(Ns[b]);
+  }
+  const size_t ne = static_cast<size_t>(nb) * M;
+  w.table = c.take<sm90::BagDev>(ne);
+  w.keys = c.take<unsigned long long>(ne * (kMaxC + 1));   // keys, then the two per-entry counters (carve_phase1)
+  w.counters = reinterpret_cast<unsigned int*>(w.keys ? w.keys + ne * kMaxC : nullptr);
+  w.done = w.counters ? w.counters + ne : nullptr;
+  w.models = c.take<sm90::ModelDev>(M);
+  const uintptr_t img = reinterpret_cast<uintptr_t>(c.take<uint8_t>(M * sm90::wimg_bytes(p->D) + 1024));
+  w.wimg = reinterpret_cast<uint8_t*>((img + 1023) & ~uintptr_t(1023));
+  w.pred_part = c.take<float>(ne * sm90::kFinSlices * kMaxC);
+  w.Q = c.take<float>(static_cast<size_t>(M) * tiles * sm90::kTileM * kQ);
+  w.recs = c.take<float>(static_cast<size_t>(M) * nrec * rec_floats(p->C, p->D));
+  w.row_offsets = nullptr;
+  w.qmax = nullptr;
+  w.bytes = c.off;
+  *ok = c.ok();
+  return w;
+}
+
+static int forward_bags_models_impl(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
+                                    int nb, int64_t total, float* classes, float* pred, float* A, float* B,
+                                    int64_t* crit, void* ws, size_t ws_bytes, cudaStream_t st) {
+  const int C = ps[0].C, D = ps[0].D, ne = nb * M;
+  bool ok;
+  ModelsWs w = carve_models(&ps[0], M, Ns, nb, ws, ws_bytes, &ok);
+  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+  if (rc) return rc;
+  std::vector<sm90::BagDev> tbl(ne);
+  long long row = 0;
+  int tile = 0, rec = 0;
+  for (int b = 0; b < nb; ++b) {
+    for (int m = 0; m < M; ++m) {
+      long long r = row;
+      sm90::BagDev& e = tbl[static_cast<size_t>(b) * M + m];
+      e = bag_entry(Xs[b], Ns[b], r, tile, rec);
+      e.row_off = m * total + row;
+      e.pad_ = m;
+    }
+    row += Ns[b];
+  }
+  std::vector<sm90::ModelDev> mh(M);
+  for (int m = 0; m < M; ++m) {
+    const dsmil_params_t& p = ps[m];
+    mh[m] = sm90::ModelDev{p.Wi, p.bi, p.W1, p.b1, p.W2, p.b2, p.Wf, p.bf};
+  }
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * ne, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.models, mh.data(), sizeof(sm90::ModelDev) * M, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * ne, st));
+  if ((rc = sm90::launch_prep_wimg_models(w.models, M, D, w.wimg, st))) return rc;
+  // overlapped as in forward_bags_impl: not under capture, not while kernels are timed
+  const bool overlap = !g_prof_on && !stream_is_capturing(st);
+  if ((rc = sm90::launch_qmlp_models(w.models, M, D, C, w.table, ne, tile, classes, w.keys, w.Q, w.wimg,
+                                     overlap ? overlap_phase1_ctas(tile) : num_sms(), st,
+                                     overlap ? w.done : nullptr)))
+    return rc;
+  sm90::AttendArgs aa{w.table, ne, D, C, w.Q, true, w.keys, A, w.recs, nullptr, nullptr, overlap ? w.done : nullptr};
+  if ((rc = sm90::launch_attend_b(aa, rec, st))) return rc;
+  sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, nullptr, nullptr, A, B, pred,
+                        reinterpret_cast<long long*>(crit), w.pred_part, w.counters, nullptr, 0, 0,
+                        w.models, M, nb};
+  return sm90::launch_finalize_b(fa, ne, st);
+}
+
+int dsmil_models_supported(const dsmil_params_t* ps, int32_t M) {
+  if (!ps || M < 1 || M > sm90::kMaxModels || check_models(ps, M) != 0 || !models_batched(ps, M)) return 0;
+  return sm90::qmlp_models_fit(ps[0].C, ps[0].D, M) ? 1 : 0;
+}
+
+size_t dsmil_forward_bags_models_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int64_t* Ns, int32_t nb) {
+  if (!ps || M < 1 || M > sm90::kMaxModels || !Ns || nb < 1) return 0;
+  size_t bytes = 0;
+  for (int m = 0; m < M; ++m) {   // the per-model loop
+    const size_t b = dsmil_forward_bags_workspace_bytes(&ps[m], Ns, nb);
+    if (b == 0) return 0;
+    bytes = std::max(bytes, b);
+  }
+  // the fused layout on every batched shape, whether or not M members fit in shared memory: the size then grows with
+  // M, nb and N alike
+  bool ok;
+  if (models_batched(ps, M)) bytes = std::max(bytes, carve_models(&ps[0], M, Ns, nb, nullptr, 0, &ok).bytes);
+  return bytes;
+}
+
+int dsmil_forward_bags_models(const dsmil_params_t* ps, int32_t M, const float* const* Xs, const int64_t* Ns,
+                              int32_t nb, float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                              void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_models(ps, M);
+  if (rc) return rc;
+  DSMIL_REQUIRE(Xs && Ns && nb >= 1 && classes && pred && A && B, "NULL pointer or nb < 1");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int64_t total;
+  bool aligned;
+  if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
+  const size_t need = dsmil_forward_bags_models_workspace_bytes(ps, M, Ns, nb);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  if (aligned && dsmil_models_supported(ps, M) && static_cast<int64_t>(nb) * M <= 65535)
+    return forward_bags_models_impl(ps, M, Xs, Ns, nb, total, classes, pred, A, B, crit_idx, workspace,
+                                    workspace_bytes, st);
+  // off the fused route: each model's dsmil_forward_bags into its slice
+  const int C = ps[0].C, D = ps[0].D;
+  for (int m = 0; m < M; ++m) {
+    rc = dsmil_forward_bags(&ps[m], Xs, Ns, nb, classes + m * total * C, pred + static_cast<size_t>(m) * nb * C,
+                            A + m * total * C, B + static_cast<size_t>(m) * nb * C * D,
+                            crit_idx ? crit_idx + static_cast<size_t>(m) * nb * C : nullptr, workspace,
+                            workspace_bytes, stream);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
 size_t dsmil_shard_workspace_bytes(const dsmil_params_t* p, int64_t N_local) {
   return dsmil_forward_workspace_bytes(p, N_local);
 }

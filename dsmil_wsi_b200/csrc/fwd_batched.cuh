@@ -291,6 +291,10 @@ struct FinalizeArgs {
   // ext_P per-rank records at recs[(p * ext_nb + b) * stride] (an all-gather result), not the bag table's.
   float* emit;
   int ext_P, ext_nb;
+  // ensemble table (k_finalize_b<true>): entry e = b * nmodels + m takes Wf / bf from models[m] (Wf, bf unused) and
+  // writes pred / B / crit to slot m * nb_out + b, model-major
+  const ModelDev* models;
+  int nmodels, nb_out;
 };
 
 constexpr int kFinSlices = 32;
@@ -300,7 +304,8 @@ constexpr int kFinSlices = 32;
 // all its loads in flight, partials added in a fixed order (deterministic) -- and contributes a partial Conv1d dot
 // product; the last CTA of the bag to finish adds the kFinSlices partials in slice order (dsmil.py:59-61) and writes
 // the critical indices.  4 CTAs per SM (64 registers): left free, ptxas squeezes the kernel under 48 registers for a
-// fifth CTA and spills.
+// fifth CTA and spills.  MODELS: an ensemble table (FinalizeArgs::models).
+template <bool MODELS = false>
 __global__ void __launch_bounds__(256, 4)
 k_finalize_b(const FinalizeArgs a) {
   __shared__ float sw[kMaxRecPerBag][kMaxC];
@@ -312,6 +317,9 @@ k_finalize_b(const FinalizeArgs a) {
   const int C = a.C, D = a.D;
   const int bag = blockIdx.y;
   const BagDev bg = a.bags[bag];
+  const size_t slot = MODELS ? static_cast<size_t>(bg.pad_) * a.nb_out + bag / a.nmodels : bag;   // output bag
+  const float* Wf = MODELS ? a.models[bg.pad_].Wf : a.Wf;
+  const float* bf = MODELS ? a.models[bg.pad_].bf : a.bf;
   const size_t rstride = rec_floats(C, D);
   const bool ext = a.ext_P > 0;
   const float* recs = ext ? a.recs + static_cast<size_t>(bag) * rstride : a.recs + static_cast<size_t>(bg.rec_off) * rstride;
@@ -378,8 +386,8 @@ k_finalize_b(const FinalizeArgs a) {
       } else {
         const int k = e / D;
         const float bval = __fdiv_rn(tot, sS[k]);
-        a.B[static_cast<size_t>(bag) * CD + e] = bval;
-        for (int kk = 0; kk < C; ++kk) ppart[kk] = fmaf(__ldg(a.Wf + static_cast<size_t>(kk) * CD + e), bval, ppart[kk]);
+        a.B[slot * CD + e] = bval;
+        for (int kk = 0; kk < C; ++kk) ppart[kk] = fmaf(__ldg(Wf + static_cast<size_t>(kk) * CD + e), bval, ppart[kk]);
       }
     }
     __syncthreads();
@@ -411,8 +419,8 @@ k_finalize_b(const FinalizeArgs a) {
     const volatile float* pp = a.pred_part + static_cast<size_t>(bag) * kFinSlices * kMaxC;
     float sacc = 0.f;
     for (int sl = 0; sl < kFinSlices; ++sl) sacc += pp[sl * kMaxC + tid];
-    a.pred[static_cast<size_t>(bag) * C + tid] = sacc + __ldg(a.bf + tid);
-    if (a.crit) a.crit[static_cast<size_t>(bag) * C + tid] = key_row(a.keys[static_cast<size_t>(bag) * kMaxC + tid]);
+    a.pred[slot * C + tid] = sacc + __ldg(bf + tid);
+    if (a.crit) a.crit[slot * C + tid] = key_row(a.keys[static_cast<size_t>(bag) * kMaxC + tid]);
   }
 }
 
@@ -486,7 +494,8 @@ inline int launch_attend_b(const AttendArgs& a, int nrecs, cudaStream_t st) {
 
 inline int launch_finalize_b(const FinalizeArgs& a, int nb, cudaStream_t st) {
   prof_begin(PROF_FINAL, st);
-  k_finalize_b<<<dim3(kFinSlices, nb), 256, 0, st>>>(a);
+  if (a.models != nullptr) k_finalize_b<true><<<dim3(kFinSlices, nb), 256, 0, st>>>(a);
+  else k_finalize_b<<<dim3(kFinSlices, nb), 256, 0, st>>>(a);
   prof_end(PROF_FINAL, st);
   DSMIL_LAUNCH_OK("k_finalize_b");
   return 0;

@@ -19,9 +19,11 @@
 //                          chunks and, per tile, the two W2 chunks into a kWStages-deep smem ring (mbarrier full /
 //                          empty pairs; a stage is freed when both consumer warpgroups' MMAs on it have retired)
 //   smem: W ring kWStages x 32 KB | Wi rows (C rounded up to 1/2/4/8)
+//         (MODELS, an ensemble table: the M members' Wi rows | their b1 / b2 / bi; DESIGN §4.2e)
 #pragma once
 #include <cuda_bf16.h>
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -144,10 +146,19 @@ struct BagDev {
   int tile_off;         // first 128-row tile of this bag in the batch-wide tile numbering
   int rec_off;          // first partial record of this bag
   int nrec;             // partial records (== attend CTAs) of this bag
-  int pad_;
+  int pad_;             // ensemble tables (MODELS kernels): the entry's model; 0 elsewhere
 };
 
 constexpr int kSmemBags = 96;
+
+// One member of an ensemble forward (device memory, built by the host per call): the kernels' MODELS forms take each
+// entry's weights from models[entry.pad_].
+constexpr int kMaxModels = 8;
+struct ModelDev {
+  const float *Wi, *bi, *W1, *b1, *W2, *b2, *Wf, *bf;
+};
+// per model after the M sets of Wi rows in the MODELS kernel's shared memory: b1 | b2 | bi (kMaxC slots)
+constexpr int kModelBiasFloats = 2 * kQ + kMaxC;
 
 struct QmlpArgs {
   const BagDev* bags;
@@ -169,6 +180,20 @@ struct QmlpArgs {
   unsigned int* done;     // [nb] or NULL: each consumer warpgroup adds 1 to its bag's count once its half of a tile
                           // (scores, key, Q, H1) is in global memory -- k_attend_b waits for 2 x tiles of the bag
 };
+// The MODELS kernels' arguments (QmlpArgs' Wi, bi, b1, b2 and w2img unused): the nmodels members, and model m's W1 / W2
+// images at w1img + m * wimg_stride.  A type of its own, so that the one-model instantiations keep their parameter block.
+struct QmlpModelsArgs : QmlpArgs {
+  const ModelDev* models;
+  int nmodels;
+  size_t wimg_stride;
+};
+template <bool MODELS> using QmlpArgsOf = typename std::conditional<MODELS, QmlpModelsArgs, QmlpArgs>::type;
+__device__ __forceinline__ const ModelDev* models_of(const QmlpArgs&) { return nullptr; }
+__device__ __forceinline__ const ModelDev* models_of(const QmlpModelsArgs& a) { return a.models; }
+__device__ __forceinline__ int nmodels_of(const QmlpArgs&) { return 1; }
+__device__ __forceinline__ int nmodels_of(const QmlpModelsArgs& a) { return a.nmodels; }
+__device__ __forceinline__ size_t wimg_stride_of(const QmlpArgs&) { return 0; }
+__device__ __forceinline__ size_t wimg_stride_of(const QmlpModelsArgs& a) { return a.wimg_stride; }
 
 // Walks the bag table as a role's tile index increases monotonically.
 struct TileCursor {
@@ -199,9 +224,11 @@ constexpr int kSmemFixed = kOffWi;
 // CT: classes rounded up to 1/2/4/8.  DT: compile-time feature size (512 = every shipped configuration:
 // the chunk loops unroll and the load offsets become immediates) or 0 = run-time D.  DEV: the dev calls' form, whose
 // live tile count is read on the device (a.ntiles_dev); the eager form's code does not carry that test.
-template <int CT, int DT, bool DEV = false>
+// MODELS: an ensemble table, whose entries name their model (BagDev::pad_).  All members' Wi rows and biases are staged
+// in shared memory once (CT*D + kModelBiasFloats floats each); the producer streams the entry's W1 / W2 images.
+template <int CT, int DT, bool DEV = false, bool MODELS = false>
 __global__ void __launch_bounds__(kThreads, 1)
-k_qmlp_sm90(const QmlpArgs a) {
+k_qmlp_sm90(const QmlpArgsOf<MODELS> a) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment (SWIZZLE_128B atoms)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -225,9 +252,19 @@ k_qmlp_sm90(const QmlpArgs a) {
 
   float* sWi = reinterpret_cast<float*>(smem + kOffWi);
   const bool do_scores = a.classes != nullptr;   // bag form (scores given): Wi/bi may be NULL
-  if (do_scores)
-    for (int i = tid; i < CT * D; i += kThreads) sWi[i] = (i < C * D) ? a.Wi[i] : 0.f;
-  if (tid < kQ) { s_b1[tid] = a.b1[tid]; s_b2[tid] = a.b2[tid]; }
+  float* sMb = sWi + (MODELS ? nmodels_of(a) * CT * D : 0);   // MODELS: the members' biases
+  if (MODELS) {
+    for (int m = 0; m < nmodels_of(a); ++m) {
+      const ModelDev md = models_of(a)[m];
+      for (int i = tid; i < CT * D; i += kThreads) sWi[m * CT * D + i] = (i < C * D) ? md.Wi[i] : 0.f;
+      for (int i = tid; i < kModelBiasFloats; i += kThreads)
+        sMb[m * kModelBiasFloats + i] = i < kQ ? md.b1[i] : (i < 2 * kQ ? md.b2[i - kQ] : (i - 2 * kQ < C ? md.bi[i - 2 * kQ] : 0.f));
+    }
+  } else {
+    if (do_scores)
+      for (int i = tid; i < CT * D; i += kThreads) sWi[i] = (i < C * D) ? a.Wi[i] : 0.f;
+    if (tid < kQ) { s_b1[tid] = a.b1[tid]; s_b2[tid] = a.b2[tid]; }
+  }
   const bool tbl_in_smem = a.nb <= kSmemBags;
   if (tbl_in_smem)
     for (int i = tid; i < a.nb; i += kThreads) s_bags[i] = a.bags[i];
@@ -250,10 +287,22 @@ k_qmlp_sm90(const QmlpArgs a) {
         bulk_g2s(smem_u32(smem + kOffWRing + stage * kChunkBytes), src, kChunkBytes, bar(W_FULL + stage));
         if (++stage == kWStages) { stage = 0; phase ^= 1; }
       };
-      for (int tile = blockIdx.x; live(tile); tile += gridDim.x) {
-        for (int kc = 0; kc < nchunks; ++kc) push(a.w1img + static_cast<size_t>(kc) * kChunkBytes);
-        push(a.w2img);
-        push(a.w2img + kChunkBytes);
+      if (MODELS) {   // the entry's model's images
+        TileCursor pcur(tbl, a.nb);
+        for (int tile = blockIdx.x; live(tile); tile += gridDim.x) {
+          pcur.seek(tile);
+          const uint8_t* w1 = a.w1img + static_cast<size_t>(tbl[pcur.bag].pad_) * wimg_stride_of(a);
+          const uint8_t* w2 = w1 + static_cast<size_t>(nchunks) * kChunkBytes;
+          for (int kc = 0; kc < nchunks; ++kc) push(w1 + static_cast<size_t>(kc) * kChunkBytes);
+          push(w2);
+          push(w2 + kChunkBytes);
+        }
+      } else {
+        for (int tile = blockIdx.x; live(tile); tile += gridDim.x) {
+          for (int kc = 0; kc < nchunks; ++kc) push(a.w1img + static_cast<size_t>(kc) * kChunkBytes);
+          push(a.w2img);
+          push(a.w2img + kChunkBytes);
+        }
       }
     }
     return;
@@ -284,10 +333,12 @@ k_qmlp_sm90(const QmlpArgs a) {
   uint32_t ld_N = 0, ld_row = 0;               // rows in the bag, this thread's first row in the bag
   bool ld_full = false;                        // whole 128-row tile inside the bag: unpredicated loads
   long long ld_rowoff = 0;
+  int ld_model = 0;                            // MODELS: the entry's model
   const float* xrow = nullptr;
   auto open_tile = [&](int t) {
     cur_bag.seek(t);
     const BagDev* bp = tbl + cur_bag.bag;
+    if (MODELS) ld_model = bp->pad_;
     ld_N = static_cast<uint32_t>(bp->N);
     ld_rowoff = bp->row_off;
     ld_row = static_cast<uint32_t>(t - bp->tile_off) * kTileM + rloc;
@@ -310,6 +361,7 @@ k_qmlp_sm90(const QmlpArgs a) {
       }
   };
   float sc[2][CT];
+  uint32_t swi_t = swi_u32;                    // MODELS: this tile's model's Wi rows
   // scores of chunk kc + the bf16 hi/lo A fragments of its four k steps (register 4s + 2 pair + row half)
   // sWi rows >= C are zero-filled (CT rows are staged), so the class loop needs no bound check
   auto convert = [&](const float4 (&x)[8], int kc, uint32_t (&hi)[16], uint32_t (&lo)[16]) {
@@ -318,7 +370,7 @@ k_qmlp_sm90(const QmlpArgs a) {
       if (do_scores) {
 #pragma unroll
         for (int k = 0; k < CT; ++k) {
-          const float4 w = lds128(swi_u32 + static_cast<uint32_t>(k * D + kc * kChunkK + 16 * s) * 4u);
+          const float4 w = lds128((MODELS ? swi_t : swi_u32) + static_cast<uint32_t>(k * D + kc * kChunkK + 16 * s) * 4u);
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
             const float4 v = x[2 * s + i];
@@ -366,6 +418,8 @@ k_qmlp_sm90(const QmlpArgs a) {
     const int my_bag = cur_bag.bag;   // this tile's bag (the load state moves on below)
     const uint32_t t_N = ld_N, t_row = ld_row;
     const long long t_rowoff = ld_rowoff;
+    const int t_model = MODELS ? ld_model : 0;
+    if (MODELS) swi_t = swi_u32 + static_cast<uint32_t>(t_model * CT * D) * 4u;
     const int next_tile = tile + gridDim.x;
 #pragma unroll
     for (int i = 0; i < 2; ++i)
@@ -407,7 +461,7 @@ k_qmlp_sm90(const QmlpArgs a) {
           v += __shfl_xor_sync(0xffffffffu, v, 2);
           v += __shfl_xor_sync(0xffffffffu, v, 1);
           if (q == 0 && k < C && n < t_N) {
-            v += a.bi[k];
+            v += MODELS ? sMb[t_model * kModelBiasFloats + 2 * kQ + k] : a.bi[k];
             a.classes[(t_rowoff + n) * C + k] = v;
             const unsigned long long key = pack_key(v, n);
             best[k] = key > best[k] ? key : best[k];
@@ -425,7 +479,8 @@ k_qmlp_sm90(const QmlpArgs a) {
     uint32_t h2[32], l2[32];
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
-      const float2 bb = *reinterpret_cast<const float2*>(&s_b1[8 * j + 2 * q]);
+      const float2 bb = *reinterpret_cast<const float2*>(MODELS ? &sMb[t_model * kModelBiasFloats + 8 * j + 2 * q]
+                                                                : &s_b1[8 * j + 2 * q]);
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const float h0 = fmaxf(acc[4 * j + 2 * i] + bb.x, 0.f), h1 = fmaxf(acc[4 * j + 2 * i + 1] + bb.y, 0.f);
@@ -463,7 +518,7 @@ k_qmlp_sm90(const QmlpArgs a) {
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       const int c = 8 * j + 2 * q;
-      const float2 bb = *reinterpret_cast<const float2*>(&s_b2[c]);
+      const float2 bb = *reinterpret_cast<const float2*>(MODELS ? &sMb[t_model * kModelBiasFloats + kQ + c] : &s_b2[c]);
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const float z0 = qa[4 * j + 2 * i] + bb.x, z1 = qa[4 * j + 2 * i + 1] + bb.y;
@@ -492,9 +547,8 @@ k_qmlp_sm90(const QmlpArgs a) {
 }
 
 // one kernel for both images
-__global__ void __launch_bounds__(256)
-k_prep_wimg2(const float* __restrict__ W1, int D, const float* __restrict__ W2, uint8_t* __restrict__ img1,
-             uint8_t* __restrict__ img2) {
+__device__ __forceinline__ void prep_wimg2(const float* __restrict__ W1, int D, const float* __restrict__ W2,
+                                           uint8_t* __restrict__ img1, uint8_t* __restrict__ img2) {
   const int t1 = 128 * D, total = t1 + 128 * kQ;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const bool first = i < t1;
@@ -510,17 +564,34 @@ k_prep_wimg2(const float* __restrict__ W1, int D, const float* __restrict__ W2, 
     *reinterpret_cast<__nv_bfloat16*>(chunk + kTileBytes + off) = lo;
   }
 }
+__global__ void __launch_bounds__(256)
+k_prep_wimg2(const float* __restrict__ W1, int D, const float* __restrict__ W2, uint8_t* __restrict__ img1,
+             uint8_t* __restrict__ img2) {
+  prep_wimg2(W1, D, W2, img1, img2);
+}
+// the image pairs of an ensemble's members: model blockIdx.y at img + blockIdx.y * stride
+__global__ void __launch_bounds__(256)
+k_prep_wimg2_models(const ModelDev* __restrict__ models, int D, uint8_t* __restrict__ img, size_t stride) {
+  uint8_t* img1 = img + blockIdx.y * stride;
+  prep_wimg2(models[blockIdx.y].W1, D, models[blockIdx.y].W2, img1, img1 + static_cast<size_t>(D / kChunkK) * kChunkBytes);
+}
 
+inline int ct_of(int C) { return C <= 1 ? 1 : (C <= 2 ? 2 : (C <= 4 ? 4 : 8)); }
 inline size_t qmlp_smem_bytes(int C, int D) {   // Wi is staged with C rounded up to 1, 2, 4, 8 rows
-  const int ct = C <= 1 ? 1 : (C <= 2 ? 2 : (C <= 4 ? 4 : 8));
+  const int ct = ct_of(C);
   return kSmemFixed + sizeof(float) * ct * D + 1024;
+}
+// MODELS: the M members' Wi rows and biases
+inline size_t qmlp_models_smem_bytes(int C, int D, int M) {
+  return kSmemFixed + sizeof(float) * M * (static_cast<size_t>(ct_of(C)) * D + kModelBiasFloats) + 1024;
 }
 inline size_t wimg_bytes(int D) { return static_cast<size_t>(D / kChunkK) * kChunkBytes + 2 * kChunkBytes; }
 // 227 KB of shared memory per block on sm_90, less the kernel's static arrays (barriers, biases, bag table)
+constexpr size_t kQmlpStaticSmem = 2 * kQ * sizeof(float) + kSmemBags * sizeof(BagDev) + 256;
 inline bool qmlp_supported(const dsmil_params_t* p) {
-  return p->nonlinear && p->D % (2 * kChunkK) == 0 &&
-         qmlp_smem_bytes(p->C, p->D) + 2 * kQ * sizeof(float) + kSmemBags * sizeof(BagDev) + 256 <= 232448;
+  return p->nonlinear && p->D % (2 * kChunkK) == 0 && qmlp_smem_bytes(p->C, p->D) + kQmlpStaticSmem <= 232448;
 }
+inline bool qmlp_models_fit(int C, int D, int M) { return qmlp_models_smem_bytes(C, D, M) + kQmlpStaticSmem <= 232448; }
 
 inline int launch_prep_wimg(const dsmil_params_t* p, uint8_t* wimg, cudaStream_t st) {
   uint8_t* w2img = wimg + static_cast<size_t>(p->D / kChunkK) * kChunkBytes;
@@ -575,6 +646,39 @@ inline int launch_qmlp(const dsmil_params_t* p, const BagDev* bags_dev, int nb, 
   if (C == 2) return go(k_qmlp_sm90<2, 0>);
   if (C <= 4) return go(k_qmlp_sm90<4, 0>);
   return go(k_qmlp_sm90<8, 0>);
+}
+
+// Ensemble forms (models_dev: M members in device memory; table entries name their model).  The images of model m are
+// at wimg + m * wimg_bytes(D), which keeps each 1024-byte aligned.
+inline int launch_prep_wimg_models(const ModelDev* models_dev, int M, int D, uint8_t* wimg, cudaStream_t st) {
+  k_prep_wimg2_models<<<dim3(80, M), 256, 0, st>>>(models_dev, D, wimg, wimg_bytes(D));
+  DSMIL_LAUNCH_OK("k_prep_wimg2_models");
+  return 0;
+}
+// Scores, arg-max keys and tile-blocked Q of every entry; C <= 4 (the batched shapes), done as in launch_qmlp.
+inline int launch_qmlp_models(const ModelDev* models_dev, int M, int D, int C, const BagDev* bags_dev, int nb,
+                              int ntiles, float* classes, unsigned long long* keys, float* Q, const uint8_t* wimg,
+                              int max_ctas, cudaStream_t st, unsigned int* done) {
+  QmlpModelsArgs a{{bags_dev, nb, ntiles, D, C, nullptr, nullptr, nullptr, nullptr, wimg, nullptr, classes, keys, Q,
+                    nullptr, true, nullptr, done}, models_dev, M, wimg_bytes(D)};
+  const size_t smem = qmlp_models_smem_bytes(C, D, M);
+  const int grid = ntiles < max_ctas ? ntiles : max_ctas;
+  auto go = [&](auto kern) -> int {
+    DSMIL_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    prof_begin(PROF_FUSED, st);
+    kern<<<grid, kThreads, smem, st>>>(a);
+    prof_end(PROF_FUSED, st);
+    DSMIL_LAUNCH_OK("k_qmlp_sm90");
+    return 0;
+  };
+  if (D == 512) {
+    if (C == 1) return go(k_qmlp_sm90<1, 512, false, true>);
+    if (C == 2) return go(k_qmlp_sm90<2, 512, false, true>);
+    return go(k_qmlp_sm90<4, 512, false, true>);
+  }
+  if (C == 1) return go(k_qmlp_sm90<1, 0, false, true>);
+  if (C == 2) return go(k_qmlp_sm90<2, 0, false, true>);
+  return go(k_qmlp_sm90<4, 0, false, true>);
 }
 
 }  // namespace sm90

@@ -245,6 +245,46 @@ def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, 
     return loss, torch.stack(labels).cpu().numpy().astype(int), torch.stack(preds).cpu().numpy()
 
 
+def eval_epoch_models(milnets, store: DeviceBagStore, criterion, average: bool = False, bags_per_launch: int = 16):
+    """eval_epoch for an ensemble (the fold models of train_tcga.py:395-404) over the same bags: one (loss, labels,
+    preds) per model, each bit for bit `eval_epoch(milnets[m], store, criterion, average, bags_per_launch)` without
+    patch dropout.  Each group of bags_per_launch > 1 bags is one ensemble.forward_bags_models call, and the whole
+    call makes one host sync.  The thresholds and the vote over the models (train_tcga.py:113-124, 401-404) are the
+    caller's, on these arrays."""
+    from .ensemble import forward_bags_models
+    milnets = list(milnets)
+    for m in milnets:
+        m.eval()
+    n, k = len(store), max(1, bags_per_launch)
+    if n == 0:
+        raise ValueError("eval_epoch_models over an empty store")
+    losses = [[] for _ in milnets]
+    preds = [[] for _ in milnets]
+    with torch.no_grad():
+        for s in range(0, n, k):
+            group = store.bags[s:s + k]
+            xs = [f for f, _ in group]
+            # one bag per launch: each model's milnet(x), as eval_epoch takes it
+            outs = forward_bags_models(milnets, xs) if k > 1 else [[net(x) for x in xs] for net in milnets]
+            for m, out in enumerate(outs):
+                for (ins_prediction, bag_prediction, _, _), (_, label) in zip(out, group):
+                    max_prediction, _ = torch.max(ins_prediction, 0)
+                    losses[m].append(0.5 * criterion(bag_prediction.view(1, -1), label.view(1, -1)) +
+                                     0.5 * criterion(max_prediction.view(1, -1), label.view(1, -1)))
+                    p = torch.sigmoid(bag_prediction).view(-1)
+                    preds[m].append(torch.sigmoid(max_prediction).view(-1) + p if average else p)
+        M = len(milnets)
+        loss = torch.stack([torch.stack([l.reshape(()) for l in ls]).mean() for ls in losses])
+        labels = torch.stack([label.view(-1) for _, label in store.bags])
+        pred = torch.stack([torch.stack(ps) for ps in preds])
+        # the one host sync (float32 and the integer labels are exact in float64)
+        host = torch.cat([loss.double(), labels.double().view(-1), pred.double().view(-1)]).cpu().numpy()
+    C = int(labels.shape[1])
+    lab = host[M:M + n * C].reshape(n, C).astype(int)
+    pr = host[M + n * C:].reshape(M, n, C).astype(np.float32)
+    return [(float(host[m]), lab.copy(), pr[m]) for m in range(M)]
+
+
 # model -> {(bags per graph, max_rows, average): EvalBagsGraph}: later epochs replay the graphs of earlier ones (the
 # graphs read the parameters in place, so training between epochs is seen); kept off the model itself, as
 # embed._GRAPHS, so that deepcopy / pickling of the caller's model never meets a CUDA graph

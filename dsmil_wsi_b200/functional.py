@@ -426,6 +426,48 @@ def mil_forward_bags_dev(xs: torch.Tensor, Ns: torch.Tensor, status: torch.Tenso
     return classes, pred, A, B, crit
 
 
+MAX_MODELS = 8   # members of one dsmil_forward_bags_models call
+
+
+@torch.no_grad()
+def mil_forward_bags_models(bags: Sequence[torch.Tensor], params_list: Sequence[Sequence[Optional[torch.Tensor]]]):
+    """An ensemble forward: M parameter sets (1 <= M <= 8, the same D, C and q form, identity v) over the same bags in
+    one dsmil_forward_bags_models call.  Returns M BagOutputs, one per model, over model-major packed tensors, each
+    with `.crit` [nb, C]; model m's are bit for bit what mil_forward_bags(bags, params_list[m]) gives.  On the batched
+    tensor-core shapes the whole ensemble costs one launch of each kernel and the passes over a bag follow each
+    other while it is in L2."""
+    lib = _lib.load()
+    packs = [ParamPack(*p) for p in params_list]
+    M = len(packs)
+    if not 1 <= M <= MAX_MODELS:
+        raise ValueError(f"an ensemble forward takes 1 to {MAX_MODELS} models, got {M}")
+    P0 = packs[0]
+    for m, P in enumerate(packs[1:], 1):
+        for what in ("D", "C", "nonlinear", "passing_v"):
+            if getattr(P, what) != getattr(P0, what):
+                raise ValueError(f"model {m}: {what}={getattr(P, what)} differs from model 0's {getattr(P0, what)}")
+        if P.device != P0.device:
+            raise ValueError(f"model {m} is on {P.device}, model 0 on {P0.device}")
+    if P0.passing_v:
+        raise NotImplementedError("forward_bags: passing_v models go through MILNet.forward per bag")
+    nb = len(bags)
+    if nb == 0:
+        return [BagOutputs(None, None, None, None, [], None) for _ in range(M)]
+    xs, Ns, c_X, c_N = _bag_table(bags, P0)
+    total, Cc, D, dev = sum(Ns), P0.C, P0.D, P0.device
+    ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
+    with torch.cuda.device(dev):
+        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        classes, A = new(M, total, Cc), new(M, total, Cc)
+        pred, B = new(M, nb, Cc), new(M, nb, Cc, D)
+        crit = torch.empty(M, nb, Cc, dtype=torch.int64, device=dev)
+        ws = _workspace(lib.dsmil_forward_bags_models_workspace_bytes(ps, M, c_N, nb), dev)
+        rc = lib.dsmil_forward_bags_models(ps, M, c_X, c_N, nb, _ptr(classes), _ptr(pred), _ptr(A), _ptr(B),
+                                           _ptr(crit), _ptr(ws), ws.numel(), _stream())
+        _lib.check(rc, "dsmil_forward_bags_models")
+    return [BagOutputs(classes[m], pred[m], A[m], B[m], Ns, crit[m]) for m in range(M)]
+
+
 @torch.no_grad()
 def _mil_forward_bags_infer(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]]):
     lib = _lib.load()

@@ -149,6 +149,22 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
  * has finished.  The grid changes no result; tests use it to place batches at its edges.  0 for tiles < 1. */
 int32_t dsmil_forward_bags_phase1_ctas(int64_t tiles);
 
+/* An ensemble of M models (1 <= M <= 8, e.g. the fold models of a cross-validation) over the same batch of bags in
+ * one call.  ps[0..M-1] are M parameter sets with the same D, C, nonlinear and passing_v, each valid for
+ * dsmil_forward_bags; otherwise DSMIL_ERR_ARG before any CUDA work.  Outputs are model-major: classes / A
+ * [M, sum N, C], pred [M, nb, C], B [M, nb, C, D], crit_idx [M, nb, C] (or NULL).  Slice m is, bit for bit, what
+ * dsmil_forward_bags(&ps[m], ...) writes for the same bags.
+ * dsmil_models_supported: the ensemble runs fused -- one weight-image prep, one phase-1, one attend and one finalize
+ * launch for all M models, the M passes over a bag following each other while it is in L2 -- when every member is on
+ * dsmil_shard_bags_supported and the M members' weights fit in shared memory; the call also needs every bag 16-byte
+ * aligned.  Other calls loop dsmil_forward_bags over the models into the same slices.  The workspace size covers
+ * both forms and is never below dsmil_forward_bags_workspace_bytes for the same bags; 0 for invalid arguments. */
+int dsmil_models_supported(const dsmil_params_t* ps, int32_t M);
+size_t dsmil_forward_bags_models_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int64_t* Ns, int32_t nb);
+int dsmil_forward_bags_models(const dsmil_params_t* ps, int32_t M, const float* const* Xs, const int64_t* Ns,
+                              int32_t nb, float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                              void* workspace, size_t workspace_bytes, void* stream);
+
 /* Training form of dsmil_forward_bags: the same packed outputs, plus save_Q [sum N,128] (after the tanh) and, for a
  * nonlinear q, save_H1 [sum N,128], packed in bag order -- what dsmil_backward_bags needs.  crit_idx [nb,C] is
  * required; its entries are rows within each bag.  Identity v only (passing_v: DSMIL_ERR_ARG).  Shapes or bags off
