@@ -685,8 +685,11 @@ static bool models_batched(const dsmil_params_t* ps, int M) {
 struct ModelsWs : BagsWs {
   sm90::ModelDev* models;   // [M]
 };
-static ModelsWs carve_models(const dsmil_params_t* p, int M, const int64_t* Ns, int nb, void* ws, size_t cap,
-                             bool* ok) {
+// The fused layout of M members over a table of nb * reps entries: the nb bags Ns, each `reps` times (the ensemble
+// forward: reps = M, every model over the same bags; the training form: reps = 1, every model's own bags listed
+// model-major).  need_Q: room for tile-blocked Q (the training form writes the caller's row-major save_Q instead).
+static ModelsWs carve_models(const dsmil_params_t* p, int M, const int64_t* Ns, int nb, int reps, bool need_Q,
+                             void* ws, size_t cap, bool* ok) {
   Carver c(ws, cap);
   ModelsWs w;
   int64_t tiles = 0, nrec = 0;
@@ -694,7 +697,7 @@ static ModelsWs carve_models(const dsmil_params_t* p, int M, const int64_t* Ns, 
     tiles += tiles_for_bag(Ns[b]);
     nrec += recs_for_bag(Ns[b]);
   }
-  const size_t ne = static_cast<size_t>(nb) * M;
+  const size_t ne = static_cast<size_t>(nb) * reps;
   w.table = c.take<sm90::BagDev>(ne);
   w.keys = c.take<unsigned long long>(ne * (kMaxC + 1));   // keys, then the two per-entry counters (carve_phase1)
   w.counters = reinterpret_cast<unsigned int*>(w.keys ? w.keys + ne * kMaxC : nullptr);
@@ -703,8 +706,8 @@ static ModelsWs carve_models(const dsmil_params_t* p, int M, const int64_t* Ns, 
   const uintptr_t img = reinterpret_cast<uintptr_t>(c.take<uint8_t>(M * sm90::wimg_bytes(p->D) + 1024));
   w.wimg = reinterpret_cast<uint8_t*>((img + 1023) & ~uintptr_t(1023));
   w.pred_part = c.take<float>(ne * sm90::kFinSlices * kMaxC);
-  w.Q = c.take<float>(static_cast<size_t>(M) * tiles * sm90::kTileM * kQ);
-  w.recs = c.take<float>(static_cast<size_t>(M) * nrec * rec_floats(p->C, p->D));
+  w.Q = need_Q ? c.take<float>(static_cast<size_t>(reps) * tiles * sm90::kTileM * kQ) : nullptr;
+  w.recs = c.take<float>(static_cast<size_t>(reps) * nrec * rec_floats(p->C, p->D));
   w.row_offsets = nullptr;
   w.qmax = nullptr;
   w.bytes = c.off;
@@ -712,12 +715,45 @@ static ModelsWs carve_models(const dsmil_params_t* p, int M, const int64_t* Ns, 
   return w;
 }
 
+// The fused launches over a host table `tbl` (tiles / recs: its 128-row tiles and partial records): one weight-image
+// prep, one phase 1, one attend and one finalize for all M members.  Q (+ H1) as launch_qmlp_models takes them.
+// nb_out > 0: the ensemble's table, whose entry b * M + m writes pred / B / crit to slot m * nb_out + b; nb_out == 0:
+// a table of each model's own bags, model-major, whose entry e writes slot e.
+static int models_launch(const dsmil_params_t* ps, int M, const ModelsWs& w, const std::vector<sm90::BagDev>& tbl,
+                         int tile, int rec, float* classes, float* Q, float* H1, bool q_blocked, float* pred, float* A,
+                         float* B, int64_t* crit, int nb_out, cudaStream_t st) {
+  const int C = ps[0].C, D = ps[0].D, ne = static_cast<int>(tbl.size());
+  int rc;
+  std::vector<sm90::ModelDev> mh(M);
+  for (int m = 0; m < M; ++m) {
+    const dsmil_params_t& p = ps[m];
+    mh[m] = sm90::ModelDev{p.Wi, p.bi, p.W1, p.b1, p.W2, p.b2, p.Wf, p.bf};
+  }
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * ne, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.models, mh.data(), sizeof(sm90::ModelDev) * M, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * ne, st));
+  if ((rc = sm90::launch_prep_wimg_models(w.models, M, D, w.wimg, st))) return rc;
+  // overlapped as in forward_bags_impl: not under capture, not while kernels are timed
+  const bool overlap = !g_prof_on && !stream_is_capturing(st);
+  if ((rc = sm90::launch_qmlp_models(w.models, M, D, C, w.table, ne, tile, classes, w.keys, Q, H1, q_blocked, w.wimg,
+                                     overlap ? overlap_phase1_ctas(tile) : num_sms(), st,
+                                     overlap ? w.done : nullptr)))
+    return rc;
+  sm90::AttendArgs aa{w.table, ne, D, C, Q, q_blocked, w.keys, A, w.recs, nullptr, nullptr, overlap ? w.done : nullptr};
+  if ((rc = sm90::launch_attend_b(aa, rec, st))) return rc;
+  // slot = pad_ * nb_out + entry / nmodels: nmodels = 1 and nb_out = 0 make it the entry itself
+  sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, nullptr, nullptr, A, B, pred,
+                        reinterpret_cast<long long*>(crit), w.pred_part, w.counters, nullptr, 0, 0,
+                        w.models, nb_out > 0 ? M : 1, nb_out};
+  return sm90::launch_finalize_b(fa, ne, st);
+}
+
 static int forward_bags_models_impl(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
                                     int nb, int64_t total, float* classes, float* pred, float* A, float* B,
                                     int64_t* crit, void* ws, size_t ws_bytes, cudaStream_t st) {
-  const int C = ps[0].C, D = ps[0].D, ne = nb * M;
+  const int ne = nb * M;
   bool ok;
-  ModelsWs w = carve_models(&ps[0], M, Ns, nb, ws, ws_bytes, &ok);
+  ModelsWs w = carve_models(&ps[0], M, Ns, nb, M, true, ws, ws_bytes, &ok);
   int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
   if (rc) return rc;
   std::vector<sm90::BagDev> tbl(ne);
@@ -733,27 +769,7 @@ static int forward_bags_models_impl(const dsmil_params_t* ps, int M, const float
     }
     row += Ns[b];
   }
-  std::vector<sm90::ModelDev> mh(M);
-  for (int m = 0; m < M; ++m) {
-    const dsmil_params_t& p = ps[m];
-    mh[m] = sm90::ModelDev{p.Wi, p.bi, p.W1, p.b1, p.W2, p.b2, p.Wf, p.bf};
-  }
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * ne, cudaMemcpyHostToDevice, st));
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.models, mh.data(), sizeof(sm90::ModelDev) * M, cudaMemcpyHostToDevice, st));
-  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * ne, st));
-  if ((rc = sm90::launch_prep_wimg_models(w.models, M, D, w.wimg, st))) return rc;
-  // overlapped as in forward_bags_impl: not under capture, not while kernels are timed
-  const bool overlap = !g_prof_on && !stream_is_capturing(st);
-  if ((rc = sm90::launch_qmlp_models(w.models, M, D, C, w.table, ne, tile, classes, w.keys, w.Q, w.wimg,
-                                     overlap ? overlap_phase1_ctas(tile) : num_sms(), st,
-                                     overlap ? w.done : nullptr)))
-    return rc;
-  sm90::AttendArgs aa{w.table, ne, D, C, w.Q, true, w.keys, A, w.recs, nullptr, nullptr, overlap ? w.done : nullptr};
-  if ((rc = sm90::launch_attend_b(aa, rec, st))) return rc;
-  sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, nullptr, nullptr, A, B, pred,
-                        reinterpret_cast<long long*>(crit), w.pred_part, w.counters, nullptr, 0, 0,
-                        w.models, M, nb};
-  return sm90::launch_finalize_b(fa, ne, st);
+  return models_launch(ps, M, w, tbl, tile, rec, classes, w.Q, nullptr, true, pred, A, B, crit, nb, st);
 }
 
 int dsmil_models_supported(const dsmil_params_t* ps, int32_t M) {
@@ -772,7 +788,7 @@ size_t dsmil_forward_bags_models_workspace_bytes(const dsmil_params_t* ps, int32
   // the fused layout on every batched shape, whether or not M members fit in shared memory: the size then grows with
   // M, nb and N alike
   bool ok;
-  if (models_batched(ps, M)) bytes = std::max(bytes, carve_models(&ps[0], M, Ns, nb, nullptr, 0, &ok).bytes);
+  if (models_batched(ps, M)) bytes = std::max(bytes, carve_models(&ps[0], M, Ns, nb, M, true, nullptr, 0, &ok).bytes);
   return bytes;
 }
 
@@ -1482,6 +1498,390 @@ int dsmil_backward_bags(const dsmil_params_t* p, const float* const* Xs, const i
   if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
   return backward_bags_impl(p, Xs, Ns, nb, total, aligned, Q, H1, A, B, crit_idx, d_classes, d_pred, d_A, d_B, grads,
                             workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+// ---- the fold models of a cross-validation in one training step: each model over its own bags ---------------------
+// Model m's bags are entries [bag[m], bag[m + 1]) of Xs / Ns; its rows start at packed row row[m].  Per-row buffers are
+// packed model-major, and so are the per-bag ones.
+struct ModelsBags {
+  std::vector<int> bag;
+  std::vector<int64_t> row;
+  int ne;          // entries: the bags of all models
+  bool aligned;    // every bag 16-byte aligned
+};
+static int check_models_bags(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
+                             const int32_t* nbs, ModelsBags* mb) {
+  int rc = check_models(ps, M);
+  if (rc) return rc;
+  DSMIL_REQUIRE(!ps[0].passing_v, "batched training supports the identity v only (passing_v: one bag per call)");
+  DSMIL_REQUIRE(Xs && Ns && nbs, "NULL bag list");
+  mb->bag.assign(M + 1, 0);
+  mb->row.assign(M + 1, 0);
+  for (int m = 0; m < M; ++m) {
+    DSMIL_REQUIRE(nbs[m] >= 1 && nbs[m] <= 65535, "model %d: nb=%d outside [1, 65535]", m, nbs[m]);
+    mb->bag[m + 1] = mb->bag[m] + nbs[m];
+  }
+  mb->ne = mb->bag[M];
+  for (int m = 0; m < M; ++m) {
+    int64_t rows;
+    bool al;
+    if ((rc = check_bags(Xs + mb->bag[m], Ns + mb->bag[m], nbs[m], &rows, &al))) return rc;
+    mb->row[m + 1] = mb->row[m] + rows;
+    mb->aligned = (m == 0 || mb->aligned) && al;
+  }
+  return 0;
+}
+// The loop route gives each model its own slice of the workspace, 256-byte aligned.
+static size_t ws_slice(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+
+size_t dsmil_forward_bags_models_train_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int64_t* Ns,
+                                                       const int32_t* nbs) {
+  if (!ps || M < 1 || M > sm90::kMaxModels || !Ns || !nbs) return 0;
+  size_t loop = 0;
+  int ne = 0;
+  for (int m = 0; m < M; ++m) {
+    if (nbs[m] < 1) return 0;
+    const size_t b = dsmil_forward_bags_train_workspace_bytes(&ps[m], Ns + ne, nbs[m]);
+    if (b == 0) return 0;
+    loop += ws_slice(b);
+    ne += nbs[m];
+  }
+  bool ok;
+  if (!models_batched(ps, M)) return loop;
+  return std::max(loop, carve_models(&ps[0], M, Ns, ne, 1, false, nullptr, 0, &ok).bytes);
+}
+
+int dsmil_forward_bags_models_train(const dsmil_params_t* ps, int32_t M, const float* const* Xs, const int64_t* Ns,
+                                    const int32_t* nbs, float* classes, float* pred, float* A, float* B,
+                                    int64_t* crit_idx, float* save_Q, float* save_H1, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  ModelsBags mb;
+  int rc = check_models_bags(ps, M, Xs, Ns, nbs, &mb);
+  if (rc) return rc;
+  DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && (!ps[0].nonlinear || save_H1),
+                "NULL output pointer");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t need = dsmil_forward_bags_models_train_workspace_bytes(ps, M, Ns, nbs);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  const int C = ps[0].C, D = ps[0].D;
+  if (mb.aligned && dsmil_models_supported(ps, M) && mb.ne <= 65535) {
+    bool ok;
+    ModelsWs w = carve_models(&ps[0], M, Ns, mb.ne, 1, false, workspace, workspace_bytes, &ok);
+    if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
+    // entry e is bag e of the list, its model in pad_; rows and tiles numbered across all models
+    std::vector<sm90::BagDev> tbl(mb.ne);
+    long long row = 0;
+    int tile = 0, rec = 0;
+    for (int m = 0; m < M; ++m)
+      for (int e = mb.bag[m]; e < mb.bag[m + 1]; ++e) {
+        tbl[e] = bag_entry(Xs[e], Ns[e], row, tile, rec);
+        tbl[e].pad_ = m;
+      }
+    return models_launch(ps, M, w, tbl, tile, rec, classes, save_Q, save_H1, false, pred, A, B, crit_idx, 0, st);
+  }
+  // off the fused route: each model's dsmil_forward_bags_train into its slices
+  size_t off = 0;
+  for (int m = 0; m < M; ++m) {
+    const int b0 = mb.bag[m];
+    const int64_t r0 = mb.row[m];
+    const size_t wb = dsmil_forward_bags_train_workspace_bytes(&ps[m], Ns + b0, nbs[m]);
+    rc = dsmil_forward_bags_train(&ps[m], Xs + b0, Ns + b0, nbs[m], classes + r0 * C, pred + static_cast<size_t>(b0) * C,
+                                  A + r0 * C, B + static_cast<size_t>(b0) * C * D, crit_idx + static_cast<size_t>(b0) * C,
+                                  save_Q + r0 * kQ, save_H1 ? save_H1 + r0 * kQ : nullptr,
+                                  static_cast<char*>(workspace) + off, wb, stream);
+    if (rc) return rc;
+    off += ws_slice(wb);
+  }
+  return 0;
+}
+
+// The fused backward's host plan: every split the one-model backward would choose for each model's own batch, on
+// the model-major packing.  Xs == NULL: counts only (the workspace size); H1 may then be NULL too.
+struct BwdModelsPlan {
+  std::vector<sm90::BagDev> table;                 // per entry: X, N, row_off; tile_off = G_m, rec_off, pad_ = m
+  std::vector<TnChunk> chi, ch1, ch2, chc;         // gWi, gW1, gW2 and the column sums' chunks
+  std::vector<int> nci, nc1, nc2, ncs;             // per model
+  int Gmax = 1, slots = 0;                         // largest G, per-CTA partial slots of all entries
+  int64_t max_rows = 1;                            // rows of the largest model
+};
+static void plan_bwd_models(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
+                            const int32_t* nbs, const float* H1, BwdModelsPlan& pl) {
+  const int C = ps[0].C, D = ps[0].D;
+  const bool gemv = tn_use_gemv(C, D);   // the fused route has every bag 16-byte aligned
+  pl.nci.assign(M, 0); pl.nc1.assign(M, 0); pl.nc2.assign(M, 0); pl.ncs.assign(M, 0);
+  int e = 0;
+  long long row = 0;
+  for (int m = 0; m < M; ++m) {
+    const int nb = nbs[m];
+    const int64_t* N = Ns + e;
+    int64_t total = 0, mx = 1;
+    for (int b = 0; b < nb; ++b) {
+      total += N[b];
+      mx = std::max<int64_t>(mx, N[b]);
+    }
+    const long long r0 = row;
+    const int G = bwd_bags_ctas(nb, mx);
+    pl.Gmax = std::max(pl.Gmax, G);
+    pl.max_rows = std::max(pl.max_rows, total);
+    for (int b = 0; b < nb; ++b, ++e) {
+      pl.table.push_back(sm90::BagDev{Xs ? Xs[e] : nullptr, N[b], row, G, pl.slots, 0, m});
+      row += N[b];
+      pl.slots += G;
+    }
+    // gWi and gW1: chunks of each bag's rows, as carve_bwd_bags cuts them
+    auto rag = [&](std::vector<TnChunk>& out, int64_t rps) {
+      const int n = rag_chunks(nullptr, N, nb, D, rps, nullptr);
+      const size_t at = out.size();
+      out.resize(at + n);
+      if (Xs) {
+        rag_chunks(Xs + (e - nb), N, nb, D, rps, out.data() + at);
+        for (int z = 0; z < n; ++z) out[at + z].prow += r0;
+      }
+      return n;
+    };
+    pl.nci[m] = rag(pl.chi, rag_rows_per_chunk(C, D, total, gemv));
+    pl.nc1[m] = rag(pl.ch1, rag_rows_per_chunk(kQ, D, total, false));
+    // gW2 = dz2^T H1 and the column sums: launch_gemm_tn's tile form and launch_colsum split the model's rows
+    const RowSplit t2 = gemm_tn_split(kQ, kQ, total), cs = colsum_split(total);
+    for (int z = 0; z < t2.S; ++z) {
+      const long long lo = z * t2.rps;
+      pl.ch2.push_back(TnChunk{H1 ? H1 + (r0 + lo) * kQ : nullptr, r0 + lo, std::min<long long>(total, lo + t2.rps) - lo});
+    }
+    for (int z = 0; z < cs.S; ++z) {
+      const long long lo = z * cs.rps;
+      pl.chc.push_back(TnChunk{nullptr, r0 + lo, std::min<long long>(total, lo + cs.rps) - lo});
+    }
+    pl.nc2[m] = t2.S;
+    pl.ncs[m] = cs.S;
+  }
+}
+
+struct BwdModelsWs {
+  sm90::BagDev* table;
+  BwdModelDev* models;
+  TnChunk *chi, *ch1, *ch2, *chc;
+  SumSeg* segs;              // [6][M]: gWi, gbi, gW2, gb2, gW1, gb1
+  LinSeg* lin;               // [2][M]: dz1, gX
+  float *dB, *dA, *dL, *tpart, *dpart, *dqm, *dz2, *dz1, *part;
+  size_t bytes;
+};
+static BwdModelsWs carve_bwd_models(const dsmil_params_t* ps, int M, const BwdModelsPlan& pl, int64_t total,
+                                    void* ws, size_t cap, bool* ok) {
+  const int C = ps[0].C, D = ps[0].D;
+  const size_t ne = pl.table.size(), T = std::max<int64_t>(total, 1);
+  Carver c(ws, cap);
+  BwdModelsWs w;
+  w.table = c.take<sm90::BagDev>(ne);
+  w.models = c.take<BwdModelDev>(M);
+  w.chi = c.take<TnChunk>(pl.chi.size());
+  w.ch1 = c.take<TnChunk>(pl.ch1.size());
+  w.ch2 = c.take<TnChunk>(pl.ch2.size());
+  w.chc = c.take<TnChunk>(pl.chc.size());
+  w.segs = c.take<SumSeg>(6 * M);
+  w.lin = c.take<LinSeg>(2 * M);
+  w.dB = c.take<float>(ne * C * D);
+  w.dA = c.take<float>(T * C);
+  w.dL = c.take<float>(T * C);
+  w.tpart = c.take<float>(static_cast<size_t>(pl.slots) * C);
+  w.dpart = c.take<float>(static_cast<size_t>(pl.slots) * C * kQ);
+  w.dqm = c.take<float>(ne * C * kQ);
+  w.dz2 = c.take<float>(T * kQ);
+  w.dz1 = c.take<float>(T * kQ);
+  size_t part = pl.chi.size() * C * D;
+  part = std::max(part, pl.ch1.size() * kQ * D);
+  part = std::max(part, pl.ch2.size() * kQ * kQ);
+  part = std::max(part, pl.chc.size() * kQ);
+  w.part = c.take<float>(part);
+  w.bytes = c.off;
+  *ok = c.ok();
+  return w;
+}
+
+// One launch per stage for all M models (nonlinear q, C <= 4: the dsmil_models_supported shapes; aligned bags).
+static int backward_bags_models_impl(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
+                                     const int32_t* nbs, const ModelsBags& mb, const float* Q, const float* H1,
+                                     const float* A, const float* B, const int64_t* crit, const float* d_classes,
+                                     const float* d_pred, const float* d_A, const float* d_B,
+                                     const dsmil_grads_t* g, void* ws, size_t ws_bytes, cudaStream_t st) {
+  const int C = ps[0].C, D = ps[0].D, ne = mb.ne;
+  BwdModelsPlan pl;
+  plan_bwd_models(ps, M, Xs, Ns, nbs, H1, pl);
+  bool ok;
+  BwdModelsWs w = carve_bwd_models(ps, M, pl, mb.row[M], ws, ws_bytes, &ok);
+  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+  if (rc) return rc;
+  std::vector<BwdModelDev> md(M);
+  std::vector<SumSeg> segs(6 * M);
+  std::vector<LinSeg> lin(2 * M);
+  bool any_gX = false;
+  int zi = 0, z1 = 0, z2 = 0;
+  for (int m = 0; m < M; ++m) {
+    const long long r0 = mb.row[m], rows = mb.row[m + 1] - r0;
+    md[m] = BwdModelDev{ps[m].Wf, ps[m].Wi, g[m].gWf, g[m].gbf, g[m].gX, mb.bag[m], nbs[m], r0};
+    const bool dc = d_classes != nullptr;
+    segs[0 * M + m] = SumSeg{dc ? g[m].gWi : nullptr, zi, pl.nci[m]};
+    segs[1 * M + m] = SumSeg{dc ? g[m].gbi : nullptr, 0, 0};   // z0 filled below: the column-sum chunks
+    segs[2 * M + m] = SumSeg{g[m].gW2, z2, pl.nc2[m]};
+    segs[3 * M + m] = SumSeg{g[m].gb2, 0, 0};
+    segs[4 * M + m] = SumSeg{g[m].gW1, z1, pl.nc1[m]};
+    segs[5 * M + m] = SumSeg{g[m].gb1, 0, 0};
+    zi += pl.nci[m];
+    z1 += pl.nc1[m];
+    z2 += pl.nc2[m];
+    lin[m] = LinSeg{w.dz2 + r0 * kQ, ps[m].W2, H1 + r0 * kQ, w.dz1 + r0 * kQ, rows};
+    lin[M + m] = LinSeg{w.dz1 + r0 * kQ, ps[m].W1, nullptr, g[m].gX, rows};
+    any_gX = any_gX || g[m].gX != nullptr;
+    if (!dc) {   // no gradient through the scores: zero instance-classifier gradients, as the one-model call
+      if (g[m].gWi) DSMIL_CUDA_OK(cudaMemsetAsync(g[m].gWi, 0, sizeof(float) * C * D, st));
+      if (g[m].gbi) DSMIL_CUDA_OK(cudaMemsetAsync(g[m].gbi, 0, sizeof(float) * C, st));
+    }
+  }
+  for (int m = 0, zc = 0; m < M; zc += pl.ncs[m], ++m)
+    for (int r : {1, 3, 5}) {
+      segs[r * M + m].z0 = zc;
+      segs[r * M + m].S = pl.ncs[m];
+    }
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, pl.table.data(), sizeof(sm90::BagDev) * ne, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.models, md.data(), sizeof(BwdModelDev) * M, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.chi, pl.chi.data(), sizeof(TnChunk) * pl.chi.size(), cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.ch1, pl.ch1.data(), sizeof(TnChunk) * pl.ch1.size(), cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.ch2, pl.ch2.data(), sizeof(TnChunk) * pl.ch2.size(), cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.chc, pl.chc.data(), sizeof(TnChunk) * pl.chc.size(), cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.segs, segs.data(), sizeof(SumSeg) * 6 * M, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.lin, lin.data(), sizeof(LinSeg) * 2 * M, cudaMemcpyHostToDevice, st));
+
+  // each model's partials into its gradients: reduction r of the six
+  auto sums = [&](int r, int64_t L) -> int {
+    k_sum_partials_models<<<dim3(static_cast<unsigned>(ceil_div(L, 32)), M), 256, 0, st>>>(w.part, w.segs + r * M, L);
+    DSMIL_LAUNCH_OK("k_sum_partials_models");
+    return 0;
+  };
+  auto colsums = [&](const float* P, int L, int r) -> int {
+    k_colsum_rag<<<static_cast<unsigned>(pl.chc.size()), 256, 0, st>>>(P, L, w.chc, w.part);
+    DSMIL_LAUNCH_OK("k_colsum_rag");
+    return sums(r, L);
+  };
+  const dim3 per_entry(pl.Gmax, ne);
+  // phase 1: bag classifier, instance classifier, dA and t's partials
+  k_bwd_bag_models<<<dim3(ceil_div(static_cast<int64_t>(C) * D, 256), M), 256, 0, st>>>(w.models, B, d_pred, d_B, C,
+                                                                                       D, w.dB);
+  DSMIL_LAUNCH_OK("k_bwd_bag_models");
+  if (d_classes) {
+    const int nz = static_cast<int>(pl.chi.size());
+    if (tn_use_gemv(C, D)) {
+      switch (C) {
+        case 1: k_gemv_tn_rag<1><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nullptr); break;
+        case 2: k_gemv_tn_rag<2><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nullptr); break;
+        case 3: k_gemv_tn_rag<3><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nullptr); break;
+        default: k_gemv_tn_rag<4><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nullptr); break;
+      }
+      DSMIL_LAUNCH_OK("k_gemv_tn_rag");
+    } else {
+      k_gemm_tn_rag<<<dim3(ceil_div(D, TBM), ceil_div(C, TBM), nz), 256, 0, st>>>(d_classes, C, D, w.chi, w.part,
+                                                                                 nullptr);
+      DSMIL_LAUNCH_OK("k_gemm_tn_rag");
+    }
+    if ((rc = sums(0, static_cast<int64_t>(C) * D)) || (rc = colsums(d_classes, C, 1))) return rc;
+  }
+  const size_t smem = sizeof(float) * C * D;
+  if (smem > 48 * 1024)
+    DSMIL_CUDA_OK(cudaFuncSetAttribute(k_bwd_rowdot_models, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_bwd_rowdot_models<<<per_entry, 256, smem, st>>>(w.table, D, w.dB, C, A, d_A, w.dA, w.tpart);
+  DSMIL_LAUNCH_OK("k_bwd_rowdot_models");
+  // phase 2: dL and dq_max
+  k_bwd_dL_models<<<per_entry, 256, 0, st>>>(w.table, C, A, w.dA, w.tpart, Q, w.dL, w.dpart);
+  DSMIL_LAUNCH_OK("k_bwd_dL_models");
+  k_sum_segments_models<<<dim3(ceil_div(C * kQ, 256), ne), 256, 0, st>>>(w.table, w.dpart, C * kQ, w.dqm);
+  DSMIL_LAUNCH_OK("k_sum_segments_models");
+  // phase 3: dz2, back through the Q-MLP
+  k_bwd_dq_b<<<per_entry, 256, 0, st>>>(w.table, C, w.dL, Q, nullptr, w.dqm, crit, nullptr, 1, w.dz2);
+  DSMIL_LAUNCH_OK("k_bwd_dq_b");
+  k_gemm_tn_rag<<<dim3(1, 1, static_cast<unsigned>(pl.ch2.size())), 256, 0, st>>>(w.dz2, kQ, kQ, w.ch2, w.part,
+                                                                                   nullptr);
+  DSMIL_LAUNCH_OK("k_gemm_tn_rag");
+  if ((rc = sums(2, static_cast<int64_t>(kQ) * kQ)) || (rc = colsums(w.dz2, kQ, 3))) return rc;
+  const unsigned row_tiles = static_cast<unsigned>(ceil_div(pl.max_rows, LBM));
+  k_linear_models<ACT_MASK_POS, true><<<dim3(row_tiles, 1, M), 256, 0, st>>>(w.lin, kQ, kQ);
+  DSMIL_LAUNCH_OK("k_linear_models");
+  k_gemm_tn_rag<<<dim3(ceil_div(D, TBM), 1, static_cast<unsigned>(pl.ch1.size())), 256, 0, st>>>(w.dz1, kQ, D, w.ch1,
+                                                                                                 w.part, nullptr);
+  DSMIL_LAUNCH_OK("k_gemm_tn_rag");
+  if ((rc = sums(4, static_cast<int64_t>(kQ) * D)) || (rc = colsums(w.dz1, kQ, 5))) return rc;
+  if (any_gX) {
+    k_linear_models<ACT_NONE, true><<<dim3(row_tiles, ceil_div(D, LBN), M), 256, 0, st>>>(w.lin + M, kQ, D);
+    DSMIL_LAUNCH_OK("k_linear_models");
+    k_bwd_dx_extra_models<<<per_entry, 256, 0, st>>>(w.table, w.models, d_classes, A, w.dB, C, D);
+    DSMIL_LAUNCH_OK("k_bwd_dx_extra_models");
+  }
+  return 0;
+}
+// Whether the fused backward takes these members and bags: the forward's fused shapes, aligned bags, and every grid
+// within its limits.
+static bool bwd_models_fused(const dsmil_params_t* ps, int M, const int64_t* Ns, const int32_t* nbs, int ne,
+                             bool aligned) {
+  if (!aligned || ne > 65535 || !dsmil_models_supported(ps, M)) return false;
+  BwdModelsPlan pl;
+  plan_bwd_models(ps, M, nullptr, Ns, nbs, nullptr, pl);
+  return pl.chi.size() <= 65535 && pl.ch1.size() <= 65535 && pl.ch2.size() <= 65535;
+}
+
+size_t dsmil_backward_bags_models_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int64_t* Ns,
+                                                  const int32_t* nbs, int need_gX) {
+  if (!ps || M < 1 || M > sm90::kMaxModels || !Ns || !nbs) return 0;
+  size_t bytes = 0;
+  int ne = 0;
+  for (int m = 0; m < M; ++m) {
+    if (nbs[m] < 1) return 0;
+    const size_t b = dsmil_backward_bags_workspace_bytes(&ps[m], Ns + ne, nbs[m], need_gX);
+    if (b == 0) return 0;
+    bytes += ws_slice(b);
+    ne += nbs[m];
+  }
+  if (!models_batched(ps, M)) return bytes;
+  // the fused layout on every batched shape, so the size grows with M, the bags and the rows alike
+  BwdModelsPlan pl;
+  plan_bwd_models(ps, M, nullptr, Ns, nbs, nullptr, pl);
+  int64_t total = 0;
+  for (int e = 0; e < ne; ++e) total += Ns[e];
+  bool ok;
+  return std::max(bytes, carve_bwd_models(ps, M, pl, total, nullptr, 0, &ok).bytes);
+}
+
+int dsmil_backward_bags_models(const dsmil_params_t* ps, int32_t M, const float* const* Xs, const int64_t* Ns,
+                               const int32_t* nbs, const float* Q, const float* H1, const float* A, const float* B,
+                               const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
+                               const float* d_B, const dsmil_grads_t* grads, void* workspace, size_t workspace_bytes,
+                               void* stream) {
+  ModelsBags mb;
+  int rc = check_models_bags(ps, M, Xs, Ns, nbs, &mb);
+  if (rc) return rc;
+  DSMIL_REQUIRE(Q && A && B && crit_idx && grads, "NULL pointer");
+  DSMIL_REQUIRE(!ps[0].nonlinear || H1, "nonlinear q backward needs saved H1");
+  bool gX = false;
+  for (int m = 0; m < M; ++m) gX = gX || grads[m].gX != nullptr;
+  const size_t need = dsmil_backward_bags_models_workspace_bytes(ps, M, Ns, nbs, gX);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (bwd_models_fused(ps, M, Ns, nbs, mb.ne, mb.aligned))
+    return backward_bags_models_impl(ps, M, Xs, Ns, nbs, mb, Q, H1, A, B, crit_idx, d_classes, d_pred, d_A, d_B, grads,
+                                     workspace, workspace_bytes, st);
+  // off the fused route: each model's dsmil_backward_bags on its slices
+  const int C = ps[0].C, D = ps[0].D;
+  size_t off = 0;
+  for (int m = 0; m < M; ++m) {
+    const int b0 = mb.bag[m];
+    const int64_t r0 = mb.row[m];
+    const size_t bo = static_cast<size_t>(b0);
+    const size_t wb = dsmil_backward_bags_workspace_bytes(&ps[m], Ns + b0, nbs[m], gX);
+    rc = dsmil_backward_bags(&ps[m], Xs + b0, Ns + b0, nbs[m], Q + r0 * kQ, H1 ? H1 + r0 * kQ : nullptr, A + r0 * C,
+                             B + bo * C * D, crit_idx + bo * C, d_classes ? d_classes + r0 * C : nullptr,
+                             d_pred ? d_pred + bo * C : nullptr, d_A ? d_A + r0 * C : nullptr,
+                             d_B ? d_B + bo * C * D : nullptr, &grads[m], static_cast<char*>(workspace) + off, wb,
+                             stream);
+    if (rc) return rc;
+    off += ws_slice(wb);
+  }
+  return 0;
 }
 
 

@@ -292,7 +292,8 @@ struct FinalizeArgs {
   float* emit;
   int ext_P, ext_nb;
   // ensemble table (k_finalize_b<true>): entry e = b * nmodels + m takes Wf / bf from models[m] (Wf, bf unused) and
-  // writes pred / B / crit to slot m * nb_out + b, model-major
+  // writes pred / B / crit to slot m * nb_out + b, model-major.  A table of each model's own bags, listed model-major
+  // (the ensemble's training forward), passes nmodels = 1 and nb_out = 0: entry e then writes slot e.
   const ModelDev* models;
   int nmodels, nb_out;
 };

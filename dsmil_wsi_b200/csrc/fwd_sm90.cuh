@@ -655,12 +655,13 @@ inline int launch_prep_wimg_models(const ModelDev* models_dev, int M, int D, uin
   DSMIL_LAUNCH_OK("k_prep_wimg2_models");
   return 0;
 }
-// Scores, arg-max keys and tile-blocked Q of every entry; C <= 4 (the batched shapes), done as in launch_qmlp.
+// Scores, arg-max keys and Q (+ H1 when non-NULL; Q tile-blocked when q_blocked, else row-major after the tanh, as the
+// training forward keeps it) of every entry; C <= 4 (the batched shapes), done as in launch_qmlp.
 inline int launch_qmlp_models(const ModelDev* models_dev, int M, int D, int C, const BagDev* bags_dev, int nb,
-                              int ntiles, float* classes, unsigned long long* keys, float* Q, const uint8_t* wimg,
-                              int max_ctas, cudaStream_t st, unsigned int* done) {
+                              int ntiles, float* classes, unsigned long long* keys, float* Q, float* H1,
+                              bool q_blocked, const uint8_t* wimg, int max_ctas, cudaStream_t st, unsigned int* done) {
   QmlpModelsArgs a{{bags_dev, nb, ntiles, D, C, nullptr, nullptr, nullptr, nullptr, wimg, nullptr, classes, keys, Q,
-                    nullptr, true, nullptr, done}, models_dev, M, wimg_bytes(D)};
+                    H1, q_blocked, nullptr, done}, models_dev, M, wimg_bytes(D)};
   const size_t smem = qmlp_models_smem_bytes(C, D, M);
   const int grid = ntiles < max_ctas ? ntiles : max_ctas;
   auto go = [&](auto kern) -> int {

@@ -14,20 +14,15 @@ constexpr int LBM = 64, LBN = 128, LBK = 16;
 
 // Y[N,M] (+)= act(X[N,K] * op(W) + b);  op(W)[k,m] = WT ? W[k*M+m] : W[m*K+k].
 // ACT_MASK_POS: y = aux[n,m] > 0 ? y : 0  (ReLU backward through a saved activation).
+// The body of CTA (blockIdx.x, blockIdx.y), whose rows start at n0.
 template <int ACT, bool WT>
-__global__ void __launch_bounds__(256)
-k_linear(const float* __restrict__ X, int64_t N, int K, const float* __restrict__ W,
-         const float* __restrict__ b, int M, float* __restrict__ Y, const float* __restrict__ aux,
-         int accumulate, const long long* __restrict__ N_dev) {
+__device__ __forceinline__ void linear_tile(const float* __restrict__ X, int64_t N, int64_t n0, int K,
+                                            const float* __restrict__ W, const float* __restrict__ b, int M,
+                                            float* __restrict__ Y, const float* __restrict__ aux, int accumulate) {
   __shared__ __align__(16) float As[LBK][LBM + 4];
   __shared__ __align__(16) float Bs[LBK][LBN + 4];
   const int tid = threadIdx.x;
   const int ty = tid >> 4, tx = tid & 15;
-  const int64_t n0 = static_cast<int64_t>(blockIdx.x) * LBM;
-  if (N_dev) {               // the live row count of a capacity grid
-    N = *N_dev;
-    if (n0 >= N) return;
-  }
   const int m0 = blockIdx.y * LBN;
   float acc[4][8];
 #pragma unroll
@@ -103,6 +98,18 @@ k_linear(const float* __restrict__ X, int64_t N, int K, const float* __restrict_
       *dst = accumulate ? (*dst + y) : y;
     }
   }
+}
+template <int ACT, bool WT>
+__global__ void __launch_bounds__(256)
+k_linear(const float* __restrict__ X, int64_t N, int K, const float* __restrict__ W,
+         const float* __restrict__ b, int M, float* __restrict__ Y, const float* __restrict__ aux,
+         int accumulate, const long long* __restrict__ N_dev) {
+  const int64_t n0 = static_cast<int64_t>(blockIdx.x) * LBM;
+  if (N_dev) {               // the live row count of a capacity grid
+    N = *N_dev;
+    if (n0 >= N) return;
+  }
+  linear_tile<ACT, WT>(X, N, n0, K, W, b, M, Y, aux, accumulate);
 }
 
 // N_dev != NULL: N is the row capacity (the grid), *N_dev the live row count, read on the device.
@@ -298,10 +305,8 @@ k_colsum(const float* __restrict__ P, int M, int64_t N, int64_t rows_per_split, 
 // out[i] = sum_z part[z][i]  (fixed order: warp w of the CTA adds z = w, w + 8, ... with four independent running sums,
 // the eight warp sums are then added in warp order).  32 outputs per CTA, so a short vector (a bias gradient: 128
 // values from 235 partials) is no longer one CTA walking 235 dependent steps.
-__global__ void __launch_bounds__(256)
-k_sum_partials(const float* __restrict__ part, int S, int64_t L, float* __restrict__ out, const int* __restrict__ S_dev) {
+__device__ __forceinline__ void sum_partials(const float* __restrict__ part, int S, int64_t L, float* __restrict__ out) {
   __shared__ float s_w[8][32];
-  if (S_dev) S = *S_dev;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t i = static_cast<int64_t>(blockIdx.x) * 32 + lane;
   float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -320,6 +325,11 @@ k_sum_partials(const float* __restrict__ part, int S, int64_t L, float* __restri
   if (w == 0 && i < L)
     out[i] = ((s_w[0][lane] + s_w[1][lane]) + (s_w[2][lane] + s_w[3][lane])) +
              ((s_w[4][lane] + s_w[5][lane]) + (s_w[6][lane] + s_w[7][lane]));
+}
+__global__ void __launch_bounds__(256)
+k_sum_partials(const float* __restrict__ part, int S, int64_t L, float* __restrict__ out, const int* __restrict__ S_dev) {
+  if (S_dev) S = *S_dev;
+  sum_partials(part, S, L, out);
 }
 inline int launch_sum_partials(const float* part, int S, int64_t L, float* out, cudaStream_t st,
                                const int* S_dev = nullptr) {

@@ -150,6 +150,82 @@ def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_pat
     return float(total.item()) / max(1, len(order))
 
 
+def fold_steps(sizes: Sequence[int], k: int) -> List[List[Tuple[int, int, int]]]:
+    """The steps of train_epoch_models over folds of `sizes` bags, k bags per step: step s holds (fold, start, stop)
+    for every fold that still has bags, its group being bags [start, stop) of its order.  A fold whose bags have run
+    out is not in the step."""
+    k = max(1, int(k))
+    steps = []
+    for s in range(0, max(sizes, default=0), k):
+        steps.append([(m, s, min(s + k, n)) for m, n in enumerate(sizes) if s < n])
+    return steps
+
+
+def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[int]], criterion,
+                       optimizers, dropout_patch: float = 0.0, orders: Optional[Sequence[Sequence[int]]] = None,
+                       generators: Optional[Sequence[Optional[torch.Generator]]] = None,
+                       bags_per_step: int = 1) -> List[float]:
+    """One epoch of every fold model of a cross-validation (train_tcga.py:252-288, train_mil.py:164-187), the folds
+    taking their steps together; returns each fold's mean loss per bag.  folds[m] lists the store indices of fold m's
+    training split; orders[m], when given, is the order fold m visits them in (a permutation of folds[m]), else a
+    random one (torch.randperm).
+
+    Each step, every fold that still has bags takes its next group of k = bags_per_step (fold_steps): it draws its
+    dropout_patches with generators[m], all groups go through one ensemble.forward_bags_per_model call, the step's loss
+    is the sum of the folds' minibatch_loss (so each fold's own loss gets a gradient of exactly 1), one backward fills
+    every fold's gradients, and each fold's optimizers[m].step() follows.  A fold with no group left is not in the
+    call and its optimizer is not stepped.  The epoch makes one host sync.
+
+    With per-fold generators (or no patch dropout) and the same orders, fold m's losses and parameters are bit for bit
+    those of train_epoch(milnets[m], store, criterion, optimizers[m], dropout_patch, orders[m], generators[m], k, graph=True)
+    (and of the eager minibatch epoch for k >= 2).  Without generators, or with one generator shared by the folds,
+    the folds' permutation draws interleave in step order (fold 0's group, then fold 1's, ...), so each fold sees
+    different draws than it would alone."""
+    from .ensemble import forward_bags_per_model
+    milnets, M = list(milnets), len(folds)
+    if not 1 <= M <= Fn.MAX_MODELS:
+        raise ValueError(f"a fold step takes 1 to {Fn.MAX_MODELS} folds, got {M}")
+    for what, seq in (("milnets", milnets), ("optimizers", optimizers), ("orders", orders),
+                      ("generators", generators)):
+        if seq is not None and len(seq) != M:
+            raise ValueError(f"{len(seq)} {what} for {M} folds")
+    for m, fold in enumerate(folds):
+        if len(fold) == 0:
+            raise ValueError(f"fold {m} has no training bags")
+        bad = [i for i in fold if not 0 <= i < len(store)]
+        if bad:
+            raise IndexError(f"fold {m}: store index {bad[0]} outside [0, {len(store)})")
+    if orders is None:
+        orders = [[fold[i] for i in torch.randperm(len(fold)).tolist()] for fold in folds]
+    else:
+        orders = [list(o) for o in orders]
+        for m, (o, fold) in enumerate(zip(orders, folds)):
+            if sorted(o) != sorted(fold):
+                raise ValueError(f"orders[{m}] is not a permutation of folds[{m}]")
+    gens = list(generators) if generators is not None else [None] * M
+    for net in milnets:
+        net.train()
+    totals = [torch.zeros((), device=store.device) for _ in range(M)]
+    for step in fold_steps([len(o) for o in orders], bags_per_step):
+        groups = [(m, orders[m][lo:hi]) for m, lo, hi in step]
+        for m, _ in groups:
+            optimizers[m].zero_grad()
+        xs = [[dropout_patches(store.bags[i][0], 1 - dropout_patch, gens[m]) for i in group] for m, group in groups]
+        outs = forward_bags_per_model([milnets[m] for m, _ in groups], xs, grad=True)
+        loss = None
+        for (m, group), out in zip(groups, outs):
+            labels = torch.cat([store.bags[i][1].view(1, -1) for i in group])
+            bag_prediction, max_prediction = _group_predictions(out)
+            lm = minibatch_loss(criterion, bag_prediction, max_prediction, labels)
+            totals[m] += lm.detach() * len(group)
+            loss = lm if loss is None else loss + lm
+        loss.backward()
+        for m, _ in groups:
+            optimizers[m].step()
+    host = torch.stack(totals).double().tolist()    # the epoch's one host sync
+    return [t / len(o) for t, o in zip(host, orders)]
+
+
 def minibatch_loss(criterion, bag_prediction, max_prediction, labels):
     """The minibatch step's loss over a group's [k, C] predictions and labels."""
     return 0.5 * criterion(bag_prediction, labels) + 0.5 * criterion(max_prediction, labels)

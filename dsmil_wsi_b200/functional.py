@@ -429,14 +429,9 @@ def mil_forward_bags_dev(xs: torch.Tensor, Ns: torch.Tensor, status: torch.Tenso
 MAX_MODELS = 8   # members of one dsmil_forward_bags_models call
 
 
-@torch.no_grad()
-def mil_forward_bags_models(bags: Sequence[torch.Tensor], params_list: Sequence[Sequence[Optional[torch.Tensor]]]):
-    """An ensemble forward: M parameter sets (1 <= M <= 8, the same D, C and q form, identity v) over the same bags in
-    one dsmil_forward_bags_models call.  Returns M BagOutputs, one per model, over model-major packed tensors, each
-    with `.crit` [nb, C]; model m's are bit for bit what mil_forward_bags(bags, params_list[m]) gives.  On the batched
-    tensor-core shapes the whole ensemble costs one launch of each kernel and the passes over a bag follow each
-    other while it is in L2."""
-    lib = _lib.load()
+def _model_packs(params_list) -> list:
+    """ParamPacks of an ensemble's members: 1 to MAX_MODELS of them, with the same D, C and q form, identity v, on one
+    device; ValueError naming the first mismatch."""
     packs = [ParamPack(*p) for p in params_list]
     M = len(packs)
     if not 1 <= M <= MAX_MODELS:
@@ -450,6 +445,126 @@ def mil_forward_bags_models(bags: Sequence[torch.Tensor], params_list: Sequence[
             raise ValueError(f"model {m} is on {P.device}, model 0 on {P0.device}")
     if P0.passing_v:
         raise NotImplementedError("forward_bags: passing_v models go through MILNet.forward per bag")
+    return packs
+
+
+PARAM_NAMES = ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")
+
+
+class MILBagsModelsFn(torch.autograd.Function):
+    """MILBagsFn for M members, each over its own bags: dsmil_forward_bags_models_train forward and
+    dsmil_backward_bags_models backward, one call each for all members.  args: nbs (each member's bag count), the
+    sum(nbs) bags (member 0's, then member 1's, ...), then the M members' ten parameter tensors each.  The packed
+    outputs are model-major; member m's parameter gradients are sums over its own bags."""
+
+    @staticmethod
+    def forward(ctx, nbs, *args):
+        lib = _lib.load()
+        ctx.set_materialize_grads(False)
+        M, ne = len(nbs), sum(nbs)
+        packs = _model_packs([args[ne + 10 * m:ne + 10 * (m + 1)] for m in range(M)])
+        P0 = packs[0]
+        xs, Ns, c_X, c_N = _bag_table(args[:ne], P0)
+        total, Cc, D, dev = sum(Ns), P0.C, P0.D, P0.device
+        ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
+        c_nb = (C.c_int32 * M)(*nbs)
+        with torch.cuda.device(dev):
+            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+            classes, A = new(total, Cc), new(total, Cc)
+            pred, B = new(ne, Cc), new(ne, Cc, D)
+            crit = torch.empty(ne, Cc, dtype=torch.int64, device=dev)
+            sQ = new(total, Q_DIM)
+            sH = new(total, Q_DIM) if P0.nonlinear else None
+            ws = _workspace(lib.dsmil_forward_bags_models_train_workspace_bytes(ps, M, c_N, c_nb), dev)
+            rc = lib.dsmil_forward_bags_models_train(ps, M, c_X, c_N, c_nb, _ptr(classes), _ptr(pred), _ptr(A),
+                                                     _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(ws), ws.numel(),
+                                                     _stream())
+            _lib.check(rc, "dsmil_forward_bags_models_train")
+        ctx.nbs, ctx.Ns = tuple(nbs), Ns
+        ctx.save_for_backward(*xs, sQ, sH, A, B, crit, *[t for P in packs for t in P.tensors])
+        ctx.mark_non_differentiable(crit)
+        return classes, pred, A, B, crit
+
+    @staticmethod
+    def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
+        lib = _lib.load()
+        nbs, Ns = ctx.nbs, ctx.Ns
+        M, ne = len(nbs), sum(nbs)
+        saved = ctx.saved_tensors
+        xs, (sQ, sH, A, B, crit) = saved[:ne], saved[ne:ne + 5]
+        packs = [ParamPack(*saved[ne + 5 + 10 * m:ne + 5 + 10 * (m + 1)]) for m in range(M)]
+        need_bags, need_params = ctx.needs_input_grad[1:1 + ne], ctx.needs_input_grad[1 + ne:]
+        P0, dev = packs[0], packs[0].device
+        c_X = (C.c_void_p * ne)(*[x.data_ptr() for x in xs])
+        c_N = (C.c_int64 * ne)(*Ns)
+        c_nb = (C.c_int32 * M)(*nbs)
+        ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
+        with torch.cuda.device(dev):
+            outs = [{nm: (torch.empty_like(t) if t is not None and need else None)
+                     for nm, t, need in zip(PARAM_NAMES, P.tensors, need_params[10 * m:10 * (m + 1)])}
+                    for m, P in enumerate(packs)]
+            gX = torch.empty(sum(Ns), P0.D, dtype=torch.float32, device=dev) if any(need_bags) else None
+            grads, lo, b = (_lib.DsmilGrads * M)(), 0, 0
+            for m in range(M):
+                rows = sum(Ns[b:b + nbs[m]])
+                grads[m] = _lib.DsmilGrads(*[_ptr(outs[m][n]) for n in PARAM_NAMES],
+                                           None if gX is None else _ptr(gX[lo:lo + rows]))
+                lo, b = lo + rows, b + nbs[m]
+            dc, dp, dA, dB = (_f32c(t) for t in (g_classes, g_pred, g_A, g_B))
+            ws = _workspace(lib.dsmil_backward_bags_models_workspace_bytes(ps, M, c_N, c_nb, int(gX is not None)),
+                            dev)
+            rc = lib.dsmil_backward_bags_models(ps, M, c_X, c_N, c_nb, _ptr(sQ), _ptr(sH), _ptr(A), _ptr(B),
+                                                _ptr(crit), _ptr(dc), _ptr(dp), _ptr(dA), _ptr(dB), grads, _ptr(ws),
+                                                ws.numel(), _stream())
+            _lib.check(rc, "dsmil_backward_bags_models")
+        gxs, lo = [], 0
+        for n, need in zip(Ns, need_bags):
+            gxs.append(gX[lo:lo + n] if need else None)
+            lo += n
+        return (None, *gxs, *[o[n] for o in outs for n in PARAM_NAMES])
+
+
+def mil_forward_bags_per_model(bag_lists: Sequence[Sequence[torch.Tensor]],
+                               params_list: Sequence[Sequence[Optional[torch.Tensor]]], *, grad: bool = False):
+    """M parameter sets (1 <= M <= 8, the same D, C and q form, identity v), each over its OWN non-empty list of bags,
+    in one dsmil_forward_bags_models_train call.  Returns M BagOutputs over model-major packed tensors, each with
+    `.crit`; model m's are bit for bit what mil_forward_bags(bag_lists[m], params_list[m], grad=True) gives.
+
+    grad=True with grad mode on: the packed outputs carry autograd history (MILBagsModelsFn), and one backward over a
+    loss of every member's outputs fills every member's gradients with one dsmil_backward_bags_models call."""
+    M = len(bag_lists)
+    if not 1 <= M <= MAX_MODELS:
+        raise ValueError(f"an ensemble forward takes 1 to {MAX_MODELS} models, got {M}")
+    if M != len(params_list):
+        raise ValueError(f"{M} bag lists for {len(params_list)} parameter sets")
+    for m, bags in enumerate(bag_lists):
+        if len(bags) == 0:
+            raise ValueError(f"model {m} has no bags: every member of a fold step needs at least one")
+    nbs = tuple(len(bags) for bags in bag_lists)
+    flat = [b for bags in bag_lists for b in bags]
+    params = [t for p in params_list for t in p]
+    with torch.set_grad_enabled(grad and torch.is_grad_enabled()):
+        classes, pred, A, B, crit = MILBagsModelsFn.apply(nbs, *flat, *params)
+    outs, row, b = [], 0, 0
+    for bags in bag_lists:
+        Ns = [int(x.shape[0]) for x in bags]
+        rows, nb = sum(Ns), len(bags)
+        outs.append(BagOutputs(classes[row:row + rows], pred[b:b + nb], A[row:row + rows], B[b:b + nb], Ns,
+                               crit[b:b + nb]))
+        row, b = row + rows, b + nb
+    return outs
+
+
+@torch.no_grad()
+def mil_forward_bags_models(bags: Sequence[torch.Tensor], params_list: Sequence[Sequence[Optional[torch.Tensor]]]):
+    """An ensemble forward: M parameter sets (1 <= M <= 8, the same D, C and q form, identity v) over the same bags in
+    one dsmil_forward_bags_models call.  Returns M BagOutputs, one per model, over model-major packed tensors, each
+    with `.crit` [nb, C]; model m's are bit for bit what mil_forward_bags(bags, params_list[m]) gives.  On the batched
+    tensor-core shapes the whole ensemble costs one launch of each kernel and the passes over a bag follow each
+    other while it is in L2."""
+    lib = _lib.load()
+    packs = _model_packs(params_list)
+    M, P0 = len(packs), packs[0]
     nb = len(bags)
     if nb == 0:
         return [BagOutputs(None, None, None, None, [], None) for _ in range(M)]

@@ -184,6 +184,34 @@ int dsmil_backward_bags(const dsmil_params_t* p, const float* const* Xs, const i
                         const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
                         const dsmil_grads_t* grads, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Training forms of the ensemble, for the fold models of a cross-validation taking one step together: M members
+ * (1 <= M <= 8, checked as dsmil_forward_bags_models checks them; identity v only), each over its OWN bags.  nbs[m]
+ * >= 1 is model m's bag count; Xs / Ns list model 0's bags, then model 1's, and so on.  Every buffer is packed
+ * model-major: classes / A [sum_m sum N_m, C], save_Q / save_H1 [sum_m sum N_m, 128], pred / crit_idx [sum nb_m, C],
+ * B [sum nb_m, C, D], and the upstream gradients of the backward likewise.
+ * dsmil_forward_bags_models_train: model m's slices are, bit for bit, what dsmil_forward_bags_train(&ps[m], ...)
+ * writes for model m's bags.  When dsmil_models_supported(ps, M) holds, every bag is 16-byte aligned and there are at
+ * most 65535 bags in all, it is one weight-image prep, one phase-1, one attend and one finalize launch for all
+ * models; otherwise it loops dsmil_forward_bags_train over the models into the same slices.
+ * dsmil_backward_bags_models: grads[m] receives model m's gradients (sums over model m's bags; grads[m].gX, when
+ * non-NULL, is model m's [sum N_m, D]), bit for bit what dsmil_backward_bags(&ps[m], ...) gives on model m's slices.
+ * On the forward's fused route it is one launch per backward stage for all models (20 with gX), every per-model sum
+ * split as the one-model call splits it on that model's bags; otherwise it loops dsmil_backward_bags over the models.
+ * Both workspace sizes are never below the sum of the one-model calls' sizes; 0 for invalid arguments. */
+size_t dsmil_forward_bags_models_train_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int64_t* Ns,
+                                                       const int32_t* nbs);
+int dsmil_forward_bags_models_train(const dsmil_params_t* ps, int32_t M, const float* const* Xs, const int64_t* Ns,
+                                    const int32_t* nbs, float* classes, float* pred, float* A, float* B,
+                                    int64_t* crit_idx, float* save_Q, float* save_H1, void* workspace,
+                                    size_t workspace_bytes, void* stream);
+size_t dsmil_backward_bags_models_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int64_t* Ns,
+                                                  const int32_t* nbs, int need_gX);
+int dsmil_backward_bags_models(const dsmil_params_t* ps, int32_t M, const float* const* Xs, const int64_t* Ns,
+                               const int32_t* nbs, const float* Q, const float* H1, const float* A, const float* B,
+                               const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
+                               const float* d_B, const dsmil_grads_t* grads, void* workspace, size_t workspace_bytes,
+                               void* stream);
+
 /* Capture-safe forms of dsmil_forward_bags_train / dsmil_backward_bags, for a training step recorded once as a CUDA
  * graph and replayed over batches of different bag sizes.  The bag list is in DEVICE memory: Xs_dev [nb] feature
  * pointers, Ns_dev [nb] row counts.  max_rows is the per-bag row capacity: classes, A, save_Q and save_H1 (and
