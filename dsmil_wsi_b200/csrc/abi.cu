@@ -1607,7 +1607,6 @@ struct BwdModelsPlan {
 static void plan_bwd_models(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
                             const int32_t* nbs, const float* H1, BwdModelsPlan& pl) {
   const int C = ps[0].C, D = ps[0].D;
-  const bool gemv = tn_use_gemv(C, D);   // the fused route has every bag 16-byte aligned
   pl.nci.assign(M, 0); pl.nc1.assign(M, 0); pl.nc2.assign(M, 0); pl.ncs.assign(M, 0);
   int e = 0;
   long long row = 0;
@@ -1620,7 +1619,8 @@ static void plan_bwd_models(const dsmil_params_t* ps, int M, const float* const*
       mx = std::max<int64_t>(mx, N[b]);
     }
     const long long r0 = row;
-    const int G = bwd_bags_ctas(nb, mx);
+    const ModelSplits sp = model_splits(C, D, nb, total, mx);
+    const int G = sp.G;
     pl.Gmax = std::max(pl.Gmax, G);
     pl.max_rows = std::max(pl.max_rows, total);
     for (int b = 0; b < nb; ++b, ++e) {
@@ -1629,30 +1629,21 @@ static void plan_bwd_models(const dsmil_params_t* ps, int M, const float* const*
       pl.slots += G;
     }
     // gWi and gW1: chunks of each bag's rows, as carve_bwd_bags cuts them
+    const BagList L{Xs ? Xs + (e - nb) : nullptr, N, nullptr};
     auto rag = [&](std::vector<TnChunk>& out, int64_t rps) {
-      const int n = rag_chunks(nullptr, N, nb, D, rps, nullptr);
+      const int n = rag_chunks_list(L, nb, D, rps, r0, nullptr);
       const size_t at = out.size();
       out.resize(at + n);
-      if (Xs) {
-        rag_chunks(Xs + (e - nb), N, nb, D, rps, out.data() + at);
-        for (int z = 0; z < n; ++z) out[at + z].prow += r0;
-      }
+      if (Xs) rag_chunks_list(L, nb, D, rps, r0, out.data() + at);
       return n;
     };
-    pl.nci[m] = rag(pl.chi, rag_rows_per_chunk(C, D, total, gemv));
-    pl.nc1[m] = rag(pl.ch1, rag_rows_per_chunk(kQ, D, total, false));
+    pl.nci[m] = rag(pl.chi, sp.rps_i);
+    pl.nc1[m] = rag(pl.ch1, sp.rps_1);
     // gW2 = dz2^T H1 and the column sums: launch_gemm_tn's tile form and launch_colsum split the model's rows
-    const RowSplit t2 = gemm_tn_split(kQ, kQ, total), cs = colsum_split(total);
-    for (int z = 0; z < t2.S; ++z) {
-      const long long lo = z * t2.rps;
-      pl.ch2.push_back(TnChunk{H1 ? H1 + (r0 + lo) * kQ : nullptr, r0 + lo, std::min<long long>(total, lo + t2.rps) - lo});
-    }
-    for (int z = 0; z < cs.S; ++z) {
-      const long long lo = z * cs.rps;
-      pl.chc.push_back(TnChunk{nullptr, r0 + lo, std::min<long long>(total, lo + cs.rps) - lo});
-    }
-    pl.nc2[m] = t2.S;
-    pl.ncs[m] = cs.S;
+    for (int z = 0; z < sp.t2.S; ++z) pl.ch2.push_back(split_chunk(sp.t2, z, r0, H1, kQ));
+    for (int z = 0; z < sp.cs.S; ++z) pl.chc.push_back(split_chunk(sp.cs, z, r0, nullptr, 0));
+    pl.nc2[m] = sp.t2.S;
+    pl.ncs[m] = sp.cs.S;
   }
 }
 
@@ -1695,6 +1686,87 @@ static BwdModelsWs carve_bwd_models(const dsmil_params_t* ps, int M, const BwdMo
   w.bytes = c.off;
   *ok = c.ok();
   return w;
+}
+
+// The fused backward's launches over the tables in w: one per stage for all M models.  The grids are those of gr; in a
+// dev call they are capacities, the tables are the planner's and the live chunk counts are read from gr.live.
+struct BwdModelsGrid {
+  int Gmax, nci, nc1, nc2, ncs;   // per-row CTAs per entry, and the chunks of gWi, gW1, gW2 and the column sums
+  int64_t max_rows;               // rows of the largest model
+  bool any_gX;
+  const ModelsPlan* live;         // dev call: the planner's counts (device memory); NULL: eager
+};
+static int bwd_models_launch(int C, int D, int M, int ne, const BwdModelsWs& w, const BwdModelsGrid& gr,
+                             const float* Q, const float* H1, const float* A, const float* B, const int64_t* crit,
+                             const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                             cudaStream_t st) {
+  const ModelsPlan* live = gr.live;
+  int rc;
+  // each model's partials into its gradients: reduction r of the six
+  auto sums = [&](int r, int64_t L) -> int {
+    k_sum_partials_models<<<dim3(static_cast<unsigned>(ceil_div(L, 32)), M), 256, 0, st>>>(w.part, w.segs + r * M, L);
+    DSMIL_LAUNCH_OK("k_sum_partials_models");
+    return 0;
+  };
+  auto colsums = [&](const float* P, int L, int r) -> int {
+    k_colsum_rag<<<static_cast<unsigned>(gr.ncs), 256, 0, st>>>(P, L, w.chc, w.part);
+    DSMIL_LAUNCH_OK("k_colsum_rag");
+    return sums(r, L);
+  };
+  const dim3 per_entry(gr.Gmax, ne);
+  // phase 1: bag classifier, instance classifier, dA and t's partials
+  k_bwd_bag_models<<<dim3(ceil_div(static_cast<int64_t>(C) * D, 256), M), 256, 0, st>>>(w.models, B, d_pred, d_B, C,
+                                                                                       D, w.dB);
+  DSMIL_LAUNCH_OK("k_bwd_bag_models");
+  if (d_classes) {
+    const int nz = gr.nci;
+    const int* nzd = live ? &live->nci : nullptr;
+    if (tn_use_gemv(C, D)) {
+      switch (C) {
+        case 1: k_gemv_tn_rag<1><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nzd); break;
+        case 2: k_gemv_tn_rag<2><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nzd); break;
+        case 3: k_gemv_tn_rag<3><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nzd); break;
+        default: k_gemv_tn_rag<4><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nzd); break;
+      }
+      DSMIL_LAUNCH_OK("k_gemv_tn_rag");
+    } else {
+      k_gemm_tn_rag<<<dim3(ceil_div(D, TBM), ceil_div(C, TBM), nz), 256, 0, st>>>(d_classes, C, D, w.chi, w.part,
+                                                                                 nzd);
+      DSMIL_LAUNCH_OK("k_gemm_tn_rag");
+    }
+    if ((rc = sums(0, static_cast<int64_t>(C) * D)) || (rc = colsums(d_classes, C, 1))) return rc;
+  }
+  const size_t smem = sizeof(float) * C * D;
+  if (smem > 48 * 1024)
+    DSMIL_CUDA_OK(cudaFuncSetAttribute(k_bwd_rowdot_models, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_bwd_rowdot_models<<<per_entry, 256, smem, st>>>(w.table, D, w.dB, C, A, d_A, w.dA, w.tpart);
+  DSMIL_LAUNCH_OK("k_bwd_rowdot_models");
+  // phase 2: dL and dq_max
+  k_bwd_dL_models<<<per_entry, 256, 0, st>>>(w.table, C, A, w.dA, w.tpart, Q, w.dL, w.dpart);
+  DSMIL_LAUNCH_OK("k_bwd_dL_models");
+  k_sum_segments_models<<<dim3(ceil_div(C * kQ, 256), ne), 256, 0, st>>>(w.table, w.dpart, C * kQ, w.dqm);
+  DSMIL_LAUNCH_OK("k_sum_segments_models");
+  // phase 3: dz2, back through the Q-MLP
+  k_bwd_dq_b<<<per_entry, 256, 0, st>>>(w.table, C, w.dL, Q, nullptr, w.dqm, crit, nullptr, 1, w.dz2);
+  DSMIL_LAUNCH_OK("k_bwd_dq_b");
+  k_gemm_tn_rag<<<dim3(1, 1, static_cast<unsigned>(gr.nc2)), 256, 0, st>>>(w.dz2, kQ, kQ, w.ch2, w.part,
+                                                                           live ? &live->nc2 : nullptr);
+  DSMIL_LAUNCH_OK("k_gemm_tn_rag");
+  if ((rc = sums(2, static_cast<int64_t>(kQ) * kQ)) || (rc = colsums(w.dz2, kQ, 3))) return rc;
+  const unsigned row_tiles = static_cast<unsigned>(ceil_div(gr.max_rows, LBM));
+  k_linear_models<ACT_MASK_POS, true><<<dim3(row_tiles, 1, M), 256, 0, st>>>(w.lin, kQ, kQ);
+  DSMIL_LAUNCH_OK("k_linear_models");
+  k_gemm_tn_rag<<<dim3(ceil_div(D, TBM), 1, static_cast<unsigned>(gr.nc1)), 256, 0, st>>>(
+      w.dz1, kQ, D, w.ch1, w.part, live ? &live->nc1 : nullptr);
+  DSMIL_LAUNCH_OK("k_gemm_tn_rag");
+  if ((rc = sums(4, static_cast<int64_t>(kQ) * D)) || (rc = colsums(w.dz1, kQ, 5))) return rc;
+  if (gr.any_gX) {
+    k_linear_models<ACT_NONE, true><<<dim3(row_tiles, ceil_div(D, LBN), M), 256, 0, st>>>(w.lin + M, kQ, D);
+    DSMIL_LAUNCH_OK("k_linear_models");
+    k_bwd_dx_extra_models<<<per_entry, 256, 0, st>>>(w.table, w.models, d_classes, A, w.dB, C, D);
+    DSMIL_LAUNCH_OK("k_bwd_dx_extra_models");
+  }
+  return 0;
 }
 
 // One launch per stage for all M models (nonlinear q, C <= 4: the dsmil_models_supported shapes; aligned bags).
@@ -1750,70 +1822,9 @@ static int backward_bags_models_impl(const dsmil_params_t* ps, int M, const floa
   DSMIL_CUDA_OK(cudaMemcpyAsync(w.segs, segs.data(), sizeof(SumSeg) * 6 * M, cudaMemcpyHostToDevice, st));
   DSMIL_CUDA_OK(cudaMemcpyAsync(w.lin, lin.data(), sizeof(LinSeg) * 2 * M, cudaMemcpyHostToDevice, st));
 
-  // each model's partials into its gradients: reduction r of the six
-  auto sums = [&](int r, int64_t L) -> int {
-    k_sum_partials_models<<<dim3(static_cast<unsigned>(ceil_div(L, 32)), M), 256, 0, st>>>(w.part, w.segs + r * M, L);
-    DSMIL_LAUNCH_OK("k_sum_partials_models");
-    return 0;
-  };
-  auto colsums = [&](const float* P, int L, int r) -> int {
-    k_colsum_rag<<<static_cast<unsigned>(pl.chc.size()), 256, 0, st>>>(P, L, w.chc, w.part);
-    DSMIL_LAUNCH_OK("k_colsum_rag");
-    return sums(r, L);
-  };
-  const dim3 per_entry(pl.Gmax, ne);
-  // phase 1: bag classifier, instance classifier, dA and t's partials
-  k_bwd_bag_models<<<dim3(ceil_div(static_cast<int64_t>(C) * D, 256), M), 256, 0, st>>>(w.models, B, d_pred, d_B, C,
-                                                                                       D, w.dB);
-  DSMIL_LAUNCH_OK("k_bwd_bag_models");
-  if (d_classes) {
-    const int nz = static_cast<int>(pl.chi.size());
-    if (tn_use_gemv(C, D)) {
-      switch (C) {
-        case 1: k_gemv_tn_rag<1><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nullptr); break;
-        case 2: k_gemv_tn_rag<2><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nullptr); break;
-        case 3: k_gemv_tn_rag<3><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nullptr); break;
-        default: k_gemv_tn_rag<4><<<nz, 256, 0, st>>>(d_classes, D, w.chi, w.part, nullptr); break;
-      }
-      DSMIL_LAUNCH_OK("k_gemv_tn_rag");
-    } else {
-      k_gemm_tn_rag<<<dim3(ceil_div(D, TBM), ceil_div(C, TBM), nz), 256, 0, st>>>(d_classes, C, D, w.chi, w.part,
-                                                                                 nullptr);
-      DSMIL_LAUNCH_OK("k_gemm_tn_rag");
-    }
-    if ((rc = sums(0, static_cast<int64_t>(C) * D)) || (rc = colsums(d_classes, C, 1))) return rc;
-  }
-  const size_t smem = sizeof(float) * C * D;
-  if (smem > 48 * 1024)
-    DSMIL_CUDA_OK(cudaFuncSetAttribute(k_bwd_rowdot_models, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_bwd_rowdot_models<<<per_entry, 256, smem, st>>>(w.table, D, w.dB, C, A, d_A, w.dA, w.tpart);
-  DSMIL_LAUNCH_OK("k_bwd_rowdot_models");
-  // phase 2: dL and dq_max
-  k_bwd_dL_models<<<per_entry, 256, 0, st>>>(w.table, C, A, w.dA, w.tpart, Q, w.dL, w.dpart);
-  DSMIL_LAUNCH_OK("k_bwd_dL_models");
-  k_sum_segments_models<<<dim3(ceil_div(C * kQ, 256), ne), 256, 0, st>>>(w.table, w.dpart, C * kQ, w.dqm);
-  DSMIL_LAUNCH_OK("k_sum_segments_models");
-  // phase 3: dz2, back through the Q-MLP
-  k_bwd_dq_b<<<per_entry, 256, 0, st>>>(w.table, C, w.dL, Q, nullptr, w.dqm, crit, nullptr, 1, w.dz2);
-  DSMIL_LAUNCH_OK("k_bwd_dq_b");
-  k_gemm_tn_rag<<<dim3(1, 1, static_cast<unsigned>(pl.ch2.size())), 256, 0, st>>>(w.dz2, kQ, kQ, w.ch2, w.part,
-                                                                                   nullptr);
-  DSMIL_LAUNCH_OK("k_gemm_tn_rag");
-  if ((rc = sums(2, static_cast<int64_t>(kQ) * kQ)) || (rc = colsums(w.dz2, kQ, 3))) return rc;
-  const unsigned row_tiles = static_cast<unsigned>(ceil_div(pl.max_rows, LBM));
-  k_linear_models<ACT_MASK_POS, true><<<dim3(row_tiles, 1, M), 256, 0, st>>>(w.lin, kQ, kQ);
-  DSMIL_LAUNCH_OK("k_linear_models");
-  k_gemm_tn_rag<<<dim3(ceil_div(D, TBM), 1, static_cast<unsigned>(pl.ch1.size())), 256, 0, st>>>(w.dz1, kQ, D, w.ch1,
-                                                                                                 w.part, nullptr);
-  DSMIL_LAUNCH_OK("k_gemm_tn_rag");
-  if ((rc = sums(4, static_cast<int64_t>(kQ) * D)) || (rc = colsums(w.dz1, kQ, 5))) return rc;
-  if (any_gX) {
-    k_linear_models<ACT_NONE, true><<<dim3(row_tiles, ceil_div(D, LBN), M), 256, 0, st>>>(w.lin + M, kQ, D);
-    DSMIL_LAUNCH_OK("k_linear_models");
-    k_bwd_dx_extra_models<<<per_entry, 256, 0, st>>>(w.table, w.models, d_classes, A, w.dB, C, D);
-    DSMIL_LAUNCH_OK("k_bwd_dx_extra_models");
-  }
-  return 0;
+  BwdModelsGrid gr{pl.Gmax, static_cast<int>(pl.chi.size()), static_cast<int>(pl.ch1.size()),
+                   static_cast<int>(pl.ch2.size()), static_cast<int>(pl.chc.size()), pl.max_rows, any_gX, nullptr};
+  return bwd_models_launch(C, D, M, ne, w, gr, Q, H1, A, B, crit, d_classes, d_pred, d_A, d_B, st);
 }
 // Whether the fused backward takes these members and bags: the forward's fused shapes, aligned bags, and every grid
 // within its limits.
@@ -2148,6 +2159,216 @@ int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev,
   DSMIL_LAUNCH_OK("k_plan_bags");
   return backward_bags_run(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, A, B, crit_idx,
                            d_classes, d_pred, nullptr, nullptr, grads, w, st);
+}
+
+// ---- capture-safe fold step: M models, each over its own device bag list ------------------------------------------
+// The grids and workspace regions a fold dev call sizes on the host, from (M, nbs, max_rows) alone.
+struct ModelsDevCaps {
+  int ne;                     // entries: the bags of all models
+  int Gcap;                   // per-row CTAs per entry at most
+  int nci, nc1, nc2, ncs;     // chunk capacities over all models
+  int64_t max_model_rows;     // row capacity of the largest model
+};
+static bool models_dev_caps(const dsmil_params_t* ps, int M, const int32_t* nbs, int64_t max_rows, ModelsDevCaps* c) {
+  if (!ps || !nbs || !dsmil_models_supported(ps, M) || max_rows < 1 || max_rows >= 0xffffffffll) return false;
+  const int C = ps[0].C, D = ps[0].D;
+  int64_t ne = 0, nci = 0, nc1 = 0;
+  *c = ModelsDevCaps{0, 1, 0, 0, M * kModelSplitsCap, M * kModelSplitsCap, 1};
+  for (int m = 0; m < M; ++m) {
+    if (nbs[m] < 1 || nbs[m] > 65535) return false;
+    ne += nbs[m];
+    nci += rag_chunks_cap(C, D, tn_use_gemv(C, D), nbs[m]);
+    nc1 += rag_chunks_cap(kQ, D, false, nbs[m]);
+    c->Gcap = std::max(c->Gcap, bwd_bags_ctas(nbs[m], max_rows));
+    c->max_model_rows = std::max<int64_t>(c->max_model_rows, nbs[m] * max_rows);
+  }
+  // every grid within its limits: entries and chunk capacities in 16 bits, the capacity tiles in an int
+  if (ne > 65535 || nci > 65535 || nc1 > 65535 || ne * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) > INT_MAX)
+    return false;
+  c->ne = static_cast<int>(ne);
+  c->nci = static_cast<int>(nci);
+  c->nc1 = static_cast<int>(nc1);
+  return true;
+}
+static int check_models_dev(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
+                            const int32_t* nbs, int64_t max_rows, const int32_t* status, ModelsDevCaps* caps) {
+  int rc = check_models(ps, M);
+  if (rc) return rc;
+  DSMIL_REQUIRE(dsmil_models_supported(ps, M), "shape not supported by the fused fold step (D=%d, C=%d, nonlinear=%d, "
+                "passing_v=%d, M=%d)", ps[0].D, ps[0].C, ps[0].nonlinear, ps[0].passing_v, M);
+  DSMIL_REQUIRE(Xs && Ns && nbs && status, "NULL bag list or status");
+  DSMIL_REQUIRE(models_dev_caps(ps, M, nbs, max_rows, caps),
+                "a model's nb outside [1, 65535], too many bags in all, or max_rows=%lld out of range",
+                (long long)max_rows);
+  return 0;
+}
+// What the planner is told of the models (weights; with g, where their gradients go).
+static PlanModelsArgs plan_models_args(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
+                                       const int32_t* nbs, int64_t max_rows, int32_t* status,
+                                       const dsmil_grads_t* g) {
+  PlanModelsArgs a{};
+  a.Xs = Xs; a.Ns = Ns; a.M = M; a.C = ps[0].C; a.D = ps[0].D; a.max_rows = max_rows; a.status = status;
+  for (int m = 0, e0 = 0; m < M; e0 += nbs[m], ++m) {
+    const dsmil_params_t& p = ps[m];
+    a.m[m].w = sm90::ModelDev{p.Wi, p.bi, p.W1, p.b1, p.W2, p.b2, p.Wf, p.bf};
+    if (g) {
+      a.m[m].gWi = g[m].gWi; a.m[m].gbi = g[m].gbi; a.m[m].gW1 = g[m].gW1; a.m[m].gb1 = g[m].gb1;
+      a.m[m].gW2 = g[m].gW2; a.m[m].gb2 = g[m].gb2; a.m[m].gWf = g[m].gWf; a.m[m].gbf = g[m].gbf;
+    }
+    a.m[m].e0 = e0;
+    a.m[m].nb = nbs[m];
+  }
+  return a;
+}
+
+// The forward's carve for the capacity batch (every bag max_rows rows), then the planner's counts and the zero row.
+static ModelsWs carve_models_dev(const dsmil_params_t* ps, int M, int ne, int64_t max_rows, void* ws, size_t cap,
+                                 bool* ok, ModelsPlan** plan, float** zero_row) {
+  const std::vector<int64_t> Ns(ne, max_rows);
+  ModelsWs w = carve_models(&ps[0], M, Ns.data(), ne, 1, false, ws, cap, ok);
+  Carver c(ws, cap);
+  c.off = w.bytes;
+  *plan = c.take<ModelsPlan>(1);
+  *zero_row = c.take<float>(ps[0].D);
+  w.bytes = c.off;
+  *ok = c.ok();
+  return w;
+}
+
+size_t dsmil_forward_bags_models_train_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                           int64_t max_rows) {
+  ModelsDevCaps caps;
+  if (!models_dev_caps(ps, M, nbs, max_rows, &caps)) return 0;
+  bool ok;
+  ModelsPlan* plan;
+  float* zero_row;
+  size_t bytes = carve_models_dev(ps, M, caps.ne, max_rows, nullptr, 0, &ok, &plan, &zero_row).bytes;
+  // never below the eager fold call's size for the same capacity, nor the one-model dev calls' sizes together
+  const std::vector<int64_t> Ns(caps.ne, max_rows);
+  bytes = std::max(bytes, dsmil_forward_bags_models_train_workspace_bytes(ps, M, Ns.data(), nbs));
+  size_t each = 0;
+  for (int m = 0; m < M; ++m) each += ws_slice(dsmil_forward_bags_train_dev_workspace_bytes(&ps[m], nbs[m], max_rows));
+  return std::max(bytes, each);
+}
+
+int dsmil_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                        const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, float* classes,
+                                        float* pred, float* A, float* B, int64_t* crit_idx, float* save_Q,
+                                        float* save_H1, int32_t* status, void* workspace, size_t workspace_bytes,
+                                        void* stream) {
+  ModelsDevCaps caps;
+  int rc = check_models_dev(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, &caps);
+  if (rc) return rc;
+  DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && save_H1, "NULL output pointer");
+  const size_t need = dsmil_forward_bags_models_train_dev_workspace_bytes(ps, M, nbs, max_rows);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int C = ps[0].C, D = ps[0].D, ne = caps.ne;
+  bool ok;
+  ModelsPlan* plan;
+  float* zero_row;
+  ModelsWs w = carve_models_dev(ps, M, ne, max_rows, workspace, workspace_bytes, &ok, &plan, &zero_row);
+  PlanModelsArgs pa = plan_models_args(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, nullptr);
+  pa.zero_row = zero_row;
+  pa.plan = plan;
+  pa.ftable = w.table;
+  pa.fmodels = w.models;
+  k_plan_bags_models<<<1, 32 * M, 0, st>>>(pa);
+  DSMIL_LAUNCH_OK("k_plan_bags_models");
+  // as dsmil_forward_bags_train_dev: the weight images rebuilt on every call, phase 1 on the capacity grid of tiles,
+  // the attend pass a plain launch on the capacity grid of records
+  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * ne, st));
+  if ((rc = sm90::launch_prep_wimg_models(w.models, M, D, w.wimg, st))) return rc;
+  if ((rc = sm90::launch_qmlp_models(w.models, M, D, C, w.table, ne, ne * tiles_for_bag(max_rows), classes, w.keys,
+                                     save_Q, save_H1, false, w.wimg, num_sms(), st, nullptr, &plan->tiles)))
+    return rc;
+  sm90::AttendArgs aa{w.table, ne, D, C, save_Q, false, w.keys, A, w.recs, nullptr, &plan->recs, nullptr};
+  if ((rc = sm90::launch_attend_b(aa, ne * recs_for_bag(max_rows), st))) return rc;
+  sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, nullptr, nullptr, A, B, pred,
+                        reinterpret_cast<long long*>(crit_idx), w.pred_part, w.counters, nullptr, 0, 0, w.models, 1, 0};
+  return sm90::launch_finalize_b(fa, ne, st);
+}
+
+// The backward's carve at the capacities, then the planner's counts and the zero row.
+static BwdModelsWs carve_bwd_models_dev(const dsmil_params_t* ps, int M, const ModelsDevCaps& caps, int64_t max_rows,
+                                        void* ws, size_t cap, bool* ok, ModelsPlan** plan, float** zero_row) {
+  BwdModelsPlan pl;
+  pl.table.resize(caps.ne);
+  pl.chi.resize(caps.nci);
+  pl.ch1.resize(caps.nc1);
+  pl.ch2.resize(caps.nc2);
+  pl.chc.resize(caps.ncs);
+  pl.slots = caps.ne * caps.Gcap;
+  BwdModelsWs w = carve_bwd_models(ps, M, pl, caps.ne * max_rows, ws, cap, ok);
+  Carver c(ws, cap);
+  c.off = w.bytes;
+  *plan = c.take<ModelsPlan>(1);
+  *zero_row = c.take<float>(ps[0].D);
+  w.bytes = c.off;
+  *ok = c.ok();
+  return w;
+}
+
+size_t dsmil_backward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                      int64_t max_rows) {
+  ModelsDevCaps caps;
+  if (!models_dev_caps(ps, M, nbs, max_rows, &caps)) return 0;
+  bool ok;
+  ModelsPlan* plan;
+  float* zero_row;
+  size_t bytes = carve_bwd_models_dev(ps, M, caps, max_rows, nullptr, 0, &ok, &plan, &zero_row).bytes;
+  const std::vector<int64_t> Ns(caps.ne, max_rows);
+  bytes = std::max(bytes, dsmil_backward_bags_models_workspace_bytes(ps, M, Ns.data(), nbs, 0));
+  size_t each = 0;
+  for (int m = 0; m < M; ++m) each += ws_slice(dsmil_backward_bags_dev_workspace_bytes(&ps[m], nbs[m], max_rows));
+  return std::max(bytes, each);
+}
+
+int dsmil_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                   const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, const float* Q,
+                                   const float* H1, const float* A, const float* B, const int64_t* crit_idx,
+                                   const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                                   const dsmil_grads_t* grads, int32_t* status, void* workspace,
+                                   size_t workspace_bytes, void* stream) {
+  ModelsDevCaps caps;
+  int rc = check_models_dev(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, &caps);
+  if (rc) return rc;
+  DSMIL_REQUIRE(Q && H1 && A && B && crit_idx && grads, "NULL pointer");
+  bool gX = false;
+  for (int m = 0; m < M; ++m) gX = gX || grads[m].gX != nullptr;
+  DSMIL_REQUIRE(!d_A && !d_B && !gX,
+                "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
+  const size_t need = dsmil_backward_bags_models_dev_workspace_bytes(ps, M, nbs, max_rows);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int C = ps[0].C, D = ps[0].D;
+  bool ok;
+  ModelsPlan* plan;
+  float* zero_row;
+  BwdModelsWs w = carve_bwd_models_dev(ps, M, caps, max_rows, workspace, workspace_bytes, &ok, &plan, &zero_row);
+  PlanModelsArgs pa = plan_models_args(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, grads);
+  pa.Gcap = caps.Gcap;
+  pa.zero_row = zero_row;
+  pa.plan = plan;
+  pa.btable = w.table;
+  pa.bmodels = w.models;
+  pa.chi = w.chi; pa.ch1 = w.ch1; pa.ch2 = w.ch2; pa.chc = w.chc;
+  pa.ncs_cap = caps.ncs;
+  pa.segs = w.segs;
+  pa.lin = w.lin;
+  pa.H1 = H1;
+  pa.dz2 = w.dz2;
+  pa.dz1 = w.dz1;
+  pa.dc = d_classes != nullptr;
+  k_plan_bags_models<<<1, 32 * M, 0, st>>>(pa);
+  DSMIL_LAUNCH_OK("k_plan_bags_models");
+  if (!d_classes)   // no gradient through the scores: zero instance-classifier gradients, as the eager call
+    for (int m = 0; m < M; ++m) {
+      if (grads[m].gWi) DSMIL_CUDA_OK(cudaMemsetAsync(grads[m].gWi, 0, sizeof(float) * C * D, st));
+      if (grads[m].gbi) DSMIL_CUDA_OK(cudaMemsetAsync(grads[m].gbi, 0, sizeof(float) * C, st));
+    }
+  BwdModelsGrid gr{caps.Gcap, caps.nci, caps.nc1, caps.nc2, caps.ncs, caps.max_model_rows, false, plan};
+  return bwd_models_launch(C, D, M, caps.ne, w, gr, Q, H1, A, B, crit_idx, d_classes, d_pred, nullptr, nullptr, st);
 }
 
 // ---- capture-safe row-sharded batch training: the six calls of the sharded step in dev form -----------------------

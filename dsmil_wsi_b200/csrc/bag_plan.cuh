@@ -75,6 +75,28 @@ __host__ __device__ inline int rag_chunks(const float* const* Xs, const int64_t*
   }
   return z;
 }
+// A bag list as a planner walks it: the caller's (host or device memory), or, with zero_row set, the stand-in batch of
+// a refused list, every bag one row of zeros.
+struct BagList {
+  const float* const* Xs;
+  const int64_t* Ns;
+  const float* zero_row;
+  __host__ __device__ const float* X(int b) const { return zero_row ? zero_row : Xs[b]; }
+  __host__ __device__ int64_t N(int b) const { return zero_row ? 1 : Ns[b]; }
+};
+// rag_chunks over a BagList whose packed rows start at row0.  out == NULL: count only (the features are not read).
+__host__ __device__ inline int rag_chunks_list(const BagList& L, int nb, int M2, int64_t rps, long long row0,
+                                               TnChunk* out) {
+  int z = 0;
+  long long row = row0;
+  for (int b = 0; b < nb; ++b) {
+    const int64_t N = L.N(b);
+    for (int64_t r0 = 0; r0 < N; r0 += rps, ++z)
+      if (out) out[z] = TnChunk{L.X(b) + r0 * M2, row + r0, N - r0 < rps ? N - r0 : rps};
+    row += N;
+  }
+  return z;
+}
 // Most chunks rag_chunks can give for nb bags at any total: rps >= total / rag_splits, so the whole chunks number at
 // most rag_splits, and each bag adds at most one short chunk.
 __host__ __device__ inline int rag_chunks_cap(int M1, int M2, bool gemv, int nb) { return rag_splits(M1, M2, gemv) + nb; }
@@ -166,6 +188,190 @@ k_plan_bags(const float* const* __restrict__ Xs, const int64_t* __restrict__ Ns,
   pl.cs = colsum_split(row);
   pl.tn2 = gemm_tn_split(kQ, kQ, row);
   *plan = pl;
+}
+
+// ---- the fold step: M models, each over its own bags (dsmil_*_bags_models*) --------------------------------------
+// What the fused backward's kernels read per model (bwd_bags.cuh).  The eager call fills these on the host; the dev
+// call's planner, k_plan_bags_models, on the device.
+struct BwdModelDev {
+  const float *Wf, *Wi;
+  float *gWf, *gbf, *gX;
+  int e0, nb;            // the model's first entry, its bags
+  long long r0;          // its first packed row
+};
+// One model's share of a chunked reduction: partials [z0, z0 + S) summed into out (NULL: the gradient is not wanted).
+struct SumSeg {
+  float* out;
+  int z0, S;
+};
+// One model's rows of a row-wise linear layer (k_linear_models): Y = X op(W) (+ the ReLU mask of aux); Y NULL: skip.
+struct LinSeg {
+  const float *X, *W, *aux;
+  float* Y;
+  long long N;
+};
+
+// Every split the one-model backward would choose for one model's own batch of nb bags, `total` rows, the largest of
+// mx: the per-row kernels' CTAs per bag, the rows per chunk of gWi and gW1, and the row splits of gW2 and of the
+// column sums.  They follow from that model's live sizes alone, which is what keeps its gradients' bits.
+struct ModelSplits {
+  int G;
+  int64_t rps_i, rps_1;
+  RowSplit t2, cs;
+};
+__host__ __device__ inline ModelSplits model_splits(int C, int D, int nb, int64_t total, int64_t mx) {
+  ModelSplits s;
+  s.G = bwd_bags_ctas(nb, mx);
+  s.rps_i = rag_rows_per_chunk(C, D, total, tn_use_gemv(C, D));   // the fused route's bags are 16-byte aligned
+  s.rps_1 = rag_rows_per_chunk(kQ, D, total, false);
+  s.t2 = gemm_tn_split(kQ, kQ, total);
+  s.cs = colsum_split(total);
+  return s;
+}
+// Split z of `s` as a chunk of a model whose packed rows start at r0; R: the packed right operand ([*, ldr]) or NULL.
+__host__ __device__ inline TnChunk split_chunk(const RowSplit& s, int z, long long r0, const float* R, int ldr) {
+  const long long lo = z * s.rps, hi = lo + s.rps < s.N ? lo + s.rps : s.N;
+  return TnChunk{R ? R + (r0 + lo) * ldr : nullptr, r0 + lo, hi - lo};
+}
+// Most splits gemm_tn_split(kQ, kQ, .) and colsum_split give at any row count.
+constexpr int kModelSplitsCap = kSplits;
+
+// The live counts of a fold dev call, over all models: the forward's tiles and records, the backward's chunks.
+struct ModelsPlan {
+  int tiles, recs;
+  int nci, nc1, nc2, ncs;
+};
+// What the host knows of model m in a dev call, passed to the planner by value (a dev call uploads nothing).
+struct PlanModel {
+  sm90::ModelDev w;
+  float *gWi, *gbi, *gW1, *gb1, *gW2, *gb2, *gWf, *gbf;   // backward: the model's gradients (NULL: not wanted)
+  int e0, nb;                                              // its first entry of the list, its bags
+};
+struct PlanModelsArgs {
+  const float* const* Xs;     // [sum nb] device memory, model-major
+  const int64_t* Ns;
+  int M, C, D;
+  int Gcap;                   // backward: per-CTA partial slots per entry
+  long long max_rows;
+  float* zero_row;            // [D]
+  int* status;                // [M]
+  ModelsPlan* plan;
+  sm90::BagDev* ftable;       // forward call: the table in the forward numbering, and the members
+  sm90::ModelDev* fmodels;
+  sm90::BagDev* btable;       // backward call: the table in the backward numbering (bwd_bags.cuh) ...
+  BwdModelDev* bmodels;
+  TnChunk *chi, *ch1, *ch2, *chc;   // ... the compacted chunk tables (chc padded to ncs_cap with empty chunks) ...
+  int ncs_cap;
+  SumSeg* segs;               // ... [6][M] and [2][M], as backward_bags_models_impl lays them out
+  LinSeg* lin;
+  const float* H1;
+  float *dz2, *dz1;
+  int dc;                     // gradients flow through the scores (d_classes != NULL)
+  PlanModel m[sm90::kMaxModels];
+};
+
+// The planner of a fold dev call: warp m plans model m from its own bags, as k_plan_bags plans one model, so model
+// m's tables are what its one-model dev call would build, shifted to its capacity block (rows from max_rows * e0).
+// The models meet only at prefix sums of their counts: tiles and records of the forward numbering, and the chunk
+// tables, which are compacted (model m's chunks follow model m - 1's live ones), so that the GEMM grids' live
+// counts are single numbers and the partial buffer is indexed as in the eager call.  A model with a bad bag (N
+// outside [1, max_rows], features NULL or not 16-byte aligned) sets status[m] = 1 + the bag's index within the model
+// and is planned on its stand-in batch (every bag one row of zeros); the other models' plans do not change.
+__global__ void __launch_bounds__(32 * sm90::kMaxModels)
+k_plan_bags_models(const PlanModelsArgs a) {
+  enum { TILES, RECS, NCI, NC1, NC2, NCS, NCNT };
+  __shared__ int s_cnt[NCNT][sm90::kMaxModels];
+  const int m = threadIdx.x >> 5, lane = threadIdx.x & 31, M = a.M;
+  const int e0 = a.m[m].e0, nb = a.m[m].nb;
+  const long long cap0 = a.max_rows * e0;
+  const bool bwd = a.btable != nullptr;
+  // the first bad bag and the largest bag, the lanes sharing the list
+  int bad = nb + 1;
+  long long mx = 0;
+  for (int b = lane; b < nb; b += 32) {
+    const int64_t N = a.Ns[e0 + b];
+    const float* X = a.Xs[e0 + b];
+    if ((N < 1 || N > a.max_rows || X == nullptr || (reinterpret_cast<uintptr_t>(X) & 15) != 0) && b + 1 < bad)
+      bad = b + 1;
+    mx = N > mx ? N : mx;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    const int ob = __shfl_xor_sync(0xffffffffu, bad, o);
+    const long long om = __shfl_xor_sync(0xffffffffu, mx, o);
+    bad = ob < bad ? ob : bad;
+    mx = om > mx ? om : mx;
+  }
+  if (bad > nb) bad = 0;
+  if (bad) {
+    if (lane == 0) a.status[m] = bad;
+    for (int i = lane; i < a.D; i += 32) a.zero_row[i] = 0.f;
+    mx = 1;
+  }
+  const BagList L{a.Xs + e0, a.Ns + e0, bad ? a.zero_row : nullptr};
+  long long total = 0;
+  if (lane == 0) {
+    int tiles = 0, recs = 0;
+    for (int b = 0; b < nb; ++b) {
+      const int64_t N = L.N(b);
+      total += N;
+      tiles += tiles_for_bag(N);
+      recs += recs_for_bag(N);
+    }
+    s_cnt[TILES][m] = tiles;
+    s_cnt[RECS][m] = recs;
+  }
+  total = __shfl_sync(0xffffffffu, total, 0);
+  const ModelSplits sp = model_splits(a.C, a.D, nb, total, mx);
+  if (lane == 0) {
+    s_cnt[NCI][m] = bwd ? rag_chunks_list(L, nb, a.D, sp.rps_i, 0, nullptr) : 0;
+    s_cnt[NC1][m] = bwd ? rag_chunks_list(L, nb, a.D, sp.rps_1, 0, nullptr) : 0;
+    s_cnt[NC2][m] = bwd ? sp.t2.S : 0;
+    s_cnt[NCS][m] = bwd ? sp.cs.S : 0;
+  }
+  __syncthreads();
+  int at[NCNT], all[NCNT];   // this model's first index of each numbering, and the totals
+  for (int i = 0; i < NCNT; ++i) {
+    at[i] = all[i] = 0;
+    for (int j = 0; j < M; ++j) {
+      if (j < m) at[i] += s_cnt[i][j];
+      all[i] += s_cnt[i][j];
+    }
+  }
+  if (threadIdx.x == 0) *a.plan = ModelsPlan{all[TILES], all[RECS], all[NCI], all[NC1], all[NC2], all[NCS]};
+  if (a.ftable && lane == 0) {
+    long long row = cap0;
+    int tile = at[TILES], rec = at[RECS];
+    for (int b = 0; b < nb; ++b) {
+      sm90::BagDev e = bag_entry(L.X(b), L.N(b), row, tile, rec);
+      e.pad_ = m;
+      a.ftable[e0 + b] = e;
+    }
+    a.fmodels[m] = a.m[m].w;
+  }
+  if (!bwd) return;
+  if (lane == 0) {
+    const PlanModel& pm = a.m[m];
+    long long row = cap0;
+    for (int b = 0; b < nb; ++b) {
+      a.btable[e0 + b] = sm90::BagDev{L.X(b), L.N(b), row, sp.G, (e0 + b) * a.Gcap, 0, m};
+      row += L.N(b);
+    }
+    rag_chunks_list(L, nb, a.D, sp.rps_i, cap0, a.chi + at[NCI]);
+    rag_chunks_list(L, nb, a.D, sp.rps_1, cap0, a.ch1 + at[NC1]);
+    a.bmodels[m] = BwdModelDev{pm.w.Wf, pm.w.Wi, pm.gWf, pm.gbf, nullptr, e0, nb, cap0};
+    a.segs[0 * M + m] = SumSeg{a.dc ? pm.gWi : nullptr, at[NCI], s_cnt[NCI][m]};
+    a.segs[1 * M + m] = SumSeg{a.dc ? pm.gbi : nullptr, at[NCS], sp.cs.S};
+    a.segs[2 * M + m] = SumSeg{pm.gW2, at[NC2], sp.t2.S};
+    a.segs[3 * M + m] = SumSeg{pm.gb2, at[NCS], sp.cs.S};
+    a.segs[4 * M + m] = SumSeg{pm.gW1, at[NC1], s_cnt[NC1][m]};
+    a.segs[5 * M + m] = SumSeg{pm.gb1, at[NCS], sp.cs.S};
+    a.lin[m] = LinSeg{a.dz2 + cap0 * kQ, pm.w.W2, a.H1 + cap0 * kQ, a.dz1 + cap0 * kQ, total};
+    a.lin[M + m] = LinSeg{a.dz1 + cap0 * kQ, pm.w.W1, nullptr, nullptr, total};
+  }
+  for (int z = lane; z < sp.t2.S; z += 32) a.ch2[at[NC2] + z] = split_chunk(sp.t2, z, cap0, a.H1, kQ);
+  for (int z = lane; z < sp.cs.S; z += 32) a.chc[at[NCS] + z] = split_chunk(sp.cs, z, cap0, nullptr, 0);
+  // k_colsum_rag runs on the capacity grid: the chunks past the live ones are empty (their partial is not read)
+  for (int z = all[NCS] + threadIdx.x; z < a.ncs_cap; z += blockDim.x) a.chc[z] = TnChunk{nullptr, 0, 0};
 }
 
 }  // namespace dsmil

@@ -273,24 +273,8 @@ inline int launch_gemm_tn_rag(const float* P, int M1, int M2, const TnChunk* chu
 // model; its spare fields carry what the one-model call derives from its own batch: tile_off = G of the entry's model
 // (bwd_bags_ctas of that model's bags), rec_off = the entry's first per-CTA partial slot in tpart / dpart, pad_ = its
 // model.  Each stage reproduces, entry by entry or model by model, the split sums of dsmil_backward_bags on that
-// model's bags alone, so every model's gradients keep its bits.
-struct BwdModelDev {
-  const float *Wf, *Wi;
-  float *gWf, *gbf, *gX;
-  int e0, nb;            // the model's first entry, its bags
-  long long r0;          // its first packed row
-};
-// One model's share of a chunked reduction: partials [z0, z0 + S) summed into out (NULL: the gradient is not wanted).
-struct SumSeg {
-  float* out;
-  int z0, S;
-};
-// One model's rows of a row-wise linear layer (k_linear_models): Y = X op(W) (+ the ReLU mask of aux); Y NULL: skip.
-struct LinSeg {
-  const float *X, *W, *aux;
-  float* Y;
-  long long N;
-};
+// model's bags alone, so every model's gradients keep its bits.  (BwdModelDev, SumSeg and LinSeg: bag_plan.cuh, where
+// the dev calls' planner fills them.)
 
 // dB, gWf and gbf of model blockIdx.y over its bags, as k_bwd_bag_b
 __global__ void __launch_bounds__(256)

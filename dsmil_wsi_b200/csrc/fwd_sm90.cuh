@@ -656,12 +656,14 @@ inline int launch_prep_wimg_models(const ModelDev* models_dev, int M, int D, uin
   return 0;
 }
 // Scores, arg-max keys and Q (+ H1 when non-NULL; Q tile-blocked when q_blocked, else row-major after the tanh, as the
-// training forward keeps it) of every entry; C <= 4 (the batched shapes), done as in launch_qmlp.
+// training forward keeps it) of every entry; C <= 4 (the batched shapes), done as in launch_qmlp.  ntiles_dev != NULL
+// (the fold dev call): ntiles is the capacity, *ntiles_dev the live count.
 inline int launch_qmlp_models(const ModelDev* models_dev, int M, int D, int C, const BagDev* bags_dev, int nb,
                               int ntiles, float* classes, unsigned long long* keys, float* Q, float* H1,
-                              bool q_blocked, const uint8_t* wimg, int max_ctas, cudaStream_t st, unsigned int* done) {
+                              bool q_blocked, const uint8_t* wimg, int max_ctas, cudaStream_t st, unsigned int* done,
+                              const int* ntiles_dev = nullptr) {
   QmlpModelsArgs a{{bags_dev, nb, ntiles, D, C, nullptr, nullptr, nullptr, nullptr, wimg, nullptr, classes, keys, Q,
-                    H1, q_blocked, nullptr, done}, models_dev, M, wimg_bytes(D)};
+                    H1, q_blocked, ntiles_dev, done}, models_dev, M, wimg_bytes(D)};
   const size_t smem = qmlp_models_smem_bytes(C, D, M);
   const int grid = ntiles < max_ctas ? ntiles : max_ctas;
   auto go = [&](auto kern) -> int {
@@ -672,6 +674,16 @@ inline int launch_qmlp_models(const ModelDev* models_dev, int M, int D, int C, c
     DSMIL_LAUNCH_OK("k_qmlp_sm90");
     return 0;
   };
+  if (ntiles_dev != nullptr) {
+    if (D == 512) {
+      if (C == 1) return go(k_qmlp_sm90<1, 512, true, true>);
+      if (C == 2) return go(k_qmlp_sm90<2, 512, true, true>);
+      return go(k_qmlp_sm90<4, 512, true, true>);
+    }
+    if (C == 1) return go(k_qmlp_sm90<1, 0, true, true>);
+    if (C == 2) return go(k_qmlp_sm90<2, 0, true, true>);
+    return go(k_qmlp_sm90<4, 0, true, true>);
+  }
   if (D == 512) {
     if (C == 1) return go(k_qmlp_sm90<1, 512, false, true>);
     if (C == 2) return go(k_qmlp_sm90<2, 512, false, true>);

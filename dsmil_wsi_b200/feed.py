@@ -164,7 +164,7 @@ def fold_steps(sizes: Sequence[int], k: int) -> List[List[Tuple[int, int, int]]]
 def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[int]], criterion,
                        optimizers, dropout_patch: float = 0.0, orders: Optional[Sequence[Sequence[int]]] = None,
                        generators: Optional[Sequence[Optional[torch.Generator]]] = None,
-                       bags_per_step: int = 1) -> List[float]:
+                       bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None) -> List[float]:
     """One epoch of every fold model of a cross-validation (train_tcga.py:252-288, train_mil.py:164-187), the folds
     taking their steps together; returns each fold's mean loss per bag.  folds[m] lists the store indices of fold m's
     training split; orders[m], when given, is the order fold m visits them in (a permutation of folds[m]), else a
@@ -180,7 +180,14 @@ def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[
     those of train_epoch(milnets[m], store, criterion, optimizers[m], dropout_patch, orders[m], generators[m], k, graph=True)
     (and of the eager minibatch epoch for k >= 2).  Without generators, or with one generator shared by the folds,
     the folds' permutation draws interleave in step order (fold 0's group, then fold 1's, ...), so each fold sees
-    different draws than it would alone."""
+    different draws than it would alone.
+
+    graph=True: every step is a replay of a train_graph.FoldTrainStepGraph, recorded once per (folds in the step, their
+    group sizes) -- for folds whose sizes differ by at most one bag, at most three graphs an epoch -- with the same
+    bits.  The bags go through dropout_patches straight into the graph's slots; max_rows is the per-bag row capacity
+    (default: the largest bag of the store), and a bag over it raises ValueError before any step.  Needs the fused fold
+    shapes (dsmil_models_supported) and capture-safe optimizers, and records its graphs afresh on every call, as
+    train_epoch(graph=True) does."""
     from .ensemble import forward_bags_per_model
     milnets, M = list(milnets), len(folds)
     if not 1 <= M <= Fn.MAX_MODELS:
@@ -205,6 +212,9 @@ def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[
     gens = list(generators) if generators is not None else [None] * M
     for net in milnets:
         net.train()
+    if graph:
+        return _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_patch, orders, gens,
+                                         bags_per_step, max_rows)
     totals = [torch.zeros((), device=store.device) for _ in range(M)]
     for step in fold_steps([len(o) for o in orders], bags_per_step):
         groups = [(m, orders[m][lo:hi]) for m, lo, hi in step]
@@ -260,6 +270,50 @@ def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order
     if bad:
         raise RuntimeError(f"training graph: a batch held a bag outside [1, {cap}] rows (planner status {int(bad)})")
     return loss / max(1, len(order))
+
+
+def _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_patch, orders, gens, k, max_rows):
+    from .train_graph import FoldTrainStepGraph, fold_step_shape
+    fold_step_shape(milnets)                                   # shapes off the fused fold route raise here
+    p = 1 - dropout_patch
+    keep = {i: int(int(store.bags[i][0].shape[0]) * p) for o in orders for i in o}   # dropout_patches' row counts
+    cap = int(max_rows) if max_rows is not None else max([int(f.shape[0]) for f, _ in store.bags], default=1)
+    for m, o in enumerate(orders):
+        for i in o:
+            if keep[i] > cap:
+                raise ValueError(f"fold {m}, bag {i}: {keep[i]} rows exceed the training graph's max_rows={cap}")
+            if keep[i] < 1:
+                raise IndexError(f"dsmil_b200: fold {m}, bag {i} is empty after patch dropout (N == 0)")
+    graphs = {}
+    totals = [torch.zeros((), device=store.device) for _ in orders]
+    bad = torch.zeros(len(orders), dtype=torch.int32, device=store.device)
+    for step in fold_steps([len(o) for o in orders], k):
+        key = tuple((m, hi - lo) for m, lo, hi in step)
+        g = graphs.get(key)
+        if g is None:                                          # the full step, short last groups, fewer folds
+            g = graphs[key] = FoldTrainStepGraph([milnets[m] for m, _ in key], criterion,
+                                                 [optimizers[m] for m, _ in key], [n for _, n in key], cap)
+        e = 0
+        for j, (m, lo, hi) in enumerate(step):
+            group = orders[m][lo:hi]
+            for b, i in enumerate(group):
+                dropout_patches(store.bags[i][0], p, gens[m], out=g.slots[j][b])
+                g.Ns[e + b].fill_(keep[i])
+            torch.cat([store.bags[i][1].view(1, -1) for i in group], out=g.labels[e:e + len(group)])
+            e += len(group)
+        losses = g.step()
+        for j, (m, lo, hi) in enumerate(step):
+            totals[m] += losses[j] * (hi - lo)
+    for key, g in graphs.items():
+        for j, (m, _) in enumerate(key):
+            bad[m] = torch.where(bad[m] != 0, bad[m], g.status[j])
+    # the epoch's one host sync, which also reads the planners' status words
+    host = torch.cat([torch.stack(totals).double(), bad.double()]).tolist()
+    for m, st in enumerate(host[len(orders):]):
+        if st:
+            raise RuntimeError(f"training graph: fold {m} held a bag outside [1, {cap}] rows (planner status "
+                               f"{int(st)})")
+    return [t / len(o) for t, o in zip(host, orders)]
 
 
 def _group_predictions(outs):

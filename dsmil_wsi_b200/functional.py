@@ -524,6 +524,78 @@ class MILBagsModelsFn(torch.autograd.Function):
         return (None, *gxs, *[o[n] for o in outs for n in PARAM_NAMES])
 
 
+class MILBagsModelsDevFn(torch.autograd.Function):
+    """MILBagsModelsFn over the capture-safe entry points (dsmil_forward_bags_models_train_dev /
+    dsmil_backward_bags_models_dev): every member's bag list lives on the device, so one recorded call serves every
+    step of the same group sizes.
+
+    args: nbs (each member's bag count), slots [sum(nbs), max_rows, D] (member-major; bag e is slots[e, :Ns[e]]),
+    Ns [sum(nbs)] int64 and status [M] int32 on the device, then the M members' ten parameter tensors each.  The
+    packed per-row outputs (classes, A) have sum(nbs) * max_rows rows: member m's block starts at row
+    max_rows * sum(nbs[:m]) and packs its live rows at the prefix sums of its own Ns.  Parameter gradients only."""
+
+    @staticmethod
+    def forward(ctx, nbs, slots, Ns, status, *params):
+        lib = _lib.load()
+        ctx.set_materialize_grads(False)
+        M, ne = len(nbs), sum(nbs)
+        packs = _model_packs([params[10 * m:10 * (m + 1)] for m in range(M)])
+        P0 = packs[0]
+        ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
+        if min(nbs) < 1 or not lib.dsmil_models_supported(ps, M):
+            raise ValueError(f"the graph-captured fold step runs on the fused fold shapes only; M={M}, D={P0.D}, "
+                             f"C={P0.C}, nonlinear={P0.nonlinear}, group sizes {tuple(nbs)} are not on them")
+        if slots.dim() != 3 or slots.shape[0] != ne or slots.shape[2] != P0.D or slots.dtype != torch.float32 \
+                or not slots.is_contiguous():
+            raise ValueError(f"slots must be contiguous float32 [{ne}, max_rows, {P0.D}], got {tuple(slots.shape)}")
+        max_rows, dev = int(slots.shape[1]), P0.device
+        c_nb = (C.c_int32 * M)(*nbs)
+        with torch.cuda.device(dev):
+            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+            rows = ne * max_rows
+            classes, A = new(rows, P0.C), new(rows, P0.C)
+            pred, B = new(ne, P0.C), new(ne, P0.C, P0.D)
+            crit = torch.empty(ne, P0.C, dtype=torch.int64, device=dev)
+            sQ, sH = new(rows, Q_DIM), new(rows, Q_DIM)
+            xs = slots.data_ptr() + 4 * max_rows * P0.D * torch.arange(ne, dtype=torch.int64, device=dev)
+            ws = _workspace(lib.dsmil_forward_bags_models_train_dev_workspace_bytes(ps, M, c_nb, max_rows), dev)
+            rc = lib.dsmil_forward_bags_models_train_dev(ps, M, _ptr(xs), _ptr(Ns), c_nb, max_rows, _ptr(classes),
+                                                         _ptr(pred), _ptr(A), _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH),
+                                                         _ptr(status), _ptr(ws), ws.numel(), _stream())
+            _lib.check(rc, "dsmil_forward_bags_models_train_dev")
+        ctx.save_for_backward(xs, Ns, status, sQ, sH, A, B, crit, *[t for P in packs for t in P.tensors])
+        ctx.nbs, ctx.max_rows = tuple(nbs), max_rows
+        ctx.mark_non_differentiable(crit)
+        return classes, pred, A, B, crit
+
+    @staticmethod
+    def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
+        if ctx.needs_input_grad[1] or g_A is not None or g_B is not None:
+            raise NotImplementedError("the graph-captured fold step takes gradients through the instance scores "
+                                      "and the bag prediction only (no gradient to A, B or the features)")
+        lib = _lib.load()
+        xs, Ns, status, sQ, sH, A, B, crit, *params = ctx.saved_tensors
+        nbs, max_rows = ctx.nbs, ctx.max_rows
+        M = len(nbs)
+        packs = [ParamPack(*params[10 * m:10 * (m + 1)]) for m in range(M)]
+        dev = packs[0].device
+        ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
+        c_nb = (C.c_int32 * M)(*nbs)
+        need = ctx.needs_input_grad[4:]
+        with torch.cuda.device(dev):
+            outs = [{nm: (torch.empty_like(t) if t is not None and nd else None)
+                     for nm, t, nd in zip(PARAM_NAMES, P.tensors, need[10 * m:10 * (m + 1)])}
+                    for m, P in enumerate(packs)]
+            grads = (_lib.DsmilGrads * M)(*[_lib.DsmilGrads(*[_ptr(o[n]) for n in PARAM_NAMES], None) for o in outs])
+            dc, dp = _f32c(g_classes), _f32c(g_pred)
+            ws = _workspace(lib.dsmil_backward_bags_models_dev_workspace_bytes(ps, M, c_nb, max_rows), dev)
+            rc = lib.dsmil_backward_bags_models_dev(ps, M, _ptr(xs), _ptr(Ns), c_nb, max_rows, _ptr(sQ), _ptr(sH),
+                                                    _ptr(A), _ptr(B), _ptr(crit), _ptr(dc), _ptr(dp), None, None,
+                                                    grads, _ptr(status), _ptr(ws), ws.numel(), _stream())
+            _lib.check(rc, "dsmil_backward_bags_models_dev")
+        return (None, None, None, None, *[o[n] for o in outs for n in PARAM_NAMES])
+
+
 def mil_forward_bags_per_model(bag_lists: Sequence[Sequence[torch.Tensor]],
                                params_list: Sequence[Sequence[Optional[torch.Tensor]]], *, grad: bool = False):
     """M parameter sets (1 <= M <= 8, the same D, C and q form, identity v), each over its OWN non-empty list of bags,

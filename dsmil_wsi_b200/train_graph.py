@@ -55,6 +55,78 @@ def step_shape(milnet):
     return D, C
 
 
+def fold_step_shape(milnets):
+    """(D, C) of MILNets whose fold step the graph can record: each on step_shape's route, all of one D, C and q form,
+    1 to 8 of them, together on the fused fold shapes (dsmil_models_supported).  Else ValueError."""
+    milnets = list(milnets)
+    if not 1 <= len(milnets) <= Fn.MAX_MODELS:
+        raise ValueError(f"a fold step takes 1 to {Fn.MAX_MODELS} folds, got {len(milnets)}")
+    shapes = [step_shape(net) for net in milnets]
+    for m, sh in enumerate(shapes):
+        if sh != shapes[0]:
+            raise ValueError(f"fold {m}: (D, C)={sh} differs from fold 0's {shapes[0]}")
+    D, C = shapes[0]
+    ps = (_lib.DsmilParams * len(milnets))()
+    for p in ps:                       # the shape test reads no weights: any non-NULL address will do
+        p.D, p.C, p.nonlinear, p.passing_v = D, C, 1, 0
+        for name in ("Wi", "bi", "W1", "b1", "W2", "b2", "Wf", "bf"):
+            setattr(p, name, 16)
+    if not _lib.load().dsmil_models_supported(ps, len(milnets)):
+        raise ValueError(f"the graph-captured fold step runs on the fused fold shapes only; M={len(milnets)}, D={D}, "
+                         f"C={C} is not on them: train these folds one at a time (train_epoch(graph=True))")
+    return D, C
+
+
+def _flat(tensors):
+    with torch.no_grad():
+        return torch.cat([t.detach().reshape(-1).float() for t in tensors])
+
+
+def _snapshot(optimizer, params):
+    with torch.no_grad():
+        values = [p.detach().clone() for p in params]
+        state = {p: {k: (v.clone() if torch.is_tensor(v) else v) for k, v in optimizer.state[p].items()}
+                 for p in params if optimizer.state.get(p)}
+    return values, state
+
+
+def _restore(optimizer, params, snap):
+    """Puts parameters and optimizer state back in place; state created since the snapshot is reset to zeros."""
+    values, state = snap
+    with torch.no_grad():
+        for p, v in zip(params, values):
+            p.copy_(v)
+        for p in params:
+            cur, old = optimizer.state.get(p), state.get(p, {})
+            for k, v in (cur or {}).items():
+                if torch.is_tensor(v):
+                    v.copy_(old[k]) if k in old else v.zero_()
+                elif k in old:
+                    cur[k] = old[k]
+
+
+def _kept_tensors(optimizer, params):
+    """What a refused step puts back: the parameters and every tensor of the optimizer state."""
+    return params + [v for p in params for v in optimizer.state.get(p, {}).values() if torch.is_tensor(v)]
+
+
+def _keep_if(ok, kept, before):
+    """The stepped values of `kept` stand only where ok (bit for bit: a copy of them); else `before` returns."""
+    new = torch.where(ok, _flat(kept), before)
+    with torch.no_grad():
+        torch._foreach_copy_(kept, [v.view_as(t) for v, t in zip(new.split([t.numel() for t in kept]), kept)])
+
+
+def _warm_up(dev, steps, run):
+    """`run` `steps` times on a side stream, as torch.cuda.graph asks before a capture."""
+    side = torch.cuda.Stream(dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side):
+        for _ in range(max(1, steps)):
+            run()
+    torch.cuda.current_stream(dev).wait_stream(side)
+
+
 class TrainStepGraph:
     """One recorded minibatch step of nb bags of up to max_rows rows.
 
@@ -86,19 +158,15 @@ class TrainStepGraph:
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
         self._step_status = torch.zeros(1, dtype=torch.int32, device=dev)   # this replay's planners
         self._buffers(dev)
-        snap = self._snapshot()
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(max(1, warmup)):
-                optimizer.zero_grad(set_to_none=True)
-                self._step()
-        torch.cuda.current_stream(dev).wait_stream(side)
-        self._restore(snap)
+        snap = _snapshot(optimizer, self.params)
+
+        def warm():
+            optimizer.zero_grad(set_to_none=True)
+            self._step()
+        _warm_up(dev, warmup, warm)
+        _restore(optimizer, self.params, snap)
         optimizer.zero_grad(set_to_none=True)
-        # what a refused step puts back: the parameters and every tensor of the optimizer state (it exists now)
-        self._kept = self.params + [v for p in self.params for v in optimizer.state.get(p, {}).values()
-                                    if torch.is_tensor(v)]
+        self._kept = _kept_tensors(optimizer, self.params)   # the optimizer state exists now
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.loss = self._step(guard=True)
@@ -129,45 +197,16 @@ class TrainStepGraph:
         loss = torch.where(ok, loss, torch.full_like(loss, float("nan")))
         loss.backward()
         if guard:
-            before = self._flat(self._kept)
+            before = _flat(self._kept)
         self.optimizer.step()
         if guard:
-            # the update stands only for an accepted batch (bit for bit: a copy of the stepped values)
-            kept = torch.where(ok, self._flat(self._kept), before)
-            with torch.no_grad():
-                torch._foreach_copy_(self._kept, [v.view_as(t) for v, t in
-                                                  zip(kept.split([t.numel() for t in self._kept]), self._kept)])
+            _keep_if(ok, self._kept, before)   # the update stands only for an accepted batch
         self.status.copy_(torch.where(self.status != 0, self.status, self._step_status))
         return loss.detach()
-
-    @staticmethod
-    def _flat(tensors):
-        with torch.no_grad():
-            return torch.cat([t.detach().reshape(-1).float() for t in tensors])
 
     def step(self) -> torch.Tensor:
         self.graph.replay()
         return self.loss
-
-    def _snapshot(self):
-        with torch.no_grad():
-            params = [p.detach().clone() for p in self.params]
-            state = {p: {k: (v.clone() if torch.is_tensor(v) else v) for k, v in self.optimizer.state[p].items()}
-                     for p in self.params if self.optimizer.state.get(p)}
-        return params, state
-
-    def _restore(self, snap):
-        params, state = snap
-        with torch.no_grad():
-            for p, v in zip(self.params, params):
-                p.copy_(v)
-            for p in self.params:
-                cur, old = self.optimizer.state.get(p), state.get(p, {})
-                for k, v in (cur or {}).items():
-                    if torch.is_tensor(v):
-                        v.copy_(old[k]) if k in old else v.zero_()
-                    elif k in old:
-                        cur[k] = old[k]
 
 
 class ShardedTrainStepGraph(TrainStepGraph):
@@ -200,3 +239,95 @@ class ShardedTrainStepGraph(TrainStepGraph):
                                                               self.Ns.clamp(0, self.max_rows),
                                                               self._step_status[0] != 0, self.group)
         return feed.minibatch_loss(self.criterion, pred, mx, self.labels), ~refused
+
+
+class FoldTrainStepGraph:
+    """One recorded step of the fold models of a cross-validation: fold m takes nbs[m] bags of up to max_rows rows.
+
+    The step is feed.train_epoch_models' step over the capture-safe fold calls (MILBagsModelsDevFn): one forward for
+    all folds, each fold's feed.minibatch_loss on its own slices, the sum of the folds' losses, one backward, every
+    fold's optimizer.step().  Fill `slots[m][b, :n]` with bag b of fold m, `Ns` [sum nbs] (fold-major) with the row
+    counts and `labels` [sum nbs, C], then `step()` replays the graph and returns the M losses (a device tensor,
+    overwritten by the next replay).  With the same batches, fold m's losses, gradients and parameters are bit for
+    bit those of its own TrainStepGraph.
+
+    Refusal is per fold: a fold with a bag outside 1..max_rows has `status[m]` set (the first refusal's 1 + bag index
+    within the fold; never cleared here), a NaN loss, and its parameters and optimizer state left as they were; the
+    other folds step normally.  Warm-up, capture and hyperparameters behave as in TrainStepGraph."""
+
+    def __init__(self, milnets, criterion, optimizers, nbs, max_rows: int, warmup: int = 1):
+        milnets, optimizers, nbs = list(milnets), list(optimizers), [int(n) for n in nbs]
+        M = len(milnets)
+        if len(optimizers) != M or len(nbs) != M:
+            raise ValueError(f"FoldTrainStepGraph: {M} milnets, {len(optimizers)} optimizers and {len(nbs)} group "
+                             "sizes")
+        for opt in optimizers:
+            check_optimizer(opt)
+        D, C = fold_step_shape(milnets)
+        ne, max_rows = sum(nbs), int(max_rows)
+        if min(nbs) < 1 or ne > 65535 or max_rows < 1:
+            raise ValueError(f"FoldTrainStepGraph: group sizes {nbs} outside [1, 65535] or max_rows={max_rows} < 1")
+        self.milnets, self.criterion, self.optimizers = milnets, criterion, optimizers
+        self.nbs, self.max_rows = tuple(nbs), max_rows
+        self.params = [[p for g in opt.param_groups for p in g["params"]] for opt in optimizers]
+        dev = milnets[0].b_classifier.fcc.weight.device
+        for net in milnets:
+            Fn.require_cuda(net.b_classifier.fcc.weight, "the model")
+        self._bag0 = [sum(nbs[:m]) for m in range(M)]                      # each fold's first entry
+        self._slots = torch.zeros(ne, max_rows, D, device=dev)
+        self.slots = [self._slots[e:e + n] for e, n in zip(self._bag0, nbs)]
+        self.Ns = torch.ones(ne, dtype=torch.int64, device=dev)
+        self.labels = torch.zeros(ne, C, device=dev)
+        self.status = torch.zeros(M, dtype=torch.int32, device=dev)
+        self._step_status = torch.zeros(M, dtype=torch.int32, device=dev)   # this replay's planners
+        snaps = [_snapshot(o, p) for o, p in zip(optimizers, self.params)]
+
+        def warm():
+            for opt in optimizers:
+                opt.zero_grad(set_to_none=True)
+            self._step()
+        _warm_up(dev, warmup, warm)
+        for o, p, snap in zip(optimizers, self.params, snaps):
+            _restore(o, p, snap)
+            o.zero_grad(set_to_none=True)
+        self._kept = [_kept_tensors(o, p) for o, p in zip(optimizers, self.params)]
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self.loss = self._step(guard=True)
+        self.status.zero_()
+
+    def _step(self, guard=False):
+        from .sharded import milnet_params
+        self._step_status.zero_()
+        params = [t for net in self.milnets for t in milnet_params(net)]
+        classes, pred, _, _, crit = Fn.MILBagsModelsDevFn.apply(self.nbs, self._slots, self.Ns, self._step_status,
+                                                                *params)
+        n = self.Ns.clamp(0, self.max_rows)                # the live sizes (a refused fold's stay in range)
+        losses, oks = [], []
+        for m, (e, nb) in enumerate(zip(self._bag0, self.nbs)):
+            nm = n[e:e + nb]
+            first = torch.cumsum(nm, 0) - nm + e * self.max_rows          # each bag's first packed row
+            mx = classes.gather(0, crit[e:e + nb] + first[:, None])
+            lm = feed.minibatch_loss(self.criterion, pred[e:e + nb], mx, self.labels[e:e + nb])
+            ok = self._step_status[m] == 0
+            # a refused fold: NaN loss and no gradient (where's backward sends none to the unselected side)
+            losses.append(torch.where(ok, lm, torch.full_like(lm, float("nan"))))
+            oks.append(ok)
+        total = losses[0]
+        for lm in losses[1:]:
+            total = total + lm
+        total.backward()
+        if guard:
+            before = [_flat(k) for k in self._kept]
+        for opt in self.optimizers:
+            opt.step()
+        if guard:
+            for ok, kept, b in zip(oks, self._kept, before):
+                _keep_if(ok, kept, b)
+        self.status.copy_(torch.where(self.status != 0, self.status, self._step_status))
+        return torch.stack([lm.detach() for lm in losses])
+
+    def step(self) -> torch.Tensor:
+        self.graph.replay()
+        return self.loss
+

@@ -240,6 +240,44 @@ int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev,
                             const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
                             const float* d_B, const dsmil_grads_t* grads, int32_t* status, void* workspace,
                             size_t workspace_bytes, void* stream);
+/* Capture-safe forms of dsmil_forward_bags_models_train / dsmil_backward_bags_models: the fold step of a
+ * cross-validation recorded once as a CUDA graph.  The rules are those of the two families above, combined.
+ * From the dev calls: Xs_dev / Ns_dev [sum nbs] live in DEVICE memory; a call only enqueues work on `stream` (no
+ * host<->device copy, allocation or synchronisation, nothing read from Ns on the host; what the host knows of the
+ * models travels as kernel arguments); row-indexed buffers have capacity rows; d_A, d_B and every grads[m].gX must be
+ * NULL; the W1/W2 images are rebuilt on every call; a short workspace is DSMIL_ERR_WORKSPACE.
+ * From the fold calls: nbs[m] >= 1 is model m's bag count, a HOST array fixed per call (one recorded graph per set of
+ * group sizes).  Lists and buffers are model-major.  Model m's packed rows start at the fixed capacity offset
+ * max_rows * sum_{j<m} nbs[j], and inside that block its live rows are packed at its own live prefix sums: model m's
+ * block of every buffer is what the one-model dev call would be given.  classes / A / save_Q / save_H1 / d_classes
+ * have max_rows * sum nbs rows; pred, B, crit_idx are [sum nbs, ...].
+ * Shapes: dsmil_models_supported(ps, M) must hold (there is no per-model loop route: the one-model dev calls serve
+ * the other shapes one fold at a time), 1 <= nbs[m], sum nbs <= 65535 less a chunk allowance of at most 296 per model
+ * (the ragged GEMM grids number their chunks in 16 bits), 1 <= max_rows < 2^32 with the capacity tiles in an int.
+ * Anything else is DSMIL_ERR_ARG before any CUDA work, and the workspace functions return 0.
+ * Refusal is per model: a bag of model m with N outside [1, max_rows], or features NULL or not 16-byte aligned, sets
+ * status[m] (device int32 [M]) to 1 + the index within model m of the first such bag, and puts MODEL m ONLY on the
+ * stand-in batch (each of its bags one row of zeros: finite outputs, indices in range).  The other models' results
+ * are untouched.  A status word is never cleared by the library.
+ * On the same bags every output and gradient is, bit for bit, the eager fold call's, and so model m's slices are the
+ * one-model dev calls' on model m's bags: every partial-sum layout follows from model m's live sizes alone.
+ * The workspace sizes depend on (M, nbs, max_rows) only and are never below the eager fold calls' for nbs bags of
+ * max_rows rows, nor below the sum of the one-model dev calls' sizes. */
+size_t dsmil_forward_bags_models_train_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                           int64_t max_rows);
+int dsmil_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                        const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, float* classes,
+                                        float* pred, float* A, float* B, int64_t* crit_idx, float* save_Q,
+                                        float* save_H1, int32_t* status, void* workspace, size_t workspace_bytes,
+                                        void* stream);
+size_t dsmil_backward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                      int64_t max_rows);
+int dsmil_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                   const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, const float* Q,
+                                   const float* H1, const float* A, const float* B, const int64_t* crit_idx,
+                                   const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                                   const dsmil_grads_t* grads, int32_t* status, void* workspace,
+                                   size_t workspace_bytes, void* stream);
 /* Capture-safe form of dsmil_forward_bags (inference), under the rules of dsmil_forward_bags_train_dev above: the bag
  * list in device memory, classes and A sized for nb * max_rows rows with the live rows packed at the live prefix sums,
  * no host<->device copy, allocation or synchronisation, the same refusal through *status and the same stand-in batch,
