@@ -125,6 +125,22 @@ SIGNATURES = {
     "dsmil_forward_bags_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_int32, c_i64,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_generic_bags_supported": (C.c_int, [C.POINTER(DsmilParams)]),
+    "dsmil_generic_forward_bags_train_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
+    "dsmil_generic_forward_bags_train_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_int32,
+                                                       c_i64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                       C.c_size_t, C.c_void_p]),
+    "dsmil_generic_forward_bags_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
+    "dsmil_generic_forward_bags_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_int32, c_i64,
+                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_generic_backward_bags_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
+    "dsmil_generic_backward_bags_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_int32, c_i64,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.POINTER(DsmilGrads), C.c_void_p, C.c_void_p, C.c_size_t,
+                                                  C.c_void_p]),
     "dsmil_backward_bags_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
     "dsmil_backward_bags_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_int32, c_i64,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

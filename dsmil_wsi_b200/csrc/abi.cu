@@ -18,6 +18,7 @@
 #include "fwd_sm90.cuh"
 #include "fwd_batched.cuh"
 #include "bag_plan.cuh"
+#include "fwd_generic_b.cuh"
 #include "embed_kernels.cuh"
 #include "jpeg_kernels.cuh"
 
@@ -136,11 +137,6 @@ static int check_bags(const float* const* Xs, const int64_t* Ns, int nb, int64_t
   return 0;
 }
 
-static inline int attend_ctas(int64_t N) {
-  const int64_t tiles = (N + kAttendRows - 1) / kAttendRows;
-  return static_cast<int>(tiles < kSplits ? (tiles < 1 ? 1 : tiles) : kSplits);
-}
-
 static int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
@@ -257,8 +253,7 @@ static int launch_scores(const dsmil_params_t* p, const float* X, int64_t N, flo
                          unsigned long long* keys, cudaStream_t st) {
   const int C = p->C, D = p->D;
   const size_t smem = sizeof(float) * C * D;
-  const bool vec = (D % 4 == 0) && ((reinterpret_cast<uintptr_t>(X) & 15) == 0);
-  const int mode = !vec ? 0 : (D % 64 == 0 ? 2 : 1);
+  const int mode = scores_mode(X, D);
   const int grid = static_cast<int>(std::min<int64_t>(ceil_div(N, mode == 2 ? 64 : 8), kSms * 8));
   prof_begin(PROF_SCORES, st);
   if (mode == 2) {
@@ -486,6 +481,145 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
   return bags_attend_finalize(p, w, nb, Q, q_blocked, pred, A, B, crit, recs, nullptr, st, overlap);
 }
 
+// ---- batched forward on the generic shapes: identity v off the tensor-core batch, one launch per stage -----------
+// Every bag's outputs are the bits dsmil_forward gives it alone (fwd_generic_b.cuh, DESIGN §4.2h).  Phase 1 is the
+// one the single-bag forward takes on the shape: k_qmlp_sm90 where it runs (D % 128 == 0, nonlinear q, 16-byte
+// aligned bags), else k_scores at each bag's MODE and the FFMA Q-MLP.
+static bool gen_shape(const dsmil_params_t* p) { return !p->passing_v && !sm90::batched_supported(p); }
+
+struct GenWs : Phase1Ws {
+  float *Q, *H1;            // row-major [rows][128] where the caller keeps none
+  float* qmax;              // [nb][C][128]
+  int64_t* crit;            // [nb][C] where the caller wants none
+  float *recs, *rec;        // the partial records; each bag's combined one [nb]
+  BagsPlan* plan;           // dev calls: the planner's live counts and the stand-in row of a refused batch
+  float* zero_row;
+  size_t bytes;
+};
+// rows, recs: the packed rows and partial records (dev calls: their capacities).
+static GenWs carve_gen(const dsmil_params_t* p, int nb, int64_t rows, int64_t recs, bool need_Q, bool need_H1,
+                       bool dev, void* ws, size_t cap, bool* ok) {
+  Carver c(ws, cap);
+  GenWs w;
+  carve_phase1(c, p, nb, w);
+  w.Q = need_Q ? c.take<float>(rows * kQ) : nullptr;
+  w.H1 = need_H1 ? c.take<float>(rows * kQ) : nullptr;
+  w.qmax = c.take<float>(static_cast<size_t>(nb) * p->C * kQ);
+  w.crit = c.take<int64_t>(static_cast<size_t>(nb) * p->C);
+  w.recs = c.take<float>(recs * rec_floats(p->C, p->D));
+  w.rec = c.take<float>(static_cast<size_t>(nb) * rec_floats(p->C, p->D));
+  w.plan = dev ? c.take<BagsPlan>(1) : nullptr;
+  w.zero_row = dev ? c.take<float>(p->D) : nullptr;
+  w.bytes = c.off;
+  *ok = c.ok();
+  return w;
+}
+static GenWs carve_gen_eager(const dsmil_params_t* p, const int64_t* Ns, int nb, bool need_Q, bool need_H1, void* ws,
+                             size_t cap, bool* ok) {
+  int64_t rows = 0, recs = 0;
+  for (int b = 0; b < nb; ++b) {
+    rows += Ns[b];
+    recs += attend_ctas(Ns[b]);
+  }
+  return carve_gen(p, nb, rows, recs, need_Q, need_H1, false, ws, cap, ok);
+}
+static GenWs carve_gen_dev(const dsmil_params_t* p, int nb, int64_t max_rows, bool need_Q, bool need_H1, void* ws,
+                           size_t cap, bool* ok) {
+  return carve_gen(p, nb, nb * max_rows, static_cast<int64_t>(nb) * attend_ctas(max_rows), need_Q, need_H1, true, ws,
+                   cap, ok);
+}
+
+template <int CT>
+static int launch_attend_gb_j(int J, int grid, cudaStream_t st, const sm90::BagDev* bags, int nb, const int* recs_dev,
+                              int D, int C, const float* Q, const float* qmax, float* A, float* recs) {
+  switch (J) {
+    case 1: k_attend_gb<CT, 1><<<grid, 256, 0, st>>>(bags, nb, recs_dev, D, C, Q, qmax, A, recs); break;
+    case 2: k_attend_gb<CT, 2><<<grid, 256, 0, st>>>(bags, nb, recs_dev, D, C, Q, qmax, A, recs); break;
+    case 4: k_attend_gb<CT, 4><<<grid, 256, 0, st>>>(bags, nb, recs_dev, D, C, Q, qmax, A, recs); break;
+    case 8: k_attend_gb<CT, 8><<<grid, 256, 0, st>>>(bags, nb, recs_dev, D, C, Q, qmax, A, recs); break;
+    default: k_attend_gb<CT, 16><<<grid, 256, 0, st>>>(bags, nb, recs_dev, D, C, Q, qmax, A, recs); break;
+  }
+  DSMIL_LAUNCH_OK("k_attend_gb");
+  return 0;
+}
+
+// The generic forward over w.table: `tiles` and `recs` are the table's 128-row tiles and records and `rows` its packed
+// rows (dev calls: capacities, the live counts in w.plan); max_N bounds the bags' rows.  Q (and H1 for nonlinear q)
+// receive the Q-MLP's outputs row-major.
+static int gen_forward_run(const dsmil_params_t* p, const GenWs& w, int nb, int64_t rows, int tiles, int recs,
+                           int64_t max_N, float* classes, float* pred, float* A, float* B, int64_t* crit, float* Q,
+                           float* H1, cudaStream_t st) {
+  const int C = p->C, D = p->D;
+  const BagsPlan* pl = w.plan;
+  int rc;
+  DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * kMaxC * nb, st));
+  if (sm90::qmlp_supported(p)) {
+    if ((rc = sm90::launch_prep_wimg(p, w.wimg, st))) return rc;
+    if ((rc = sm90::launch_qmlp(p, w.table, nb, tiles, classes, w.keys, Q, H1, w.wimg, num_sms(), st, false,
+                                pl ? &pl->tiles : nullptr, nullptr)))
+      return rc;
+  } else {
+    const size_t smem = sizeof(float) * C * D;
+    if (smem > 48 * 1024)
+      DSMIL_CUDA_OK(cudaFuncSetAttribute(k_scores_b, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    prof_begin(PROF_SCORES, st);
+    k_scores_b<<<tiles, 256, smem, st>>>(w.table, nb, pl ? &pl->tiles : nullptr, D, p->Wi, p->bi, C, classes, w.keys);
+    prof_end(PROF_SCORES, st);
+    DSMIL_LAUNCH_OK("k_scores_b");
+    prof_begin(PROF_QMLP, st);
+    const dim3 g1(2 * tiles, ceil_div(kQ, LBN));
+    if (p->nonlinear) k_linear_b<ACT_RELU><<<g1, 256, 0, st>>>(w.table, nb, pl ? &pl->tiles : nullptr, D, p->W1, p->b1, kQ, H1);
+    else k_linear_b<ACT_NONE><<<g1, 256, 0, st>>>(w.table, nb, pl ? &pl->tiles : nullptr, D, p->W1, p->b1, kQ, Q);
+    DSMIL_LAUNCH_OK("k_linear_b");
+    if (p->nonlinear &&
+        (rc = launch_linear<ACT_TANH, false>(H1, rows, kQ, p->W2, p->b2, kQ, Q, nullptr, 0, st, pl ? &pl->total : nullptr)))
+      return rc;
+    prof_end(PROF_QMLP, st);
+  }
+  k_crit_qmax_b<<<dim3(C, nb), kQ, 0, st>>>(w.table, w.keys, Q, C, w.qmax, crit);
+  DSMIL_LAUNCH_OK("k_crit_qmax_b");
+  int j = ceil_div(D, 256), J = 1;
+  while (J < j) J <<= 1;
+  const int* recs_dev = pl ? &pl->recs : nullptr;
+  prof_begin(PROF_ATTEND, st);
+  if (C == 1) rc = launch_attend_gb_j<1>(J, recs, st, w.table, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
+  else if (C == 2) rc = launch_attend_gb_j<2>(J, recs, st, w.table, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
+  else if (C <= 4) rc = launch_attend_gb_j<4>(J, recs, st, w.table, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
+  else rc = launch_attend_gb_j<8>(J, recs, st, w.table, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
+  prof_end(PROF_ATTEND, st);
+  if (rc) return rc;
+  k_combine_rec_b<<<dim3(C, ceil_div(D, 256), nb), 256, 0, st>>>(w.table, C, D, w.recs, w.rec);
+  DSMIL_LAUNCH_OK("k_combine_rec_b");
+  const int fgrid = static_cast<int>(std::min<int64_t>(std::max<int64_t>(ceil_div(max_N * C, 256), 1), kSplits));
+  prof_begin(PROF_FINAL, st);
+  k_finalize_gb<<<dim3(fgrid, nb), 256, 0, st>>>(w.table, w.rec, C, D, p->Wf, p->bf, A, B, pred);
+  prof_end(PROF_FINAL, st);
+  DSMIL_LAUNCH_OK("k_finalize_gb");
+  return 0;
+}
+
+// The eager generic forward: the table built on the host (each bag's MODE from its own alignment) and uploaded.
+// save_Q / save_H1: the training form's row-major Q and H1 (NULL: inference, into the workspace).
+static int forward_bags_gen(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb, float* classes,
+                            float* pred, float* A, float* B, int64_t* crit, float* save_Q, float* save_H1, void* ws,
+                            size_t ws_bytes, cudaStream_t st) {
+  bool ok;
+  GenWs w = carve_gen_eager(p, Ns, nb, !save_Q, p->nonlinear && !save_H1, ws, ws_bytes, &ok);
+  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+  if (rc) return rc;
+  std::vector<sm90::BagDev> tbl(nb);
+  long long row = 0;
+  int tile = 0, rec = 0;
+  int64_t mx = 1;
+  for (int b = 0; b < nb; ++b) {
+    tbl[b] = gen_bag_entry(Xs[b], Ns[b], p->D, row, tile, rec);
+    mx = std::max<int64_t>(mx, Ns[b]);
+  }
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
+  return gen_forward_run(p, w, nb, row, tile, rec, mx, classes, pred, A, B, crit ? crit : w.crit,
+                         save_Q ? save_Q : w.Q, p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr, st);
+}
+
 }  // namespace dsmil
 
 using namespace dsmil;
@@ -624,6 +758,7 @@ size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t
   for (int b = 0; b < nb; ++b) mx = std::max<int64_t>(mx, Ns[b]);
   size_t bytes = carve_fwd(p, mx, nullptr, 0, &ok).bytes;
   if (sm90::batched_supported(p)) bytes = std::max(bytes, carve_bags(p, Ns, nb, true, false, nullptr, 0, &ok).bytes);
+  if (gen_shape(p)) bytes = std::max(bytes, carve_gen_eager(p, Ns, nb, true, p->nonlinear, nullptr, 0, &ok).bytes);
   return bytes;
 }
 
@@ -643,7 +778,10 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
   if (sm90::batched_supported(p) && aligned)
     return forward_bags_impl(p, Xs, Ns, nb, nullptr, classes, pred, A, B, crit_idx, nullptr, nullptr, workspace,
                              workspace_bytes, st);
-  // shapes the tensor-core kernels do not take: same packed outputs, one bag at a time
+  if (gen_shape(p) && (aligned || !sm90::qmlp_supported(p)))
+    return forward_bags_gen(p, Xs, Ns, nb, classes, pred, A, B, crit_idx, nullptr, nullptr, workspace, workspace_bytes,
+                            st);
+  // passing_v, and bags the batched routes do not take: same packed outputs, one bag at a time
   int64_t row = 0;
   for (int b = 0; b < nb; ++b) {
     rc = forward_impl(p, Xs[b], nullptr, nullptr, Ns[b], classes + row * p->C, pred + static_cast<size_t>(b) * p->C,
@@ -1458,7 +1596,10 @@ int dsmil_forward_bags_train(const dsmil_params_t* p, const float* const* Xs, co
   if (sm90::batched_supported(p) && aligned)
     return forward_bags_impl(p, Xs, Ns, nb, nullptr, classes, pred, A, B, crit_idx, save_Q, save_H1, workspace,
                              workspace_bytes, st);
-  // shapes or bags off the tensor-core batch: one bag at a time into the same packed buffers
+  if (gen_shape(p) && (aligned || !sm90::qmlp_supported(p)))
+    return forward_bags_gen(p, Xs, Ns, nb, classes, pred, A, B, crit_idx, save_Q, save_H1, workspace, workspace_bytes,
+                            st);
+  // bags the batched routes do not take: one bag at a time into the same packed buffers
   int64_t row = 0;
   for (int b = 0; b < nb; ++b) {
     rc = forward_impl(p, Xs[b], nullptr, nullptr, Ns[b], classes + row * p->C, pred + static_cast<size_t>(b) * p->C,
@@ -2157,6 +2298,128 @@ int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev,
   k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, w.zero_row, w.table, w.chi, w.ch1, w.plan,
                                 status, nullptr, nullptr);
   DSMIL_LAUNCH_OK("k_plan_bags");
+  return backward_bags_run(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, A, B, crit_idx,
+                           d_classes, d_pred, nullptr, nullptr, grads, w, st);
+}
+
+// ---- capture-safe calls on the generic shapes: the dev calls' contract, planned by k_plan_bags_gen ----------------
+int dsmil_generic_bags_supported(const dsmil_params_t* p) {
+  return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && gen_shape(p)) ? 1 : 0;
+}
+
+}  // extern "C"
+namespace dsmil {
+// check_bags_dev of the generic calls: their shapes, and a capacity whose 128-row tiles k_linear_b's grid can number
+// twice over in an int.
+static int check_generic_dev(const dsmil_params_t* p, bool need_scores, const float* const* Xs, const int64_t* Ns,
+                             int nb, int64_t max_rows, const int32_t* status) {
+  int rc = check_params(p, need_scores);
+  if (rc) return rc;
+  DSMIL_REQUIRE(dsmil_generic_bags_supported(p),
+                "shape not on the generic batched route, i.e. identity v off dsmil_shard_bags_supported (D=%d, C=%d, "
+                "nonlinear=%d, passing_v=%d)", p->D, p->C, p->nonlinear, p->passing_v);
+  DSMIL_REQUIRE(Xs && Ns && status, "NULL bag list or status");
+  DSMIL_REQUIRE(nb >= 1 && nb <= 65535, "nb=%d outside [1, 65535]", nb);
+  DSMIL_REQUIRE(max_rows >= 1 && max_rows < 0xffffffffll &&
+                2 * static_cast<int64_t>(nb) * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) <= INT_MAX,
+                "max_rows=%lld out of range for nb=%d", (long long)max_rows, nb);
+  return 0;
+}
+static bool generic_dev_sizes(const dsmil_params_t* p, int nb, int64_t max_rows) {
+  return dsmil_generic_bags_supported(p) && nb >= 1 && nb <= 65535 && max_rows >= 1 && max_rows < 0xffffffffll;
+}
+
+// The generic shapes' dev forward: k_plan_bags_gen writes the table and the live counts, then the generic forward runs
+// on the capacity grids.  save_Q == NULL: inference (Q and H1 in the workspace).
+static int forward_bags_gen_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev, int nb,
+                                int64_t max_rows, float* classes, float* pred, float* A, float* B, int64_t* crit,
+                                float* save_Q, float* save_H1, int32_t* status, void* ws, size_t ws_bytes,
+                                cudaStream_t st) {
+  bool ok;
+  GenWs w = carve_gen_dev(p, nb, max_rows, !save_Q, p->nonlinear && !save_H1, ws, ws_bytes, &ok);
+  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+  if (rc) return rc;
+  k_plan_bags_gen<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, w.zero_row, w.table, nullptr, nullptr,
+                                    w.plan, status);
+  DSMIL_LAUNCH_OK("k_plan_bags_gen");
+  return gen_forward_run(p, w, nb, nb * max_rows, nb * tiles_for_bag(max_rows), nb * attend_ctas(max_rows), max_rows,
+                         classes, pred, A, B, crit ? crit : w.crit, save_Q ? save_Q : w.Q,
+                         p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr, st);
+}
+}  // namespace dsmil
+extern "C" {
+
+size_t dsmil_generic_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  if (!generic_dev_sizes(p, nb, max_rows)) return 0;
+  bool ok;
+  const size_t dev = carve_gen_dev(p, nb, max_rows, false, false, nullptr, 0, &ok).bytes;
+  // never below the eager call's size for the same capacity: one buffer serves both forms
+  const std::vector<int64_t> Ns(nb, max_rows);
+  return std::max(dev, dsmil_forward_bags_train_workspace_bytes(p, Ns.data(), nb));
+}
+
+int dsmil_generic_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                         int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
+                                         int64_t* crit_idx, float* save_Q, float* save_H1, int32_t* status,
+                                         void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_generic_dev(p, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && (!p->nonlinear || save_H1), "NULL output pointer");
+  const size_t need = dsmil_generic_forward_bags_train_dev_workspace_bytes(p, nb, max_rows);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  return forward_bags_gen_dev(p, Xs_dev, Ns_dev, nb, max_rows, classes, pred, A, B, crit_idx, save_Q, save_H1, status,
+                              workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+size_t dsmil_generic_forward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  if (!generic_dev_sizes(p, nb, max_rows)) return 0;
+  bool ok;
+  const size_t dev = carve_gen_dev(p, nb, max_rows, true, p->nonlinear, nullptr, 0, &ok).bytes;
+  const std::vector<int64_t> Ns(nb, max_rows);
+  return std::max(dev, dsmil_forward_bags_workspace_bytes(p, Ns.data(), nb));
+}
+
+int dsmil_generic_forward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                   int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
+                                   int64_t* crit_idx, int32_t* status, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+  int rc = check_generic_dev(p, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(classes && pred && A && B, "NULL output pointer");
+  const size_t need = dsmil_generic_forward_bags_dev_workspace_bytes(p, nb, max_rows);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  return forward_bags_gen_dev(p, Xs_dev, Ns_dev, nb, max_rows, classes, pred, A, B, crit_idx, nullptr, nullptr, status,
+                              workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+size_t dsmil_generic_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  if (!generic_dev_sizes(p, nb, max_rows)) return 0;
+  bool ok;
+  const size_t dev = carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
+  const std::vector<int64_t> Ns(nb, max_rows);
+  return std::max(dev, dsmil_backward_bags_workspace_bytes(p, Ns.data(), nb, 0));
+}
+
+int dsmil_generic_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                    int32_t nb, int64_t max_rows, const float* Q, const float* H1, const float* A,
+                                    const float* B, const int64_t* crit_idx, const float* d_classes,
+                                    const float* d_pred, const float* d_A, const float* d_B, const dsmil_grads_t* grads,
+                                    int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_generic_dev(p, false, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(Q && (!p->nonlinear || H1) && A && B && crit_idx && grads, "NULL pointer");
+  DSMIL_REQUIRE(!d_A && !d_B && !grads->gX,
+                "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
+  const size_t need = dsmil_generic_backward_bags_dev_workspace_bytes(p, nb, max_rows);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  bool ok;
+  BwdBagsWs w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
+  // the alignment rule (gen_bag_aligned) keeps each form the eager call would choose: gWi streams (tn_use_gemv) only
+  // where D % 4 == 0, and there the bags are 16-byte aligned
+  k_plan_bags_gen<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, w.zero_row, w.table, w.chi, w.ch1,
+                                    w.plan, status);
+  DSMIL_LAUNCH_OK("k_plan_bags_gen");
   return backward_bags_run(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, A, B, crit_idx,
                            d_classes, d_pred, nullptr, nullptr, grads, w, st);
 }

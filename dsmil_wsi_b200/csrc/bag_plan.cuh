@@ -37,6 +37,30 @@ __host__ __device__ inline sm90::BagDev bag_entry(const float* X, int64_t N, lon
   return e;
 }
 
+// The generic forward (fwd_generic_b.cuh, and the per-bag forward it matches): attend CTAs (== partial records) of a
+// bag of N rows, one per kAttendRows-row tile up to kSplits.
+__host__ __device__ inline int attend_ctas(int64_t N) {
+  const int64_t tiles = (N + kAttendRows - 1) / kAttendRows;
+  return static_cast<int>(tiles < kSplits ? (tiles < 1 ? 1 : tiles) : kSplits);
+}
+// The next bag of a generic-forward table: bag_entry's row and 128-row tile numbering, attend_ctas(N) records, and
+// the bag's k_scores MODE in pad_.
+__host__ __device__ inline sm90::BagDev gen_bag_entry(const float* X, int64_t N, int D, long long& row, int& tile,
+                                                      int& rec) {
+  const int nrec = attend_ctas(N);
+  const sm90::BagDev e{X, N, row, tile, rec, nrec, scores_mode(X, D)};
+  row += N;
+  tile += tiles_for_bag(N);
+  rec += nrec;
+  return e;
+}
+// The alignment a dev call asks of a bag's features on the generic shapes: 16 bytes when D % 4 == 0 (so that the
+// MODE of k_scores and the form of the gWi reduction follow from D alone, as the eager calls choose them for aligned
+// bags), 4 bytes otherwise (rows of an odd D are never 16-byte aligned; every form there reads scalars).
+__host__ __device__ inline bool gen_bag_aligned(const float* X, int D) {
+  return (reinterpret_cast<uintptr_t>(X) & (D % 4 == 0 ? 15 : 3)) == 0;
+}
+
 // CTAs per bag of the batched backward's per-row kernels, from the batch size and its largest bag.  It fixes how the
 // per-bag sums t_b and dq_max_b are split, so it follows the shapes only.
 __host__ __device__ inline int bwd_bags_ctas(int nb, int64_t max_N) {
@@ -124,10 +148,10 @@ struct BagsPlan {
 
 // The planner of a dev call: one thread reads the bag list (Xs, Ns: device memory) and writes the bag table, the live
 // counts and, when chi / ch1 are non-NULL, the backward's chunk tables.  A bag with N outside [1, max_rows] or
-// features that are NULL or not 16-byte aligned sets *status to 1 + its index (the first such bag; a set status is
-// never cleared here), and the call then runs on a stand-in batch instead: every bag becomes one row of zeros
-// (zero_row, D floats of the workspace).  Every output of a refused call is then finite and every index in range
-// (crit_idx 0, pred = bf, B = 0), and nothing reads the caller's bag list.  A row-sharded batch also passes each bag's
+// features that are NULL or not 16-byte aligned (k_plan_bags_gen: not gen_bag_aligned) sets *status to 1 + its index
+// (the first such bag; a set status is never cleared here), and the call then runs on a stand-in batch instead: every
+// bag becomes one row of zeros (zero_row, D floats of the workspace).  Every output of a refused call is then finite
+// and every index in range (crit_idx 0, pred = bf, B = 0), and nothing reads the caller's bag list.  A row-sharded batch also passes each bag's
 // first global row (offs_in, device memory): the planner copies it to offs_out, a negative offset is refused like a
 // bad bag, and a refused batch's offsets are 0.
 // The walk is one thread's; the warp first stages the list of the first kPlanStaged bags into shared memory with its
@@ -181,6 +205,62 @@ k_plan_bags(const float* const* __restrict__ Xs, const int64_t* __restrict__ Ns,
   } else {
     if (chi) {
       const bool gemv = tn_use_gemv(C, D);   // the bags are 16-byte aligned
+      pl.nci = rag_chunks(Xs, Ns, nb, D, rag_rows_per_chunk(C, D, row, gemv), chi);
+    }
+    if (ch1) pl.nc1 = rag_chunks(Xs, Ns, nb, D, rag_rows_per_chunk(kQ, D, row, false), ch1);
+  }
+  pl.cs = colsum_split(row);
+  pl.tn2 = gemm_tn_split(kQ, kQ, row);
+  *plan = pl;
+}
+
+// The planner of the generic shapes' dev calls: k_plan_bags with the alignment rule of gen_bag_aligned and a table of
+// gen_bag_entry, no row offsets.  A kernel of its own, as the k_plan_bags SASS stays what it was.
+__global__ void __launch_bounds__(32)
+k_plan_bags_gen(const float* const* __restrict__ Xs, const int64_t* __restrict__ Ns, int nb, long long max_rows,
+                int C, int D, float* __restrict__ zero_row, sm90::BagDev* __restrict__ table,
+                TnChunk* __restrict__ chi, TnChunk* __restrict__ ch1, BagsPlan* __restrict__ plan,
+                int* __restrict__ status) {
+  __shared__ const float* sX[kPlanStaged];
+  __shared__ int64_t sN[kPlanStaged];
+  if (blockIdx.x != 0) return;
+  for (int b = threadIdx.x; b < nb && b < kPlanStaged; b += 32) { sX[b] = Xs[b]; sN[b] = Ns[b]; }
+  __syncwarp();
+  if (threadIdx.x != 0) return;
+  auto X_of = [&](int b) { return b < kPlanStaged ? sX[b] : Xs[b]; };
+  auto N_of = [&](int b) { return b < kPlanStaged ? sN[b] : Ns[b]; };
+  int bad = 0;
+  long long mx = 0;
+  for (int b = 0; b < nb && !bad; ++b) {
+    const int64_t N = N_of(b);
+    const float* X = X_of(b);
+    if (N < 1 || N > max_rows || X == nullptr || !gen_bag_aligned(X, D)) bad = b + 1;
+    mx = N > mx ? N : mx;
+  }
+  if (bad) {
+    *status = bad;
+    for (int i = 0; i < D; ++i) zero_row[i] = 0.f;
+    mx = 1;
+  }
+  BagsPlan pl{};
+  long long row = 0;
+  int tile = 0, rec = 0;
+  for (int b = 0; b < nb; ++b)
+    table[b] = bad ? gen_bag_entry(zero_row, 1, D, row, tile, rec) : gen_bag_entry(X_of(b), N_of(b), D, row, tile, rec);
+  pl.total = row;
+  pl.tiles = tile;
+  pl.recs = rec;
+  pl.G = bwd_bags_ctas(nb, mx);
+  if (bad) {                     // one one-row chunk per bag, as rag_chunks gives for one-row bags
+    for (int b = 0; b < nb && (chi || ch1); ++b) {
+      if (chi) chi[b] = TnChunk{zero_row, b, 1};
+      if (ch1) ch1[b] = TnChunk{zero_row, b, 1};
+    }
+    pl.nci = chi ? nb : 0;
+    pl.nc1 = ch1 ? nb : 0;
+  } else {
+    if (chi) {
+      const bool gemv = tn_use_gemv(C, D);   // true only where D % 4 == 0, and such bags are 16-byte aligned
       pl.nci = rag_chunks(Xs, Ns, nb, D, rag_rows_per_chunk(C, D, row, gemv), chi);
     }
     if (ch1) pl.nc1 = rag_chunks(Xs, Ns, nb, D, rag_rows_per_chunk(kQ, D, row, false), ch1);

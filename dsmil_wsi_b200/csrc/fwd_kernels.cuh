@@ -17,6 +17,12 @@ namespace dsmil {
 // per row with exactly the summation order of the tensor-core kernel's fused scores
 // (fwd_sm90.cuh: lane `seg` takes float4 #seg, #seg+4, ... of the row, then xor-shuffles 2,1), so
 // FCLayer/IClassifier scores are bit-identical whichever kernel produced them.
+// The MODE k_scores reads a bag with: float4 loads only from a 16-byte aligned bag of D % 4 == 0.
+__host__ __device__ inline int scores_mode(const float* X, int D) {
+  const bool vec = (D % 4 == 0) && ((reinterpret_cast<uintptr_t>(X) & 15) == 0);
+  return !vec ? 0 : (D % 64 == 0 ? 2 : 1);
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(256)
 k_scores(const float* __restrict__ X, int64_t N, int D, const float* __restrict__ Wi,
@@ -303,8 +309,8 @@ k_attend(const float* __restrict__ V, int Dv, const float* __restrict__ Q, int64
 // Combine P records (per-CTA partials, or per-rank records) into one, fixed order.
 // grid = (C, ceil(Dv/256)); P <= kMaxRecs.
 constexpr int kMaxRecs = 1024;
-__global__ void __launch_bounds__(256)
-k_combine_rec(const float* __restrict__ recs, int P, int C, int Dv, float* __restrict__ out) {
+__device__ __forceinline__ void combine_recs(const float* __restrict__ recs, int P, int C, int Dv,
+                                             float* __restrict__ out) {
   __shared__ float w[kMaxRecs];
   __shared__ float sM;
   const int k = blockIdx.x;
@@ -335,6 +341,10 @@ k_combine_rec(const float* __restrict__ recs, int P, int C, int Dv, float* __res
     for (int p = 0; p < P; ++p) b = fmaf(recs[p * stride + 2 * C + static_cast<size_t>(k) * Dv + d], w[p], b);
     out[2 * C + static_cast<size_t>(k) * Dv + d] = b;
   }
+}
+__global__ void __launch_bounds__(256)
+k_combine_rec(const float* __restrict__ recs, int P, int C, int Dv, float* __restrict__ out) {
+  combine_recs(recs, P, C, Dv, out);
 }
 
 // A[n,k] = exp(L - M_k) / S_k in place; block 0 also emits B = Bp / S and the bag logits.

@@ -607,10 +607,6 @@ inline int launch_qmlp(const dsmil_params_t* p, const BagDev* bags_dev, int nb, 
                        unsigned long long* keys, float* Q, float* H1, const uint8_t* wimg, int max_ctas, cudaStream_t st,
                        bool q_blocked, const int* ntiles_dev = nullptr, unsigned int* done = nullptr) {
   const int D = p->D, C = p->C;
-  if (ntiles_dev != nullptr && C > 4) {
-    set_error("launch_qmlp: a device tile count needs C <= 4");
-    return DSMIL_ERR_ARG;
-  }
   const uint8_t* w2img = wimg + static_cast<size_t>(D / kChunkK) * kChunkBytes;
   QmlpArgs a{bags_dev, nb, ntiles, D, C, p->Wi, p->bi, p->b1, p->b2, wimg, w2img, classes, keys, Q, H1, q_blocked,
              ntiles_dev, done};
@@ -626,15 +622,17 @@ inline int launch_qmlp(const dsmil_params_t* p, const BagDev* bags_dev, int nb, 
     DSMIL_LAUNCH_OK("k_qmlp_sm90");
     return 0;
   };
-  if (ntiles_dev != nullptr) {   // the dev calls' shapes: C <= 4
+  if (ntiles_dev != nullptr) {   // the dev calls' shapes (C > 4: the generic batched route's)
     if (D == 512) {
       if (C == 1) return go(k_qmlp_sm90<1, 512, true>);
       if (C == 2) return go(k_qmlp_sm90<2, 512, true>);
-      return go(k_qmlp_sm90<4, 512, true>);
+      if (C <= 4) return go(k_qmlp_sm90<4, 512, true>);
+      return go(k_qmlp_sm90<8, 512, true>);
     }
     if (C == 1) return go(k_qmlp_sm90<1, 0, true>);
     if (C == 2) return go(k_qmlp_sm90<2, 0, true>);
-    return go(k_qmlp_sm90<4, 0, true>);
+    if (C <= 4) return go(k_qmlp_sm90<4, 0, true>);
+    return go(k_qmlp_sm90<8, 0, true>);
   }
   if (D == 512) {
     if (C == 1) return go(k_qmlp_sm90<1, 512>);

@@ -101,7 +101,8 @@ class DeviceBagStore:
 
 def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_patch: float = 0.0,
                 order: Optional[Sequence[int]] = None, generator: Optional[torch.Generator] = None,
-                bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None) -> float:
+                bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None,
+                generic: bool = False) -> float:
     """One epoch of train_tcga.train() (train_tcga.py:55-76) over device-resident bags; one host sync per epoch.
 
     bags_per_step = 1: the reference's loop, one forward, backward and optimizer step per bag.  k > 1: minibatches of
@@ -117,13 +118,14 @@ def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_pat
     its graphs afresh (one warm-up step, one capture, new [k, max_rows, D] slots and a graph memory pool per group size,
     freed when the call returns), so a graph holds the optimizer's hyperparameters of its call, e.g. a learning rate
     that a scheduler changes between epochs.  Needs the batched tensor-core shapes and a capture-safe optimizer
-    (SGD, or Adam / AdamW with capturable=True)."""
+    (SGD, or Adam / AdamW with capturable=True); generic=True also takes the other identity-v shapes (e.g. the
+    classic-MIL D = 166 / 230, linear q), over the generic batched route, with the bits of the k-bag step."""
     milnet.train()
     total = torch.zeros((), device=store.device)
     order = list(order) if order is not None else torch.randperm(len(store)).tolist()
     if graph:
         return _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator,
-                                  max(1, bags_per_step), max_rows)
+                                  max(1, bags_per_step), max_rows, generic)
     if bags_per_step > 1:
         for s in range(0, len(order), bags_per_step):
             group = order[s:s + bags_per_step]
@@ -241,9 +243,9 @@ def minibatch_loss(criterion, bag_prediction, max_prediction, labels):
     return 0.5 * criterion(bag_prediction, labels) + 0.5 * criterion(max_prediction, labels)
 
 
-def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator, k, max_rows):
+def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator, k, max_rows, generic):
     from .train_graph import TrainStepGraph, step_shape
-    step_shape(milnet)                                         # a shape off the batched path raises here
+    step_shape(milnet, generic)                                # a shape off the batched routes raises here
     p = 1 - dropout_patch
     keep = [int(int(store.bags[i][0].shape[0]) * p) for i in order]   # dropout_patches' row counts
     cap = int(max_rows) if max_rows is not None else max([int(f.shape[0]) for f, _ in store.bags], default=1)
@@ -258,7 +260,7 @@ def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order
         group = order[s:s + k]
         g = graphs.get(len(group))
         if g is None:                                          # the first full group, and a short last one
-            g = graphs[len(group)] = TrainStepGraph(milnet, criterion, optimizer, len(group), cap)
+            g = graphs[len(group)] = TrainStepGraph(milnet, criterion, optimizer, len(group), cap, generic=generic)
         for b, i in enumerate(group):
             dropout_patches(store.bags[i][0], p, generator, out=g.slots[b])
             g.Ns[b].fill_(keep[s + b])
@@ -331,7 +333,7 @@ def _group_predictions(outs):
 
 def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, bags_per_launch: int = 16,
                dropout_patch: float = 0.0, generator: Optional[torch.Generator] = None, graph: bool = False,
-               max_rows: Optional[int] = None):
+               max_rows: Optional[int] = None, generic: bool = False):
     """The measuring half of train_tcga.test() (train_tcga.py:85-107): mean loss, labels [n_bags, C] and
     sigmoid predictions [n_bags, C] (`average=True`: sigmoid(max) + sigmoid(bag), as `args.average`).  The ROC /
     threshold logic that follows in the reference (:108-132) is the caller's and works on these arrays.
@@ -349,14 +351,14 @@ def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, 
     bag of the store); a bag over it raises ValueError before any launch.  The graphs stay cached with the model (held
     weakly) and later calls with the same group sizes, capacity, `average` and criterion object replay them: the first
     call pays the recording, and a model whose parameter tensors were replaced gets new graphs.  Needs the batched
-    tensor-core shapes."""
+    tensor-core shapes; generic=True also takes the other identity-v shapes, over the generic batched route."""
     milnet.eval()
     n = len(store)
     if n == 0:
         raise ValueError("eval_epoch over an empty store")
     if graph:
         return _eval_epoch_graph(milnet, store, criterion, average, max(1, bags_per_launch), dropout_patch, generator,
-                                 max_rows)
+                                 max_rows, generic)
     losses, labels, preds = [], [], []
     batched = hasattr(milnet, "forward_bags") and bags_per_launch > 1
     with torch.no_grad():
@@ -421,10 +423,10 @@ def eval_epoch_models(milnets, store: DeviceBagStore, criterion, average: bool =
 _EVAL_GRAPHS = weakref.WeakKeyDictionary()
 
 
-def _eval_epoch_graph(milnet, store, criterion, average, k, dropout_patch, generator, max_rows):
+def _eval_epoch_graph(milnet, store, criterion, average, k, dropout_patch, generator, max_rows, generic):
     from .infer_graph import EvalBagsGraph
     from .train_graph import step_shape
-    step_shape(milnet)                                         # a shape off the batched path raises here
+    step_shape(milnet, generic)                                # a shape off the batched routes raises here
     p = 1 - dropout_patch
     keep = [int(int(f.shape[0]) * p) if dropout_patch > 0 else int(f.shape[0]) for f, _ in store.bags]
     cap = int(max_rows) if max_rows is not None else max(int(f.shape[0]) for f, _ in store.bags)
@@ -446,7 +448,7 @@ def _eval_epoch_graph(milnet, store, criterion, average, k, dropout_patch, gener
             key = (len(group), cap, bool(average))
             g = cached.get(key)
             if g is None or g.criterion is not criterion or not g.current():
-                g = cached[key] = EvalBagsGraph(milnet, criterion, len(group), cap, average)
+                g = cached[key] = EvalBagsGraph(milnet, criterion, len(group), cap, average, generic=generic)
             graphs[len(group)] = g
         xs = [dropout_patches(f, p, generator) if dropout_patch > 0 else f for f, _ in group]
         g.labels.copy_(labels[s:s + len(group)])
@@ -501,13 +503,19 @@ def compute_pos_weight(bags: Sequence[Tuple[int, object]]) -> float:
 
 
 def mil_epoch_train(milnet, store: DeviceBagStore, criterion, optimizer, order: Optional[Sequence[int]] = None,
-                    bags_per_step: int = 1) -> float:
+                    bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None) -> float:
     """train_mil.epoch_train (train_mil.py:42-59): per bag, shuffle the instances, forward, 0.5/0.5 loss, step
-    (bags_per_step > 1: one step per group of bags, as train_epoch)."""
-    return train_epoch(milnet, store, criterion, optimizer, dropout_patch=0.0, order=order, bags_per_step=bags_per_step)
+    (bags_per_step > 1: one step per group of bags, as train_epoch).  graph, max_rows: as train_epoch's, on the generic
+    batched route too (the classic-MIL shapes are off the tensor-core batch): bags of a few dozen rows cost little on
+    the device, so the replayed step saves most of an epoch's host work."""
+    return train_epoch(milnet, store, criterion, optimizer, dropout_patch=0.0, order=order, bags_per_step=bags_per_step,
+                       graph=graph, max_rows=max_rows, generic=True)
 
 
-def mil_epoch_test(milnet, store: DeviceBagStore, criterion, bags_per_launch: int = 16):
-    """train_mil.epoch_test (train_mil.py:61-80): (mean loss, bag labels, sigmoid bag predictions)."""
-    loss, labels, preds = eval_epoch(milnet, store, criterion, average=False, bags_per_launch=bags_per_launch)
+def mil_epoch_test(milnet, store: DeviceBagStore, criterion, bags_per_launch: int = 16, graph: bool = False,
+                   max_rows: Optional[int] = None):
+    """train_mil.epoch_test (train_mil.py:61-80): (mean loss, bag labels, sigmoid bag predictions).  graph, max_rows:
+    as eval_epoch's, on the generic batched route too."""
+    loss, labels, preds = eval_epoch(milnet, store, criterion, average=False, bags_per_launch=bags_per_launch,
+                                     graph=graph, max_rows=max_rows, generic=True)
     return loss, [int(l[0]) for l in labels], [p.squeeze() for p in preds]

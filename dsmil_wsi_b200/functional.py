@@ -322,22 +322,31 @@ class MILBagsFn(torch.autograd.Function):
         return (None, *gxs, *[out[n] for n in names])
 
 
+def _dev_prefix(lib, P, what):
+    """The name prefix of the capture-safe calls that take P's shape: the tensor-core ones, or their generic forms."""
+    if lib.dsmil_shard_bags_supported(P.ref):
+        return "dsmil_"
+    if lib.dsmil_generic_bags_supported(P.ref):
+        return "dsmil_generic_"
+    raise ValueError(f"{what} takes identity v only; D={P.D}, C={P.C}, nonlinear={P.nonlinear}, "
+                     f"passing_v={P.passing_v} is on no batched route")
+
+
 class MILBagsDevFn(torch.autograd.Function):
     """MILBagsFn over the capture-safe entry points (dsmil_forward_bags_train_dev / dsmil_backward_bags_dev): the bag
     list lives on the device, so one recorded call serves every batch of nb bags of 1..max_rows rows.
 
     args: slots [nb, max_rows, D] (bag b is slots[b, :Ns[b]]), Ns [nb] int64 and status [1] int32 on the device, then
     the ten parameter tensors.  The packed per-row outputs (classes, A) have nb * max_rows rows; the live ones are
-    packed at the prefix sums of Ns, as MILBagsFn packs them.  Parameter gradients only (no gradient to the slots)."""
+    packed at the prefix sums of Ns, as MILBagsFn packs them.  Parameter gradients only (no gradient to the slots).
+    The tensor-core shapes call the dev entry points; the other identity-v shapes their dsmil_generic_* forms."""
 
     @staticmethod
     def forward(ctx, slots, Ns, status, *params):
         lib = _lib.load()
         ctx.set_materialize_grads(False)
         P = ParamPack(*params)
-        if not lib.dsmil_shard_bags_supported(P.ref):
-            raise ValueError(f"graph-captured training runs on the batched tensor-core path only; D={P.D}, C={P.C}, "
-                             f"nonlinear={P.nonlinear}, passing_v={P.passing_v} is not on it")
+        pre = _dev_prefix(lib, P, "graph-captured training")
         if slots.dim() != 3 or slots.shape[2] != P.D or slots.dtype != torch.float32 or not slots.is_contiguous():
             raise ValueError(f"slots must be contiguous float32 [nb, max_rows, {P.D}], got {tuple(slots.shape)}")
         nb, max_rows = int(slots.shape[0]), int(slots.shape[1])
@@ -350,13 +359,14 @@ class MILBagsDevFn(torch.autograd.Function):
             crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
             sQ, sH = new(rows, Q_DIM), new(rows, Q_DIM)
             xs = slots.data_ptr() + 4 * max_rows * P.D * torch.arange(nb, dtype=torch.int64, device=dev)
-            ws = _workspace(lib.dsmil_forward_bags_train_dev_workspace_bytes(P.ref, nb, max_rows), dev)
-            rc = lib.dsmil_forward_bags_train_dev(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred),
+            ws = _workspace(getattr(lib, pre + "forward_bags_train_dev_workspace_bytes")(P.ref, nb, max_rows), dev)
+            call = getattr(lib, pre + "forward_bags_train_dev")
+            rc = call(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred),
                                                   _ptr(A), _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(status),
                                                   _ptr(ws), ws.numel(), _stream())
-            _lib.check(rc, "dsmil_forward_bags_train_dev")
+            _lib.check(rc, pre + "forward_bags_train_dev")
         ctx.save_for_backward(xs, Ns, status, sQ, sH, A, B, crit, *P.tensors)
-        ctx.shape = (nb, max_rows)
+        ctx.shape, ctx.pre = (nb, max_rows), pre
         ctx.mark_non_differentiable(crit)
         return classes, pred, A, B, crit
 
@@ -376,11 +386,12 @@ class MILBagsDevFn(torch.autograd.Function):
                    for nm, t, need in zip(names, P.tensors, ctx.needs_input_grad[3:])}
             G = _lib.DsmilGrads(*[_ptr(out[n]) for n in names], None)
             dc, dp = _f32c(g_classes), _f32c(g_pred)
-            ws = _workspace(lib.dsmil_backward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
-            rc = lib.dsmil_backward_bags_dev(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(sQ), _ptr(sH), _ptr(A),
+            ws = _workspace(getattr(lib, ctx.pre + "backward_bags_dev_workspace_bytes")(P.ref, nb, max_rows), dev)
+            call = getattr(lib, ctx.pre + "backward_bags_dev")
+            rc = call(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(sQ), _ptr(sH), _ptr(A),
                                              _ptr(B), _ptr(crit), _ptr(dc), _ptr(dp), None, None, C.byref(G),
                                              _ptr(status), _ptr(ws), ws.numel(), _stream())
-            _lib.check(rc, "dsmil_backward_bags_dev")
+            _lib.check(rc, ctx.pre + "backward_bags_dev")
         return (None, None, None, *[out[n] for n in names])
 
 
@@ -407,22 +418,22 @@ def mil_forward_bags_dev(xs: torch.Tensor, Ns: torch.Tensor, status: torch.Tenso
 
     xs [nb] int64 (the bags' feature addresses: contiguous float32 [N_b, D]), Ns [nb] int64 and status [1] int32 on
     the device.  Returns the packed (classes, pred, A, B, crit): classes and A have nb * max_rows rows, the live ones
-    packed at the prefix sums of Ns, as dsmil_forward_bags packs them.  A refused batch sets status (see the header)."""
+    packed at the prefix sums of Ns, as dsmil_forward_bags packs them.  A refused batch sets status (see the header).
+    The shapes off the tensor-core batch call dsmil_generic_forward_bags_dev."""
     lib = _lib.load()
     P = ParamPack(*params)
-    if not lib.dsmil_shard_bags_supported(P.ref):
-        raise ValueError(f"the device bag list runs on the batched tensor-core path only; D={P.D}, C={P.C}, "
-                         f"nonlinear={P.nonlinear}, passing_v={P.passing_v} is not on it")
+    pre = _dev_prefix(lib, P, "the device bag list")
     nb, dev = int(xs.numel()), P.device
     with torch.cuda.device(dev):
         new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
         classes, A = new(nb * max_rows, P.C), new(nb * max_rows, P.C)
         pred, B = new(nb, P.C), new(nb, P.C, P.D)
         crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
-        ws = _workspace(lib.dsmil_forward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
-        rc = lib.dsmil_forward_bags_dev(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred), _ptr(A),
+        ws = _workspace(getattr(lib, pre + "forward_bags_dev_workspace_bytes")(P.ref, nb, max_rows), dev)
+        call = getattr(lib, pre + "forward_bags_dev")
+        rc = call(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred), _ptr(A),
                                         _ptr(B), _ptr(crit), _ptr(status), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, "dsmil_forward_bags_dev")
+        _lib.check(rc, pre + "forward_bags_dev")
     return classes, pred, A, B, crit
 
 

@@ -31,10 +31,14 @@ class ForwardBagsGraph:
     The graph reads the parameters in place: in-place updates (an optimizer step, `load_state_dict`) are seen by the
     next replay.  A parameter replaced by another tensor is not, and `run` raises RuntimeError; build a new graph.  A
     bag the library refuses (features not 16-byte aligned) sets `status` to 1 + its index (never cleared here) and the
-    batch's outputs are a finite stand-in; read `status` when you synchronise."""
+    batch's outputs are a finite stand-in; read `status` when you synchronise.
 
-    def __init__(self, milnet, nb: int, max_rows: int, warmup: int = 1):
-        self.D, self.C = step_shape(milnet)
+    generic=True: also the identity-v shapes off the tensor-core batch (train_graph.step_shape), recorded over the
+    generic batched route (dsmil_generic_forward_bags_dev, whose alignment rule refuses a bag of D % 4 == 0 that is not
+    16-byte aligned, and otherwise one that is not 4-byte aligned)."""
+
+    def __init__(self, milnet, nb: int, max_rows: int, warmup: int = 1, generic: bool = False):
+        self.D, self.C = step_shape(milnet, generic)
         nb, max_rows = int(nb), int(max_rows)
         if not 1 <= nb <= 65535 or max_rows < 1:
             raise ValueError(f"ForwardBagsGraph: nb={nb} outside [1, 65535] or max_rows={max_rows} < 1")
@@ -135,9 +139,9 @@ class EvalBagsGraph(ForwardBagsGraph):
     [1, C] rows as feed.eval_epoch computes it, and the sigmoid predictions (average: sigmoid(max) + sigmoid(bag)).
     Fill `labels` [nb, C], then `run(bags)`; `loss` [nb] and `pred` [nb, C] hold the batch's results."""
 
-    def __init__(self, milnet, criterion, nb: int, max_rows: int, average: bool = False):
+    def __init__(self, milnet, criterion, nb: int, max_rows: int, average: bool = False, generic: bool = False):
         self.criterion, self.average = criterion, bool(average)
-        super().__init__(milnet, nb, max_rows)
+        super().__init__(milnet, nb, max_rows, generic=generic)
 
     def _buffers(self, dev):
         self.labels = torch.zeros(self.nb, self.C, device=dev)

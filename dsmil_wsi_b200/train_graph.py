@@ -38,9 +38,11 @@ def check_optimizer(optimizer) -> None:
                      "or Adam / AdamW with capturable=True")
 
 
-def step_shape(milnet):
+def step_shape(milnet, generic: bool = False):
     """(D, C) of a MILNet whose training step the graph can record: FCLayer + BClassifier with identity v, on the
-    batched tensor-core shapes (dsmil_shard_bags_supported).  Anything else raises ValueError naming the shape."""
+    batched tensor-core shapes (dsmil_shard_bags_supported), or with generic=True also on the generic batched route
+    of the other identity-v shapes (dsmil_generic_bags_supported: e.g. D = 166 / 230, linear q, C > 4, D > 2048).
+    Anything else raises ValueError naming the shape."""
     ic, bc = getattr(milnet, "i_classifier", None), getattr(milnet, "b_classifier", None)
     if not (isinstance(ic, FCLayer) and isinstance(bc, BClassifier)):
         raise ValueError("graph-captured training needs MILNet(FCLayer, BClassifier); got "
@@ -49,10 +51,17 @@ def step_shape(milnet):
     Wv, _, _ = bc._v_params()
     C, D = int(bc.fcc.weight.shape[0]), int(bc.fcc.weight.shape[2])
     p = _lib.DsmilParams(D, C, int(W2 is not None), int(Wv is not None))
-    if not _lib.load().dsmil_shard_bags_supported(ctypes.byref(p)):
-        raise ValueError(f"graph-captured training runs on the batched tensor-core path only; D={D}, C={C}, "
-                         f"nonlinear={W2 is not None}, passing_v={Wv is not None} is not on it")
-    return D, C
+    lib = _lib.load()
+    if lib.dsmil_shard_bags_supported(ctypes.byref(p)):
+        return D, C
+    if generic and lib.dsmil_generic_bags_supported(ctypes.byref(p)):
+        return D, C
+    if generic:
+        raise ValueError(f"graph-captured training takes identity v only; D={D}, C={C}, "
+                         f"nonlinear={W2 is not None}, passing_v={Wv is not None} is on no batched route")
+    raise ValueError(f"graph-captured training runs on the batched tensor-core path only; D={D}, C={C}, "
+                     f"nonlinear={W2 is not None}, passing_v={Wv is not None} is not on it "
+                     "(generic=True records the generic batched route of the other identity-v shapes)")
 
 
 def fold_step_shape(milnets):
@@ -139,11 +148,13 @@ class TrainStepGraph:
     Warm-up and capture leave the parameters and the optimizer state as they found them, restored in place so the
     graph's addresses stay valid; optimizer state the warm-up creates is reset to its fresh value (zeros).  The graph
     freezes the optimizer's hyperparameters (e.g. its learning rate) at construction.  The parameters' .grad become
-    the graph's gradient buffers."""
+    the graph's gradient buffers.  generic=True: also the shapes off the tensor-core batch (step_shape), whose step
+    records the generic batched route with the bits of its eager step; their bags follow the alignment rule of
+    dsmil_generic_forward_bags_train_dev, which the slots meet."""
 
-    def __init__(self, milnet, criterion, optimizer, nb: int, max_rows: int, warmup: int = 1):
+    def __init__(self, milnet, criterion, optimizer, nb: int, max_rows: int, warmup: int = 1, generic: bool = False):
         check_optimizer(optimizer)
-        D, C = step_shape(milnet)
+        D, C = step_shape(milnet, generic)
         nb, max_rows = int(nb), int(max_rows)
         if not 1 <= nb <= 65535 or max_rows < 1:
             raise ValueError(f"TrainStepGraph: nb={nb} outside [1, 65535] or max_rows={max_rows} < 1")

@@ -138,8 +138,11 @@ int dsmil_forward(const dsmil_params_t* p, const float* X, const float* x_for_v,
 /* A stream of bags in ONE call (throughput form of the same forward; slides/sec in BASELINE.json):
  * Xs[b] -> device features [Ns[b], D] (host arrays of nb entries).  Outputs are packed in bag order:
  * classes / A [sum N, C], pred [nb, C], B [nb, C, D], crit_idx [nb, C].  On the tensor-core path the
- * whole batch costs a handful of launches (one bag table); other shapes, and bags that are not
- * 16-byte aligned, loop. */
+ * whole batch costs a handful of launches (one bag table); bags there that are not 16-byte aligned
+ * loop.  The generic shapes (identity v off dsmil_shard_bags_supported: any D <= 4096, C <= 8, either
+ * q form) run one launch per stage for the whole batch, every bag's outputs bit for bit what
+ * dsmil_forward gives it alone; on those of them whose phase 1 is k_qmlp_sm90 (nonlinear q,
+ * D % 128 == 0) a bag that is not 16-byte aligned makes the batch loop.  passing_v loops. */
 size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb);
 int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                        float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
@@ -167,8 +170,9 @@ int dsmil_forward_bags_models(const dsmil_params_t* ps, int32_t M, const float* 
 
 /* Training form of dsmil_forward_bags: the same packed outputs, plus save_Q [sum N,128] (after the tanh) and, for a
  * nonlinear q, save_H1 [sum N,128], packed in bag order -- what dsmil_backward_bags needs.  crit_idx [nb,C] is
- * required; its entries are rows within each bag.  Identity v only (passing_v: DSMIL_ERR_ARG).  Shapes or bags off
- * the tensor-core batch loop per bag (as dsmil_forward_bags does) into the same packed buffers. */
+ * required; its entries are rows within each bag.  Identity v only (passing_v: DSMIL_ERR_ARG).  Routes as
+ * dsmil_forward_bags: bags it loops over go one at a time into the same packed buffers.  save_H1 may be NULL for a
+ * linear q. */
 size_t dsmil_forward_bags_train_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb);
 int dsmil_forward_bags_train(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                              float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
@@ -291,6 +295,36 @@ size_t dsmil_forward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t n
 int dsmil_forward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev, int32_t nb,
                            int64_t max_rows, float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
                            int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+/* The three capture-safe calls above on the generic shapes: identity v off dsmil_shard_bags_supported (any D <= 4096,
+ * C <= 8, either q form; dsmil_generic_bags_supported).  Same arguments, rules, refusal, stand-in batch and workspace
+ * contract as dsmil_forward_bags_train_dev / dsmil_backward_bags_dev / dsmil_forward_bags_dev, except:
+ *  - the forward is the generic batched forward of dsmil_forward_bags (one launch per stage for the whole batch, no
+ *    phase-1 overlap), planned on the device; every bag's outputs are what dsmil_forward gives that bag alone, and on
+ *    the same bags every output and gradient is the eager calls' (dsmil_forward_bags(_train), dsmil_backward_bags).
+ *  - alignment rule: a bag must be 16-byte aligned when D % 4 == 0 and 4-byte aligned otherwise (so that [nb, max_rows,
+ *    D] slots of any D are accepted); every kernel form the eager calls would choose for such bags (the MODE of the
+ *    instance scores, gWi's streaming or tiled reduction) then follows from D alone.  A bag that breaks the rule is
+ *    refused like a bag of a bad size.
+ *  - save_H1 / H1 may be NULL for a linear q.
+ * The tensor-core shapes are DSMIL_ERR_ARG here (their calls are the ones above), and the workspace functions return 0
+ * off dsmil_generic_bags_supported. */
+int dsmil_generic_bags_supported(const dsmil_params_t* p);
+size_t dsmil_generic_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_generic_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                         int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
+                                         int64_t* crit_idx, float* save_Q, float* save_H1, int32_t* status,
+                                         void* workspace, size_t workspace_bytes, void* stream);
+size_t dsmil_generic_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_generic_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                    int32_t nb, int64_t max_rows, const float* Q, const float* H1, const float* A,
+                                    const float* B, const int64_t* crit_idx, const float* d_classes,
+                                    const float* d_pred, const float* d_A, const float* d_B, const dsmil_grads_t* grads,
+                                    int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+size_t dsmil_generic_forward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_generic_forward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                                   int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
+                                   int64_t* crit_idx, int32_t* status, void* workspace, size_t workspace_bytes,
+                                   void* stream);
 
 /* Call form (2)+(3) of the boundary (SURVEY §8b): the callers in attention_map.py:74,85 /
  * testing_tcga.py:72,83 run the instance classifier and the bag classifier separately.
