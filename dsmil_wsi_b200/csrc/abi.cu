@@ -543,12 +543,33 @@ static int launch_attend_gb_j(int J, int grid, cudaStream_t st, const sm90::BagD
   return 0;
 }
 
+// The value projection V = relu(Xv Wv^T + bv) over a table whose X are the value inputs, into packed V.  k_vproj_b;
+// DSMIL_VPROJ_LINEAR_B=1 builds the variant that runs k_linear_b (k_linear's 64 x 128 tile) instead, with the same
+// bits, for tools/bench_value_bags.py.  The library is built with the default.
+#ifndef DSMIL_VPROJ_LINEAR_B
+#define DSMIL_VPROJ_LINEAR_B 0
+#endif
+static int launch_vproj_b(const dsmil_params_t* p, const sm90::BagDev* vtab, int nb, int tiles, const int* tiles_dev,
+                          float* V, cudaStream_t st) {
+  const int D = p->D;
+#if DSMIL_VPROJ_LINEAR_B
+  k_linear_b<ACT_RELU><<<dim3(2 * tiles, ceil_div(D, LBN)), 256, 0, st>>>(vtab, nb, tiles_dev, D, p->Wv, p->bv, D, V);
+  DSMIL_LAUNCH_OK("k_linear_b");
+#else
+  k_vproj_b<<<dim3(tiles, ceil_div(D, VBN)), 256, 0, st>>>(vtab, nb, tiles_dev, D, p->Wv, p->bv, D, V);
+  DSMIL_LAUNCH_OK("k_vproj_b");
+#endif
+  return 0;
+}
+
 // The generic forward over w.table: `tiles` and `recs` are the table's 128-row tiles and records and `rows` its packed
 // rows (dev calls: capacities, the live counts in w.plan); max_N bounds the bags' rows.  Q (and H1 for nonlinear q)
-// receive the Q-MLP's outputs row-major.
+// receive the Q-MLP's outputs row-major.  vtab (passing_v, value_forward_bags): nb entries of w.table's numbering whose
+// X is each bag's value input, then nb whose X is the bag's packed rows of V; V receives the value projection and the
+// attend pass reads it through the second half.
 static int gen_forward_run(const dsmil_params_t* p, const GenWs& w, int nb, int64_t rows, int tiles, int recs,
                            int64_t max_N, float* classes, float* pred, float* A, float* B, int64_t* crit, float* Q,
-                           float* H1, cudaStream_t st) {
+                           float* H1, cudaStream_t st, const sm90::BagDev* vtab = nullptr, float* V = nullptr) {
   const int C = p->C, D = p->D;
   const BagsPlan* pl = w.plan;
   int rc;
@@ -576,16 +597,18 @@ static int gen_forward_run(const dsmil_params_t* p, const GenWs& w, int nb, int6
       return rc;
     prof_end(PROF_QMLP, st);
   }
+  if (vtab && (rc = launch_vproj_b(p, vtab, nb, tiles, pl ? &pl->tiles : nullptr, V, st))) return rc;
   k_crit_qmax_b<<<dim3(C, nb), kQ, 0, st>>>(w.table, w.keys, Q, C, w.qmax, crit);
   DSMIL_LAUNCH_OK("k_crit_qmax_b");
   int j = ceil_div(D, 256), J = 1;
   while (J < j) J <<= 1;
   const int* recs_dev = pl ? &pl->recs : nullptr;
+  const sm90::BagDev* atab = vtab ? vtab + nb : w.table;   // the rows the attend pass weighs: V, or the features
   prof_begin(PROF_ATTEND, st);
-  if (C == 1) rc = launch_attend_gb_j<1>(J, recs, st, w.table, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
-  else if (C == 2) rc = launch_attend_gb_j<2>(J, recs, st, w.table, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
-  else if (C <= 4) rc = launch_attend_gb_j<4>(J, recs, st, w.table, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
-  else rc = launch_attend_gb_j<8>(J, recs, st, w.table, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
+  if (C == 1) rc = launch_attend_gb_j<1>(J, recs, st, atab, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
+  else if (C == 2) rc = launch_attend_gb_j<2>(J, recs, st, atab, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
+  else if (C <= 4) rc = launch_attend_gb_j<4>(J, recs, st, atab, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
+  else rc = launch_attend_gb_j<8>(J, recs, st, atab, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
   prof_end(PROF_ATTEND, st);
   if (rc) return rc;
   k_combine_rec_b<<<dim3(C, ceil_div(D, 256), nb), 256, 0, st>>>(w.table, C, D, w.recs, w.rec);
@@ -618,6 +641,63 @@ static int forward_bags_gen(const dsmil_params_t* p, const float* const* Xs, con
   DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
   return gen_forward_run(p, w, nb, row, tile, rec, mx, classes, pred, A, B, crit ? crit : w.crit,
                          save_Q ? save_Q : w.Q, p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr, st);
+}
+
+// ---- batched forward of the value network (passing_v): the generic forward plus V, one launch per stage ------------
+// Phase 1 is the one dsmil_forward takes on the shape (k_qmlp_sm90 for nonlinear q with D % 128 == 0, else k_scores_b
+// and the FFMA Q-MLP), then one k_vproj_b for the V of every bag, and the attend pass over V.  Every bag's outputs and
+// saves are what dsmil_forward gives it alone (DESIGN §4.2i).
+static bool value_shape(const dsmil_params_t* p) {
+  return p && p->passing_v && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D;
+}
+
+struct ValWs {
+  GenWs g;
+  sm90::BagDev* vtab;   // [2 nb]: the value inputs' table, then the packed V's (gen_forward_run)
+  float* V;             // [rows][D] where the caller keeps none
+  size_t bytes;
+};
+static ValWs carve_value(const dsmil_params_t* p, const int64_t* Ns, int nb, bool need_Q, bool need_H1, bool need_V,
+                         void* ws, size_t cap, bool* ok) {
+  ValWs w;
+  bool gok;
+  w.g = carve_gen_eager(p, Ns, nb, need_Q, need_H1, ws, cap, &gok);
+  Carver c(ws, cap);
+  c.off = w.g.bytes;
+  int64_t rows = 0;
+  for (int b = 0; b < nb; ++b) rows += Ns[b];
+  w.vtab = c.take<sm90::BagDev>(2 * static_cast<size_t>(nb));
+  w.V = need_V ? c.take<float>(rows * p->D) : nullptr;
+  w.bytes = c.off;
+  *ok = gok && c.ok();
+  return w;
+}
+
+static int value_forward_bags(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
+                              const int64_t* Ns, int nb, float* classes, float* pred, float* A, float* B, int64_t* crit,
+                              float* save_Q, float* save_H1, float* save_V, void* ws, size_t ws_bytes,
+                              cudaStream_t st) {
+  bool ok;
+  ValWs w = carve_value(p, Ns, nb, !save_Q, p->nonlinear && !save_H1, !save_V, ws, ws_bytes, &ok);
+  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+  if (rc) return rc;
+  float* V = save_V ? save_V : w.V;
+  std::vector<sm90::BagDev> tbl(nb), vt(2 * static_cast<size_t>(nb));
+  long long row = 0;
+  int tile = 0, rec = 0;
+  int64_t mx = 1;
+  for (int b = 0; b < nb; ++b) {
+    tbl[b] = gen_bag_entry(Xs[b], Ns[b], p->D, row, tile, rec);
+    vt[b] = tbl[b];
+    vt[b].X = XVs ? XVs[b] : Xs[b];
+    vt[nb + b] = tbl[b];
+    vt[nb + b].X = V + tbl[b].row_off * p->D;
+    mx = std::max<int64_t>(mx, Ns[b]);
+  }
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.g.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.vtab, vt.data(), sizeof(sm90::BagDev) * vt.size(), cudaMemcpyHostToDevice, st));
+  return gen_forward_run(p, w.g, nb, row, tile, rec, mx, classes, pred, A, B, crit ? crit : w.g.crit,
+                         save_Q ? save_Q : w.g.Q, p->nonlinear ? (save_H1 ? save_H1 : w.g.H1) : nullptr, st, w.vtab, V);
 }
 
 }  // namespace dsmil
@@ -2784,6 +2864,60 @@ int dsmil_shard_backward_bags_phase3_dev(const dsmil_params_t* p, int32_t nb, in
   return bwd_bags_phase3_impl(p, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, dL_local, dqm_global, q_max, crit_idx,
                               reinterpret_cast<const long long*>(row_offsets_dev), &g, w, &dz1,
                               static_cast<cudaStream_t>(stream));
+}
+
+int dsmil_value_bags_supported(const dsmil_params_t* p) {
+  return value_shape(p) && p->Wv && p->bv ? 1 : 0;
+}
+
+size_t dsmil_value_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
+  if (!dsmil_value_bags_supported(p) || !Ns || nb < 1 || nb > 65535) return 0;
+  int64_t mx = 0;
+  for (int b = 0; b < nb; ++b) {
+    if (Ns[b] < 1 || Ns[b] >= 0xffffffffll) return 0;
+    mx = std::max<int64_t>(mx, Ns[b]);
+  }
+  bool ok;
+  // nonlinear q with D % 128 == 0 loops the single-bag forward when a bag is not 16-byte aligned
+  const size_t loop = sm90::qmlp_supported(p) ? carve_fwd(p, mx, nullptr, 0, &ok).bytes : 0;
+  return std::max(loop, carve_value(p, Ns, nb, true, p->nonlinear, true, nullptr, 0, &ok).bytes);
+}
+
+int dsmil_value_forward_bags(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
+                             const int64_t* Ns, int32_t nb, float* classes, float* pred, float* A, float* B,
+                             int64_t* crit_idx, float* save_Q, float* save_H1, float* save_V, void* workspace,
+                             size_t workspace_bytes, void* stream) {
+  int rc = check_params(p, true);
+  if (rc) return rc;
+  DSMIL_REQUIRE(p->passing_v, "the value route takes passing_v models (identity v: dsmil_forward_bags)");
+  DSMIL_REQUIRE(Xs && Ns && nb >= 1 && nb <= 65535 && classes && pred && A && B,
+                "NULL pointer or nb outside [1, 65535]");
+  const bool saves = save_Q || save_H1 || save_V;
+  DSMIL_REQUIRE(!saves || (save_Q && save_V && (!p->nonlinear || save_H1)),
+                "saves: save_Q, save_V (and save_H1 for a nonlinear q) together, or none");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int64_t total;
+  bool aligned;
+  if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
+  for (int b = 0; XVs && b < nb; ++b) DSMIL_REQUIRE(XVs[b], "bag %d: NULL value input", b);
+  const size_t need = dsmil_value_forward_bags_workspace_bytes(p, Ns, nb);
+  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  if (aligned || !sm90::qmlp_supported(p))
+    return value_forward_bags(p, Xs, XVs, Ns, nb, classes, pred, A, B, crit_idx, save_Q, save_H1, save_V, workspace,
+                              workspace_bytes, st);
+  // k_qmlp_sm90 reads 16-byte aligned bags only: the single-bag forward, one bag at a time into the packed buffers
+  int64_t row = 0;
+  const int C = p->C, D = p->D;
+  for (int b = 0; b < nb; ++b) {
+    rc = forward_impl(p, Xs[b], XVs ? XVs[b] : nullptr, nullptr, Ns[b], classes + row * C,
+                      pred + static_cast<size_t>(b) * C, A + row * C, B + static_cast<size_t>(b) * C * D,
+                      crit_idx ? crit_idx + static_cast<size_t>(b) * C : nullptr, save_Q ? save_Q + row * kQ : nullptr,
+                      save_H1 ? save_H1 + row * kQ : nullptr, save_V ? save_V + row * D : nullptr, workspace,
+                      workspace_bytes, st);
+    if (rc) return rc;
+    row += Ns[b];
+  }
+  return 0;
 }
 
 }  // extern "C"

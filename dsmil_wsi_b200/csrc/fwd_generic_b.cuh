@@ -9,6 +9,8 @@
 //   k_attend_gb      k_attend per (bag, record), attend_ctas(N_b) records per bag
 //   k_combine_rec_b  k_combine_rec per bag (grid.z)
 //   k_finalize_gb    k_finalize per bag (grid.y)
+//   k_vproj_b        the value network's V = relu(Xv W^T + b) per 128-row tile of a bag (passing_v; abi.cu's value
+//                    route gives k_attend_gb a table whose X is each bag's packed V)
 #pragma once
 #include "common.cuh"
 #include "gemm_generic.cuh"
@@ -337,6 +339,111 @@ k_finalize_gb(const sm90::BagDev* __restrict__ bags, const float* __restrict__ r
   const sm90::BagDev bg = bags[bag];
   finalize_bag(rec + bag * rec_floats(C, D), bg.N, C, D, Wf, bf, A + bg.row_off * C,
                B + static_cast<size_t>(bag) * C * D, pred + static_cast<size_t>(bag) * C, blockIdx.x, gridDim.x);
+}
+
+// ---- the value network's projection over the bag table (passing_v, dsmil.py:35-39) ----------------------------------
+// V[packed rows, M] = relu(Xv_b W^T + b) over each bag's own rows, bit for bit what k_linear<ACT_RELU, false> gives the
+// bag alone: every output is one fmaf chain over k = 0 .. K-1 in ascending order from 0 (zero padding past K adds
+// exact zeros, as in linear_tile), then + b[m], then the ReLU.  Within that order the tile is the k_gemm_tn one: a
+// 128 x 128 output block per CTA and 8 x 8 per thread (four 16-byte shared-memory loads per 64 FMAs, where
+// linear_tile's 4 x 8 block needs three per 32), k-tiles of Xv and W double-buffered in shared memory, the next one
+// fetched into registers while the current one is multiplied.
+constexpr int VBM = 128, VBN = 128, VBK = 16;
+static_assert(VBM == sm90::kTileM, "k_vproj_b takes one table tile per CTA");
+
+// 8 consecutive k of one row from k on (zeros past K or for a dead row).
+__device__ __forceinline__ void vproj_fetch(const float* __restrict__ row, bool live, bool vec, int k, int K,
+                                            float (&r)[8]) {
+  if (live && vec && k + 8 <= K) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(row + k));
+    const float4 c = __ldg(reinterpret_cast<const float4*>(row + k + 4));
+    r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w;
+    r[4] = c.x; r[5] = c.y; r[6] = c.z; r[7] = c.w;
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) r[i] = (live && k + i < K) ? __ldg(row + k + i) : 0.f;
+  }
+}
+
+// grid = (tiles (tiles_dev: the live count of a capacity grid), ceil(M / VBN)); X of each entry is its value input.
+__global__ void __launch_bounds__(256, 2)
+k_vproj_b(const sm90::BagDev* __restrict__ bags, int nb, const int* __restrict__ tiles_dev, int K,
+          const float* __restrict__ W, const float* __restrict__ b, int M, float* __restrict__ Y) {
+  __shared__ __align__(16) float Xs[2][VBK][VBM + 4];
+  __shared__ __align__(16) float Ws[2][VBK][VBN + 4];
+  const int t = blockIdx.x;
+  if (tiles_dev && t >= *tiles_dev) return;
+  const sm90::BagDev bg = bags[bag_of(bags, nb, t, false)];
+  const int64_t n0 = static_cast<int64_t>(t - bg.tile_off) * VBM;
+  const int m0 = blockIdx.y * VBN;
+  const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+  // loader: row lr of the X tile and of the W tile, k from lk (a warp stores 32 consecutive rows: no bank conflict)
+  const int lr = tid & 127, lk = (tid >> 7) * 8;
+  const bool xlive = n0 + lr < bg.N, wlive = m0 + lr < M;
+  const float* xrow = bg.X + (xlive ? n0 + lr : 0) * K;
+  const float* wrow = W + static_cast<int64_t>(wlive ? m0 + lr : 0) * K;
+  const bool vec = (K % 4 == 0) && ((reinterpret_cast<uintptr_t>(bg.X) & 15) == 0) &&
+                   ((reinterpret_cast<uintptr_t>(W) & 15) == 0);
+  float acc[8][8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+  float xr[8], wr[8];
+  vproj_fetch(xrow, xlive, vec, lk, K, xr);
+  vproj_fetch(wrow, wlive, vec, lk, K, wr);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { Xs[0][lk + i][lr] = xr[i]; Ws[0][lk + i][lr] = wr[i]; }
+  __syncthreads();
+  int buf = 0;
+  for (int k0 = 0; k0 < K; k0 += VBK) {
+    const bool more = k0 + VBK < K;
+    if (more) {
+      vproj_fetch(xrow, xlive, vec, k0 + VBK + lk, K, xr);
+      vproj_fetch(wrow, wlive, vec, k0 + VBK + lk, K, wr);
+    }
+#pragma unroll
+    for (int kk = 0; kk < VBK; ++kk) {
+      const float4 a0 = *reinterpret_cast<const float4*>(&Xs[buf][kk][ty * 4]);
+      const float4 a1 = *reinterpret_cast<const float4*>(&Xs[buf][kk][64 + ty * 4]);
+      const float4 b0 = *reinterpret_cast<const float4*>(&Ws[buf][kk][tx * 4]);
+      const float4 b1 = *reinterpret_cast<const float4*>(&Ws[buf][kk][64 + tx * 4]);
+      const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+      const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+    }
+    if (more) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { Xs[buf ^ 1][lk + i][lr] = xr[i]; Ws[buf ^ 1][lk + i][lr] = wr[i]; }
+    }
+    __syncthreads();   // the next buffer is written; this one is read by everyone before it is refilled
+    buf ^= 1;
+  }
+  float* Yb = Y + bg.row_off * M;
+  const bool vst = (M % 4 == 0) && ((reinterpret_cast<uintptr_t>(Y) & 15) == 0);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int64_t n = n0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4));
+    if (n >= bg.N) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int mb = m0 + h * 64 + tx * 4;
+      float y[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) y[j] = mb + j < M ? fmaxf(acc[i][h * 4 + j] + __ldg(b + mb + j), 0.f) : 0.f;
+      float* dst = Yb + n * M + mb;
+      if (vst && mb + 3 < M) {
+        *reinterpret_cast<float4*>(dst) = make_float4(y[0], y[1], y[2], y[3]);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (mb + j < M) dst[j] = y[j];
+      }
+    }
+  }
 }
 
 }  // namespace dsmil

@@ -666,6 +666,58 @@ def mil_forward_bags_models(bags: Sequence[torch.Tensor], params_list: Sequence[
     return [BagOutputs(classes[m], pred[m], A[m], B[m], Ns, crit[m]) for m in range(M)]
 
 
+MAX_VALUE_BAGS = 65535   # bags of one dsmil_value_forward_bags call
+
+
+@torch.no_grad()
+def mil_forward_value_bags(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]],
+                           v_inputs: Optional[Sequence[torch.Tensor]] = None):
+    """Inference over a stream of bags for a model with a value network (passing_v), in one
+    dsmil_value_forward_bags call: returns a lazy sequence of (classes, prediction_bag, A, B) per bag plus crit_idx
+    [nb, C], as mil_forward_bags does.  v_inputs: each bag's value input (the features after the dropout mask of
+    dsmil.py:36), or None for the features themselves (eval mode, or p = 0).  Every bag's outputs are bit for bit
+    what mil_forward gives it alone with the same value input.  A batch of more than MAX_VALUE_BAGS bags is split
+    into consecutive calls that write into the same packed outputs."""
+    lib = _lib.load()
+    P = ParamPack(*params)
+    if not P.passing_v:
+        raise ValueError("mil_forward_value_bags takes models with a value network (passing_v); identity v goes "
+                         "through mil_forward_bags")
+    nb = len(bags)
+    if nb == 0:
+        return [], None
+    xs, Ns, _, _ = _bag_table(bags, P)
+    vs = None
+    if v_inputs is not None:
+        if len(v_inputs) != nb:
+            raise ValueError(f"{len(v_inputs)} value inputs for {nb} bags")
+        vs = [_check_feats(v, P.D) for v in v_inputs]
+        for v, x in zip(vs, xs):
+            if v.shape != x.shape or v.device != x.device:
+                raise ValueError(f"a value input {tuple(v.shape)} on {v.device} does not match its bag "
+                                 f"{tuple(x.shape)} on {x.device}")
+    total, Cc, D, dev = sum(Ns), P.C, P.D, P.device
+    with torch.cuda.device(dev):
+        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        classes, A = new(total, Cc), new(total, Cc)
+        pred, B = new(nb, Cc), new(nb, Cc, D)
+        crit = torch.empty(nb, Cc, dtype=torch.int64, device=dev)
+        row = 0
+        for s in range(0, nb, MAX_VALUE_BAGS):
+            e = min(s + MAX_VALUE_BAGS, nb)
+            n, rows = e - s, sum(Ns[s:e])
+            c_X = (C.c_void_p * n)(*[x.data_ptr() for x in xs[s:e]])
+            c_V = None if vs is None else (C.c_void_p * n)(*[v.data_ptr() for v in vs[s:e]])
+            c_N = (C.c_int64 * n)(*Ns[s:e])
+            ws = _workspace(lib.dsmil_value_forward_bags_workspace_bytes(P.ref, c_N, n), dev)
+            rc = lib.dsmil_value_forward_bags(P.ref, c_X, c_V, c_N, n, _ptr(classes[row:]), _ptr(pred[s:]),
+                                              _ptr(A[row:]), _ptr(B[s:]), _ptr(crit[s:]), None, None, None, _ptr(ws),
+                                              ws.numel(), _stream())
+            _lib.check(rc, "dsmil_value_forward_bags")
+            row += rows
+    return BagOutputs(classes, pred, A, B, Ns, crit), crit
+
+
 @torch.no_grad()
 def _mil_forward_bags_infer(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]]):
     lib = _lib.load()

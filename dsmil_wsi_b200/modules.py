@@ -135,7 +135,9 @@ class MILNet(nn.Module):
         library call (bag table; see DESIGN.md).  The result is a lazy sequence of views over packed outputs
         (`.packed`).  grad=False (default): inference, no autograd.  grad=True with grad mode on: the packed outputs
         carry autograd history and one backward call covers the whole batch (a minibatch training step).  Models
-        with passing_v or a foreign instance classifier run `self.forward` per bag, under autograd when asked."""
+        with passing_v run one dsmil_value_forward_bags call for inference (in train mode each bag's dropout mask of
+        v is drawn in bag order, as `self.forward` draws it) and `self.forward` per bag with grad=True; a foreign
+        instance classifier always runs `self.forward` per bag."""
         if not (grad and torch.is_grad_enabled()):
             with torch.no_grad():
                 return self._forward_bags(bags, False)
@@ -145,14 +147,33 @@ class MILNet(nn.Module):
         ic, bc = self.i_classifier, self.b_classifier
         if not (isinstance(bc, BClassifier) and isinstance(ic, (FCLayer, IClassifier))):
             return [self.forward(b) for b in bags]
+        if bc._v_params()[0] is not None:
+            if grad:   # autograd through the per-bag forward: the gradients users get from it, bag by bag
+                return [self.forward(b) for b in bags]
+            return self._forward_value_bags(bags)
         feats = [ic.embed(b) if isinstance(ic, IClassifier) else b for b in bags]
         lin = ic._linear()
         W1, b1, W2, b2 = bc._q_params()
-        Wv, bv, _ = bc._v_params()
-        if Wv is not None:
-            return [self.forward(b) for b in bags]
         params = (lin.weight, lin.bias, W1, b1, W2, b2, None, None, bc.fcc.weight, bc.fcc.bias)
         outs, _ = Fn.mil_forward_bags(feats, params, grad=grad)
+        return outs
+
+    def _forward_value_bags(self, bags):
+        """Inference of a passing_v model over the bags in one library call, with the bits and RNG draws of the
+        per-bag loop."""
+        ic, bc = self.i_classifier, self.b_classifier
+        lin = ic._linear()
+        W1, b1, W2, b2 = bc._q_params()
+        Wv, bv, p_drop = bc._v_params()
+        draw = bc.training and p_drop > 0.0
+        feats, v_inputs = [], ([] if draw else None)
+        for b in bags:   # embedding, then v's dropout mask, bag by bag: the per-bag loop's draws in its order
+            f = ic.embed(b) if isinstance(ic, IClassifier) else b
+            feats.append(f)
+            if draw:
+                v_inputs.append(f * bc.v[0](torch.ones_like(f)))
+        params = (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
+        outs, _ = Fn.mil_forward_value_bags(feats, params, v_inputs)
         return outs
 
     @torch.no_grad()

@@ -326,6 +326,27 @@ int dsmil_generic_forward_bags_dev(const dsmil_params_t* p, const float* const* 
                                    int64_t* crit_idx, int32_t* status, void* workspace, size_t workspace_bytes,
                                    void* stream);
 
+/* The batched forward of a model with a value network (passing_v: v = Dropout-Linear(D,D)-ReLU, dsmil.py:35-39), which
+ * dsmil_forward_bags runs one bag at a time.  dsmil_value_bags_supported: passing_v with Wv/bv, 1 <= D <= 4096,
+ * 1 <= C <= 8, either q form (the shapes dsmil_forward takes with passing_v).
+ * dsmil_value_forward_bags: Xs / Ns / outputs as dsmil_forward_bags (crit_idx [nb,C] may be NULL); XVs [nb] (host
+ * array, or NULL) are the bags' value inputs -- the features after the caller applied the dropout mask of dsmil.py:36,
+ * as x_for_v of dsmil_forward; NULL means the value inputs are Xs (eval mode or p = 0).  save_Q / save_H1 [sum N,128]
+ * and save_V [sum N,D], packed in bag order, are all NULL (inference) or all given (save_H1 may be NULL for a linear
+ * q).  Every bag's outputs and saves are, bit for bit, what dsmil_forward(p, Xs[b], XVs[b], ...) writes for it alone.
+ * One launch per stage for the whole batch, whatever nb: phase 1 (k_qmlp_sm90 where dsmil_forward takes it, else the
+ * FFMA scores and Q-MLP), one value projection, attend, combine and finalize; on the shapes whose phase 1 is
+ * k_qmlp_sm90 (nonlinear q, D % 128 == 0) a bag that is not 16-byte aligned makes the batch loop dsmil_forward.
+ * Identity v, nb outside [1, 65535] or a partial set of saves is DSMIL_ERR_ARG; an empty bag DSMIL_ERR_EMPTY; a short
+ * workspace DSMIL_ERR_WORKSPACE.  The workspace size covers both routes and every save choice; 0 for invalid
+ * arguments. */
+int dsmil_value_bags_supported(const dsmil_params_t* p);
+size_t dsmil_value_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb);
+int dsmil_value_forward_bags(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
+                             const int64_t* Ns, int32_t nb, float* classes, float* pred, float* A, float* B,
+                             int64_t* crit_idx, float* save_Q, float* save_H1, float* save_V, void* workspace,
+                             size_t workspace_bytes, void* stream);
+
 /* Call form (2)+(3) of the boundary (SURVEY §8b): the callers in attention_map.py:74,85 /
  * testing_tcga.py:72,83 run the instance classifier and the bag classifier separately.
  * dsmil_instance_scores == IClassifier.fc / FCLayer.fc (dsmil.py:11,24).
