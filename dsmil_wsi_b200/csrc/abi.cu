@@ -114,6 +114,10 @@ static int check_workspace(size_t need, bool ok, const void* ws, size_t cap) {
   set_error("workspace too small: need %zu bytes, got %zu", need, cap);
   return DSMIL_ERR_WORKSPACE;
 }
+// check_workspace against the size a *_workspace_bytes call reports
+static int need_workspace(size_t need, const void* ws, size_t ws_bytes) {
+  return check_workspace(need, ws_bytes >= need, ws, ws ? ws_bytes : 0);
+}
 
 // Bags of the batch and their rows; DSMIL_ERR_EMPTY for an empty bag, as dsmil_forward_bags.  Xs == NULL checks the
 // row counts only (a phase that reads no features).
@@ -380,40 +384,6 @@ static int phase3_impl(const dsmil_params_t* p, int64_t N, const float* rec, flo
   return 0;
 }
 
-static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
-                             const float* classes_in, float* classes, float* pred, float* A, float* B,
-                             int64_t* crit, float* save_Q, float* save_H1, void* ws, size_t ws_bytes,
-                             cudaStream_t st);
-
-static int forward_impl(const dsmil_params_t* p, const float* X, const float* xv, const float* classes_in,
-                        int64_t N, float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
-                        float* save_Q, float* save_H1, float* save_V, void* ws, size_t ws_bytes, cudaStream_t st) {
-  int rc = check_params(p, classes_in == nullptr);
-  if (rc) return rc;
-  DSMIL_REQUIRE(N >= 0 && N < 0xffffffffll, "N=%lld out of range", (long long)N);
-  if (N == 0) {
-    set_error("empty bag (N == 0): the reference raises IndexError at dsmil.py:53");
-    return DSMIL_ERR_EMPTY;
-  }
-  DSMIL_REQUIRE(X && pred && A && B && (classes || classes_in), "NULL tensor pointer");
-  if (sm90::batched_supported(p) && (reinterpret_cast<uintptr_t>(X) & 15) == 0)
-    return forward_bags_impl(p, &X, &N, 1, classes_in, classes, pred, A, B, crit_idx, save_Q, save_H1, ws, ws_bytes, st);
-  bool ok;
-  FwdWs w = carve_fwd(p, N, ws, ws_bytes, &ok);
-  if ((rc = check_workspace(w.bytes, ok, ws, ws_bytes))) return rc;
-  float* Q = save_Q ? save_Q : w.Q;
-  float* H1 = p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr;
-  float* V = p->passing_v ? (save_V ? save_V : w.V) : nullptr;
-  if ((rc = phase1_impl(p, X, xv, classes_in, N, 0, classes, Q, H1, V, w.cand, w, st))) return rc;
-  int64_t* crit = crit_idx ? crit_idx : w.crit;
-  k_merge_cand<<<p->C, kQ, 0, st>>>(w.cand, 1, 1, p->C, w.qmax, crit);
-  DSMIL_LAUNCH_OK("k_merge_cand");
-  const float* Vv = p->passing_v ? V : X;
-  if ((rc = phase2_impl(p, Vv, Q, N, w.qmax, A, w.rec, w.recs, st))) return rc;
-  return phase3_impl(p, N, w.rec, A, B, pred, st);
-}
-
-
 // ---- batched forward: a stream of bags in a handful of launches (tensor-core path only) -----------
 struct BagsWs : Phase1Ws {
   float* Q;
@@ -481,10 +451,11 @@ static int forward_bags_impl(const dsmil_params_t* p, const float* const* Xs, co
   return bags_attend_finalize(p, w, nb, Q, q_blocked, pred, A, B, crit, recs, nullptr, st, overlap);
 }
 
-// ---- batched forward on the generic shapes: identity v off the tensor-core batch, one launch per stage -----------
-// Every bag's outputs are the bits dsmil_forward gives it alone (fwd_generic_b.cuh, DESIGN §4.2h).  Phase 1 is the
-// one the single-bag forward takes on the shape: k_qmlp_sm90 where it runs (D % 128 == 0, nonlinear q, 16-byte
-// aligned bags), else k_scores at each bag's MODE and the FFMA Q-MLP.
+// ---- batched forward off the tensor-core batch: the generic shapes and the value network, one launch per stage ----
+// Every bag's outputs and saves are the bits dsmil_forward gives it alone (fwd_generic_b.cuh, DESIGN §4.2h, §4.2i).
+// Phase 1 is the one the single-bag forward takes on the shape: k_qmlp_sm90 where it runs (D % 128 == 0, nonlinear q,
+// 16-byte aligned bags), else k_scores at each bag's MODE and the FFMA Q-MLP.  passing_v adds one k_vproj_b for the V
+// of every bag, and the attend pass weighs V.
 static bool gen_shape(const dsmil_params_t* p) { return !p->passing_v && !sm90::batched_supported(p); }
 
 struct GenWs : Phase1Ws {
@@ -494,39 +465,43 @@ struct GenWs : Phase1Ws {
   float *recs, *rec;        // the partial records; each bag's combined one [nb]
   BagsPlan* plan;           // dev calls: the planner's live counts and the stand-in row of a refused batch
   float* zero_row;
+  sm90::BagDev* vtab;       // passing_v: [2 nb], the value inputs' table, then the packed V's (gen_forward_run)
+  float* V;                 // passing_v: [rows][D] where the caller keeps none
   size_t bytes;
 };
-// rows, recs: the packed rows and partial records (dev calls: their capacities).
-static GenWs carve_gen(const dsmil_params_t* p, int nb, int64_t rows, int64_t recs, bool need_Q, bool need_H1,
-                       bool dev, void* ws, size_t cap, bool* ok) {
+// rows, recs: the packed rows and partial records (dev calls: their capacities).  saves: the caller keeps Q, H1 and
+// V (the training forms).
+static GenWs carve_gen(const dsmil_params_t* p, int nb, int64_t rows, int64_t recs, bool saves, bool dev, void* ws,
+                       size_t cap, bool* ok) {
   Carver c(ws, cap);
   GenWs w;
   carve_phase1(c, p, nb, w);
-  w.Q = need_Q ? c.take<float>(rows * kQ) : nullptr;
-  w.H1 = need_H1 ? c.take<float>(rows * kQ) : nullptr;
+  w.Q = saves ? nullptr : c.take<float>(rows * kQ);
+  w.H1 = p->nonlinear && !saves ? c.take<float>(rows * kQ) : nullptr;
   w.qmax = c.take<float>(static_cast<size_t>(nb) * p->C * kQ);
   w.crit = c.take<int64_t>(static_cast<size_t>(nb) * p->C);
   w.recs = c.take<float>(recs * rec_floats(p->C, p->D));
   w.rec = c.take<float>(static_cast<size_t>(nb) * rec_floats(p->C, p->D));
   w.plan = dev ? c.take<BagsPlan>(1) : nullptr;
   w.zero_row = dev ? c.take<float>(p->D) : nullptr;
+  w.vtab = p->passing_v ? c.take<sm90::BagDev>(2 * static_cast<size_t>(nb)) : nullptr;
+  w.V = p->passing_v && !saves ? c.take<float>(rows * p->D) : nullptr;
   w.bytes = c.off;
   *ok = c.ok();
   return w;
 }
-static GenWs carve_gen_eager(const dsmil_params_t* p, const int64_t* Ns, int nb, bool need_Q, bool need_H1, void* ws,
-                             size_t cap, bool* ok) {
+static GenWs carve_gen_eager(const dsmil_params_t* p, const int64_t* Ns, int nb, bool saves, void* ws, size_t cap,
+                             bool* ok) {
   int64_t rows = 0, recs = 0;
   for (int b = 0; b < nb; ++b) {
     rows += Ns[b];
     recs += attend_ctas(Ns[b]);
   }
-  return carve_gen(p, nb, rows, recs, need_Q, need_H1, false, ws, cap, ok);
+  return carve_gen(p, nb, rows, recs, saves, false, ws, cap, ok);
 }
-static GenWs carve_gen_dev(const dsmil_params_t* p, int nb, int64_t max_rows, bool need_Q, bool need_H1, void* ws,
-                           size_t cap, bool* ok) {
-  return carve_gen(p, nb, nb * max_rows, static_cast<int64_t>(nb) * attend_ctas(max_rows), need_Q, need_H1, true, ws,
-                   cap, ok);
+static GenWs carve_gen_dev(const dsmil_params_t* p, int nb, int64_t max_rows, bool saves, void* ws, size_t cap,
+                           bool* ok) {
+  return carve_gen(p, nb, nb * max_rows, static_cast<int64_t>(nb) * attend_ctas(max_rows), saves, true, ws, cap, ok);
 }
 
 template <int CT>
@@ -564,14 +539,15 @@ static int launch_vproj_b(const dsmil_params_t* p, const sm90::BagDev* vtab, int
 
 // The generic forward over w.table: `tiles` and `recs` are the table's 128-row tiles and records and `rows` its packed
 // rows (dev calls: capacities, the live counts in w.plan); max_N bounds the bags' rows.  Q (and H1 for nonlinear q)
-// receive the Q-MLP's outputs row-major.  vtab (passing_v, value_forward_bags): nb entries of w.table's numbering whose
-// X is each bag's value input, then nb whose X is the bag's packed rows of V; V receives the value projection and the
+// receive the Q-MLP's outputs row-major.  w.vtab (passing_v, eager only): nb entries of w.table's numbering whose X is
+// each bag's value input, then nb whose X is the bag's packed rows of V; V receives the value projection and the
 // attend pass reads it through the second half.
 static int gen_forward_run(const dsmil_params_t* p, const GenWs& w, int nb, int64_t rows, int tiles, int recs,
                            int64_t max_N, float* classes, float* pred, float* A, float* B, int64_t* crit, float* Q,
-                           float* H1, cudaStream_t st, const sm90::BagDev* vtab = nullptr, float* V = nullptr) {
+                           float* H1, float* V, cudaStream_t st) {
   const int C = p->C, D = p->D;
   const BagsPlan* pl = w.plan;
+  const sm90::BagDev* vtab = w.vtab;
   int rc;
   DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * kMaxC * nb, st));
   if (sm90::qmlp_supported(p)) {
@@ -621,83 +597,123 @@ static int gen_forward_run(const dsmil_params_t* p, const GenWs& w, int nb, int6
   return 0;
 }
 
-// The eager generic forward: the table built on the host (each bag's MODE from its own alignment) and uploaded.
-// save_Q / save_H1: the training form's row-major Q and H1 (NULL: inference, into the workspace).
-static int forward_bags_gen(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb, float* classes,
-                            float* pred, float* A, float* B, int64_t* crit, float* save_Q, float* save_H1, void* ws,
-                            size_t ws_bytes, cudaStream_t st) {
+// The eager generic forward: the table built on the host (each bag's MODE from its own alignment) and uploaded, and for
+// passing_v the value table, whose X are the value inputs XVs (NULL: the features) and then each bag's packed rows of
+// V.  save_Q / save_H1 / save_V: the training forms' row-major saves, all given or all NULL (inference, into the
+// workspace).
+static int forward_bags_gen(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
+                            const int64_t* Ns, int nb, float* classes, float* pred, float* A, float* B, int64_t* crit,
+                            float* save_Q, float* save_H1, float* save_V, void* ws, size_t ws_bytes, cudaStream_t st) {
   bool ok;
-  GenWs w = carve_gen_eager(p, Ns, nb, !save_Q, p->nonlinear && !save_H1, ws, ws_bytes, &ok);
+  GenWs w = carve_gen_eager(p, Ns, nb, save_Q != nullptr, ws, ws_bytes, &ok);
   int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
   if (rc) return rc;
-  std::vector<sm90::BagDev> tbl(nb);
+  float* V = save_V ? save_V : w.V;
+  std::vector<sm90::BagDev> tbl(nb), vt(p->passing_v ? 2 * static_cast<size_t>(nb) : 0);
   long long row = 0;
   int tile = 0, rec = 0;
   int64_t mx = 1;
   for (int b = 0; b < nb; ++b) {
     tbl[b] = gen_bag_entry(Xs[b], Ns[b], p->D, row, tile, rec);
     mx = std::max<int64_t>(mx, Ns[b]);
+    if (p->passing_v) {
+      vt[b] = vt[nb + b] = tbl[b];
+      vt[b].X = XVs ? XVs[b] : Xs[b];
+      vt[nb + b].X = V + tbl[b].row_off * p->D;
+    }
   }
   DSMIL_CUDA_OK(cudaMemcpyAsync(w.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
+  if (p->passing_v)
+    DSMIL_CUDA_OK(cudaMemcpyAsync(w.vtab, vt.data(), sizeof(sm90::BagDev) * vt.size(), cudaMemcpyHostToDevice, st));
   return gen_forward_run(p, w, nb, row, tile, rec, mx, classes, pred, A, B, crit ? crit : w.crit,
-                         save_Q ? save_Q : w.Q, p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr, st);
+                         save_Q ? save_Q : w.Q, p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr, V, st);
 }
 
-// ---- batched forward of the value network (passing_v): the generic forward plus V, one launch per stage ------------
-// Phase 1 is the one dsmil_forward takes on the shape (k_qmlp_sm90 for nonlinear q with D % 128 == 0, else k_scores_b
-// and the FFMA Q-MLP), then one k_vproj_b for the V of every bag, and the attend pass over V.  Every bag's outputs and
-// saves are what dsmil_forward gives it alone (DESIGN §4.2i).
 static bool value_shape(const dsmil_params_t* p) {
   return p && p->passing_v && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D;
 }
 
-struct ValWs {
-  GenWs g;
-  sm90::BagDev* vtab;   // [2 nb]: the value inputs' table, then the packed V's (gen_forward_run)
-  float* V;             // [rows][D] where the caller keeps none
-  size_t bytes;
-};
-static ValWs carve_value(const dsmil_params_t* p, const int64_t* Ns, int nb, bool need_Q, bool need_H1, bool need_V,
-                         void* ws, size_t cap, bool* ok) {
-  ValWs w;
-  bool gok;
-  w.g = carve_gen_eager(p, Ns, nb, need_Q, need_H1, ws, cap, &gok);
-  Carver c(ws, cap);
-  c.off = w.g.bytes;
-  int64_t rows = 0;
-  for (int b = 0; b < nb; ++b) rows += Ns[b];
-  w.vtab = c.take<sm90::BagDev>(2 * static_cast<size_t>(nb));
-  w.V = need_V ? c.take<float>(rows * p->D) : nullptr;
-  w.bytes = c.off;
-  *ok = gok && c.ok();
-  return w;
+// ---- the route of an eager forward -----------------------------------------------------------------------------------
+// One rule for every eager forward of nb bags: the tensor-core batch where the shape takes it and every bag is 16-byte
+// aligned; off that batch (the generic shapes and passing_v) the generic batch, unless its phase 1 is k_qmlp_sm90 and
+// a bag is not aligned, or nb passes the 65535 bags its grids number in y and z; otherwise one bag at a time.
+enum Route : unsigned { ROUTE_TC = 1, ROUTE_GEN = 2, ROUTE_LOOP = 4 };
+static Route bags_route(const dsmil_params_t* p, int nb, bool aligned) {
+  if (sm90::batched_supported(p)) return aligned ? ROUTE_TC : ROUTE_LOOP;
+  return nb <= 65535 && (aligned || !sm90::qmlp_supported(p)) ? ROUTE_GEN : ROUTE_LOOP;
+}
+// The routes bags_route gives nb bags of this shape at either alignment.
+static unsigned bags_routes(const dsmil_params_t* p, int nb) {
+  return bags_route(p, nb, true) | bags_route(p, nb, false);
+}
+// The workspace of an eager forward of these bags that may take any of `routes` (Route bits): the largest of their
+// carves as inference takes them.  The loop's is the single-bag forward's carve for the largest bag.
+static size_t routes_ws_bytes(const dsmil_params_t* p, const int64_t* Ns, int nb, unsigned routes) {
+  bool ok;
+  size_t bytes = 0;
+  if (routes & ROUTE_TC) bytes = carve_bags(p, Ns, nb, true, false, nullptr, 0, &ok).bytes;
+  if (routes & ROUTE_GEN) bytes = std::max(bytes, carve_gen_eager(p, Ns, nb, false, nullptr, 0, &ok).bytes);
+  if (routes & ROUTE_LOOP) {
+    int64_t mx = 0;
+    for (int b = 0; b < nb; ++b) mx = std::max<int64_t>(mx, Ns[b]);
+    bytes = std::max(bytes, carve_fwd(p, mx, nullptr, 0, &ok).bytes);
+  }
+  return bytes;
 }
 
-static int value_forward_bags(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
-                              const int64_t* Ns, int nb, float* classes, float* pred, float* A, float* B, int64_t* crit,
-                              float* save_Q, float* save_H1, float* save_V, void* ws, size_t ws_bytes,
-                              cudaStream_t st) {
-  bool ok;
-  ValWs w = carve_value(p, Ns, nb, !save_Q, p->nonlinear && !save_H1, !save_V, ws, ws_bytes, &ok);
-  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
+// One bag: the tensor-core batch of one where bags_route takes it, else the single-bag kernels.
+static int forward_impl(const dsmil_params_t* p, const float* X, const float* xv, const float* classes_in,
+                        int64_t N, float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                        float* save_Q, float* save_H1, float* save_V, void* ws, size_t ws_bytes, cudaStream_t st) {
+  int rc = check_params(p, classes_in == nullptr);
   if (rc) return rc;
-  float* V = save_V ? save_V : w.V;
-  std::vector<sm90::BagDev> tbl(nb), vt(2 * static_cast<size_t>(nb));
-  long long row = 0;
-  int tile = 0, rec = 0;
-  int64_t mx = 1;
-  for (int b = 0; b < nb; ++b) {
-    tbl[b] = gen_bag_entry(Xs[b], Ns[b], p->D, row, tile, rec);
-    vt[b] = tbl[b];
-    vt[b].X = XVs ? XVs[b] : Xs[b];
-    vt[nb + b] = tbl[b];
-    vt[nb + b].X = V + tbl[b].row_off * p->D;
-    mx = std::max<int64_t>(mx, Ns[b]);
+  DSMIL_REQUIRE(N >= 0 && N < 0xffffffffll, "N=%lld out of range", (long long)N);
+  if (N == 0) {
+    set_error("empty bag (N == 0): the reference raises IndexError at dsmil.py:53");
+    return DSMIL_ERR_EMPTY;
   }
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.g.table, tbl.data(), sizeof(sm90::BagDev) * nb, cudaMemcpyHostToDevice, st));
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.vtab, vt.data(), sizeof(sm90::BagDev) * vt.size(), cudaMemcpyHostToDevice, st));
-  return gen_forward_run(p, w.g, nb, row, tile, rec, mx, classes, pred, A, B, crit ? crit : w.g.crit,
-                         save_Q ? save_Q : w.g.Q, p->nonlinear ? (save_H1 ? save_H1 : w.g.H1) : nullptr, st, w.vtab, V);
+  DSMIL_REQUIRE(X && pred && A && B && (classes || classes_in), "NULL tensor pointer");
+  if (bags_route(p, 1, (reinterpret_cast<uintptr_t>(X) & 15) == 0) == ROUTE_TC)
+    return forward_bags_impl(p, &X, &N, 1, classes_in, classes, pred, A, B, crit_idx, save_Q, save_H1, ws, ws_bytes, st);
+  bool ok;
+  FwdWs w = carve_fwd(p, N, ws, ws_bytes, &ok);
+  if ((rc = check_workspace(w.bytes, ok, ws, ws_bytes))) return rc;
+  float* Q = save_Q ? save_Q : w.Q;
+  float* H1 = p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr;
+  float* V = p->passing_v ? (save_V ? save_V : w.V) : nullptr;
+  if ((rc = phase1_impl(p, X, xv, classes_in, N, 0, classes, Q, H1, V, w.cand, w, st))) return rc;
+  int64_t* crit = crit_idx ? crit_idx : w.crit;
+  k_merge_cand<<<p->C, kQ, 0, st>>>(w.cand, 1, 1, p->C, w.qmax, crit);
+  DSMIL_LAUNCH_OK("k_merge_cand");
+  const float* Vv = p->passing_v ? V : X;
+  if ((rc = phase2_impl(p, Vv, Q, N, w.qmax, A, w.rec, w.recs, st))) return rc;
+  return phase3_impl(p, N, w.rec, A, B, pred, st);
+}
+
+// The eager forward of nb checked bags on their route: the tensor-core batch, the generic (passing_v: value) batch, or
+// forward_impl per bag into the same packed outputs.  XVs: passing_v's value inputs (NULL: the features).  save_Q /
+// save_H1 / save_V: the training forms' row-major saves, or NULL.
+static int forward_bags_route(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
+                              const int64_t* Ns, int nb, bool aligned, float* classes, float* pred, float* A,
+                              float* B, int64_t* crit, float* save_Q, float* save_H1, float* save_V, void* ws,
+                              size_t ws_bytes, cudaStream_t st) {
+  const Route r = bags_route(p, nb, aligned);
+  if (r == ROUTE_TC)
+    return forward_bags_impl(p, Xs, Ns, nb, nullptr, classes, pred, A, B, crit, save_Q, save_H1, ws, ws_bytes, st);
+  if (r == ROUTE_GEN)
+    return forward_bags_gen(p, Xs, XVs, Ns, nb, classes, pred, A, B, crit, save_Q, save_H1, save_V, ws, ws_bytes, st);
+  const int C = p->C, D = p->D;
+  int64_t row = 0;
+  for (int b = 0; b < nb; ++b) {
+    const int rc = forward_impl(p, Xs[b], XVs ? XVs[b] : nullptr, nullptr, Ns[b], classes + row * C,
+                                pred + static_cast<size_t>(b) * C, A + row * C, B + static_cast<size_t>(b) * C * D,
+                                crit ? crit + static_cast<size_t>(b) * C : nullptr,
+                                save_Q ? save_Q + row * kQ : nullptr, save_H1 ? save_H1 + row * kQ : nullptr,
+                                save_V ? save_V + row * D : nullptr, ws, ws_bytes, st);
+    if (rc) return rc;
+    row += Ns[b];
+  }
+  return 0;
 }
 
 }  // namespace dsmil
@@ -823,23 +839,15 @@ size_t dsmil_rec_floats(int32_t C, int32_t Dv) { return rec_floats(C, Dv); }
 
 size_t dsmil_forward_workspace_bytes(const dsmil_params_t* p, int64_t N) {
   if (!p || p->C < 1 || p->C > DSMIL_MAX_C || p->D < 1 || p->D > DSMIL_MAX_D || N < 0) return 0;
-  bool ok;
-  size_t a = carve_fwd(p, N, nullptr, 0, &ok).bytes;
-  if (sm90::batched_supported(p) && N > 0) a = std::max(a, carve_bags(p, &N, 1, true, false, nullptr, 0, &ok).bytes);
-  return a;
+  // forward_impl takes the rule's tensor-core batch of one bag, else the single-bag kernels (the loop's carve)
+  return routes_ws_bytes(p, &N, 1, ROUTE_LOOP | (N > 0 ? bags_routes(p, 1) & ROUTE_TC : 0));
 }
 
 size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
   if (!p || !Ns || nb < 1 || p->C < 1 || p->C > DSMIL_MAX_C || p->D < 1 || p->D > DSMIL_MAX_D) return 0;
-  bool ok;
-  // Even on a shape of the tensor-core batch, a bag that is not 16-byte aligned sends dsmil_forward_bags down the
-  // per-bag loop: the workspace must cover both layouts.
-  int64_t mx = 0;
-  for (int b = 0; b < nb; ++b) mx = std::max<int64_t>(mx, Ns[b]);
-  size_t bytes = carve_fwd(p, mx, nullptr, 0, &ok).bytes;
-  if (sm90::batched_supported(p)) bytes = std::max(bytes, carve_bags(p, Ns, nb, true, false, nullptr, 0, &ok).bytes);
-  if (gen_shape(p)) bytes = std::max(bytes, carve_gen_eager(p, Ns, nb, true, p->nonlinear, nullptr, 0, &ok).bytes);
-  return bytes;
+  // The rule's routes, and on every shape the loop's carve, on identity-v shapes the generic batch's at any nb: one
+  // size for the batch whatever its alignment and nb.
+  return routes_ws_bytes(p, Ns, nb, bags_routes(p, nb) | ROUTE_LOOP | (gen_shape(p) ? ROUTE_GEN : 0));
 }
 
 int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
@@ -848,30 +856,13 @@ int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const in
   int rc = check_params(p, true);
   if (rc) return rc;
   DSMIL_REQUIRE(Xs && Ns && nb >= 1 && classes && pred && A && B, "NULL pointer or nb < 1");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   int64_t total;
   bool aligned;
   if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
-  // one contract for both routes below: the size dsmil_forward_bags_workspace_bytes reports
-  const size_t need = dsmil_forward_bags_workspace_bytes(p, Ns, nb);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
-  if (sm90::batched_supported(p) && aligned)
-    return forward_bags_impl(p, Xs, Ns, nb, nullptr, classes, pred, A, B, crit_idx, nullptr, nullptr, workspace,
-                             workspace_bytes, st);
-  if (gen_shape(p) && (aligned || !sm90::qmlp_supported(p)))
-    return forward_bags_gen(p, Xs, Ns, nb, classes, pred, A, B, crit_idx, nullptr, nullptr, workspace, workspace_bytes,
-                            st);
-  // passing_v, and bags the batched routes do not take: same packed outputs, one bag at a time
-  int64_t row = 0;
-  for (int b = 0; b < nb; ++b) {
-    rc = forward_impl(p, Xs[b], nullptr, nullptr, Ns[b], classes + row * p->C, pred + static_cast<size_t>(b) * p->C,
-                      A + row * p->C, B + static_cast<size_t>(b) * p->C * p->D,
-                      crit_idx ? crit_idx + static_cast<size_t>(b) * p->C : nullptr, nullptr, nullptr, nullptr,
-                      workspace, workspace_bytes, st);
-    if (rc) return rc;
-    row += Ns[b];
-  }
-  return 0;
+  // one contract for every route: the size dsmil_forward_bags_workspace_bytes reports
+  if ((rc = need_workspace(dsmil_forward_bags_workspace_bytes(p, Ns, nb), workspace, workspace_bytes))) return rc;
+  return forward_bags_route(p, Xs, nullptr, Ns, nb, aligned, classes, pred, A, B, crit_idx, nullptr, nullptr, nullptr,
+                            workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 int32_t dsmil_forward_bags_phase1_ctas(int64_t tiles) { return tiles < 1 ? 0 : overlap_phase1_ctas(tiles); }
 
@@ -1021,7 +1012,7 @@ int dsmil_forward_bags_models(const dsmil_params_t* ps, int32_t M, const float* 
   bool aligned;
   if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
   const size_t need = dsmil_forward_bags_models_workspace_bytes(ps, M, Ns, nb);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
   if (aligned && dsmil_models_supported(ps, M) && static_cast<int64_t>(nb) * M <= 65535)
     return forward_bags_models_impl(ps, M, Xs, Ns, nb, total, classes, pred, A, B, crit_idx, workspace,
                                     workspace_bytes, st);
@@ -1667,29 +1658,12 @@ int dsmil_forward_bags_train(const dsmil_params_t* p, const float* const* Xs, co
   DSMIL_REQUIRE(!p->passing_v, "batched training supports the identity v only (passing_v: one bag per call)");
   DSMIL_REQUIRE(Xs && Ns && nb >= 1 && classes && pred && A && B && crit_idx && save_Q && (!p->nonlinear || save_H1),
                 "NULL pointer or nb < 1");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   int64_t total;
   bool aligned;
   if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
-  const size_t need = dsmil_forward_bags_train_workspace_bytes(p, Ns, nb);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
-  if (sm90::batched_supported(p) && aligned)
-    return forward_bags_impl(p, Xs, Ns, nb, nullptr, classes, pred, A, B, crit_idx, save_Q, save_H1, workspace,
-                             workspace_bytes, st);
-  if (gen_shape(p) && (aligned || !sm90::qmlp_supported(p)))
-    return forward_bags_gen(p, Xs, Ns, nb, classes, pred, A, B, crit_idx, save_Q, save_H1, workspace, workspace_bytes,
-                            st);
-  // bags the batched routes do not take: one bag at a time into the same packed buffers
-  int64_t row = 0;
-  for (int b = 0; b < nb; ++b) {
-    rc = forward_impl(p, Xs[b], nullptr, nullptr, Ns[b], classes + row * p->C, pred + static_cast<size_t>(b) * p->C,
-                      A + row * p->C, B + static_cast<size_t>(b) * p->C * p->D, crit_idx + static_cast<size_t>(b) * p->C,
-                      save_Q + row * kQ, save_H1 ? save_H1 + row * kQ : nullptr, nullptr, workspace, workspace_bytes,
-                      st);
-    if (rc) return rc;
-    row += Ns[b];
-  }
-  return 0;
+  if ((rc = need_workspace(dsmil_forward_bags_train_workspace_bytes(p, Ns, nb), workspace, workspace_bytes))) return rc;
+  return forward_bags_route(p, Xs, nullptr, Ns, nb, aligned, classes, pred, A, B, crit_idx, save_Q, save_H1, nullptr,
+                            workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 size_t dsmil_backward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb, int need_gX) {
@@ -1716,7 +1690,7 @@ int dsmil_backward_bags(const dsmil_params_t* p, const float* const* Xs, const i
   bool aligned;
   if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
   const size_t need = dsmil_backward_bags_workspace_bytes(p, Ns, nb, grads->gX != nullptr);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
   return backward_bags_impl(p, Xs, Ns, nb, total, aligned, Q, H1, A, B, crit_idx, d_classes, d_pred, d_A, d_B, grads,
                             workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
@@ -1783,7 +1757,7 @@ int dsmil_forward_bags_models_train(const dsmil_params_t* ps, int32_t M, const f
                 "NULL output pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t need = dsmil_forward_bags_models_train_workspace_bytes(ps, M, Ns, nbs);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
   const int C = ps[0].C, D = ps[0].D;
   if (mb.aligned && dsmil_models_supported(ps, M) && mb.ne <= 65535) {
     bool ok;
@@ -2092,7 +2066,7 @@ int dsmil_backward_bags_models(const dsmil_params_t* ps, int32_t M, const float*
   bool gX = false;
   for (int m = 0; m < M; ++m) gX = gX || grads[m].gX != nullptr;
   const size_t need = dsmil_backward_bags_models_workspace_bytes(ps, M, Ns, nbs, gX);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (bwd_models_fused(ps, M, Ns, nbs, mb.ne, mb.aligned))
     return backward_bags_models_impl(ps, M, Xs, Ns, nbs, mb, Q, H1, A, B, crit_idx, d_classes, d_pred, d_A, d_B, grads,
@@ -2238,20 +2212,61 @@ int dsmil_shard_backward_bags_phase3(const dsmil_params_t* p, const float* const
 
 
 // ---- capture-safe batched training: the bag list in device memory, every launch sized for a capacity -------------
-// What every dev call checks: the batched tensor-core shapes, the bag list and status (need_list: the calls that run
-// the planner), 1 <= nb <= 65535 and a row capacity whose 128-row tiles the kernels can number (an int).
-static int check_bags_dev(const dsmil_params_t* p, bool need_scores, bool need_list, const float* const* Xs,
+// Two routes (Route): the tensor-core batch (dsmil_*_dev, planned by k_plan_bags) and the generic shapes
+// (dsmil_generic_*_dev, planned by k_plan_bags_gen).  Each pair of calls shares one body.
+static bool dev_shape(Route r, const dsmil_params_t* p) {
+  return r == ROUTE_TC ? dsmil_shard_bags_supported(p) != 0 : dsmil_generic_bags_supported(p) != 0;
+}
+// The batch every dev call sizes: 1 <= nb <= 65535 bags of at most max_rows < 2^32 rows.
+static bool dev_sizes(int nb, int64_t max_rows) {
+  return nb >= 1 && nb <= 65535 && max_rows >= 1 && max_rows < 0xffffffffll;
+}
+// A dev call's workspace is never below the eager call's for the same capacity: one buffer serves both forms.
+static size_t not_below_eager(size_t dev, size_t (*eager)(const dsmil_params_t*, const int64_t*, int32_t),
+                              const dsmil_params_t* p, int nb, int64_t max_rows) {
+  const std::vector<int64_t> Ns(nb, max_rows);
+  return std::max(dev, eager(p, Ns.data(), nb));
+}
+
+// What every dev call checks: the route's shapes, the bag list and status (need_list: the calls that run the planner),
+// 1 <= nb <= 65535 and a row capacity whose 128-row tiles the kernels can number in an int (twice over on the generic
+// route, for k_linear_b's grid).
+static int check_bags_dev(Route r, const dsmil_params_t* p, bool need_scores, bool need_list, const float* const* Xs,
                           const int64_t* Ns, int nb, int64_t max_rows, const int32_t* status) {
   int rc = check_params(p, need_scores);
   if (rc) return rc;
-  DSMIL_REQUIRE(dsmil_shard_bags_supported(p),
-                "shape not supported by the batched tensor-core path (D=%d, C=%d, nonlinear=%d, passing_v=%d)", p->D,
-                p->C, p->nonlinear, p->passing_v);
+  if (r == ROUTE_TC)
+    DSMIL_REQUIRE(dsmil_shard_bags_supported(p),
+                  "shape not supported by the batched tensor-core path (D=%d, C=%d, nonlinear=%d, passing_v=%d)", p->D,
+                  p->C, p->nonlinear, p->passing_v);
+  else
+    DSMIL_REQUIRE(dsmil_generic_bags_supported(p),
+                  "shape not on the generic batched route, i.e. identity v off dsmil_shard_bags_supported (D=%d, C=%d, "
+                  "nonlinear=%d, passing_v=%d)", p->D, p->C, p->nonlinear, p->passing_v);
   DSMIL_REQUIRE(!need_list || (Xs && Ns && status), "NULL bag list or status");
   DSMIL_REQUIRE(nb >= 1 && nb <= 65535, "nb=%d outside [1, 65535]", nb);
   DSMIL_REQUIRE(max_rows >= 1 && max_rows < 0xffffffffll &&
-                static_cast<int64_t>(nb) * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) <= INT_MAX,
+                (r == ROUTE_TC ? 1 : 2) * static_cast<int64_t>(nb) * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) <=
+                    INT_MAX,
                 "max_rows=%lld out of range for nb=%d", (long long)max_rows, nb);
+  return 0;
+}
+
+// The route's planner over the device bag list: the table, the live counts and, when chi / ch1 are non-NULL, the
+// backward's chunk tables.
+static int launch_plan_dev(Route r, const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
+                           int64_t max_rows, float* zero_row, sm90::BagDev* table, TnChunk* chi, TnChunk* ch1,
+                           BagsPlan* plan, int32_t* status, cudaStream_t st) {
+  if (r == ROUTE_TC) {
+    k_plan_bags<<<1, 32, 0, st>>>(Xs, Ns, nb, max_rows, p->C, p->D, zero_row, table, chi, ch1, plan, status, nullptr,
+                                  nullptr);
+    DSMIL_LAUNCH_OK("k_plan_bags");
+  } else {
+    // the alignment rule (gen_bag_aligned) keeps each form the eager call would choose: gWi streams (tn_use_gemv) only
+    // where D % 4 == 0, and there the bags are 16-byte aligned
+    k_plan_bags_gen<<<1, 32, 0, st>>>(Xs, Ns, nb, max_rows, p->C, p->D, zero_row, table, chi, ch1, plan, status);
+    DSMIL_LAUNCH_OK("k_plan_bags_gen");
+  }
   return 0;
 }
 
@@ -2286,222 +2301,161 @@ static int bags_phase1_dev(const dsmil_params_t* p, const BagsWs& w, const BagsP
                            overlap ? w.done : nullptr);
 }
 
-size_t dsmil_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
-  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
+// The forward pair's size: train keeps Q (+ H1) in the caller's saves, inference in the workspace.
+static size_t forward_bags_dev_ws(Route r, bool train, const dsmil_params_t* p, int nb, int64_t max_rows) {
+  if (!dev_shape(r, p) || !dev_sizes(nb, max_rows)) return 0;
   bool ok;
-  BagsPlan* plan;
-  float* zero_row;
-  const size_t dev = carve_bags_dev(p, nb, max_rows, false, false, nullptr, 0, &ok, &plan, &zero_row).bytes;
-  // never below the eager call's size for the same capacity: one buffer serves both forms
-  const std::vector<int64_t> Ns(nb, max_rows);
-  return std::max(dev, dsmil_forward_bags_train_workspace_bytes(p, Ns.data(), nb));
+  size_t dev;
+  if (r == ROUTE_TC) {
+    BagsPlan* plan;
+    float* zero_row;
+    dev = carve_bags_dev(p, nb, max_rows, !train, false, nullptr, 0, &ok, &plan, &zero_row).bytes;
+  } else {
+    dev = carve_gen_dev(p, nb, max_rows, train, nullptr, 0, &ok).bytes;
+  }
+  return not_below_eager(dev, train ? dsmil_forward_bags_train_workspace_bytes : dsmil_forward_bags_workspace_bytes, p,
+                         nb, max_rows);
 }
 
+// The forward pair's body: the planner writes the table and the live counts, then the route's forward runs on the
+// capacity grids.  train: Q (+ H1) into save_Q (save_H1).  Inference keeps Q in the workspace (tile blocks on the
+// tensor-core route), and there the attend pass is a programmatic dependent of phase 1 as in dsmil_forward_bags --
+// under stream capture too, where the launch attribute becomes a programmatic edge of the graph (DESIGN §4.3).  Only
+// kernel timing keeps the plain launch.
+static int forward_bags_dev(Route r, bool train, const dsmil_params_t* p, const float* const* Xs_dev,
+                            const int64_t* Ns_dev, int nb, int64_t max_rows, float* classes, float* pred, float* A,
+                            float* B, int64_t* crit_idx, float* save_Q, float* save_H1, int32_t* status,
+                            void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  int rc = check_bags_dev(r, p, true, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(classes && pred && A && B && (!train || (crit_idx && save_Q && (!p->nonlinear || save_H1))),
+                "NULL output pointer");
+  if ((rc = need_workspace(forward_bags_dev_ws(r, train, p, nb, max_rows), workspace, workspace_bytes))) return rc;
+  bool ok;
+  if (r == ROUTE_GEN) {
+    GenWs w = carve_gen_dev(p, nb, max_rows, train, workspace, workspace_bytes, &ok);
+    if ((rc = launch_plan_dev(r, p, Xs_dev, Ns_dev, nb, max_rows, w.zero_row, w.table, nullptr, nullptr, w.plan, status,
+                              st)))
+      return rc;
+    return gen_forward_run(p, w, nb, nb * max_rows, nb * tiles_for_bag(max_rows), nb * attend_ctas(max_rows), max_rows,
+                           classes, pred, A, B, crit_idx ? crit_idx : w.crit, train ? save_Q : w.Q,
+                           p->nonlinear ? (train ? save_H1 : w.H1) : nullptr, nullptr, st);
+  }
+  BagsPlan* plan;
+  float* zero_row;
+  BagsWs w = carve_bags_dev(p, nb, max_rows, !train, false, workspace, workspace_bytes, &ok, &plan, &zero_row);
+  if ((rc = launch_plan_dev(r, p, Xs_dev, Ns_dev, nb, max_rows, zero_row, w.table, nullptr, nullptr, plan, status, st)))
+    return rc;
+  const bool overlap = !train && !g_prof_on;
+  float* Q = train ? save_Q : w.Q;
+  if ((rc = bags_phase1_dev(p, w, plan, nb, max_rows, classes, Q, train ? save_H1 : nullptr, st, !train, overlap)))
+    return rc;
+  return bags_attend_finalize(p, w, nb, Q, !train, pred, A, B, crit_idx, nb * recs_for_bag(max_rows), &plan->recs, st,
+                              overlap);
+}
+
+// The backward pair's size.  The generic route also covers the eager backward's carve.
+static size_t backward_bags_dev_ws(Route r, const dsmil_params_t* p, int nb, int64_t max_rows) {
+  if (!dev_shape(r, p) || !dev_sizes(nb, max_rows)) return 0;
+  bool ok;
+  const size_t dev = carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
+  if (r == ROUTE_TC) return dev;
+  return not_below_eager(dev, [](const dsmil_params_t* q, const int64_t* Ns, int32_t n) {
+    return dsmil_backward_bags_workspace_bytes(q, Ns, n, 0);
+  }, p, nb, max_rows);
+}
+
+// The backward pair's body: the planner writes the bag and chunk tables, then the three phases run on the capacity
+// grids.
+static int backward_bags_dev(Route r, const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
+                             int nb, int64_t max_rows, const float* Q, const float* H1, const float* A, const float* B,
+                             const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
+                             const float* d_B, const dsmil_grads_t* grads, int32_t* status, void* workspace,
+                             size_t workspace_bytes, cudaStream_t st) {
+  int rc = check_bags_dev(r, p, false, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  if (rc) return rc;
+  DSMIL_REQUIRE(Q && (!p->nonlinear || H1) && A && B && crit_idx && grads, "NULL pointer");
+  DSMIL_REQUIRE(!d_A && !d_B && !grads->gX,
+                "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
+  if ((rc = need_workspace(backward_bags_dev_ws(r, p, nb, max_rows), workspace, workspace_bytes))) return rc;
+  bool ok;
+  BwdBagsWs w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
+  if ((rc = launch_plan_dev(r, p, Xs_dev, Ns_dev, nb, max_rows, w.zero_row, w.table, w.chi, w.ch1, w.plan, status,
+                            st)))
+    return rc;
+  return backward_bags_run(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, A, B, crit_idx,
+                           d_classes, d_pred, nullptr, nullptr, grads, w, st);
+}
+
+size_t dsmil_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  return forward_bags_dev_ws(ROUTE_TC, true, p, nb, max_rows);
+}
 int dsmil_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
                                  int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
                                  int64_t* crit_idx, float* save_Q, float* save_H1, int32_t* status, void* workspace,
                                  size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, true, true, Xs_dev, Ns_dev, nb, max_rows, status);
-  if (rc) return rc;
-  DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && save_H1, "NULL output pointer");
-  const size_t need = dsmil_forward_bags_train_dev_workspace_bytes(p, nb, max_rows);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  bool ok;
-  BagsPlan* plan;
-  float* zero_row;
-  BagsWs w = carve_bags_dev(p, nb, max_rows, false, false, workspace, workspace_bytes, &ok, &plan, &zero_row);
-  k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, zero_row, w.table, nullptr, nullptr, plan,
-                                status, nullptr, nullptr);
-  DSMIL_LAUNCH_OK("k_plan_bags");
-  if ((rc = bags_phase1_dev(p, w, plan, nb, max_rows, classes, save_Q, save_H1, st))) return rc;
-  return bags_attend_finalize(p, w, nb, save_Q, false, pred, A, B, crit_idx, nb * recs_for_bag(max_rows), &plan->recs,
-                              st);
+  return forward_bags_dev(ROUTE_TC, true, p, Xs_dev, Ns_dev, nb, max_rows, classes, pred, A, B, crit_idx, save_Q,
+                          save_H1, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 size_t dsmil_forward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
-  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
-  bool ok;
-  BagsPlan* plan;
-  float* zero_row;
-  const size_t dev = carve_bags_dev(p, nb, max_rows, true, false, nullptr, 0, &ok, &plan, &zero_row).bytes;
-  const std::vector<int64_t> Ns(nb, max_rows);
-  return std::max(dev, dsmil_forward_bags_workspace_bytes(p, Ns.data(), nb));
+  return forward_bags_dev_ws(ROUTE_TC, false, p, nb, max_rows);
 }
-
-// The inference twin of dsmil_forward_bags_train_dev: Q stays in the workspace as tile blocks, and the attend pass is
-// a programmatic dependent of phase 1 as in dsmil_forward_bags -- under stream capture too, where the launch attribute
-// becomes a programmatic edge of the graph (DESIGN §4.3).  Only kernel timing keeps the plain launch.
 int dsmil_forward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev, int32_t nb,
                            int64_t max_rows, float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
                            int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, true, true, Xs_dev, Ns_dev, nb, max_rows, status);
-  if (rc) return rc;
-  DSMIL_REQUIRE(classes && pred && A && B, "NULL output pointer");
-  const size_t need = dsmil_forward_bags_dev_workspace_bytes(p, nb, max_rows);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  bool ok;
-  BagsPlan* plan;
-  float* zero_row;
-  BagsWs w = carve_bags_dev(p, nb, max_rows, true, false, workspace, workspace_bytes, &ok, &plan, &zero_row);
-  k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, zero_row, w.table, nullptr, nullptr, plan,
-                                status, nullptr, nullptr);
-  DSMIL_LAUNCH_OK("k_plan_bags");
-  const bool overlap = !g_prof_on;
-  if ((rc = bags_phase1_dev(p, w, plan, nb, max_rows, classes, w.Q, nullptr, st, true, overlap))) return rc;
-  return bags_attend_finalize(p, w, nb, w.Q, true, pred, A, B, crit_idx, nb * recs_for_bag(max_rows), &plan->recs, st,
-                              overlap);
+  return forward_bags_dev(ROUTE_TC, false, p, Xs_dev, Ns_dev, nb, max_rows, classes, pred, A, B, crit_idx, nullptr,
+                          nullptr, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 size_t dsmil_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
-  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
-  bool ok;
-  return carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
+  return backward_bags_dev_ws(ROUTE_TC, p, nb, max_rows);
 }
-
 int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev, int32_t nb,
                             int64_t max_rows, const float* Q, const float* H1, const float* A, const float* B,
                             const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
                             const float* d_B, const dsmil_grads_t* grads, int32_t* status, void* workspace,
                             size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, false, true, Xs_dev, Ns_dev, nb, max_rows, status);
-  if (rc) return rc;
-  DSMIL_REQUIRE(Q && H1 && A && B && crit_idx && grads, "NULL pointer");
-  DSMIL_REQUIRE(!d_A && !d_B && !grads->gX,
-                "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
-  const size_t need = dsmil_backward_bags_dev_workspace_bytes(p, nb, max_rows);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  bool ok;
-  BwdBagsWs w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
-  k_plan_bags<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, w.zero_row, w.table, w.chi, w.ch1, w.plan,
-                                status, nullptr, nullptr);
-  DSMIL_LAUNCH_OK("k_plan_bags");
-  return backward_bags_run(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, A, B, crit_idx,
-                           d_classes, d_pred, nullptr, nullptr, grads, w, st);
+  return backward_bags_dev(ROUTE_TC, p, Xs_dev, Ns_dev, nb, max_rows, Q, H1, A, B, crit_idx, d_classes, d_pred, d_A,
+                           d_B, grads, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
-// ---- capture-safe calls on the generic shapes: the dev calls' contract, planned by k_plan_bags_gen ----------------
 int dsmil_generic_bags_supported(const dsmil_params_t* p) {
   return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && gen_shape(p)) ? 1 : 0;
 }
 
-}  // extern "C"
-namespace dsmil {
-// check_bags_dev of the generic calls: their shapes, and a capacity whose 128-row tiles k_linear_b's grid can number
-// twice over in an int.
-static int check_generic_dev(const dsmil_params_t* p, bool need_scores, const float* const* Xs, const int64_t* Ns,
-                             int nb, int64_t max_rows, const int32_t* status) {
-  int rc = check_params(p, need_scores);
-  if (rc) return rc;
-  DSMIL_REQUIRE(dsmil_generic_bags_supported(p),
-                "shape not on the generic batched route, i.e. identity v off dsmil_shard_bags_supported (D=%d, C=%d, "
-                "nonlinear=%d, passing_v=%d)", p->D, p->C, p->nonlinear, p->passing_v);
-  DSMIL_REQUIRE(Xs && Ns && status, "NULL bag list or status");
-  DSMIL_REQUIRE(nb >= 1 && nb <= 65535, "nb=%d outside [1, 65535]", nb);
-  DSMIL_REQUIRE(max_rows >= 1 && max_rows < 0xffffffffll &&
-                2 * static_cast<int64_t>(nb) * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) <= INT_MAX,
-                "max_rows=%lld out of range for nb=%d", (long long)max_rows, nb);
-  return 0;
-}
-static bool generic_dev_sizes(const dsmil_params_t* p, int nb, int64_t max_rows) {
-  return dsmil_generic_bags_supported(p) && nb >= 1 && nb <= 65535 && max_rows >= 1 && max_rows < 0xffffffffll;
-}
-
-// The generic shapes' dev forward: k_plan_bags_gen writes the table and the live counts, then the generic forward runs
-// on the capacity grids.  save_Q == NULL: inference (Q and H1 in the workspace).
-static int forward_bags_gen_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev, int nb,
-                                int64_t max_rows, float* classes, float* pred, float* A, float* B, int64_t* crit,
-                                float* save_Q, float* save_H1, int32_t* status, void* ws, size_t ws_bytes,
-                                cudaStream_t st) {
-  bool ok;
-  GenWs w = carve_gen_dev(p, nb, max_rows, !save_Q, p->nonlinear && !save_H1, ws, ws_bytes, &ok);
-  int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
-  if (rc) return rc;
-  k_plan_bags_gen<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, w.zero_row, w.table, nullptr, nullptr,
-                                    w.plan, status);
-  DSMIL_LAUNCH_OK("k_plan_bags_gen");
-  return gen_forward_run(p, w, nb, nb * max_rows, nb * tiles_for_bag(max_rows), nb * attend_ctas(max_rows), max_rows,
-                         classes, pred, A, B, crit ? crit : w.crit, save_Q ? save_Q : w.Q,
-                         p->nonlinear ? (save_H1 ? save_H1 : w.H1) : nullptr, st);
-}
-}  // namespace dsmil
-extern "C" {
-
 size_t dsmil_generic_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
-  if (!generic_dev_sizes(p, nb, max_rows)) return 0;
-  bool ok;
-  const size_t dev = carve_gen_dev(p, nb, max_rows, false, false, nullptr, 0, &ok).bytes;
-  // never below the eager call's size for the same capacity: one buffer serves both forms
-  const std::vector<int64_t> Ns(nb, max_rows);
-  return std::max(dev, dsmil_forward_bags_train_workspace_bytes(p, Ns.data(), nb));
+  return forward_bags_dev_ws(ROUTE_GEN, true, p, nb, max_rows);
 }
-
 int dsmil_generic_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
                                          int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
                                          int64_t* crit_idx, float* save_Q, float* save_H1, int32_t* status,
                                          void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = check_generic_dev(p, true, Xs_dev, Ns_dev, nb, max_rows, status);
-  if (rc) return rc;
-  DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && (!p->nonlinear || save_H1), "NULL output pointer");
-  const size_t need = dsmil_generic_forward_bags_train_dev_workspace_bytes(p, nb, max_rows);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
-  return forward_bags_gen_dev(p, Xs_dev, Ns_dev, nb, max_rows, classes, pred, A, B, crit_idx, save_Q, save_H1, status,
-                              workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+  return forward_bags_dev(ROUTE_GEN, true, p, Xs_dev, Ns_dev, nb, max_rows, classes, pred, A, B, crit_idx, save_Q,
+                          save_H1, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 size_t dsmil_generic_forward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
-  if (!generic_dev_sizes(p, nb, max_rows)) return 0;
-  bool ok;
-  const size_t dev = carve_gen_dev(p, nb, max_rows, true, p->nonlinear, nullptr, 0, &ok).bytes;
-  const std::vector<int64_t> Ns(nb, max_rows);
-  return std::max(dev, dsmil_forward_bags_workspace_bytes(p, Ns.data(), nb));
+  return forward_bags_dev_ws(ROUTE_GEN, false, p, nb, max_rows);
 }
-
 int dsmil_generic_forward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
                                    int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
                                    int64_t* crit_idx, int32_t* status, void* workspace, size_t workspace_bytes,
                                    void* stream) {
-  int rc = check_generic_dev(p, true, Xs_dev, Ns_dev, nb, max_rows, status);
-  if (rc) return rc;
-  DSMIL_REQUIRE(classes && pred && A && B, "NULL output pointer");
-  const size_t need = dsmil_generic_forward_bags_dev_workspace_bytes(p, nb, max_rows);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
-  return forward_bags_gen_dev(p, Xs_dev, Ns_dev, nb, max_rows, classes, pred, A, B, crit_idx, nullptr, nullptr, status,
-                              workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+  return forward_bags_dev(ROUTE_GEN, false, p, Xs_dev, Ns_dev, nb, max_rows, classes, pred, A, B, crit_idx, nullptr,
+                          nullptr, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 size_t dsmil_generic_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
-  if (!generic_dev_sizes(p, nb, max_rows)) return 0;
-  bool ok;
-  const size_t dev = carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
-  const std::vector<int64_t> Ns(nb, max_rows);
-  return std::max(dev, dsmil_backward_bags_workspace_bytes(p, Ns.data(), nb, 0));
+  return backward_bags_dev_ws(ROUTE_GEN, p, nb, max_rows);
 }
-
 int dsmil_generic_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
                                     int32_t nb, int64_t max_rows, const float* Q, const float* H1, const float* A,
                                     const float* B, const int64_t* crit_idx, const float* d_classes,
                                     const float* d_pred, const float* d_A, const float* d_B, const dsmil_grads_t* grads,
                                     int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = check_generic_dev(p, false, Xs_dev, Ns_dev, nb, max_rows, status);
-  if (rc) return rc;
-  DSMIL_REQUIRE(Q && (!p->nonlinear || H1) && A && B && crit_idx && grads, "NULL pointer");
-  DSMIL_REQUIRE(!d_A && !d_B && !grads->gX,
-                "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
-  const size_t need = dsmil_generic_backward_bags_dev_workspace_bytes(p, nb, max_rows);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  bool ok;
-  BwdBagsWs w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
-  // the alignment rule (gen_bag_aligned) keeps each form the eager call would choose: gWi streams (tn_use_gemv) only
-  // where D % 4 == 0, and there the bags are 16-byte aligned
-  k_plan_bags_gen<<<1, 32, 0, st>>>(Xs_dev, Ns_dev, nb, max_rows, p->C, p->D, w.zero_row, w.table, w.chi, w.ch1,
-                                    w.plan, status);
-  DSMIL_LAUNCH_OK("k_plan_bags_gen");
-  return backward_bags_run(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, Q, H1, A, B, crit_idx,
-                           d_classes, d_pred, nullptr, nullptr, grads, w, st);
+  return backward_bags_dev(ROUTE_GEN, p, Xs_dev, Ns_dev, nb, max_rows, Q, H1, A, B, crit_idx, d_classes, d_pred, d_A,
+                           d_B, grads, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 // ---- capture-safe fold step: M models, each over its own device bag list ------------------------------------------
@@ -2513,12 +2467,12 @@ struct ModelsDevCaps {
   int64_t max_model_rows;     // row capacity of the largest model
 };
 static bool models_dev_caps(const dsmil_params_t* ps, int M, const int32_t* nbs, int64_t max_rows, ModelsDevCaps* c) {
-  if (!ps || !nbs || !dsmil_models_supported(ps, M) || max_rows < 1 || max_rows >= 0xffffffffll) return false;
+  if (!ps || !nbs || !dsmil_models_supported(ps, M)) return false;
   const int C = ps[0].C, D = ps[0].D;
   int64_t ne = 0, nci = 0, nc1 = 0;
   *c = ModelsDevCaps{0, 1, 0, 0, M * kModelSplitsCap, M * kModelSplitsCap, 1};
   for (int m = 0; m < M; ++m) {
-    if (nbs[m] < 1 || nbs[m] > 65535) return false;
+    if (!dev_sizes(nbs[m], max_rows)) return false;
     ne += nbs[m];
     nci += rag_chunks_cap(C, D, tn_use_gemv(C, D), nbs[m]);
     nc1 += rag_chunks_cap(kQ, D, false, nbs[m]);
@@ -2604,7 +2558,7 @@ int dsmil_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, con
   if (rc) return rc;
   DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && save_H1, "NULL output pointer");
   const size_t need = dsmil_forward_bags_models_train_dev_workspace_bytes(ps, M, nbs, max_rows);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int C = ps[0].C, D = ps[0].D, ne = caps.ne;
   bool ok;
@@ -2682,7 +2636,7 @@ int dsmil_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const fl
   DSMIL_REQUIRE(!d_A && !d_B && !gX,
                 "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
   const size_t need = dsmil_backward_bags_models_dev_workspace_bytes(ps, M, nbs, max_rows);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
+  if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int C = ps[0].C, D = ps[0].D;
   bool ok;
@@ -2719,20 +2673,19 @@ int dsmil_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const fl
 // counts the planner writes, no host<->device traffic.  Forward phases 2 and 3 read phase 1's table and counts from the
 // forward workspace, backward phases 2 and 3 read backward phase 1's from the backward workspace.
 size_t dsmil_shard_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
-  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
+  if (!dev_shape(ROUTE_TC, p) || !dev_sizes(nb, max_rows)) return 0;
   bool ok;
   BagsPlan* plan;
   float* zero_row;
   const size_t dev = carve_bags_dev(p, nb, max_rows, false, true, nullptr, 0, &ok, &plan, &zero_row).bytes;
-  const std::vector<int64_t> Ns(nb, max_rows);
-  return std::max(dev, dsmil_shard_bags_workspace_bytes(p, Ns.data(), nb));
+  return not_below_eager(dev, dsmil_shard_bags_workspace_bytes, p, nb, max_rows);
 }
 
 // The forward workspace of a sharded dev call, after its checks.
 static int shard_bags_dev_ws(const dsmil_params_t* p, int nb, int64_t max_rows, void* workspace,
                              size_t workspace_bytes, BagsWs* w, BagsPlan** plan, float** zero_row) {
   const size_t need = dsmil_shard_bags_train_dev_workspace_bytes(p, nb, max_rows);
-  int rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0);
+  int rc = need_workspace(need, workspace, workspace_bytes);
   if (rc) return rc;
   bool ok;
   *w = carve_bags_dev(p, nb, max_rows, false, true, workspace, workspace_bytes, &ok, plan, zero_row);
@@ -2743,7 +2696,7 @@ int dsmil_shard_bags_phase1_train_dev(const dsmil_params_t* p, const float* cons
                                       const int64_t* row_offsets_dev, int32_t nb, int64_t max_rows, float* classes,
                                       float* save_Q, float* save_H1, float* cand_recs, int32_t* status,
                                       void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, true, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  int rc = check_bags_dev(ROUTE_TC, p, true, true, Xs_dev, Ns_dev, nb, max_rows, status);
   if (rc) return rc;
   DSMIL_REQUIRE(row_offsets_dev && classes && save_Q && save_H1 && cand_recs, "NULL pointer");
   BagsWs w;
@@ -2764,7 +2717,7 @@ int dsmil_shard_bags_phase1_train_dev(const dsmil_params_t* p, const float* cons
 int dsmil_shard_bags_phase2_train_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows, const float* Q,
                                       const float* cands_all, int32_t G, float* A, int64_t* crit_idx, float* q_max,
                                       float* recs_out, void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, true, false, nullptr, nullptr, nb, max_rows, nullptr);
+  int rc = check_bags_dev(ROUTE_TC, p, true, false, nullptr, nullptr, nb, max_rows, nullptr);
   if (rc) return rc;
   DSMIL_REQUIRE(Q && cands_all && G >= 1 && A && crit_idx && q_max && recs_out, "NULL pointer or G < 1");
   BagsWs w;
@@ -2778,7 +2731,7 @@ int dsmil_shard_bags_phase2_train_dev(const dsmil_params_t* p, int32_t nb, int64
 int dsmil_shard_bags_phase3_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows, const float* recs_all,
                                 int32_t G, float* A, float* B, float* pred, void* workspace, size_t workspace_bytes,
                                 void* stream) {
-  int rc = check_bags_dev(p, true, false, nullptr, nullptr, nb, max_rows, nullptr);
+  int rc = check_bags_dev(ROUTE_TC, p, true, false, nullptr, nullptr, nb, max_rows, nullptr);
   if (rc) return rc;
   DSMIL_REQUIRE(recs_all && G >= 1 && G <= sm90::kMaxRecPerBag && A && B && pred, "NULL pointer or G out of range");
   BagsWs w;
@@ -2791,18 +2744,17 @@ int dsmil_shard_bags_phase3_dev(const dsmil_params_t* p, int32_t nb, int64_t max
 }
 
 size_t dsmil_shard_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
-  if (!dsmil_shard_bags_supported(p) || nb < 1 || nb > 65535 || max_rows < 1 || max_rows >= 0xffffffffll) return 0;
+  if (!dev_shape(ROUTE_TC, p) || !dev_sizes(nb, max_rows)) return 0;
   bool ok;
   const size_t dev = carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
-  const std::vector<int64_t> Ns(nb, max_rows);
-  return std::max(dev, dsmil_shard_backward_bags_workspace_bytes(p, Ns.data(), nb));
+  return not_below_eager(dev, dsmil_shard_backward_bags_workspace_bytes, p, nb, max_rows);
 }
 
 // The backward workspace of a sharded dev call, after its checks.
 static int shard_bwd_bags_dev_ws(const dsmil_params_t* p, int nb, int64_t max_rows, void* workspace,
                                  size_t workspace_bytes, BwdBagsWs* w) {
   const size_t need = dsmil_shard_backward_bags_dev_workspace_bytes(p, nb, max_rows);
-  int rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0);
+  int rc = need_workspace(need, workspace, workspace_bytes);
   if (rc) return rc;
   bool ok;
   *w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
@@ -2814,7 +2766,7 @@ int dsmil_shard_backward_bags_phase1_dev(const dsmil_params_t* p, const float* c
                                          const float* d_classes_local, const float* d_pred, float* dA_local,
                                          float* t_local, float* gWi, float* gbi, float* gWf, float* gbf,
                                          int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, false, true, Xs_dev, Ns_dev, nb, max_rows, status);
+  int rc = check_bags_dev(ROUTE_TC, p, false, true, Xs_dev, Ns_dev, nb, max_rows, status);
   if (rc) return rc;
   DSMIL_REQUIRE(A && B && dA_local && t_local, "NULL tensor pointer");
   BwdBagsWs w;
@@ -2837,7 +2789,7 @@ int dsmil_shard_backward_bags_phase1_dev(const dsmil_params_t* p, const float* c
 int dsmil_shard_backward_bags_phase2_dev(const dsmil_params_t* p, int32_t nb, int64_t max_rows, const float* A,
                                          float* dA_to_dL, const float* t_global, const float* Q, float* dqm_local,
                                          void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, false, false, nullptr, nullptr, nb, max_rows, nullptr);
+  int rc = check_bags_dev(ROUTE_TC, p, false, false, nullptr, nullptr, nb, max_rows, nullptr);
   if (rc) return rc;
   DSMIL_REQUIRE(A && dA_to_dL && t_global && Q && dqm_local, "NULL tensor pointer");
   BwdBagsWs w;
@@ -2853,7 +2805,7 @@ int dsmil_shard_backward_bags_phase3_dev(const dsmil_params_t* p, int32_t nb, in
                                          const float* dL_local, const float* dqm_global, const float* q_max,
                                          const int64_t* crit_idx, float* gW1, float* gb1, float* gW2, float* gb2,
                                          void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = check_bags_dev(p, false, false, nullptr, nullptr, nb, max_rows, nullptr);
+  int rc = check_bags_dev(ROUTE_TC, p, false, false, nullptr, nullptr, nb, max_rows, nullptr);
   if (rc) return rc;
   DSMIL_REQUIRE(row_offsets_dev && Q && H1 && dL_local && dqm_global && q_max && crit_idx, "NULL tensor pointer");
   BwdBagsWs w;
@@ -2872,15 +2824,9 @@ int dsmil_value_bags_supported(const dsmil_params_t* p) {
 
 size_t dsmil_value_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
   if (!dsmil_value_bags_supported(p) || !Ns || nb < 1 || nb > 65535) return 0;
-  int64_t mx = 0;
-  for (int b = 0; b < nb; ++b) {
+  for (int b = 0; b < nb; ++b)
     if (Ns[b] < 1 || Ns[b] >= 0xffffffffll) return 0;
-    mx = std::max<int64_t>(mx, Ns[b]);
-  }
-  bool ok;
-  // nonlinear q with D % 128 == 0 loops the single-bag forward when a bag is not 16-byte aligned
-  const size_t loop = sm90::qmlp_supported(p) ? carve_fwd(p, mx, nullptr, 0, &ok).bytes : 0;
-  return std::max(loop, carve_value(p, Ns, nb, true, p->nonlinear, true, nullptr, 0, &ok).bytes);
+  return routes_ws_bytes(p, Ns, nb, bags_routes(p, nb));
 }
 
 int dsmil_value_forward_bags(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
@@ -2895,29 +2841,13 @@ int dsmil_value_forward_bags(const dsmil_params_t* p, const float* const* Xs, co
   const bool saves = save_Q || save_H1 || save_V;
   DSMIL_REQUIRE(!saves || (save_Q && save_V && (!p->nonlinear || save_H1)),
                 "saves: save_Q, save_V (and save_H1 for a nonlinear q) together, or none");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   int64_t total;
   bool aligned;
   if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
   for (int b = 0; XVs && b < nb; ++b) DSMIL_REQUIRE(XVs[b], "bag %d: NULL value input", b);
-  const size_t need = dsmil_value_forward_bags_workspace_bytes(p, Ns, nb);
-  if ((rc = check_workspace(need, workspace_bytes >= need, workspace, workspace ? workspace_bytes : 0))) return rc;
-  if (aligned || !sm90::qmlp_supported(p))
-    return value_forward_bags(p, Xs, XVs, Ns, nb, classes, pred, A, B, crit_idx, save_Q, save_H1, save_V, workspace,
-                              workspace_bytes, st);
-  // k_qmlp_sm90 reads 16-byte aligned bags only: the single-bag forward, one bag at a time into the packed buffers
-  int64_t row = 0;
-  const int C = p->C, D = p->D;
-  for (int b = 0; b < nb; ++b) {
-    rc = forward_impl(p, Xs[b], XVs ? XVs[b] : nullptr, nullptr, Ns[b], classes + row * C,
-                      pred + static_cast<size_t>(b) * C, A + row * C, B + static_cast<size_t>(b) * C * D,
-                      crit_idx ? crit_idx + static_cast<size_t>(b) * C : nullptr, save_Q ? save_Q + row * kQ : nullptr,
-                      save_H1 ? save_H1 + row * kQ : nullptr, save_V ? save_V + row * D : nullptr, workspace,
-                      workspace_bytes, st);
-    if (rc) return rc;
-    row += Ns[b];
-  }
-  return 0;
+  if ((rc = need_workspace(dsmil_value_forward_bags_workspace_bytes(p, Ns, nb), workspace, workspace_bytes))) return rc;
+  return forward_bags_route(p, Xs, XVs, Ns, nb, aligned, classes, pred, A, B, crit_idx, save_Q, save_H1, save_V,
+                            workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

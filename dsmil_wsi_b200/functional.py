@@ -287,7 +287,7 @@ class MILBagsFn(torch.autograd.Function):
             rc = lib.dsmil_forward_bags_train(P.ref, c_X, c_N, nb, _ptr(classes), _ptr(pred), _ptr(A), _ptr(B),
                                               _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(ws), ws.numel(), _stream())
             _lib.check(rc, "dsmil_forward_bags_train")
-        ctx.nb, ctx.Ns = nb, Ns
+        ctx.nb, ctx.Ns, ctx.c_X, ctx.c_N = nb, Ns, c_X, c_N
         ctx.save_for_backward(*xs, sQ, sH, A, B, crit, *P.tensors)
         ctx.mark_non_differentiable(crit)
         return classes, pred, A, B, crit
@@ -295,15 +295,13 @@ class MILBagsFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
         lib = _lib.load()
-        nb, Ns = ctx.nb, ctx.Ns
+        nb, Ns, c_X, c_N = ctx.nb, ctx.Ns, ctx.c_X, ctx.c_N
         saved = ctx.saved_tensors
-        xs, (sQ, sH, A, B, crit), params = saved[:nb], saved[nb:nb + 5], saved[nb + 5:]
+        (sQ, sH, A, B, crit), params = saved[nb:nb + 5], saved[nb + 5:]   # saved[:nb]: the bags c_X points at
         P = ParamPack(*params)
         need_bags, need_params = ctx.needs_input_grad[1:1 + nb], ctx.needs_input_grad[1 + nb:]
         names = ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")
         dev = P.device
-        c_X = (C.c_void_p * nb)(*[x.data_ptr() for x in xs])
-        c_N = (C.c_int64 * nb)(*Ns)
         with torch.cuda.device(dev):
             out = {nm: (torch.empty_like(t) if t is not None and need else None)
                    for nm, t, need in zip(names, P.tensors, need_params)}
@@ -724,20 +722,12 @@ def _mil_forward_bags_infer(bags: Sequence[torch.Tensor], params: Sequence[Optio
     P = ParamPack(*params)
     if P.passing_v:
         raise NotImplementedError("forward_bags: passing_v models go through MILNet.forward per bag")
-    xs = [_check_feats(b, P.D) for b in bags]
-    nb = len(xs)
+    nb = len(bags)
     if nb == 0:
         return [], None
-    Ns = [int(x.shape[0]) for x in xs]
-    if min(Ns) == 0:
-        raise IndexError("dsmil_b200: empty bag (N == 0) in the batch")
+    xs, Ns, c_X, c_N = _bag_table(bags, P)
     dev = P.device
-    for x in xs:
-        if x.device != dev:
-            raise RuntimeError(f"dsmil_b200: bag on {x.device} but parameters on {dev}")
     total, Cc, D = sum(Ns), P.C, P.D
-    c_N = (C.c_int64 * nb)(*Ns)
-    c_X = (C.c_void_p * nb)(*[x.data_ptr() for x in xs])
     with torch.cuda.device(dev):
         new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
         classes, A = new(total, Cc), new(total, Cc)

@@ -142,7 +142,9 @@ int dsmil_forward(const dsmil_params_t* p, const float* X, const float* x_for_v,
  * loop.  The generic shapes (identity v off dsmil_shard_bags_supported: any D <= 4096, C <= 8, either
  * q form) run one launch per stage for the whole batch, every bag's outputs bit for bit what
  * dsmil_forward gives it alone; on those of them whose phase 1 is k_qmlp_sm90 (nonlinear q,
- * D % 128 == 0) a bag that is not 16-byte aligned makes the batch loop.  passing_v loops. */
+ * D % 128 == 0) a bag that is not 16-byte aligned makes the batch loop.  passing_v takes the value
+ * batch of dsmil_value_forward_bags (value inputs = Xs) on the same terms.  Off the tensor-core
+ * shapes a batch of more than 65535 bags loops. */
 size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb);
 int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                        float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
@@ -327,7 +329,7 @@ int dsmil_generic_forward_bags_dev(const dsmil_params_t* p, const float* const* 
                                    void* stream);
 
 /* The batched forward of a model with a value network (passing_v: v = Dropout-Linear(D,D)-ReLU, dsmil.py:35-39), which
- * dsmil_forward_bags runs one bag at a time.  dsmil_value_bags_supported: passing_v with Wv/bv, 1 <= D <= 4096,
+ * dsmil_forward_bags also takes with the features as value inputs.  dsmil_value_bags_supported: passing_v with Wv/bv, 1 <= D <= 4096,
  * 1 <= C <= 8, either q form (the shapes dsmil_forward takes with passing_v).
  * dsmil_value_forward_bags: Xs / Ns / outputs as dsmil_forward_bags (crit_idx [nb,C] may be NULL); XVs [nb] (host
  * array, or NULL) are the bags' value inputs -- the features after the caller applied the dropout mask of dsmil.py:36,

@@ -60,7 +60,8 @@ def _pack(net):
     return Fn.ParamPack(*milnet_params(net))
 
 
-def _value_call(lib, P, xs, vs, saves):
+def _value_call(lib, P, xs, vs, saves, forward_bags=False):
+    """dsmil_value_forward_bags, or with forward_bags dsmil_forward_bags (value inputs = the features, no saves)."""
     nb, Ns = len(xs), [int(x.shape[0]) for x in xs]
     total, Cc, D = sum(Ns), P.C, P.D
     new = lambda *s: torch.full(s, float("nan"), device="cuda")
@@ -71,9 +72,14 @@ def _value_call(lib, P, xs, vs, saves):
     c_N = (C.c_int64 * nb)(*Ns)
     c_X = (C.c_void_p * nb)(*[x.data_ptr() for x in xs])
     c_V = None if vs is None else (C.c_void_p * nb)(*[v.data_ptr() for v in vs])
-    ws = torch.empty(max(lib.dsmil_value_forward_bags_workspace_bytes(P.ref, c_N, nb), 256), dtype=torch.uint8,
-                     device="cuda")
+    size = lib.dsmil_forward_bags_workspace_bytes if forward_bags else lib.dsmil_value_forward_bags_workspace_bytes
+    ws = torch.empty(max(size(P.ref, c_N, nb), 256), dtype=torch.uint8, device="cuda")
     g = lambda k: None if out.get(k) is None else out[k].data_ptr()
+    if forward_bags:
+        rc = lib.dsmil_forward_bags(P.ref, c_X, c_N, nb, g("classes"), g("pred"), g("A"), g("B"), g("crit"),
+                                    ws.data_ptr(), ws.numel(), torch.cuda.current_stream().cuda_stream)
+        assert rc == 0, lib.dsmil_last_error()
+        return out
     rc = lib.dsmil_value_forward_bags(P.ref, c_X, c_V, c_N, nb, g("classes"), g("pred"), g("A"), g("B"), g("crit"),
                                       g("Q"), g("H1"), g("V"), ws.data_ptr(), ws.numel(),
                                       torch.cuda.current_stream().cuda_stream)
@@ -98,14 +104,14 @@ def _single_call(lib, P, x, v):
 
 # bags 1 float off a 16-byte boundary: at (512, 2) the batch loops dsmil_forward (k_qmlp_sm90 needs aligned bags); at
 # (512, 3, linear) and (96, 2) k_vproj_b reads them through its scalar path although D % 4 == 0; at 166 every row is
-# off
+# off.  Mode "bags": eval through dsmil_forward_bags, which takes passing_v on the same route.
 OFFSETS = {(512, 2): (0, 1), (166, 1): (1,), (512, 3): (0, 1), (1024, 6): (0,), (96, 2): (0, 1)}
 
 
 def _cases():
     for D, C_, nl in SHAPES:
         for off in OFFSETS[(D, C_)]:
-            for mode in ("eval", "train"):
+            for mode in ("eval", "train") + (("bags",) if (D, C_) == (512, 2) else ()):
                 yield pytest.param(D, C_, nl, off, mode, id=f"D{D}C{C_}{'nl' if nl else 'lin'}-off{off}-{mode}")
 
 
@@ -121,7 +127,12 @@ def test_every_bag_gets_its_single_bag_bits(lib, D, C_, nl, offset, mode):
         batch = _value_call(lib, P, xs, vs, saves=True)
         again = _value_call(lib, P, xs, vs, saves=True)
         infer = _value_call(lib, P, xs, vs, saves=False)
+        if mode == "bags":
+            fb = _value_call(lib, P, xs, None, saves=False, forward_bags=True)
     torch.cuda.synchronize()
+    if mode == "bags":
+        for k, t in fb.items():
+            assert torch.equal(t, infer[k]), ("dsmil_forward_bags", k)
     for k, t in batch.items():
         if t is not None:
             assert torch.equal(t, again[k]), ("run to run", k)
