@@ -13,10 +13,13 @@
 //   k_instnorm_nhwc    the channels-last form (the embedding loop runs the ResNet-18 convolutions in cuDNN's NHWC
 //                      kernels, tools/exp_channels_last.py compares the two layouts).  Memory is [n][HW][C]; one CTA per (sample, 32-channel group),
 //                      lane = channel, warps stride over the pixels, so every warp load is one 128-byte row segment.
-//                      Statistics in ONE pass as shifted sums (x - x0, x0 = the channel's first pixel: no
-//                      catastrophic cancellation for activations whose mean is far from 0), second pass normalises;
-//                      the slab a CTA reads twice is <= 1.6 MB and was just written by the convolution, i.e. the
-//                      second read is an L2 hit for every layer but the 112x112 stem.
+//                      Statistics in ONE pass: each thread runs Welford's update over its strided pixels, then the 16
+//                      warp partials are merged in a fixed order with Chan's pairwise formula.  Both work on
+//                      deviations from a running mean, so the variance keeps its accuracy relative to var itself
+//                      however far any pixel lies from the mean (the first pixel is the image corner, the pixel with
+//                      the most zero padding: an outlier of its plane on flat slide background).  The second pass
+//                      normalises; the slab a CTA reads twice is <= 1.6 MB and was just written by the convolution,
+//                      i.e. the second read is an L2 hit for every layer but the 112x112 stem.
 //
 // HBM-bound: algorithmic bytes = 8 B per element (+ 4 with a residual).  fp32 contiguous; in place allowed.
 #pragma once
@@ -124,34 +127,52 @@ k_instnorm_warp(const float* __restrict__ x, const float* __restrict__ res, floa
 }
 
 constexpr int kNhwcWarps = 16;
+constexpr int kNhwcChunk = 8;          // pixels per statistics step: their loads are all in flight together
 
 __global__ void __launch_bounds__(32 * kNhwcWarps)
 k_instnorm_nhwc(const float* __restrict__ x, const float* __restrict__ res, float* __restrict__ y, int HW, int C, float eps,
                 int relu) {
-  __shared__ float s_a[kNhwcWarps][32], s_b[kNhwcWarps][32];
+  __shared__ float s_mean[kNhwcWarps][32], s_m2[kNhwcWarps][32];
   const int groups = C >> 5;
   const int n = blockIdx.x / groups, g = blockIdx.x - n * groups;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const size_t base = (static_cast<size_t>(n) * HW) * C + (g << 5) + lane;
   const float* xp = x + base;
-  const float x0 = __ldg(xp);
-  float s1 = 0.f, s2 = 0.f;
-#pragma unroll 4
-  for (int p = warp; p < HW; p += kNhwcWarps) {
-    const float d = __ldg(xp + static_cast<size_t>(p) * C) - x0;
-    s1 += d;
-    s2 = fmaf(d, d, s2);
-  }
-  s_a[warp][lane] = s1;
-  s_b[warp][lane] = s2;
-  __syncthreads();
-  s1 = 0.f; s2 = 0.f;
+  // Welford over the thread's pixels warp, warp + 16, ..., in chunks of up to 8 (the last may be short): the chunk's
+  // mean and squared deviations in registers, then Chan's update of the running (count, mean, M2)
+  float mean = 0.f, m2 = 0.f;
+  int cnt = 0;
+  for (int p = warp; p < HW; p += kNhwcChunk * kNhwcWarps) {
+    const int t = min(kNhwcChunk, (HW - p + kNhwcWarps - 1) / kNhwcWarps);
+    float v[kNhwcChunk];
 #pragma unroll
-  for (int w = 0; w < kNhwcWarps; ++w) { s1 += s_a[w][lane]; s2 += s_b[w][lane]; }   // fixed order
-  const float inv = 1.f / static_cast<float>(HW);
-  const float dm = s1 * inv;                                    // mean - x0
-  const float mean = x0 + dm;
-  const float var = fmaxf(fmaf(-dm, s1, s2) * inv, 0.f);        // (S2 - S1^2 / HW) / HW, biased as F.instance_norm
+    for (int k = 0; k < kNhwcChunk; ++k) v[k] = k < t ? __ldg(xp + static_cast<size_t>(p + k * kNhwcWarps) * C) : 0.f;
+    const float mc = (((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]))) / static_cast<float>(t);
+    float q = 0.f;
+#pragma unroll
+    for (int k = 0; k < kNhwcChunk; ++k) { const float d = k < t ? v[k] - mc : 0.f; q = fmaf(d, d, q); }
+    const float f = static_cast<float>(t) / static_cast<float>(cnt + t);
+    const float d = mc - mean;
+    mean = fmaf(d, f, mean);
+    m2 = fmaf(d * d, static_cast<float>(cnt) * f, m2 + q);
+    cnt += t;
+  }
+  s_mean[warp][lane] = mean;
+  s_m2[warp][lane] = m2;
+  __syncthreads();
+  // Chan's formula over the 16 partials in warp order: mean = sum n_w mean_w / HW, M2 = sum M2_w + n_w (mean_w - mean)^2;
+  // warp w holds ceil((HW - w) / 16) pixels (none, and a zero partial, when w >= HW)
+  float s = 0.f;
+#pragma unroll
+  for (int w = 0; w < kNhwcWarps; ++w) s = fmaf(static_cast<float>((HW - w + kNhwcWarps - 1) / kNhwcWarps), s_mean[w][lane], s);
+  mean = s / static_cast<float>(HW);
+  m2 = 0.f;
+#pragma unroll
+  for (int w = 0; w < kNhwcWarps; ++w) {
+    const float d = s_mean[w][lane] - mean;
+    m2 += fmaf(static_cast<float>((HW - w + kNhwcWarps - 1) / kNhwcWarps) * d, d, s_m2[w][lane]);
+  }
+  const float var = m2 / static_cast<float>(HW);               // biased, as F.instance_norm
   const float rstd = rsqrtf(var + eps);
   float* yp = y + base;
   const float* rp = res ? res + base : nullptr;

@@ -48,6 +48,22 @@ def test_u8_to_float_is_to_tensor():
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("Cc", [1, 3])
+def test_u8_to_float_is_to_tensor_past_one_grid(Cc):
+    """12 x 224 x 224 pixels: more than the kernel's grid covers in one sweep (kSms * 16 CTAs x 256 threads = 540 672),
+    so the grid-stride loop takes a second turn."""
+    import torchvision.transforms.functional as VF
+    from PIL import Image
+    from dsmil_wsi_b200.embed import patches_to_float
+    rng = np.random.default_rng(3 + Cc)
+    u8 = rng.integers(0, 256, size=(12, 224, 224, Cc), dtype=np.uint8)
+    assert 12 * 224 * 224 > 132 * 16 * 256
+    out = patches_to_float(torch.from_numpy(u8).cuda()).cpu()
+    ref = torch.stack([VF.to_tensor(Image.fromarray(a[..., 0] if Cc == 1 else a)) for a in u8])
+    assert out.shape == (12, Cc, 224, 224) and torch.equal(out, ref)
+
+
+@pytest.mark.gpu
 def test_embedding_loop_matches_reference_style_loop(tmp_path):
     """compute_feats(...) on synthetic JPEG patches vs the reference's loop shape (to_tensor -> .cuda() ->
     i_classifier -> .cpu()), same IClassifier (ResNet-18 + InstanceNorm as compute_feats.py:146-170)."""
