@@ -204,21 +204,38 @@ SINGLE = [
     Case("pv_gen_d96_c2_mask", "single", 96, 2, (4097,), passing_v=True, masked=True),
     Case("pv_gen_d166_c1", "single", 166, 1, (2049,), passing_v=True),
     Case("pv_gen_d166_c1_mask", "single", 166, 1, (2049,), passing_v=True, masked=True),
+    # gWi through k_gemv_tn<3> and <4> (tn_use_gemv: C <= 4, D % 4 == 0, D <= 1024) and the tile kernel one step past it
+    Case("tc_d1024_c1_n2049", "single", 1024, 1, (2049,)),
+    Case("tc_d1024_c3_n2049", "single", 1024, 3, (2049,)),
+    Case("tc_d1024_c4_n2049", "single", 1024, 4, (2049,)),
+    Case("gen_d1028_c4_n2049", "single", 1028, 4, (2049,)),
+    Case("tc_d512_c8_n2049", "single", 512, 8, (2049,)),
+    Case("tc_d4096_c1_n1025", "single", 4096, 1, (1025,)),
 ]
 BAGS = [
     Case("bags_d512_rps128", "bags", 512, 2, (64, 63, 65, 1, 128, 129, 127, 2049)),
     Case("bags_d2048", "bags", 2048, 2, (256, 255, 257, 1, 3831)),
     Case("bags_d512_misaligned", "bags", 512, 2, (128, 127, 129, 1, 5319), misaligned=(4,)),
     Case("bags_gen_d166", "bags", 166, 1, (128, 127, 129, 1, 3000)),
+    # gWi through k_gemv_tn_rag<3> and <4>, and k_gemm_tn_rag one step past D = 1024
+    Case("bags_d1024_c1", "bags", 1024, 1, (128, 127, 129, 1, 2049)),
+    Case("bags_d1024_c3", "bags", 1024, 3, (128, 127, 129, 1, 2049)),
+    Case("bags_d1024_c4", "bags", 1024, 4, (128, 127, 129, 1, 2049)),
+    Case("bags_gen_d1028_c4", "bags", 1028, 4, (128, 127, 129, 1, 2049)),
+    Case("bags_d512_c8", "bags", 512, 8, (128, 127, 129, 1, 2049)),
 ]
 DEV = [
     Case("dev_d512_rps128", "dev", 512, 2, (64, 63, 65, 1, 128, 129, 127, 2049)),
     Case("dev_gen_d166", "dev", 166, 1, (128, 127, 129, 1, 3000)),
     Case("dev_gen_d230_linear", "dev", 230, 2, (128, 127, 129, 1, 2305), nonlinear=False),
+    Case("dev_d1024_c3", "dev", 1024, 3, (128, 127, 129, 1, 2049)),
+    Case("dev_d1024_c4", "dev", 1024, 4, (128, 127, 129, 1, 2049)),
 ]
 MODELS = [
     Case("models_m2", "models", 512, 2, ((64, 129, 2049), (128, 1, 700))),
     Case("models_m3", "models", 512, 2, ((127, 3000), (1, 128, 129), (65, 63, 513, 2))),
+    Case("models_d1024_c3", "models", 1024, 3, ((129, 1500), (1, 128, 700))),
+    Case("models_d1024_c4", "models", 1024, 4, ((129, 1500), (1, 128, 700))),
 ]
 SHARD = [
     Case("shard_bags_d512", "shard_bags", 512, 2, (70, 69, 71, 3, 4097)),
@@ -434,6 +451,17 @@ def test_case_sits_on_its_split_boundary(case):
     if case.route in ("bags", "dev"):
         rps = lay.info["rps1"]
         assert {rps - 1, rps, rps + 1, 1} <= set(Ns), (case.name, rps, Ns)
+
+
+def test_cases_reach_every_gwi_form():
+    """gWi = d_classes^T X streams through k_gemv_tn<C> (one bag) or k_gemv_tn_rag<C> (a batch) for C = 1..4 while
+    tn_use_gemv holds, and through the tile kernels one multiple of 4 past D = 1024 at the same C."""
+    for route in ("single", "bags"):
+        cases = [c for c in ALL if c.route == route]
+        assert {c.C for c in cases if tn_use_gemv(c.C, c.D)} >= {1, 2, 3, 4}, route
+        assert any(c.C == 4 and c.D == 1024 for c in cases) and any(c.C == 4 and c.D == 1028 for c in cases), route
+    assert tn_use_gemv(4, 1024) and not tn_use_gemv(4, 1028)
+    assert {c.C for c in ALL} >= {3, 4, 8} and any(c.D == 4096 and c.route == "single" for c in ALL)
 
 
 def test_fold_and_rank_layouts_cover_every_row_once():

@@ -30,8 +30,10 @@ Routes: dsmil_forward (training, eval overlapped and plain) and dsmil_bag_forwar
 capture-safe pair (dsmil_forward_bags[_train]_dev or dsmil_generic_*); the fold forms (dsmil_forward_bags_models,
 _models_train, _models_train_dev); dsmil_value_forward_bags with and without v's mask; and the row-sharded phases at
 G = 1, 2, 3 per bag (CudaShardOps, with an empty rank, a probe-free rank whose combine weight underflows, and a crafted Q
-given to phase 2) and batched (CudaShardBagOps).  Forms without saves keep Q in tile blocks and apply the same tanh_ex2
-on read, so they are checked against the restatement on the training call's Q, after asserting that they give its
+given to phase 2) and batched (CudaShardBagOps).  The cases reach every instance of k_qmlp_sm90, k_attend,
+k_attend_gb and k_attend_b (test_kernel_instances_gpu.py checks it), with the last column group of each J or NJ full
+and partly empty, and k_qmlp_sm90 at D = 128 and at the largest D of each CT (a mirror of qmlp_smem_bytes).  Forms
+without saves keep Q in tile blocks and apply the same tanh_ex2 on read, so they are checked against the restatement on the training call's Q, after asserting that they give its
 classes and crit bits.
 
 Peaked bags.  Column d0 of W1 is zero and Wi[0, d0] = 1: the class-0 critical row has x[d0] = 8.  Probe rows copy it
@@ -77,6 +79,9 @@ SCALE = orc.SCALE_F32
 # mirrored from the sources (checked below): fwd_batched.cuh, fwd_kernels.cuh, common.cuh
 K_ATT_ROWS, K_MAX_REC_PER_BAG, K_FIN_SLICES = 128, 128, 32
 K_ATTEND_ROWS, K_SPLITS = 32, 296
+# fwd_sm90.cuh: k_qmlp_sm90's shared memory (W ring of K_WSTAGES chunks, Wi at C rounded up to 1/2/4/8 rows, M members'
+# rows and biases in the fold form) against the 227 KB a block may have on sm_90; include/dsmil_b200.h: DSMIL_MAX_D
+K_WSTAGES, K_CHUNK_K, K_SMEM_BAGS, BAGDEV_BYTES, K_MAX_C, SMEM_CAP, MAX_D = 4, 64, 96, 40, 8, 232448, 4096
 # bar constants (multiples of u); the CPU part shows each is >= 4x the fp32 restatement's error on the same inputs
 C_CLS = 64.0
 C_MM = 64.0
@@ -102,6 +107,45 @@ def recs_for_bag(N):
 def attend_ctas(N):
     """bag_plan.cuh: generic k_attend records of a bag of N rows."""
     return min(max(ceil_div(N, K_ATTEND_ROWS), 1), K_SPLITS)
+
+
+def ct_of(C_):
+    return 1 if C_ <= 1 else 2 if C_ <= 2 else 4 if C_ <= 4 else 8
+
+
+def qmlp_smem_bytes(C_, D, M=0):
+    """fwd_sm90.cuh: qmlp_smem_bytes (M = 0) or qmlp_models_smem_bytes (M members), plus kQmlpStaticSmem."""
+    fixed = K_WSTAGES * 2 * (KQ * K_CHUNK_K * 2)
+    wi = ct_of(C_) * D if M == 0 else M * (ct_of(C_) * D + 2 * KQ + K_MAX_C)
+    return fixed + 4 * wi + 1024 + 2 * KQ * 4 + K_SMEM_BAGS * BAGDEV_BYTES + 256
+
+
+def qmlp_supported(C_, D, nonlinear=True):
+    return nonlinear and D % (2 * K_CHUNK_K) == 0 and qmlp_smem_bytes(C_, D) <= SMEM_CAP
+
+
+def batched_supported(C_, D, nonlinear=True):
+    """fwd_batched.cuh (passing_v aside)."""
+    return qmlp_supported(C_, D, nonlinear) and D % 4 == 0 and D <= 2048 and (C_ <= 2 or (C_ <= 4 and D <= 1024))
+
+
+def models_supported(C_, D, M):
+    """dsmil_models_supported: every member on the batched route and the fold kernel's shared memory fits."""
+    return batched_supported(C_, D) and qmlp_smem_bytes(C_, D, M) <= SMEM_CAP
+
+
+def route_edges():
+    """{CT: (largest D k_qmlp_sm90 takes, the next multiple of 128 or None at DSMIL_MAX_D)} and the same for the fold
+    form of two models."""
+    out = {}
+    for M in (0, 2):
+        for ct in (1, 2, 4, 8):
+            ok = (lambda D: qmlp_supported(ct, D)) if M == 0 else (lambda D: models_supported(ct, D, M))
+            if ct == 8 and M:
+                continue                              # the fold form stops at C = 4
+            top = max(D for D in range(128, MAX_D + 1, 128) if ok(D))
+            out[(ct, M)] = (top, top + 128 if top + 128 <= MAX_D else None)
+    return out
 
 
 def records(N, kind):
@@ -145,14 +189,14 @@ class Case:
 
     @property
     def tc_phase1(self):
-        return self.nonlinear and self.D % 128 == 0
+        return qmlp_supported(self.C, self.D, self.nonlinear)
 
     @property
     def attend(self):
         """'b': k_attend_b / k_finalize_b (batched_supported); 'g': the generic attend, combine and finalize (also the
         value route's, and the per-bag sharded phase 2's; the batched sharded form, held to the same mirror, walks
         fewer rows per record)."""
-        ok = self.tc_phase1 and self.D <= 2048 and (self.C <= 2 or (self.C <= 4 and self.D <= 1024))
+        ok = batched_supported(self.C, self.D, self.nonlinear)
         return "b" if ok and not self.passing_v and self.route != "shard" else "g"
 
 
@@ -164,6 +208,28 @@ SINGLE = [
     Case("gen_d166_c2_n2500", "single", 166, 2, (2500,)),
     Case("genlin_d230_c3_n12000_rescale", "single", 230, 3, (12000,), nonlinear=False, rescale=True),
     Case("genlin_d166_c1_n3000", "single", 166, 1, (3000,), nonlinear=False),
+    # the generic k_attend<CT, J> (J = ceil(D / 256) rounded up to a power of two; its last 256-column group full or
+    # partly empty) and k_qmlp_sm90 at the largest D of each CT, DSMIL_MAX_D = 4096 for CT <= 4
+    Case("tc_d4096_c1_n1500", "single", 4096, 1, (1500,)),
+    Case("tc_d4096_c2_n1200", "single", 4096, 2, (1200,)),
+    Case("tc_d4096_c4_n1000", "single", 4096, 4, (1000,)),
+    Case("tc_d2944_c8_n1000", "single", 2944, 8, (1000,)),          # CT = 8: the largest D k_qmlp_sm90 takes
+    Case("gen_d3072_c8_n1000", "single", 3072, 8, (1000,)),         # ... and the next multiple of 128: FFMA phase 1
+    Case("gen_d4095_c7_n1000", "single", 4095, 7, (1000,)),
+    Case("gen_d2049_c2_n1500", "single", 2049, 2, (1500,)),
+    Case("genlin_d2048_c2_n2000", "single", 2048, 2, (2000,), nonlinear=False),
+    Case("genlin_d1920_c1_n2000", "single", 1920, 1, (2000,), nonlinear=False),
+    Case("genlin_d1024_c1_n2000", "single", 1024, 1, (2000,), nonlinear=False),
+    Case("genlin_d512_c1_n2000", "single", 512, 1, (2000,), nonlinear=False),
+    Case("gen_d300_c2_n2000", "single", 300, 2, (2000,)),
+    Case("gen_d1000_c2_n2000", "single", 1000, 2, (2000,)),
+    Case("genlin_d512_c3_n2000", "single", 512, 3, (2000,), nonlinear=False),
+    Case("gen_d1020_c4_n1500", "single", 1020, 4, (1500,)),
+    Case("tc_d1152_c3_n1500", "single", 1152, 3, (1500,)),
+    Case("tc_d256_c8_n2000", "single", 256, 8, (2000,)),
+    Case("tc_d768_c5_n1500", "single", 768, 5, (1500,)),
+    Case("tc_d2048_c8_n1000", "single", 2048, 8, (1000,)),
+    Case("tc_d128_c2_n3000", "single", 128, 2, (3000,)),              # k_qmlp_sm90's shortest K loop
 ]
 BAGS = [
     Case("bags_tc_d512_c2", "bags", 512, 2, (1, 127, 128, 129, 3000, 17000), rescale=True, bias=2.5),
@@ -172,16 +238,50 @@ BAGS = [
     Case("bags_tc_d512_c1", "bags", 512, 1, (129, 4000)),
     Case("bags_tc_d512_c3", "bags", 512, 3, (2, 128, 2500)),
     Case("bags_gen_d7_c2", "bags", 7, 2, (1, 33, 3000)),
+    # k_attend_b<CT, NJ> with its last 512-column group full (D = 512 NJ) or partly empty, and k_qmlp_sm90 at DT = 0
+    # in both forms; D = 2048 against 2176 for batched_supported
+    Case("bags_tc_d1024_c1", "bags", 1024, 1, (1, 129, 2000)),
+    Case("bags_tc_d1024_c2", "bags", 1024, 2, (2, 128, 1500)),
+    Case("bags_tc_d2048_c1", "bags", 2048, 1, (129, 1200)),
+    Case("bags_tc_d2048_c2", "bags", 2048, 2, (1, 127, 1000)),
+    Case("bags_tc_d640_c1", "bags", 640, 1, (33, 1500)),
+    Case("bags_tc_d1920_c2", "bags", 1920, 2, (129, 1000)),
+    Case("bags_tc_d128_c2", "bags", 128, 2, (1, 129, 3000)),
+    Case("bags_tc_d1024_c4", "bags", 1024, 4, (128, 1500)),
+    # k_attend_gb<CT, J> over the generic batch, its dev form on the same shapes
+    Case("bags_genlin_d256_c1", "bags", 256, 1, (33, 2000), nonlinear=False),
+    Case("bags_genlin_d512_c1", "bags", 512, 1, (1, 33, 2000), nonlinear=False),
+    Case("bags_genlin_d1024_c1", "bags", 1024, 1, (33, 1500), nonlinear=False),
+    Case("bags_genlin_d1920_c1", "bags", 1920, 1, (33, 1200), nonlinear=False),
+    Case("bags_tc_d4096_c1", "bags", 4096, 1, (129, 800)),
+    Case("bags_gen_d1000_c2", "bags", 1000, 2, (33, 1500)),
+    Case("bags_tc_d2176_c2", "bags", 2176, 2, (129, 1200)),
+    Case("bags_genlin_d384_c4", "bags", 384, 4, (33, 1500), nonlinear=False),
+    Case("bags_gen_d1020_c3", "bags", 1020, 3, (33, 1500)),
+    Case("bags_tc_d2048_c3", "bags", 2048, 3, (129, 1000)),
+    Case("bags_tc_d4096_c4", "bags", 4096, 4, (33, 700)),
+    Case("bags_tc_d512_c6", "bags", 512, 6, (1, 129, 1500)),
+    Case("bags_tc_d1280_c8", "bags", 1280, 8, (33, 1000)),
+    Case("bags_gen_d777_c5", "bags", 777, 5, (33, 1200)),
+    Case("bags_gen_d4095_c8", "bags", 4095, 8, (33, 600)),
 ]
 # the ensemble forms: two models (their own weights) over the same bags
 MODELS = [
     Case("models_tc_d512_c2", "models", 512, 2, (129, 3000)),
+    Case("models_tc_d512_c1", "models", 512, 1, (129, 1000)),
+    Case("models_tc_d512_c3", "models", 512, 3, (129, 1000)),
+    Case("models_tc_d1024_c1", "models", 1024, 1, (129, 1000)),
+    Case("models_tc_d1024_c2", "models", 1024, 2, (129, 1000)),
+    Case("models_tc_d1024_c4", "models", 1024, 4, (129, 800)),      # CT = 4: the largest D of the fold form
+    Case("models_tc_d2048_c1", "models", 2048, 1, (129, 800)),      # CT = 1 and 2: the largest (batched_supported)
+    Case("models_tc_d2048_c2", "models", 2048, 2, (129, 800)),
 ]
 # dsmil_value_forward_bags (passing_v): V is checked too, and B = A^T V on the kernel's own V
 VALUE = [
     Case("value_tc_d512_c2", "value", 512, 2, (129, 2000), passing_v=True),
     Case("value_tc_d512_c2_mask", "value", 512, 2, (129, 2000), passing_v=True, masked=True),
     Case("value_gen_d166_c3_mask", "value", 166, 3, (33, 1500), passing_v=True, masked=True),
+    Case("value_tc_d2048_c2", "value", 2048, 2, (129, 800), passing_v=True),
 ]
 # the row-sharded phases at G = 1, 2, 3 virtual ranks: per bag (CudaShardOps) and batched (CudaShardBagOps)
 SHARD = [
@@ -419,10 +519,72 @@ def test_mirror_constants_are_the_sources():
     plan = _src("bag_plan.cuh")
     assert "t < sm90::kMaxRecPerBag ? (t < 1 ? 1 : t) : sm90::kMaxRecPerBag" in plan
     assert "tiles < kSplits ? (tiles < 1 ? 1 : tiles) : kSplits" in plan
+    sm, hd = _src("fwd_sm90.cuh"), _src(os.path.join("..", "..", "include", "dsmil_b200.h"))
+    assert (const(sm, "kWStages"), const(sm, "kChunkK"), const(sm, "kSmemBags"), const(sm, "kTileM")) == \
+        (K_WSTAGES, K_CHUNK_K, K_SMEM_BAGS, KQ)
+    for line in ("constexpr int kTileBytes = kQ * kChunkK * 2;", "constexpr int kChunkBytes = 2 * kTileBytes;",
+                 "constexpr int kOffWi = kOffWRing + kWStages * kChunkBytes;", "constexpr int kSmemFixed = kOffWi;",
+                 "return kSmemFixed + sizeof(float) * ct * D + 1024;",
+                 "return kSmemFixed + sizeof(float) * M * (static_cast<size_t>(ct_of(C)) * D + kModelBiasFloats) + 1024;",
+                 "constexpr int kModelBiasFloats = 2 * kQ + kMaxC;",
+                 "constexpr size_t kQmlpStaticSmem = 2 * kQ * sizeof(float) + kSmemBags * sizeof(BagDev) + 256;",
+                 f"p->D % (2 * kChunkK) == 0 && qmlp_smem_bytes(p->C, p->D) + kQmlpStaticSmem <= {SMEM_CAP};",
+                 f"return qmlp_models_smem_bytes(C, D, M) + kQmlpStaticSmem <= {SMEM_CAP};",
+                 "inline int ct_of(int C) { return C <= 1 ? 1 : (C <= 2 ? 2 : (C <= 4 ? 4 : 8)); }"):
+        assert line in sm, line
+    # sizeof(BagDev) = 40: a pointer, three 8-byte integers' worth of fields, four ints
+    bag = re.search(r"struct BagDev \{(.*?)\};", sm, re.S).group(1)
+    assert re.findall(r"^\s*(const float\*|long long|int) ", bag, re.M) == \
+        ["const float*", "long long", "long long", "int", "int", "int", "int"]
+    assert "return qmlp_supported(p) && !p->passing_v && p->D % 4 == 0 && p->D <= 2048 && p->C <= 4 &&\n" \
+           "         ((p->C <= 2) || p->D <= 1024);" in fb
+    assert (int(re.search(r"#define DSMIL_MAX_D (\d+)", hd).group(1)),
+            int(re.search(r"#define DSMIL_MAX_C (\d+)", hd).group(1))) == (MAX_D, K_MAX_C)
     from dsmil_wsi_b200.sharded import shard_bounds
     for N in (1, 2, 7, 128, 20000):
         for G in (1, 2, 3):
             assert list(shard_bounds(N, G)) == list(orc.shard_bounds(N, G))
+
+
+def attend_instance(case: Case):
+    """(kernel, CT, J or NJ) of the attend pass the case's forward launches."""
+    if case.attend == "b":
+        return ("k_attend_b", ct_of(case.C), 1 if case.D <= 512 else 2 if case.D <= 1024 else 4)
+    J = 1
+    while 256 * J < case.D:
+        J *= 2
+    return ("k_attend" if case.route in ("single", "shard") else "k_attend_gb", ct_of(case.C), J)
+
+
+def test_cases_reach_every_column_edge_and_route_edge():
+    """Each J of the generic attend passes and each NJ of k_attend_b has a case whose last column group is full and
+    one where it is partly empty; k_qmlp_sm90 runs at D = 128, at the largest D of each CT (one- and two-model forms)
+    and one multiple of 128 beyond it falls to the generic phase 1; D = 2048 and 2176 straddle batched_supported."""
+    seen = {}
+    for case in ALL:
+        kern, ct, j = attend_instance(case)
+        width = 512 if kern == "k_attend_b" else 256
+        seen.setdefault((kern, j), set()).add(case.D == width * j)
+        seen.setdefault((kern, ct, j), set()).add(True)
+    for kern, js in (("k_attend", (1, 2, 4, 8, 16)), ("k_attend_gb", (1, 2, 4, 8, 16)), ("k_attend_b", (1, 2, 4))):
+        for j in js:
+            assert seen.get((kern, j)) == {True, False}, (kern, j, seen.get((kern, j)))
+    for ct in (1, 2, 4, 8):
+        for kern in ("k_attend", "k_attend_gb"):
+            assert all((kern, ct, j) in seen for j in (1, 2, 4, 8, 16)), (kern, ct)
+    edges = route_edges()
+    assert edges[(8, 0)] == (2944, 3072) and edges[(4, 0)] == (4096, None) and edges[(4, 2)] == (1024, 1152)
+    for (ct, M), (top, nxt) in edges.items():
+        pool = SINGLE + BAGS if M == 0 else MODELS
+        assert any(ct_of(c.C) == ct and c.D == top and c.tc_phase1 for c in pool), (ct, M, top)
+        if nxt is not None and M == 0:
+            assert any(ct_of(c.C) == ct and c.D == nxt and c.nonlinear and not c.tc_phase1 for c in pool), (ct, nxt)
+        if nxt is not None and M:
+            assert not models_supported(ct, nxt, M) and qmlp_supported(ct, nxt)
+    assert any(c.D == 128 and c.tc_phase1 for c in ALL)
+    on_b = {c.D for c in BAGS if c.attend == "b" and c.C <= 2}
+    off_b = {c.D for c in BAGS if c.attend == "g" and c.tc_phase1 and c.C <= 2}
+    assert 2048 in on_b and 2176 in off_b
 
 
 def test_records_tile_every_row_once_and_cases_sit_on_their_boundaries():
