@@ -67,6 +67,13 @@ SIGNATURES = {
                                            C.POINTER(c_i64), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_size_t, C.c_void_p]),
+    "dsmil_value_backward_bags_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.POINTER(c_i64), C.c_int32,
+                                                               C.c_int]),
+    "dsmil_value_backward_bags": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                            C.POINTER(c_i64), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.POINTER(DsmilGrads), C.c_void_p,
+                                            C.c_size_t, C.c_void_p]),
     "dsmil_instance_scores": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, c_i64, C.c_void_p, C.c_void_p]),
     "dsmil_instance_scores_backward": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, c_i64, C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,

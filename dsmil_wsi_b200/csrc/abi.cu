@@ -1433,10 +1433,12 @@ static BwdBagsWs carve_bwd_bags_dev(const dsmil_params_t* p, int nb, int64_t max
 // depends on the live rows reads its count from w.plan.
 
 // Phase 1: dB, gWf/gbf, gWi/gbi, dA = X dB_b^T (+ d_A) into dA, and t_b's per-CTA partials in w.tpart (w.G per bag).
+// V (eager passing_v): the packed V rows [total, D]; the table's X is then each bag's rows of V, so dA = V dB_b^T,
+// while gWi and gW1 still reduce against the features Xs.
 static int bwd_bags_phase1_impl(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
                                 int64_t total, const float* A, const float* B, const float* d_classes,
                                 const float* d_pred, const float* d_A, const float* d_B, const dsmil_grads_t* g,
-                                float* dA, const BwdBagsWs& w, cudaStream_t st) {
+                                float* dA, const BwdBagsWs& w, cudaStream_t st, const float* V = nullptr) {
   const int C = p->C, D = p->D;
   const BagsPlan* pl = w.plan;
   int rc;
@@ -1445,7 +1447,7 @@ static int bwd_bags_phase1_impl(const dsmil_params_t* p, const float* const* Xs,
     std::vector<sm90::BagDev> tbl(nb);
     long long row = 0;
     for (int b = 0; b < nb; ++b) {
-      tbl[b] = sm90::BagDev{Xs[b], Ns[b], row, 0, 0, 0, 0};
+      tbl[b] = sm90::BagDev{V ? V + row * D : Xs[b], Ns[b], row, 0, 0, 0, 0};
       row += Ns[b];
     }
     std::vector<TnChunk> chi(w.nci), ch1(w.nc1);
@@ -1554,6 +1556,90 @@ static int backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, c
   int rc = check_workspace(w.bytes, ok, ws, ws_bytes);
   if (rc) return rc;
   return backward_bags_run(p, Xs, Ns, nb, total, Q, H1, A, B, crit, d_classes, d_pred, d_A, d_B, g, w, st);
+}
+
+// ---- batched value backward (passing_v): dsmil_backward_bags's phases over V, then the value network -------------
+// The three phases run with the packed V in the table (dA = V dB_b^T).  Then dzv_b = (A_b dB_b) * [V_b > 0] for every
+// bag in one k_linear_models launch (one LinSeg per bag: X = A rows, W = dB_b, K = C, aux = V rows), gWv = dzv^T Xv
+// over chunks of the value inputs (k_gemm_tn_rag), gbv the column sums of dzv.  gX (eager only) adds dz1 W1,
+// d_classes Wi (no A dB term: with a value network B weighs V, not X) and (dzv Wv) * the packed v mask.
+struct ValueBwdWs {
+  BwdBagsWs b;               // the identity-v backward's carve
+  LinSeg* segs;              // [nb] dzv segments
+  TnChunk* chv;              // gWv chunks over the value inputs
+  float *dzv, *tmp;          // [total, D]; tmp (gX only) holds dzv Wv
+  float *tnpart, *cspart;    // gWv's chunk partials, gbv's split partials
+  int ncv;
+  int64_t rps_v;
+  size_t bytes;
+};
+static ValueBwdWs carve_value_bwd(const dsmil_params_t* p, const int64_t* Ns, int nb, bool aligned, bool need_gX,
+                                  void* ws, size_t cap, bool* ok) {
+  ValueBwdWs w;
+  const int D = p->D;
+  w.b = carve_bwd_bags(p, Ns, nb, aligned, false, ws, cap, ok);
+  int64_t total = 0;
+  for (int b = 0; b < nb; ++b) total += Ns[b];
+  const int64_t n = std::max<int64_t>(total, 1);
+  w.rps_v = rag_rows_per_chunk(D, D, total, false);
+  w.ncv = rag_chunks(nullptr, Ns, nb, D, w.rps_v, nullptr);
+  Carver c(ws, cap);
+  c.off = w.b.bytes;
+  w.segs = c.take<LinSeg>(nb);
+  w.chv = c.take<TnChunk>(w.ncv);
+  w.dzv = c.take<float>(n * D);
+  w.tmp = need_gX ? c.take<float>(n * D) : nullptr;
+  w.tnpart = c.take<float>(static_cast<size_t>(w.ncv) * D * D);
+  w.cspart = c.take<float>(static_cast<size_t>(kSplits) * D);
+  w.bytes = c.off;
+  *ok = c.ok();
+  return w;
+}
+
+// The tile-form ragged GEMMs number their chunks in grid z.  gWi's tile form (unaligned bags) chunks the rows as gW1
+// does (rag_splits is the same for C and 128 left columns), so nc1 bounds it at either alignment.
+static bool value_bwd_grids_ok(const ValueBwdWs& w) { return w.ncv <= 65535 && w.b.nc1 <= 65535; }
+
+static int value_backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
+                                    const int64_t* Ns, int nb, int64_t total, const float* Q, const float* H1,
+                                    const float* V, const float* A, const float* B, const int64_t* crit,
+                                    const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                                    const float* v_mask, const dsmil_grads_t* g, const ValueBwdWs& w,
+                                    cudaStream_t st) {
+  const int C = p->C, D = p->D;
+  const BwdBagsWs& wb = w.b;
+  int rc;
+  const float* dz1;
+  if ((rc = bwd_bags_phase1_impl(p, Xs, Ns, nb, total, A, B, d_classes, d_pred, d_A, d_B, g, wb.dA, wb, st, V)) ||
+      (rc = bwd_bags_phase2_impl(p, nb, A, wb.dA, wb.tpart, wb.G, Q, wb.dL, wb.dqm, wb, st)) ||
+      (rc = bwd_bags_phase3_impl(p, nb, total, Q, H1, wb.dL, wb.dqm, nullptr, crit, nullptr, g, wb, &dz1, st)))
+    return rc;
+  std::vector<LinSeg> segs(nb);
+  std::vector<TnChunk> chv(w.ncv);
+  int64_t row = 0, mx = 1;
+  for (int b = 0; b < nb; ++b) {
+    segs[b] = LinSeg{A + row * C, wb.dB + static_cast<size_t>(b) * C * D, V + row * D, w.dzv + row * D, Ns[b]};
+    mx = std::max<int64_t>(mx, Ns[b]);
+    row += Ns[b];
+  }
+  rag_chunks(XVs ? XVs : Xs, Ns, nb, D, w.rps_v, chv.data());
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.segs, segs.data(), sizeof(LinSeg) * nb, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.chv, chv.data(), sizeof(TnChunk) * w.ncv, cudaMemcpyHostToDevice, st));
+  k_linear_models<ACT_MASK_POS, true><<<dim3(ceil_div(mx, LBM), ceil_div(D, LBN), nb), 256, 0, st>>>(w.segs, C, D);
+  DSMIL_LAUNCH_OK("k_linear_models");
+  if (g->gWv && (rc = launch_gemm_tn_rag(w.dzv, D, D, w.chv, w.ncv, false, w.tnpart, g->gWv, st))) return rc;
+  if (g->gbv && (rc = launch_colsum(w.dzv, D, total, w.cspart, g->gbv, st))) return rc;
+  if (!g->gX) return 0;
+  const int ge = static_cast<int>(std::min<int64_t>(ceil_div(total * D, 256), kSms * 8));
+  if ((rc = launch_linear<ACT_NONE, true>(dz1, total, kQ, p->W1, nullptr, D, g->gX, nullptr, 0, st))) return rc;
+  if (d_classes) {
+    k_bwd_dx_extra<<<ge, 256, 0, st>>>(d_classes, p->Wi, nullptr, nullptr, total, C, D, 1, g->gX);
+    DSMIL_LAUNCH_OK("k_bwd_dx_extra");
+  }
+  if ((rc = launch_linear<ACT_NONE, true>(w.dzv, total, D, p->Wv, nullptr, D, w.tmp, nullptr, 0, st))) return rc;
+  k_axpy_mask<<<ge, 256, 0, st>>>(w.tmp, v_mask, total * D, g->gX);
+  DSMIL_LAUNCH_OK("k_axpy_mask");
+  return 0;
 }
 
 // ---- sharded batch ABI ---------------------------------------------------------------------------
@@ -2848,6 +2934,41 @@ int dsmil_value_forward_bags(const dsmil_params_t* p, const float* const* Xs, co
   if ((rc = need_workspace(dsmil_value_forward_bags_workspace_bytes(p, Ns, nb), workspace, workspace_bytes))) return rc;
   return forward_bags_route(p, Xs, XVs, Ns, nb, aligned, classes, pred, A, B, crit_idx, save_Q, save_H1, save_V,
                             workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+size_t dsmil_value_backward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb, int need_gX) {
+  if (!dsmil_value_bags_supported(p) || !Ns || nb < 1 || nb > 65535) return 0;
+  for (int b = 0; b < nb; ++b)
+    if (Ns[b] < 1 || Ns[b] >= 0xffffffffll) return 0;
+  bool ok;
+  const ValueBwdWs w = carve_value_bwd(p, Ns, nb, true, need_gX != 0, nullptr, 0, &ok);
+  return value_bwd_grids_ok(w) ? w.bytes : 0;
+}
+
+int dsmil_value_backward_bags(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
+                              const int64_t* Ns, int32_t nb, const float* Q, const float* H1, const float* V,
+                              const float* A, const float* B, const int64_t* crit_idx, const float* d_classes,
+                              const float* d_pred, const float* d_A, const float* d_B, const float* v_mask,
+                              const dsmil_grads_t* grads, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_params(p);
+  if (rc) return rc;
+  DSMIL_REQUIRE(p->passing_v, "the value backward takes passing_v models (identity v: dsmil_backward_bags)");
+  DSMIL_REQUIRE(Xs && Ns && nb >= 1 && nb <= 65535 && Q && V && A && B && crit_idx && grads,
+                "NULL pointer or nb outside [1, 65535]");
+  DSMIL_REQUIRE(!p->nonlinear || H1, "nonlinear q backward needs saved H1");
+  DSMIL_REQUIRE(!(grads->gX && d_classes) || p->Wi, "gX through d_classes needs Wi");
+  int64_t total;
+  bool aligned;
+  if ((rc = check_bags(Xs, Ns, nb, &total, &aligned))) return rc;
+  for (int b = 0; XVs && b < nb; ++b) DSMIL_REQUIRE(XVs[b], "bag %d: NULL value input", b);
+  bool ok;
+  const ValueBwdWs w = carve_value_bwd(p, Ns, nb, aligned, grads->gX != nullptr, workspace, workspace_bytes, &ok);
+  DSMIL_REQUIRE(value_bwd_grids_ok(w), "too many bags for the ragged GEMM grids (%d gW1 chunks, %d gWv chunks)",
+                w.b.nc1, w.ncv);
+  const size_t need = dsmil_value_backward_bags_workspace_bytes(p, Ns, nb, grads->gX != nullptr);
+  if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
+  return value_backward_bags_impl(p, Xs, XVs, Ns, nb, total, Q, H1, V, A, B, crit_idx, d_classes, d_pred, d_A, d_B,
+                                  v_mask, grads, w, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

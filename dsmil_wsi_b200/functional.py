@@ -664,36 +664,139 @@ def mil_forward_bags_models(bags: Sequence[torch.Tensor], params_list: Sequence[
     return [BagOutputs(classes[m], pred[m], A[m], B[m], Ns, crit[m]) for m in range(M)]
 
 
-MAX_VALUE_BAGS = 65535   # bags of one dsmil_value_forward_bags call
+MAX_VALUE_BAGS = 65535   # bags of one dsmil_value_forward_bags / dsmil_value_backward_bags call
 
 
-@torch.no_grad()
-def mil_forward_value_bags(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]],
-                           v_inputs: Optional[Sequence[torch.Tensor]] = None):
-    """Inference over a stream of bags for a model with a value network (passing_v), in one
-    dsmil_value_forward_bags call: returns a lazy sequence of (classes, prediction_bag, A, B) per bag plus crit_idx
-    [nb, C], as mil_forward_bags does.  v_inputs: each bag's value input (the features after the dropout mask of
-    dsmil.py:36), or None for the features themselves (eval mode, or p = 0).  Every bag's outputs are bit for bit
-    what mil_forward gives it alone with the same value input.  A batch of more than MAX_VALUE_BAGS bags is split
-    into consecutive calls that write into the same packed outputs."""
-    lib = _lib.load()
+def _value_pack(params) -> ParamPack:
     P = ParamPack(*params)
     if not P.passing_v:
         raise ValueError("mil_forward_value_bags takes models with a value network (passing_v); identity v goes "
                          "through mil_forward_bags")
+    return P
+
+
+def _per_bag(vals, xs, P: ParamPack, what: str):
+    """Checked, contiguous per-bag tensors shaped like their bags (value inputs or v masks), or None."""
+    if vals is None:
+        return None
+    if len(vals) != len(xs):
+        raise ValueError(f"{len(vals)} {what}s for {len(xs)} bags")
+    vs = [_check_feats(v, P.D) for v in vals]
+    for v, x in zip(vs, xs):
+        if v.shape != x.shape or v.device != x.device:
+            raise ValueError(f"a {what} {tuple(v.shape)} on {v.device} does not match its bag "
+                             f"{tuple(x.shape)} on {x.device}")
+    return vs
+
+
+def _ptr_array(ts):
+    return None if ts is None else (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+
+class MILValueBagsFn(torch.autograd.Function):
+    """Packed (classes, pred, A, B, crit) of a batch of bags of a passing_v model, differentiable:
+    dsmil_value_forward_bags with saves forward, dsmil_value_backward_bags backward (one call each for the whole
+    batch).  args: nb, v_inputs (nb value inputs, or None), v_masks (their nb dropout masks, or None), the nb bags,
+    then the ten parameter tensors.  Parameter gradients are sums over the bags, gWv and gbv included; a bag's
+    gradient includes the value path, through its mask, so value inputs that are not the bags need their masks when a
+    bag gradient is wanted.  The value inputs and masks get no gradient; both are saved for the backward (an in-place
+    write to a value input before it fails there, as for any saved tensor)."""
+
+    @staticmethod
+    def forward(ctx, nb, v_inputs, v_masks, *args):
+        lib = _lib.load()
+        ctx.set_materialize_grads(False)
+        P = _value_pack(args[nb:])
+        xs, Ns, c_X, c_N = _bag_table(args[:nb], P)
+        vs, ms = _per_bag(v_inputs, xs, P, "value input"), _per_bag(v_masks, xs, P, "v mask")
+        if ms is not None and vs is None:
+            raise ValueError("v_masks without v_inputs: the masks are the factors of the value inputs")
+        if vs is not None and ms is None and any(ctx.needs_input_grad[3:3 + nb]):
+            raise ValueError("the bags' gradients through v_inputs need their v_masks (v_inputs == bags * v_masks)")
+        total, Cc, D, dev = sum(Ns), P.C, P.D, P.device
+        with torch.cuda.device(dev):
+            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+            classes, A = new(total, Cc), new(total, Cc)
+            pred, B = new(nb, Cc), new(nb, Cc, D)
+            crit = torch.empty(nb, Cc, dtype=torch.int64, device=dev)
+            sQ, sV = new(total, Q_DIM), new(total, D)
+            sH = new(total, Q_DIM) if P.nonlinear else None
+            mask = torch.cat(ms) if ms is not None else None   # packed [sum N, D], as the backward reads it
+            ws = _workspace(lib.dsmil_value_forward_bags_workspace_bytes(P.ref, c_N, nb), dev)
+            rc = lib.dsmil_value_forward_bags(P.ref, c_X, _ptr_array(vs), c_N, nb, _ptr(classes), _ptr(pred), _ptr(A),
+                                              _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(sV), _ptr(ws),
+                                              ws.numel(), _stream())
+            _lib.check(rc, "dsmil_value_forward_bags")
+        ctx.nb, ctx.Ns, ctx.c_N, ctx.nv = nb, Ns, c_N, 0 if vs is None else nb
+        ctx.save_for_backward(*xs, *(vs or ()), mask, sQ, sH, sV, A, B, crit, *P.tensors)
+        ctx.mark_non_differentiable(crit)
+        return classes, pred, A, B, crit
+
+    @staticmethod
+    def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
+        lib = _lib.load()
+        nb, nv, Ns, c_N = ctx.nb, ctx.nv, ctx.Ns, ctx.c_N
+        saved = ctx.saved_tensors
+        xs, vs = saved[:nb], saved[nb:nb + nv]
+        (mask, sQ, sH, sV, A, B, crit), params = saved[nb + nv:nb + nv + 7], saved[nb + nv + 7:]
+        P = ParamPack(*params)
+        need_bags, need_params = ctx.needs_input_grad[3:3 + nb], ctx.needs_input_grad[3 + nb:]
+        dev = P.device
+        with torch.cuda.device(dev):
+            out = {nm: (torch.empty_like(t) if t is not None and need else None)
+                   for nm, t, need in zip(PARAM_NAMES, P.tensors, need_params)}
+            gX = torch.empty(sum(Ns), P.D, dtype=torch.float32, device=dev) if any(need_bags) else None
+            G = _lib.DsmilGrads(*[_ptr(out[n]) for n in PARAM_NAMES], _ptr(gX))
+            dc, dp, dA, dB = (_f32c(t) for t in (g_classes, g_pred, g_A, g_B))
+            ws = _workspace(lib.dsmil_value_backward_bags_workspace_bytes(P.ref, c_N, nb, int(gX is not None)), dev)
+            rc = lib.dsmil_value_backward_bags(P.ref, _ptr_array(xs), _ptr_array(vs or None), c_N, nb, _ptr(sQ),
+                                               _ptr(sH), _ptr(sV), _ptr(A), _ptr(B), _ptr(crit), _ptr(dc), _ptr(dp),
+                                               _ptr(dA), _ptr(dB), _ptr(mask), C.byref(G), _ptr(ws), ws.numel(),
+                                               _stream())
+            _lib.check(rc, "dsmil_value_backward_bags")
+        gxs, lo = [], 0
+        for n, need in zip(Ns, need_bags):
+            gxs.append(gX[lo:lo + n] if need else None)
+            lo += n
+        return (None, None, None, *gxs, *[out[n] for n in PARAM_NAMES])
+
+
+def mil_forward_value_bags(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]],
+                           v_inputs: Optional[Sequence[torch.Tensor]] = None, *, grad: bool = False,
+                           v_masks: Optional[Sequence[torch.Tensor]] = None):
+    """Forward of a stream of bags for a model with a value network (passing_v), in one dsmil_value_forward_bags
+    call: returns a lazy sequence of (classes, prediction_bag, A, B) per bag plus crit_idx [nb, C], as
+    mil_forward_bags does.  v_inputs: each bag's value input (the features after the dropout mask of dsmil.py:36), or
+    None for the features themselves (eval mode, or p = 0).  Every bag's outputs are bit for bit what mil_forward
+    gives it alone with the same value input.
+
+    grad=False (default): inference under no_grad.  A batch of more than MAX_VALUE_BAGS bags is split into
+    consecutive calls that write into the same packed outputs.
+    grad=True with grad mode on: the packed outputs carry autograd history (MILValueBagsFn), and one backward over a
+    loss of them runs one dsmil_value_backward_bags call for the whole batch, at most MAX_VALUE_BAGS bags.  v_masks:
+    each bag's dropout mask (v_inputs[b] == bags[b] * v_masks[b]), for the value path's share of the bags' gradients,
+    required with v_inputs when a bag needs a gradient; None when there is no dropout."""
+    if grad and torch.is_grad_enabled():
+        nb = len(bags)
+        if nb > MAX_VALUE_BAGS:
+            raise ValueError(f"a differentiable value batch takes at most {MAX_VALUE_BAGS} bags, got {nb}")
+        _value_pack(params)   # identity v is refused before any work
+        if nb == 0:
+            return [], None
+        classes, pred, A, B, crit = MILValueBagsFn.apply(nb, v_inputs, v_masks, *bags, *params)
+        return BagOutputs(classes, pred, A, B, [int(b.shape[0]) for b in bags], crit), crit
+    return _mil_forward_value_bags_infer(bags, params, v_inputs)
+
+
+@torch.no_grad()
+def _mil_forward_value_bags_infer(bags, params, v_inputs):
+    lib = _lib.load()
+    P = _value_pack(params)
     nb = len(bags)
     if nb == 0:
         return [], None
     xs, Ns, _, _ = _bag_table(bags, P)
-    vs = None
-    if v_inputs is not None:
-        if len(v_inputs) != nb:
-            raise ValueError(f"{len(v_inputs)} value inputs for {nb} bags")
-        vs = [_check_feats(v, P.D) for v in v_inputs]
-        for v, x in zip(vs, xs):
-            if v.shape != x.shape or v.device != x.device:
-                raise ValueError(f"a value input {tuple(v.shape)} on {v.device} does not match its bag "
-                                 f"{tuple(x.shape)} on {x.device}")
+    vs = _per_bag(v_inputs, xs, P, "value input")
     total, Cc, D, dev = sum(Ns), P.C, P.D, P.device
     with torch.cuda.device(dev):
         new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)

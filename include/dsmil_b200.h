@@ -348,6 +348,28 @@ int dsmil_value_forward_bags(const dsmil_params_t* p, const float* const* Xs, co
                              const int64_t* Ns, int32_t nb, float* classes, float* pred, float* A, float* B,
                              int64_t* crit_idx, float* save_Q, float* save_H1, float* save_V, void* workspace,
                              size_t workspace_bytes, void* stream);
+/* Reverse of dsmil_value_forward_bags with saves, for all nb bags in one call: the training step of a passing_v model
+ * over a minibatch of bags.  Xs / XVs / Ns / nb as the forward took them (XVs NULL: the value inputs are Xs); Q, H1,
+ * V, A, B and crit_idx are the forward's outputs and saves, packed in bag order.  Upstream gradients are packed as in
+ * dsmil_backward_bags (d_classes / d_A [sum N,C], d_pred [nb,C], d_B [nb,C,D]; each may be NULL == zero).
+ * grads->g* are SUMS over the bags, gWv and gbv included; grads->gX, when non-NULL, is packed [sum N,D] and includes
+ * the value path.  v_mask [sum N,D] (or NULL == ones), packed in bag order like gX, is v's dropout mask: each value
+ * input is its features times the mask (XVs[b] == Xs[b] * rows of v_mask, as dsmil_backward's x_for_v / v_mask);
+ * only gX reads it.  One launch per stage for the whole batch, whatever nb, every kernel one the identity-v and
+ * single-bag backwards already run.  Any D and C of dsmil_value_bags_supported and any alignment of the bags; split
+ * sums follow the shapes only and there are no float atomics, so two runs give the same bits.
+ * Workspace: besides the [sum N,D] buffers (dzv, and dzv Wv with gX), gWv = dzv^T Xv keeps one D x D partial per chunk
+ * of the value inputs, and every bag is at least one chunk: about (296 / ceil(D/128)^2 + nb) * D^2 * 4 bytes, so a
+ * batch of many small bags at a large D needs a large workspace (1000 bags at D = 512: about 1 GB).
+ * Identity v, nb outside [1, 65535], a missing save or a batch whose ragged GEMMs would need more than 65535 chunks
+ * (only near nb = 65535) is DSMIL_ERR_ARG; an empty bag DSMIL_ERR_EMPTY; a short workspace DSMIL_ERR_WORKSPACE.  The
+ * workspace size is 0 for every batch the call refuses with DSMIL_ERR_ARG or DSMIL_ERR_EMPTY. */
+size_t dsmil_value_backward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb, int need_gX);
+int dsmil_value_backward_bags(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
+                              const int64_t* Ns, int32_t nb, const float* Q, const float* H1, const float* V,
+                              const float* A, const float* B, const int64_t* crit_idx, const float* d_classes,
+                              const float* d_pred, const float* d_A, const float* d_B, const float* v_mask,
+                              const dsmil_grads_t* grads, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Call form (2)+(3) of the boundary (SURVEY §8b): the callers in attention_map.py:74,85 /
  * testing_tcga.py:72,83 run the instance classifier and the bag classifier separately.
