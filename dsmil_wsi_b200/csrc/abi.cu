@@ -636,18 +636,21 @@ static bool value_shape(const dsmil_params_t* p) {
 // ---- the route of an eager forward -----------------------------------------------------------------------------------
 // One rule for every eager forward of nb bags: the tensor-core batch where the shape takes it and every bag is 16-byte
 // aligned; off that batch (the generic shapes and passing_v) the generic batch, unless its phase 1 is k_qmlp_sm90 and
-// a bag is not aligned, or nb passes the 65535 bags its grids number in y and z; otherwise one bag at a time.
+// a bag is not aligned; otherwise one bag at a time.  Either batch numbers its bags in grid y (k_finalize_b, the
+// generic per-bag kernels), so past 65535 bags every shape takes the loop.
 enum Route : unsigned { ROUTE_TC = 1, ROUTE_GEN = 2, ROUTE_LOOP = 4 };
 static Route bags_route(const dsmil_params_t* p, int nb, bool aligned) {
+  if (nb > 65535) return ROUTE_LOOP;
   if (sm90::batched_supported(p)) return aligned ? ROUTE_TC : ROUTE_LOOP;
-  return nb <= 65535 && (aligned || !sm90::qmlp_supported(p)) ? ROUTE_GEN : ROUTE_LOOP;
+  return aligned || !sm90::qmlp_supported(p) ? ROUTE_GEN : ROUTE_LOOP;
 }
 // The routes bags_route gives nb bags of this shape at either alignment.
 static unsigned bags_routes(const dsmil_params_t* p, int nb) {
   return bags_route(p, nb, true) | bags_route(p, nb, false);
 }
 // The workspace of an eager forward of these bags that may take any of `routes` (Route bits): the largest of their
-// carves as inference takes them.  The loop's is the single-bag forward's carve for the largest bag.
+// carves as inference takes them.  The loop's is the single-bag forward's for the largest bag: the single-bag kernels'
+// carve and, where forward_impl takes an aligned bag to the tensor-core batch of one, that batch's.
 static size_t routes_ws_bytes(const dsmil_params_t* p, const int64_t* Ns, int nb, unsigned routes) {
   bool ok;
   size_t bytes = 0;
@@ -657,6 +660,8 @@ static size_t routes_ws_bytes(const dsmil_params_t* p, const int64_t* Ns, int nb
     int64_t mx = 0;
     for (int b = 0; b < nb; ++b) mx = std::max<int64_t>(mx, Ns[b]);
     bytes = std::max(bytes, carve_fwd(p, mx, nullptr, 0, &ok).bytes);
+    if (mx > 0 && bags_route(p, 1, true) == ROUTE_TC)
+      bytes = std::max(bytes, carve_bags(p, &mx, 1, true, false, nullptr, 0, &ok).bytes);
   }
   return bytes;
 }
@@ -839,8 +844,7 @@ size_t dsmil_rec_floats(int32_t C, int32_t Dv) { return rec_floats(C, Dv); }
 
 size_t dsmil_forward_workspace_bytes(const dsmil_params_t* p, int64_t N) {
   if (!p || p->C < 1 || p->C > DSMIL_MAX_C || p->D < 1 || p->D > DSMIL_MAX_D || N < 0) return 0;
-  // forward_impl takes the rule's tensor-core batch of one bag, else the single-bag kernels (the loop's carve)
-  return routes_ws_bytes(p, &N, 1, ROUTE_LOOP | (N > 0 ? bags_routes(p, 1) & ROUTE_TC : 0));
+  return routes_ws_bytes(p, &N, 1, ROUTE_LOOP);   // the loop's carve is forward_impl's
 }
 
 size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
@@ -1646,8 +1650,9 @@ static int value_backward_bags_impl(const dsmil_params_t* p, const float* const*
 int dsmil_shard_bags_supported(const dsmil_params_t* p) {
   return (p && p->C >= 1 && p->C <= DSMIL_MAX_C && p->D >= 1 && p->D <= DSMIL_MAX_D && sm90::batched_supported(p)) ? 1 : 0;
 }
+// The batch numbers its bags in grid y (k_gather_cand_b, k_merge_cand, k_finalize_b): 1 <= nb <= 65535.
 size_t dsmil_shard_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
-  if (!dsmil_shard_bags_supported(p) || !Ns || nb < 1) return 0;
+  if (!dsmil_shard_bags_supported(p) || !Ns || nb < 1 || nb > 65535) return 0;
   bool ok;
   return carve_bags(p, Ns, nb, true, true, nullptr, 0, &ok).bytes;
 }
@@ -1690,7 +1695,8 @@ int dsmil_shard_bags_phase1(const dsmil_params_t* p, const float* const* Xs, con
   int rc = check_params(p, true);
   if (rc) return rc;
   DSMIL_REQUIRE(dsmil_shard_bags_supported(p), "shape not supported by the batched tensor-core path");
-  DSMIL_REQUIRE(Xs && Ns && nb >= 1 && row_offsets && classes && cand_recs, "NULL pointer or nb < 1");
+  DSMIL_REQUIRE(Xs && Ns && row_offsets && classes && cand_recs, "NULL pointer");
+  DSMIL_REQUIRE(nb >= 1 && nb <= 65535, "nb=%d outside [1, 65535]", nb);
   bool ok;
   BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
@@ -1702,8 +1708,9 @@ int dsmil_shard_bags_phase2(const dsmil_params_t* p, const float* const* Xs, con
                             void* workspace, size_t workspace_bytes, void* stream) {
   int rc = check_params(p, true);
   if (rc) return rc;
-  DSMIL_REQUIRE(dsmil_shard_bags_supported(p) && Xs && Ns && nb >= 1 && cands_all && G >= 1 && A && crit_idx && recs_out,
+  DSMIL_REQUIRE(dsmil_shard_bags_supported(p) && Xs && Ns && cands_all && G >= 1 && A && crit_idx && recs_out,
                 "bad arguments");
+  DSMIL_REQUIRE(nb >= 1 && nb <= 65535, "nb=%d outside [1, 65535]", nb);
   bool ok;
   BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
   if ((rc = check_workspace(w.bytes, ok, workspace, workspace_bytes))) return rc;
@@ -1718,8 +1725,9 @@ int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, con
                             size_t workspace_bytes, void* stream) {
   int rc = check_params(p, true);
   if (rc) return rc;
-  DSMIL_REQUIRE(dsmil_shard_bags_supported(p) && Xs && Ns && nb >= 1 && recs_all && G >= 1 && G <= sm90::kMaxRecPerBag && A && B && pred,
+  DSMIL_REQUIRE(dsmil_shard_bags_supported(p) && Xs && Ns && recs_all && G >= 1 && G <= sm90::kMaxRecPerBag && A && B && pred,
                 "bad arguments");
+  DSMIL_REQUIRE(nb >= 1 && nb <= 65535, "nb=%d outside [1, 65535]", nb);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   bool ok;
   BagsWs w = carve_bags(p, Ns, nb, true, true, workspace, workspace_bytes, &ok);
@@ -2440,9 +2448,15 @@ static int forward_bags_dev(Route r, bool train, const dsmil_params_t* p, const 
                               overlap);
 }
 
+// The backward pair's ragged GEMMs launch one CTA per chunk of the capacity in grid z (k_gemm_tn_rag) or x
+// (k_gemv_tn_rag), which holds at most 65535 of them: rag_splits plus one short chunk per bag.
+static bool dev_chunks_ok(const dsmil_params_t* p, int nb) {
+  return rag_chunks_cap(p->C, p->D, true, nb) <= 65535 && rag_chunks_cap(p->C, p->D, false, nb) <= 65535 &&
+         rag_chunks_cap(kQ, p->D, false, nb) <= 65535;
+}
 // The backward pair's size.  The generic route also covers the eager backward's carve.
 static size_t backward_bags_dev_ws(Route r, const dsmil_params_t* p, int nb, int64_t max_rows) {
-  if (!dev_shape(r, p) || !dev_sizes(nb, max_rows)) return 0;
+  if (!dev_shape(r, p) || !dev_sizes(nb, max_rows) || !dev_chunks_ok(p, nb)) return 0;
   bool ok;
   const size_t dev = carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
   if (r == ROUTE_TC) return dev;
@@ -2463,6 +2477,7 @@ static int backward_bags_dev(Route r, const dsmil_params_t* p, const float* cons
   DSMIL_REQUIRE(Q && (!p->nonlinear || H1) && A && B && crit_idx && grads, "NULL pointer");
   DSMIL_REQUIRE(!d_A && !d_B && !grads->gX,
                 "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
+  DSMIL_REQUIRE(dev_chunks_ok(p, nb), "nb=%d: the chunk capacity of the ragged GEMMs passes 65535", nb);
   if ((rc = need_workspace(backward_bags_dev_ws(r, p, nb, max_rows), workspace, workspace_bytes))) return rc;
   bool ok;
   BwdBagsWs w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);

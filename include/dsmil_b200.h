@@ -143,8 +143,8 @@ int dsmil_forward(const dsmil_params_t* p, const float* X, const float* x_for_v,
  * q form) run one launch per stage for the whole batch, every bag's outputs bit for bit what
  * dsmil_forward gives it alone; on those of them whose phase 1 is k_qmlp_sm90 (nonlinear q,
  * D % 128 == 0) a bag that is not 16-byte aligned makes the batch loop.  passing_v takes the value
- * batch of dsmil_value_forward_bags (value inputs = Xs) on the same terms.  Off the tensor-core
- * shapes a batch of more than 65535 bags loops. */
+ * batch of dsmil_value_forward_bags (value inputs = Xs) on the same terms.  On every shape a batch
+ * of more than 65535 bags loops dsmil_forward, bag by bag. */
 size_t dsmil_forward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb);
 int dsmil_forward_bags(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                        float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
@@ -233,7 +233,9 @@ int dsmil_backward_bags_models(const dsmil_params_t* ps, int32_t M, const float*
  * the W1/W2 weight images on every call, so a replay after an optimizer step uses the current weights.
  * Shapes: those of dsmil_shard_bags_supported (identity v).  Gradients through classes and pred only: d_A, d_B and
  * grads->gX must be NULL (DSMIL_ERR_ARG).  On the same bags the results are the eager calls' bits.
- * 1 <= nb <= 65535, max_rows >= 1; a short workspace is DSMIL_ERR_WORKSPACE.  The workspace sizes depend on
+ * 1 <= nb <= 65535, max_rows >= 1; the backward also needs its ragged GEMMs' chunk capacity (a few hundred chunks plus
+ * one per bag) within 65535, else DSMIL_ERR_ARG and a workspace size of 0, which happens only within a few hundred bags
+ * of 65535.  A short workspace is DSMIL_ERR_WORKSPACE.  The workspace sizes depend on
  * (nb, max_rows) only and are never below the eager calls' for nb bags of max_rows rows. */
 size_t dsmil_forward_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
 int dsmil_forward_bags_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
@@ -458,7 +460,9 @@ int dsmil_shard_backward_phase3(const dsmil_params_t* p, const float* X, int64_t
  * calls (it carries Q, the bag table and the per-tile partial records between the phases).
  *   phase1 -> classes (packed), cand_recs [nb][dsmil_cand_floats(C)]
  *   phase2 (cands_all [G][nb][cand]) -> A (logits, packed), crit_idx [nb][C], recs_out [nb][dsmil_rec_floats(C,D)]
- *   phase3 (recs_all  [G][nb][rec])  -> A normalised, B [nb][C][D], pred [nb][C] */
+ *   phase3 (recs_all  [G][nb][rec])  -> A normalised, B [nb][C][D], pred [nb][C]
+ * 1 <= nb <= 65535 (the kernels number the bags in grid y): another nb is DSMIL_ERR_ARG in every phase, and
+ * dsmil_shard_bags_workspace_bytes returns 0 for it. */
 int dsmil_shard_bags_supported(const dsmil_params_t* p);
 size_t dsmil_shard_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb);
 int dsmil_shard_bags_phase1(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,

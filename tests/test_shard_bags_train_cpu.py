@@ -105,6 +105,26 @@ def test_entry_point_validation(fn):
     assert fn(lib, p, Xs, n, offs, 3, FAKE, need - 1) == ERR_WORKSPACE and "workspace too small" in last_error(lib)
 
 
+def test_inference_phases_refuse_more_than_65535_bags():
+    """dsmil_shard_bags_phase1/2/3 number the bags in grid y, as the training phases do: outside [1, 65535] each is
+    DSMIL_ERR_ARG before any launch, and the workspace size is 0."""
+    lib = _lib.load()
+    p = params()
+    Xs, n, offs = arrays([3] * 65536)
+    calls = {
+        "phase1": lambda nb: lib.dsmil_shard_bags_phase1(C.byref(p), Xs, n, nb, offs, FAKE, FAKE, FAKE, 1 << 40, None),
+        "phase2": lambda nb: lib.dsmil_shard_bags_phase2(C.byref(p), Xs, n, nb, FAKE, 2, FAKE, FAKE, FAKE, FAKE,
+                                                         1 << 40, None),
+        "phase3": lambda nb: lib.dsmil_shard_bags_phase3(C.byref(p), Xs, n, nb, FAKE, 2, FAKE, FAKE, FAKE, FAKE,
+                                                         1 << 40, None),
+    }
+    for name, call in calls.items():
+        for nb in (0, 65536, 70000):
+            assert call(nb) == ERR_ARG and f"nb={nb} outside [1, 65535]" in last_error(lib), (name, nb)
+    assert lib.dsmil_shard_bags_workspace_bytes(C.byref(p), n, 65536) == 0
+    assert lib.dsmil_shard_bags_workspace_bytes(C.byref(p), n, 65535) > 0
+
+
 def test_backward_phase1_optional_buffers_pass_validation():
     """d_classes, d_pred and every gradient buffer may be NULL: those arguments fail nothing before the workspace."""
     lib = _lib.load()

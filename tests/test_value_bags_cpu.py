@@ -111,15 +111,23 @@ def test_workspace_sizes(D, C_, nl):
     assert lib.dsmil_value_forward_bags_workspace_bytes(C.byref(params(D, C_, nl, passing_v=0)), ns(10), 1) == 0
 
 
-@pytest.mark.parametrize("D,C_,nl,pv", [(166, 1, 1, 0), (512, 3, 0, 0), (512, 2, 1, 1), (166, 1, 1, 1)])
+@pytest.mark.parametrize("D,C_,nl,pv", [(166, 1, 1, 0), (512, 3, 0, 0), (512, 2, 1, 1), (166, 1, 1, 1), (512, 2, 1, 0),
+                                        (128, 1, 1, 0)])
 def test_forward_bags_workspace_covers_its_routes(D, C_, nl, pv):
-    """dsmil_forward_bags off the tensor-core batch (the generic shapes, passing_v): past 65 535 bags the batch loops the
-    single-bag forward, and on passing_v up to 65 535 bags it takes the value batch; the size covers either."""
+    """dsmil_forward_bags past 65 535 bags loops the single-bag forward on every shape, and on passing_v up to 65 535
+    bags it takes the value batch; the size covers either.  On the tensor-core shapes the loop is all the batch takes
+    past 65 535 bags: the size is then the single-bag forward's for the largest bag, which itself covers that bag's
+    tensor-core batch of one."""
     lib = _lib.load()
     p = C.byref(params(D, C_, nl, pv))
     Ns = [1 + i % 300 for i in range(65536)]
     Ns[7] = 10000
     assert lib.dsmil_forward_bags_workspace_bytes(p, ns(*Ns), 65536) >= lib.dsmil_forward_workspace_bytes(p, 10000)
+    if lib.dsmil_shard_bags_supported(p):
+        assert lib.dsmil_forward_bags_workspace_bytes(p, ns(*Ns), 65536) == lib.dsmil_forward_workspace_bytes(p, 10000)
+        assert lib.dsmil_forward_bags_workspace_bytes(p, ns(*Ns[:65535]), 65535) > lib.dsmil_forward_workspace_bytes(p, 10000)
+        assert (lib.dsmil_forward_workspace_bytes(p, 10000) >=
+                lib.dsmil_forward_bags_workspace_bytes(p, ns(10000), 1) > lib.dsmil_forward_workspace_bytes(p, 9000))
     if pv:
         assert (lib.dsmil_forward_bags_workspace_bytes(p, ns(*Ns[:16]), 16) >=
                 lib.dsmil_value_forward_bags_workspace_bytes(p, ns(*Ns[:16]), 16) > 0)
