@@ -74,7 +74,14 @@ SIGNATURES = {
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.POINTER(DsmilGrads), C.c_void_p,
                                             C.c_size_t, C.c_void_p]),
-    "dsmil_instance_scores": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, c_i64, C.c_void_p, C.c_void_p]),
+    "dsmil_value_forward_bags_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
+    "dsmil_value_forward_bags_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                               c_i64] + [C.c_void_p] * 9 + [C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_value_backward_bags_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32, c_i64]),
+    "dsmil_value_backward_bags_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_int32, c_i64] + [C.c_void_p] * 10 +
+                                      [C.POINTER(DsmilGrads), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_instance_scores":(C.c_int, [C.POINTER(DsmilParams), C.c_void_p, c_i64, C.c_void_p, C.c_void_p]),
     "dsmil_instance_scores_backward": (C.c_int, [C.POINTER(DsmilParams), C.c_void_p, c_i64, C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                                  C.c_void_p]),

@@ -637,8 +637,9 @@ static bool value_shape(const dsmil_params_t* p) {
 // One rule for every eager forward of nb bags: the tensor-core batch where the shape takes it and every bag is 16-byte
 // aligned; off that batch (the generic shapes and passing_v) the generic batch, unless its phase 1 is k_qmlp_sm90 and
 // a bag is not aligned; otherwise one bag at a time.  Either batch numbers its bags in grid y (k_finalize_b, the
-// generic per-bag kernels), so past 65535 bags every shape takes the loop.
-enum Route : unsigned { ROUTE_TC = 1, ROUTE_GEN = 2, ROUTE_LOOP = 4 };
+// generic per-bag kernels), so past 65535 bags every shape takes the loop.  ROUTE_VAL names the capture-safe calls'
+// value route (the generic batch of a passing_v model); no eager forward takes it.
+enum Route : unsigned { ROUTE_TC = 1, ROUTE_GEN = 2, ROUTE_LOOP = 4, ROUTE_VAL = 8 };
 static Route bags_route(const dsmil_params_t* p, int nb, bool aligned) {
   if (nb > 65535) return ROUTE_LOOP;
   if (sm90::batched_supported(p)) return aligned ? ROUTE_TC : ROUTE_LOOP;
@@ -1573,10 +1574,21 @@ struct ValueBwdWs {
   TnChunk* chv;              // gWv chunks over the value inputs
   float *dzv, *tmp;          // [total, D]; tmp (gX only) holds dzv Wv
   float *tnpart, *cspart;    // gWv's chunk partials, gbv's split partials
-  int ncv;
+  sm90::BagDev* vtab;        // dev calls: the planner's value table [2 nb]
+  int ncv;                   // gWv chunks (dev calls: the capacity, the live count in w.b.plan->pad_)
   int64_t rps_v;
   size_t bytes;
 };
+// The value tail's regions after w.b, for nb bags, n packed rows and w.ncv gWv chunks.
+static void layout_value_bwd(Carver& c, const dsmil_params_t* p, int nb, int64_t n, bool need_gX, ValueBwdWs& w) {
+  const int D = p->D;
+  w.segs = c.take<LinSeg>(nb);
+  w.chv = c.take<TnChunk>(w.ncv);
+  w.dzv = c.take<float>(n * D);
+  w.tmp = need_gX ? c.take<float>(n * D) : nullptr;
+  w.tnpart = c.take<float>(static_cast<size_t>(w.ncv) * D * D);
+  w.cspart = c.take<float>(static_cast<size_t>(kSplits) * D);
+}
 static ValueBwdWs carve_value_bwd(const dsmil_params_t* p, const int64_t* Ns, int nb, bool aligned, bool need_gX,
                                   void* ws, size_t cap, bool* ok) {
   ValueBwdWs w;
@@ -1584,19 +1596,31 @@ static ValueBwdWs carve_value_bwd(const dsmil_params_t* p, const int64_t* Ns, in
   w.b = carve_bwd_bags(p, Ns, nb, aligned, false, ws, cap, ok);
   int64_t total = 0;
   for (int b = 0; b < nb; ++b) total += Ns[b];
-  const int64_t n = std::max<int64_t>(total, 1);
   w.rps_v = rag_rows_per_chunk(D, D, total, false);
   w.ncv = rag_chunks(nullptr, Ns, nb, D, w.rps_v, nullptr);
+  w.vtab = nullptr;
   Carver c(ws, cap);
   c.off = w.b.bytes;
-  w.segs = c.take<LinSeg>(nb);
-  w.chv = c.take<TnChunk>(w.ncv);
-  w.dzv = c.take<float>(n * D);
-  w.tmp = need_gX ? c.take<float>(n * D) : nullptr;
-  w.tnpart = c.take<float>(static_cast<size_t>(w.ncv) * D * D);
-  w.cspart = c.take<float>(static_cast<size_t>(kSplits) * D);
+  layout_value_bwd(c, p, nb, std::max<int64_t>(total, 1), need_gX, w);
   w.bytes = c.off;
-  *ok = c.ok();
+  *ok = c.ok() && *ok;
+  return w;
+}
+// A dev call's carve: carve_bwd_bags_dev's, the value tail at its capacities (the gWv partials for
+// rag_chunks_cap(D, D, false, nb) chunks) and the planner's value table.  The phases run on its second half (X = the
+// packed V rows), w.b.table holds the planner's table of the features.
+static ValueBwdWs carve_value_bwd_dev(const dsmil_params_t* p, int nb, int64_t max_rows, void* ws, size_t cap,
+                                      bool* ok) {
+  ValueBwdWs w;
+  w.b = carve_bwd_bags_dev(p, nb, max_rows, ws, cap, ok);
+  w.rps_v = 0;
+  w.ncv = rag_chunks_cap(p->D, p->D, false, nb);
+  Carver c(ws, cap);
+  c.off = w.b.bytes;
+  layout_value_bwd(c, p, nb, static_cast<int64_t>(nb) * max_rows, false, w);
+  w.vtab = c.take<sm90::BagDev>(2 * static_cast<size_t>(nb));
+  w.bytes = c.off;
+  *ok = c.ok() && *ok;
   return w;
 }
 
@@ -1604,35 +1628,29 @@ static ValueBwdWs carve_value_bwd(const dsmil_params_t* p, const int64_t* Ns, in
 // does (rag_splits is the same for C and 128 left columns), so nc1 bounds it at either alignment.
 static bool value_bwd_grids_ok(const ValueBwdWs& w) { return w.ncv <= 65535 && w.b.nc1 <= 65535; }
 
-static int value_backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
-                                    const int64_t* Ns, int nb, int64_t total, const float* Q, const float* H1,
-                                    const float* V, const float* A, const float* B, const int64_t* crit,
-                                    const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
-                                    const float* v_mask, const dsmil_grads_t* g, const ValueBwdWs& w,
-                                    cudaStream_t st) {
+// The value backward over tables already in w: the three phases with the packed V in w.b.table (dA = V dB_b^T), then
+// dzv over w.segs, gWv over w.chv and gbv, and the eager call's gX.  mx: the largest bag (dev calls: max_rows).  In a
+// dev call (w.b.plan != NULL) `total` is the row capacity and the GEMMs read their live counts from the plan.
+static int value_backward_run(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
+                              int64_t total, int64_t mx, const float* Q, const float* H1, const float* V,
+                              const float* A, const float* B, const int64_t* crit, const float* d_classes,
+                              const float* d_pred, const float* d_A, const float* d_B, const float* v_mask,
+                              const dsmil_grads_t* g, const ValueBwdWs& w, cudaStream_t st) {
   const int C = p->C, D = p->D;
   const BwdBagsWs& wb = w.b;
+  const BagsPlan* pl = wb.plan;
   int rc;
   const float* dz1;
   if ((rc = bwd_bags_phase1_impl(p, Xs, Ns, nb, total, A, B, d_classes, d_pred, d_A, d_B, g, wb.dA, wb, st, V)) ||
-      (rc = bwd_bags_phase2_impl(p, nb, A, wb.dA, wb.tpart, wb.G, Q, wb.dL, wb.dqm, wb, st)) ||
+      (rc = bwd_bags_phase2_impl(p, nb, A, wb.dA, wb.tpart, pl ? 0 : wb.G, Q, wb.dL, wb.dqm, wb, st)) ||
       (rc = bwd_bags_phase3_impl(p, nb, total, Q, H1, wb.dL, wb.dqm, nullptr, crit, nullptr, g, wb, &dz1, st)))
     return rc;
-  std::vector<LinSeg> segs(nb);
-  std::vector<TnChunk> chv(w.ncv);
-  int64_t row = 0, mx = 1;
-  for (int b = 0; b < nb; ++b) {
-    segs[b] = LinSeg{A + row * C, wb.dB + static_cast<size_t>(b) * C * D, V + row * D, w.dzv + row * D, Ns[b]};
-    mx = std::max<int64_t>(mx, Ns[b]);
-    row += Ns[b];
-  }
-  rag_chunks(XVs ? XVs : Xs, Ns, nb, D, w.rps_v, chv.data());
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.segs, segs.data(), sizeof(LinSeg) * nb, cudaMemcpyHostToDevice, st));
-  DSMIL_CUDA_OK(cudaMemcpyAsync(w.chv, chv.data(), sizeof(TnChunk) * w.ncv, cudaMemcpyHostToDevice, st));
   k_linear_models<ACT_MASK_POS, true><<<dim3(ceil_div(mx, LBM), ceil_div(D, LBN), nb), 256, 0, st>>>(w.segs, C, D);
   DSMIL_LAUNCH_OK("k_linear_models");
-  if (g->gWv && (rc = launch_gemm_tn_rag(w.dzv, D, D, w.chv, w.ncv, false, w.tnpart, g->gWv, st))) return rc;
-  if (g->gbv && (rc = launch_colsum(w.dzv, D, total, w.cspart, g->gbv, st))) return rc;
+  if (g->gWv &&
+      (rc = launch_gemm_tn_rag(w.dzv, D, D, w.chv, w.ncv, false, w.tnpart, g->gWv, st, pl ? &pl->pad_ : nullptr)))
+    return rc;
+  if (g->gbv && (rc = launch_colsum(w.dzv, D, total, w.cspart, g->gbv, st, pl ? &pl->cs : nullptr))) return rc;
   if (!g->gX) return 0;
   const int ge = static_cast<int>(std::min<int64_t>(ceil_div(total * D, 256), kSms * 8));
   if ((rc = launch_linear<ACT_NONE, true>(dz1, total, kQ, p->W1, nullptr, D, g->gX, nullptr, 0, st))) return rc;
@@ -1644,6 +1662,30 @@ static int value_backward_bags_impl(const dsmil_params_t* p, const float* const*
   k_axpy_mask<<<ge, 256, 0, st>>>(w.tmp, v_mask, total * D, g->gX);
   DSMIL_LAUNCH_OK("k_axpy_mask");
   return 0;
+}
+
+// The eager value backward: the dzv segments and the gWv chunks built on the host and uploaded, then the shared run
+// (phase 1 uploads the V table and the chunks of gWi and gW1).
+static int value_backward_bags_impl(const dsmil_params_t* p, const float* const* Xs, const float* const* XVs,
+                                    const int64_t* Ns, int nb, int64_t total, const float* Q, const float* H1,
+                                    const float* V, const float* A, const float* B, const int64_t* crit,
+                                    const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                                    const float* v_mask, const dsmil_grads_t* g, const ValueBwdWs& w,
+                                    cudaStream_t st) {
+  const int C = p->C, D = p->D;
+  std::vector<LinSeg> segs(nb);
+  std::vector<TnChunk> chv(w.ncv);
+  int64_t row = 0, mx = 1;
+  for (int b = 0; b < nb; ++b) {
+    segs[b] = LinSeg{A + row * C, w.b.dB + static_cast<size_t>(b) * C * D, V + row * D, w.dzv + row * D, Ns[b]};
+    mx = std::max<int64_t>(mx, Ns[b]);
+    row += Ns[b];
+  }
+  rag_chunks(XVs ? XVs : Xs, Ns, nb, D, w.rps_v, chv.data());
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.segs, segs.data(), sizeof(LinSeg) * nb, cudaMemcpyHostToDevice, st));
+  DSMIL_CUDA_OK(cudaMemcpyAsync(w.chv, chv.data(), sizeof(TnChunk) * w.ncv, cudaMemcpyHostToDevice, st));
+  return value_backward_run(p, Xs, Ns, nb, total, mx, Q, H1, V, A, B, crit, d_classes, d_pred, d_A, d_B, v_mask, g, w,
+                            st);
 }
 
 // ---- sharded batch ABI ---------------------------------------------------------------------------
@@ -2306,14 +2348,21 @@ int dsmil_shard_backward_bags_phase3(const dsmil_params_t* p, const float* const
 
 
 // ---- capture-safe batched training: the bag list in device memory, every launch sized for a capacity -------------
-// Two routes (Route): the tensor-core batch (dsmil_*_dev, planned by k_plan_bags) and the generic shapes
-// (dsmil_generic_*_dev, planned by k_plan_bags_gen).  Each pair of calls shares one body.
+// Three routes (Route): the tensor-core batch (dsmil_*_dev, planned by k_plan_bags), the generic shapes
+// (dsmil_generic_*_dev, planned by k_plan_bags_gen) and the value network (dsmil_value_*_dev: the generic batch of a
+// passing_v model, planned by k_plan_bags_gen with its value tables).  Each pair of calls shares one body.
 static bool dev_shape(Route r, const dsmil_params_t* p) {
-  return r == ROUTE_TC ? dsmil_shard_bags_supported(p) != 0 : dsmil_generic_bags_supported(p) != 0;
+  if (r == ROUTE_TC) return dsmil_shard_bags_supported(p) != 0;
+  return (r == ROUTE_VAL ? dsmil_value_bags_supported(p) : dsmil_generic_bags_supported(p)) != 0;
 }
 // The batch every dev call sizes: 1 <= nb <= 65535 bags of at most max_rows < 2^32 rows.
 static bool dev_sizes(int nb, int64_t max_rows) {
   return nb >= 1 && nb <= 65535 && max_rows >= 1 && max_rows < 0xffffffffll;
+}
+// The 128-row tiles of nb bags of max_rows rows, which the kernels number in an int (twice over off the tensor-core
+// route, for k_linear_b's grid).
+static bool dev_tiles_ok(Route r, int nb, int64_t max_rows) {
+  return (r == ROUTE_TC ? 1 : 2) * static_cast<int64_t>(nb) * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) <= INT_MAX;
 }
 // A dev call's workspace is never below the eager call's for the same capacity: one buffer serves both forms.
 static size_t not_below_eager(size_t dev, size_t (*eager)(const dsmil_params_t*, const int64_t*, int32_t),
@@ -2333,24 +2382,26 @@ static int check_bags_dev(Route r, const dsmil_params_t* p, bool need_scores, bo
     DSMIL_REQUIRE(dsmil_shard_bags_supported(p),
                   "shape not supported by the batched tensor-core path (D=%d, C=%d, nonlinear=%d, passing_v=%d)", p->D,
                   p->C, p->nonlinear, p->passing_v);
+  else if (r == ROUTE_VAL)
+    DSMIL_REQUIRE(dsmil_value_bags_supported(p),
+                  "the value calls take passing_v models with Wv and bv (D=%d, C=%d, nonlinear=%d, passing_v=%d)",
+                  p->D, p->C, p->nonlinear, p->passing_v);
   else
     DSMIL_REQUIRE(dsmil_generic_bags_supported(p),
                   "shape not on the generic batched route, i.e. identity v off dsmil_shard_bags_supported (D=%d, C=%d, "
                   "nonlinear=%d, passing_v=%d)", p->D, p->C, p->nonlinear, p->passing_v);
   DSMIL_REQUIRE(!need_list || (Xs && Ns && status), "NULL bag list or status");
   DSMIL_REQUIRE(nb >= 1 && nb <= 65535, "nb=%d outside [1, 65535]", nb);
-  DSMIL_REQUIRE(max_rows >= 1 && max_rows < 0xffffffffll &&
-                (r == ROUTE_TC ? 1 : 2) * static_cast<int64_t>(nb) * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) <=
-                    INT_MAX,
+  DSMIL_REQUIRE(max_rows >= 1 && max_rows < 0xffffffffll && dev_tiles_ok(r, nb, max_rows),
                 "max_rows=%lld out of range for nb=%d", (long long)max_rows, nb);
   return 0;
 }
 
 // The route's planner over the device bag list: the table, the live counts and, when chi / ch1 are non-NULL, the
-// backward's chunk tables.
+// backward's chunk tables; on the value route also the value tables of v.
 static int launch_plan_dev(Route r, const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int nb,
                            int64_t max_rows, float* zero_row, sm90::BagDev* table, TnChunk* chi, TnChunk* ch1,
-                           BagsPlan* plan, int32_t* status, cudaStream_t st) {
+                           BagsPlan* plan, int32_t* status, cudaStream_t st, const PlanValue& v = PlanValue{}) {
   if (r == ROUTE_TC) {
     k_plan_bags<<<1, 32, 0, st>>>(Xs, Ns, nb, max_rows, p->C, p->D, zero_row, table, chi, ch1, plan, status, nullptr,
                                   nullptr);
@@ -2358,7 +2409,7 @@ static int launch_plan_dev(Route r, const dsmil_params_t* p, const float* const*
   } else {
     // the alignment rule (gen_bag_aligned) keeps each form the eager call would choose: gWi streams (tn_use_gemv) only
     // where D % 4 == 0, and there the bags are 16-byte aligned
-    k_plan_bags_gen<<<1, 32, 0, st>>>(Xs, Ns, nb, max_rows, p->C, p->D, zero_row, table, chi, ch1, plan, status);
+    k_plan_bags_gen<<<1, 32, 0, st>>>(Xs, Ns, nb, max_rows, p->C, p->D, zero_row, table, chi, ch1, plan, status, v);
     DSMIL_LAUNCH_OK("k_plan_bags_gen");
   }
   return 0;
@@ -2398,6 +2449,7 @@ static int bags_phase1_dev(const dsmil_params_t* p, const BagsWs& w, const BagsP
 // The forward pair's size: train keeps Q (+ H1) in the caller's saves, inference in the workspace.
 static size_t forward_bags_dev_ws(Route r, bool train, const dsmil_params_t* p, int nb, int64_t max_rows) {
   if (!dev_shape(r, p) || !dev_sizes(nb, max_rows)) return 0;
+  if (r == ROUTE_VAL && !dev_tiles_ok(r, nb, max_rows)) return 0;   // the value calls size no batch they refuse
   bool ok;
   size_t dev;
   if (r == ROUTE_TC) {
@@ -2407,6 +2459,7 @@ static size_t forward_bags_dev_ws(Route r, bool train, const dsmil_params_t* p, 
   } else {
     dev = carve_gen_dev(p, nb, max_rows, train, nullptr, 0, &ok).bytes;
   }
+  if (r == ROUTE_VAL) return not_below_eager(dev, dsmil_value_forward_bags_workspace_bytes, p, nb, max_rows);
   return not_below_eager(dev, train ? dsmil_forward_bags_train_workspace_bytes : dsmil_forward_bags_workspace_bytes, p,
                          nb, max_rows);
 }
@@ -2415,25 +2468,29 @@ static size_t forward_bags_dev_ws(Route r, bool train, const dsmil_params_t* p, 
 // capacity grids.  train: Q (+ H1) into save_Q (save_H1).  Inference keeps Q in the workspace (tile blocks on the
 // tensor-core route), and there the attend pass is a programmatic dependent of phase 1 as in dsmil_forward_bags --
 // under stream capture too, where the launch attribute becomes a programmatic edge of the graph (DESIGN §4.3).  Only
-// kernel timing keeps the plain launch.
+// kernel timing keeps the plain launch.  The value route (XVs_dev: the value inputs, NULL: the features) also keeps
+// V in save_V when training, and runs the value projection of the planner's value table.
 static int forward_bags_dev(Route r, bool train, const dsmil_params_t* p, const float* const* Xs_dev,
                             const int64_t* Ns_dev, int nb, int64_t max_rows, float* classes, float* pred, float* A,
                             float* B, int64_t* crit_idx, float* save_Q, float* save_H1, int32_t* status,
-                            void* workspace, size_t workspace_bytes, cudaStream_t st) {
+                            void* workspace, size_t workspace_bytes, cudaStream_t st,
+                            const float* const* XVs_dev = nullptr, float* save_V = nullptr) {
   int rc = check_bags_dev(r, p, true, true, Xs_dev, Ns_dev, nb, max_rows, status);
   if (rc) return rc;
-  DSMIL_REQUIRE(classes && pred && A && B && (!train || (crit_idx && save_Q && (!p->nonlinear || save_H1))),
+  DSMIL_REQUIRE(classes && pred && A && B &&
+                    (!train || (crit_idx && save_Q && (!p->nonlinear || save_H1) && (r != ROUTE_VAL || save_V))),
                 "NULL output pointer");
   if ((rc = need_workspace(forward_bags_dev_ws(r, train, p, nb, max_rows), workspace, workspace_bytes))) return rc;
   bool ok;
-  if (r == ROUTE_GEN) {
+  if (r != ROUTE_TC) {
     GenWs w = carve_gen_dev(p, nb, max_rows, train, workspace, workspace_bytes, &ok);
+    float* V = r == ROUTE_VAL ? (train ? save_V : w.V) : nullptr;
     if ((rc = launch_plan_dev(r, p, Xs_dev, Ns_dev, nb, max_rows, w.zero_row, w.table, nullptr, nullptr, w.plan, status,
-                              st)))
+                              st, PlanValue{XVs_dev, V, nullptr, nullptr, nullptr, w.vtab, nullptr, nullptr})))
       return rc;
     return gen_forward_run(p, w, nb, nb * max_rows, nb * tiles_for_bag(max_rows), nb * attend_ctas(max_rows), max_rows,
                            classes, pred, A, B, crit_idx ? crit_idx : w.crit, train ? save_Q : w.Q,
-                           p->nonlinear ? (train ? save_H1 : w.H1) : nullptr, nullptr, st);
+                           p->nonlinear ? (train ? save_H1 : w.H1) : nullptr, V, st);
   }
   BagsPlan* plan;
   float* zero_row;
@@ -2449,15 +2506,23 @@ static int forward_bags_dev(Route r, bool train, const dsmil_params_t* p, const 
 }
 
 // The backward pair's ragged GEMMs launch one CTA per chunk of the capacity in grid z (k_gemm_tn_rag) or x
-// (k_gemv_tn_rag), which holds at most 65535 of them: rag_splits plus one short chunk per bag.
-static bool dev_chunks_ok(const dsmil_params_t* p, int nb) {
+// (k_gemv_tn_rag), which holds at most 65535 of them: rag_splits plus one short chunk per bag (and on the value
+// route the chunks of gWv).
+static bool dev_chunks_ok(Route r, const dsmil_params_t* p, int nb) {
   return rag_chunks_cap(p->C, p->D, true, nb) <= 65535 && rag_chunks_cap(p->C, p->D, false, nb) <= 65535 &&
-         rag_chunks_cap(kQ, p->D, false, nb) <= 65535;
+         rag_chunks_cap(kQ, p->D, false, nb) <= 65535 &&
+         (r != ROUTE_VAL || rag_chunks_cap(p->D, p->D, false, nb) <= 65535);
 }
-// The backward pair's size.  The generic route also covers the eager backward's carve.
+// The backward pair's size.  The generic and value routes also cover the eager backward's carve (without gX).
 static size_t backward_bags_dev_ws(Route r, const dsmil_params_t* p, int nb, int64_t max_rows) {
-  if (!dev_shape(r, p) || !dev_sizes(nb, max_rows) || !dev_chunks_ok(p, nb)) return 0;
+  if (!dev_shape(r, p) || !dev_sizes(nb, max_rows) || !dev_chunks_ok(r, p, nb)) return 0;
   bool ok;
+  if (r == ROUTE_VAL && !dev_tiles_ok(r, nb, max_rows)) return 0;
+  if (r == ROUTE_VAL)
+    return not_below_eager(carve_value_bwd_dev(p, nb, max_rows, nullptr, 0, &ok).bytes,
+                           [](const dsmil_params_t* q, const int64_t* Ns, int32_t n) {
+                             return dsmil_value_backward_bags_workspace_bytes(q, Ns, n, 0);
+                           }, p, nb, max_rows);
   const size_t dev = carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
   if (r == ROUTE_TC) return dev;
   return not_below_eager(dev, [](const dsmil_params_t* q, const int64_t* Ns, int32_t n) {
@@ -2466,20 +2531,31 @@ static size_t backward_bags_dev_ws(Route r, const dsmil_params_t* p, int nb, int
 }
 
 // The backward pair's body: the planner writes the bag and chunk tables, then the three phases run on the capacity
-// grids.
+// grids.  The value route (XVs_dev, V: the forward's value inputs and saved V) has the planner write the value tables
+// too, and runs the value backward's phases over the V half of its value table, then its dzv, gWv and gbv.
 static int backward_bags_dev(Route r, const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
                              int nb, int64_t max_rows, const float* Q, const float* H1, const float* A, const float* B,
                              const int64_t* crit_idx, const float* d_classes, const float* d_pred, const float* d_A,
                              const float* d_B, const dsmil_grads_t* grads, int32_t* status, void* workspace,
-                             size_t workspace_bytes, cudaStream_t st) {
+                             size_t workspace_bytes, cudaStream_t st, const float* const* XVs_dev = nullptr,
+                             const float* V = nullptr) {
   int rc = check_bags_dev(r, p, false, true, Xs_dev, Ns_dev, nb, max_rows, status);
   if (rc) return rc;
-  DSMIL_REQUIRE(Q && (!p->nonlinear || H1) && A && B && crit_idx && grads, "NULL pointer");
+  DSMIL_REQUIRE(Q && (!p->nonlinear || H1) && A && B && crit_idx && grads && (r != ROUTE_VAL || V), "NULL pointer");
   DSMIL_REQUIRE(!d_A && !d_B && !grads->gX,
                 "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
-  DSMIL_REQUIRE(dev_chunks_ok(p, nb), "nb=%d: the chunk capacity of the ragged GEMMs passes 65535", nb);
+  DSMIL_REQUIRE(dev_chunks_ok(r, p, nb), "nb=%d: the chunk capacity of the ragged GEMMs passes 65535", nb);
   if ((rc = need_workspace(backward_bags_dev_ws(r, p, nb, max_rows), workspace, workspace_bytes))) return rc;
   bool ok;
+  if (r == ROUTE_VAL) {
+    ValueBwdWs w = carve_value_bwd_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
+    if ((rc = launch_plan_dev(r, p, Xs_dev, Ns_dev, nb, max_rows, w.b.zero_row, w.b.table, w.b.chi, w.b.ch1, w.b.plan,
+                              status, st, PlanValue{XVs_dev, V, A, w.b.dB, w.dzv, w.vtab, w.segs, w.chv})))
+      return rc;
+    w.b.table = w.vtab + nb;   // the phases weigh V: dA = V dB_b^T
+    return value_backward_run(p, nullptr, nullptr, nb, static_cast<int64_t>(nb) * max_rows, max_rows, Q, H1, V, A, B,
+                              crit_idx, d_classes, d_pred, nullptr, nullptr, nullptr, grads, w, st);
+  }
   BwdBagsWs w = carve_bwd_bags_dev(p, nb, max_rows, workspace, workspace_bytes, &ok);
   if ((rc = launch_plan_dev(r, p, Xs_dev, Ns_dev, nb, max_rows, w.zero_row, w.table, w.chi, w.ch1, w.plan, status,
                             st)))
@@ -2984,6 +3060,35 @@ int dsmil_value_backward_bags(const dsmil_params_t* p, const float* const* Xs, c
   if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
   return value_backward_bags_impl(p, Xs, XVs, Ns, nb, total, Q, H1, V, A, B, crit_idx, d_classes, d_pred, d_A, d_B,
                                   v_mask, grads, w, static_cast<cudaStream_t>(stream));
+}
+
+size_t dsmil_value_forward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  return forward_bags_dev_ws(ROUTE_VAL, false, p, nb, max_rows);
+}
+int dsmil_value_forward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const float* const* XVs_dev,
+                                 const int64_t* Ns_dev, int32_t nb, int64_t max_rows, float* classes, float* pred,
+                                 float* A, float* B, int64_t* crit_idx, float* save_Q, float* save_H1, float* save_V,
+                                 int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
+  const bool saves = save_Q || save_H1 || save_V;
+  DSMIL_REQUIRE(!saves || (save_Q && save_V && (!p || !p->nonlinear || save_H1)),
+                "saves: save_Q, save_V (and save_H1 for a nonlinear q) together, or none");
+  return forward_bags_dev(ROUTE_VAL, saves, p, Xs_dev, Ns_dev, nb, max_rows, classes, pred, A, B, crit_idx, save_Q,
+                          save_H1, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), XVs_dev,
+                          save_V);
+}
+
+size_t dsmil_value_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
+  return backward_bags_dev_ws(ROUTE_VAL, p, nb, max_rows);
+}
+int dsmil_value_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const float* const* XVs_dev,
+                                  const int64_t* Ns_dev, int32_t nb, int64_t max_rows, const float* Q,
+                                  const float* H1, const float* V, const float* A, const float* B,
+                                  const int64_t* crit_idx, const float* d_classes, const float* d_pred,
+                                  const float* d_A, const float* d_B, const dsmil_grads_t* grads, int32_t* status,
+                                  void* workspace, size_t workspace_bytes, void* stream) {
+  return backward_bags_dev(ROUTE_VAL, p, Xs_dev, Ns_dev, nb, max_rows, Q, H1, A, B, crit_idx, d_classes, d_pred, d_A,
+                           d_B, grads, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream), XVs_dev,
+                           V);
 }
 
 }  // extern "C"

@@ -141,7 +141,7 @@ struct BagsPlan {
   int tiles, recs;       // forward: 128-row tiles and partial records
   int G;                 // backward: CTAs per bag of the per-row kernels
   int nci, nc1;          // backward: chunks of gWi and gW1
-  int pad_;
+  int pad_;              // generic dev calls of passing_v: the live gWv chunks (k_plan_bags_gen)
   RowSplit cs;           // column sums over the packed rows
   RowSplit tn2;          // gW2 = dz2^T H1 over the packed rows
 };
@@ -214,27 +214,60 @@ k_plan_bags(const float* const* __restrict__ Xs, const int64_t* __restrict__ Ns,
   *plan = pl;
 }
 
+// One model's rows of a row-wise linear layer (k_linear_models): Y = X op(W) (+ the ReLU mask of aux); Y NULL: skip.
+struct LinSeg {
+  const float *X, *W, *aux;
+  float* Y;
+  long long N;
+};
+
+// The value network's share of a generic dev call's plan (passing_v; every member NULL elsewhere).  XVs: the bags'
+// value inputs (device memory; NULL: the features).  vtab [2 nb]: nb entries of the bag table's numbering whose X is
+// each bag's value input, then nb whose X is its packed rows of V ([rows, D] from V).  segs [nb] (backward): bag b's
+// dzv_b = (A_b dB_b) * [V_b > 0] as a LinSeg over A [rows, C], dB [nb, C, D], V and dzv [rows, D].  chv (backward):
+// the gWv chunks over the value inputs, rag_chunks' for the live total; their live count goes to BagsPlan::pad_.
+struct PlanValue {
+  const float* const* XVs;
+  const float* V;
+  const float* A;
+  const float* dB;
+  float* dzv;
+  sm90::BagDev* vtab;
+  LinSeg* segs;
+  TnChunk* chv;
+};
+
 // The planner of the generic shapes' dev calls: k_plan_bags with the alignment rule of gen_bag_aligned and a table of
-// gen_bag_entry, no row offsets.  A kernel of its own, as the k_plan_bags SASS stays what it was.
+// gen_bag_entry, no row offsets, and for passing_v the value tables of `v` (as the eager value calls build them on
+// the host).  A value input must meet its bag's rule: one that is NULL or not gen_bag_aligned refuses the batch like
+// a bad bag, and a refused batch's value tables take the stand-in's zero rows, one row per bag.  A kernel of its
+// own, as the k_plan_bags SASS stays what it was.
 __global__ void __launch_bounds__(32)
 k_plan_bags_gen(const float* const* __restrict__ Xs, const int64_t* __restrict__ Ns, int nb, long long max_rows,
                 int C, int D, float* __restrict__ zero_row, sm90::BagDev* __restrict__ table,
                 TnChunk* __restrict__ chi, TnChunk* __restrict__ ch1, BagsPlan* __restrict__ plan,
-                int* __restrict__ status) {
+                int* __restrict__ status, const PlanValue v) {
   __shared__ const float* sX[kPlanStaged];
+  __shared__ const float* sXV[kPlanStaged];
   __shared__ int64_t sN[kPlanStaged];
   if (blockIdx.x != 0) return;
-  for (int b = threadIdx.x; b < nb && b < kPlanStaged; b += 32) { sX[b] = Xs[b]; sN[b] = Ns[b]; }
+  for (int b = threadIdx.x; b < nb && b < kPlanStaged; b += 32) {
+    sX[b] = Xs[b];
+    sN[b] = Ns[b];
+    if (v.XVs) sXV[b] = v.XVs[b];
+  }
   __syncwarp();
   if (threadIdx.x != 0) return;
   auto X_of = [&](int b) { return b < kPlanStaged ? sX[b] : Xs[b]; };
   auto N_of = [&](int b) { return b < kPlanStaged ? sN[b] : Ns[b]; };
+  auto XV_of = [&](int b) { return v.XVs ? (b < kPlanStaged ? sXV[b] : v.XVs[b]) : X_of(b); };
   int bad = 0;
   long long mx = 0;
   for (int b = 0; b < nb && !bad; ++b) {
     const int64_t N = N_of(b);
     const float* X = X_of(b);
     if (N < 1 || N > max_rows || X == nullptr || !gen_bag_aligned(X, D)) bad = b + 1;
+    if (v.XVs && (XV_of(b) == nullptr || !gen_bag_aligned(XV_of(b), D))) bad = b + 1;
     mx = N > mx ? N : mx;
   }
   if (bad) {
@@ -245,25 +278,38 @@ k_plan_bags_gen(const float* const* __restrict__ Xs, const int64_t* __restrict__
   BagsPlan pl{};
   long long row = 0;
   int tile = 0, rec = 0;
-  for (int b = 0; b < nb; ++b)
-    table[b] = bad ? gen_bag_entry(zero_row, 1, D, row, tile, rec) : gen_bag_entry(X_of(b), N_of(b), D, row, tile, rec);
+  for (int b = 0; b < nb; ++b) {
+    const long long r0 = row;
+    const int64_t N = bad ? 1 : N_of(b);
+    table[b] = bad ? gen_bag_entry(zero_row, 1, D, row, tile, rec) : gen_bag_entry(X_of(b), N, D, row, tile, rec);
+    if (v.vtab) {
+      v.vtab[b] = v.vtab[nb + b] = table[b];
+      v.vtab[b].X = bad ? zero_row : XV_of(b);
+      v.vtab[nb + b].X = v.V + r0 * D;
+    }
+    if (v.segs)
+      v.segs[b] = LinSeg{v.A + r0 * C, v.dB + static_cast<size_t>(b) * C * D, v.V + r0 * D, v.dzv + r0 * D, N};
+  }
   pl.total = row;
   pl.tiles = tile;
   pl.recs = rec;
   pl.G = bwd_bags_ctas(nb, mx);
   if (bad) {                     // one one-row chunk per bag, as rag_chunks gives for one-row bags
-    for (int b = 0; b < nb && (chi || ch1); ++b) {
+    for (int b = 0; b < nb && (chi || ch1 || v.chv); ++b) {
       if (chi) chi[b] = TnChunk{zero_row, b, 1};
       if (ch1) ch1[b] = TnChunk{zero_row, b, 1};
+      if (v.chv) v.chv[b] = TnChunk{zero_row, b, 1};
     }
     pl.nci = chi ? nb : 0;
     pl.nc1 = ch1 ? nb : 0;
+    pl.pad_ = v.chv ? nb : 0;
   } else {
     if (chi) {
       const bool gemv = tn_use_gemv(C, D);   // true only where D % 4 == 0, and such bags are 16-byte aligned
       pl.nci = rag_chunks(Xs, Ns, nb, D, rag_rows_per_chunk(C, D, row, gemv), chi);
     }
     if (ch1) pl.nc1 = rag_chunks(Xs, Ns, nb, D, rag_rows_per_chunk(kQ, D, row, false), ch1);
+    if (v.chv) pl.pad_ = rag_chunks(v.XVs ? v.XVs : Xs, Ns, nb, D, rag_rows_per_chunk(D, D, row, false), v.chv);
   }
   pl.cs = colsum_split(row);
   pl.tn2 = gemm_tn_split(kQ, kQ, row);
@@ -283,12 +329,6 @@ struct BwdModelDev {
 struct SumSeg {
   float* out;
   int z0, S;
-};
-// One model's rows of a row-wise linear layer (k_linear_models): Y = X op(W) (+ the ReLU mask of aux); Y NULL: skip.
-struct LinSeg {
-  const float *X, *W, *aux;
-  float* Y;
-  long long N;
 };
 
 // Every split the one-model backward would choose for one model's own batch of nb bags, `total` rows, the largest of

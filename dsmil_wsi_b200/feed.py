@@ -102,7 +102,7 @@ class DeviceBagStore:
 def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_patch: float = 0.0,
                 order: Optional[Sequence[int]] = None, generator: Optional[torch.Generator] = None,
                 bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None,
-                generic: bool = False) -> float:
+                generic: bool = False, value: bool = False) -> float:
     """One epoch of train_tcga.train() (train_tcga.py:55-76) over device-resident bags; one host sync per epoch.
 
     bags_per_step = 1: the reference's loop, one forward, backward and optimizer step per bag.  k > 1: minibatches of
@@ -119,13 +119,44 @@ def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_pat
     freed when the call returns), so a graph holds the optimizer's hyperparameters of its call, e.g. a learning rate
     that a scheduler changes between epochs.  Needs the batched tensor-core shapes and a capture-safe optimizer
     (SGD, or Adam / AdamW with capturable=True); generic=True also takes the other identity-v shapes (e.g. the
-    classic-MIL D = 166 / 230, linear q), over the generic batched route, with the bits of the k-bag step."""
+    classic-MIL D = 166 / 230, linear q), over the generic batched route, with the bits of the k-bag step.
+
+    value=True: a model with a value network (passing_v; ValueError otherwise) trains on the batched value step
+    instead of its per-bag autograd: each group of k >= 1 bags (k = 1 included) is one
+    functional.mil_forward_value_bags(grad=True) call, one backward and one optimizer step on minibatch_loss.  The
+    group's dropout_patches are drawn first, then each bag's dropout mask of v in bag order (BClassifier._v_input), as
+    forward_bags draws them.  Its gradient sums run in another order than the per-bag step's, so its bits differ from
+    the default's, which is why it is an option.  With graph=True the step is a replayed TrainStepGraph(value=True)
+    with the same draws in the same order, written into the graph's slots and v_inputs, and the epoch gives the eager
+    value=True epoch's bits: losses, parameters, optimizer state and the RNG states after it."""
+    if value:
+        from .train_graph import step_shape
+        step_shape(milnet, value=True)                         # identity v raises here
     milnet.train()
     total = torch.zeros((), device=store.device)
     order = list(order) if order is not None else torch.randperm(len(store)).tolist()
     if graph:
         return _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator,
-                                  max(1, bags_per_step), max_rows, generic)
+                                  max(1, bags_per_step), max_rows, generic, value)
+    if value:
+        bc, lin = milnet.b_classifier, milnet.i_classifier._linear()
+        W1, b1, W2, b2 = bc._q_params()
+        Wv, bv, _ = bc._v_params()
+        params = (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
+        k = max(1, bags_per_step)
+        for s in range(0, len(order), k):
+            group = order[s:s + k]
+            optimizer.zero_grad()
+            xs = [dropout_patches(store.bags[i][0], 1 - dropout_patch, generator) for i in group]
+            vs = [bc._v_input(x) for x in xs]
+            labels = torch.cat([store.bags[i][1].view(1, -1) for i in group])
+            outs, _ = Fn.mil_forward_value_bags(xs, params, None if vs[0] is None else vs, grad=True)
+            bag_prediction, max_prediction = _group_predictions(outs)
+            loss = minibatch_loss(criterion, bag_prediction, max_prediction, labels)
+            loss.backward()
+            optimizer.step()
+            total += loss.detach() * len(group)
+        return float(total.item()) / max(1, len(order))
     if bags_per_step > 1:
         for s in range(0, len(order), bags_per_step):
             group = order[s:s + bags_per_step]
@@ -243,9 +274,10 @@ def minibatch_loss(criterion, bag_prediction, max_prediction, labels):
     return 0.5 * criterion(bag_prediction, labels) + 0.5 * criterion(max_prediction, labels)
 
 
-def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator, k, max_rows, generic):
+def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator, k, max_rows, generic,
+                       value=False):
     from .train_graph import TrainStepGraph, step_shape
-    step_shape(milnet, generic)                                # a shape off the batched routes raises here
+    step_shape(milnet, generic, value)                         # a shape off the batched routes raises here
     p = 1 - dropout_patch
     keep = [int(int(store.bags[i][0].shape[0]) * p) for i in order]   # dropout_patches' row counts
     cap = int(max_rows) if max_rows is not None else max([int(f.shape[0]) for f, _ in store.bags], default=1)
@@ -260,10 +292,14 @@ def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order
         group = order[s:s + k]
         g = graphs.get(len(group))
         if g is None:                                          # the first full group, and a short last one
-            g = graphs[len(group)] = TrainStepGraph(milnet, criterion, optimizer, len(group), cap, generic=generic)
+            g = graphs[len(group)] = TrainStepGraph(milnet, criterion, optimizer, len(group), cap, generic=generic,
+                                                    value=value)
         for b, i in enumerate(group):
             dropout_patches(store.bags[i][0], p, generator, out=g.slots[b])
             g.Ns[b].fill_(keep[s + b])
+        if value and g.v_inputs is not None:                   # then v's masks, in bag order, as the eager step
+            for b in range(len(group)):
+                milnet.b_classifier._v_input(g.slots[b, :keep[s + b]], out=g.v_inputs[b, :keep[s + b]])
         torch.cat([store.bags[i][1].view(1, -1) for i in group], out=g.labels)
         total += g.step() * len(group)
     # the epoch's one host sync, which also reads the planners' status words
@@ -333,7 +369,7 @@ def _group_predictions(outs):
 
 def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, bags_per_launch: int = 16,
                dropout_patch: float = 0.0, generator: Optional[torch.Generator] = None, graph: bool = False,
-               max_rows: Optional[int] = None, generic: bool = False):
+               max_rows: Optional[int] = None, generic: bool = False, value: bool = False):
     """The measuring half of train_tcga.test() (train_tcga.py:85-107): mean loss, labels [n_bags, C] and
     sigmoid predictions [n_bags, C] (`average=True`: sigmoid(max) + sigmoid(bag), as `args.average`).  The ROC /
     threshold logic that follows in the reference (:108-132) is the caller's and works on these arrays.
@@ -351,14 +387,21 @@ def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, 
     bag of the store); a bag over it raises ValueError before any launch.  The graphs stay cached with the model (held
     weakly) and later calls with the same group sizes, capacity, `average` and criterion object replay them: the first
     call pays the recording, and a model whose parameter tensors were replaced gets new graphs.  Needs the batched
-    tensor-core shapes; generic=True also takes the other identity-v shapes, over the generic batched route."""
+    tensor-core shapes; generic=True also takes the other identity-v shapes, over the generic batched route.
+
+    value=True: a model with a value network (passing_v; ValueError otherwise).  The eager epoch is the default one,
+    which already runs such a model's batched value forward; with graph=True the graphs record
+    dsmil_value_forward_bags_dev (EvalBagsGraph(value=True)) and give the eager epoch's bits."""
+    if value:
+        from .train_graph import step_shape
+        step_shape(milnet, value=True)                         # identity v raises here
     milnet.eval()
     n = len(store)
     if n == 0:
         raise ValueError("eval_epoch over an empty store")
     if graph:
         return _eval_epoch_graph(milnet, store, criterion, average, max(1, bags_per_launch), dropout_patch, generator,
-                                 max_rows, generic)
+                                 max_rows, generic, value)
     losses, labels, preds = [], [], []
     batched = hasattr(milnet, "forward_bags") and bags_per_launch > 1
     with torch.no_grad():
@@ -423,10 +466,10 @@ def eval_epoch_models(milnets, store: DeviceBagStore, criterion, average: bool =
 _EVAL_GRAPHS = weakref.WeakKeyDictionary()
 
 
-def _eval_epoch_graph(milnet, store, criterion, average, k, dropout_patch, generator, max_rows, generic):
+def _eval_epoch_graph(milnet, store, criterion, average, k, dropout_patch, generator, max_rows, generic, value=False):
     from .infer_graph import EvalBagsGraph
     from .train_graph import step_shape
-    step_shape(milnet, generic)                                # a shape off the batched routes raises here
+    step_shape(milnet, generic, value)                         # a shape off the batched routes raises here
     p = 1 - dropout_patch
     keep = [int(int(f.shape[0]) * p) if dropout_patch > 0 else int(f.shape[0]) for f, _ in store.bags]
     cap = int(max_rows) if max_rows is not None else max(int(f.shape[0]) for f, _ in store.bags)
@@ -448,7 +491,8 @@ def _eval_epoch_graph(milnet, store, criterion, average, k, dropout_patch, gener
             key = (len(group), cap, bool(average))
             g = cached.get(key)
             if g is None or g.criterion is not criterion or not g.current():
-                g = cached[key] = EvalBagsGraph(milnet, criterion, len(group), cap, average, generic=generic)
+                g = cached[key] = EvalBagsGraph(milnet, criterion, len(group), cap, average, generic=generic,
+                                                value=value)
             graphs[len(group)] = g
         xs = [dropout_patches(f, p, generator) if dropout_patch > 0 else f for f, _ in group]
         g.labels.copy_(labels[s:s + len(group)])
@@ -503,19 +547,20 @@ def compute_pos_weight(bags: Sequence[Tuple[int, object]]) -> float:
 
 
 def mil_epoch_train(milnet, store: DeviceBagStore, criterion, optimizer, order: Optional[Sequence[int]] = None,
-                    bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None) -> float:
+                    bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None,
+                    value: bool = False) -> float:
     """train_mil.epoch_train (train_mil.py:42-59): per bag, shuffle the instances, forward, 0.5/0.5 loss, step
     (bags_per_step > 1: one step per group of bags, as train_epoch).  graph, max_rows: as train_epoch's, on the generic
     batched route too (the classic-MIL shapes are off the tensor-core batch): bags of a few dozen rows cost little on
-    the device, so the replayed step saves most of an epoch's host work."""
+    the device, so the replayed step saves most of an epoch's host work.  value: as train_epoch's."""
     return train_epoch(milnet, store, criterion, optimizer, dropout_patch=0.0, order=order, bags_per_step=bags_per_step,
-                       graph=graph, max_rows=max_rows, generic=True)
+                       graph=graph, max_rows=max_rows, generic=True, value=value)
 
 
 def mil_epoch_test(milnet, store: DeviceBagStore, criterion, bags_per_launch: int = 16, graph: bool = False,
-                   max_rows: Optional[int] = None):
+                   max_rows: Optional[int] = None, value: bool = False):
     """train_mil.epoch_test (train_mil.py:61-80): (mean loss, bag labels, sigmoid bag predictions).  graph, max_rows:
-    as eval_epoch's, on the generic batched route too."""
+    as eval_epoch's, on the generic batched route too; value: as eval_epoch's."""
     loss, labels, preds = eval_epoch(milnet, store, criterion, average=False, bags_per_launch=bags_per_launch,
-                                     graph=graph, max_rows=max_rows, generic=True)
+                                     graph=graph, max_rows=max_rows, generic=True, value=value)
     return loss, [int(l[0]) for l in labels], [p.squeeze() for p in preds]

@@ -788,6 +788,104 @@ def mil_forward_value_bags(bags: Sequence[torch.Tensor], params: Sequence[Option
     return _mil_forward_value_bags_infer(bags, params, v_inputs)
 
 
+def _slot_addrs(slots, P: ParamPack, what: str):
+    """The device addresses of the [max_rows, D] slots of a contiguous float32 [nb, max_rows, D] buffer."""
+    if slots.dim() != 3 or slots.shape[2] != P.D or slots.dtype != torch.float32 or not slots.is_contiguous():
+        raise ValueError(f"{what} must be contiguous float32 [nb, max_rows, {P.D}], got {tuple(slots.shape)}")
+    nb, max_rows = int(slots.shape[0]), int(slots.shape[1])
+    return slots.data_ptr() + 4 * max_rows * P.D * torch.arange(nb, dtype=torch.int64, device=slots.device)
+
+
+class MILValueBagsDevFn(torch.autograd.Function):
+    """MILValueBagsFn over the capture-safe value calls (dsmil_value_forward_bags_dev / dsmil_value_backward_bags_dev),
+    as MILBagsDevFn is MILBagsFn's: the bag list lives on the device, so one recorded call serves every batch of nb
+    bags of 1..max_rows rows, with the eager calls' bits.
+
+    args: slots [nb, max_rows, D] (bag b is slots[b, :Ns[b]]), v_slots (the value inputs in the same layout, value
+    input b is v_slots[b, :Ns[b]]; None: the value inputs are the bags), Ns [nb] int64 and status [1] int32 on the
+    device, then the ten parameter tensors of a passing_v model.  The packed per-row outputs (classes, A) have
+    nb * max_rows rows, the live ones packed at the prefix sums of Ns.  Parameter gradients only (no gradient to the
+    slots), so no v mask is needed."""
+
+    @staticmethod
+    def forward(ctx, slots, v_slots, Ns, status, *params):
+        lib = _lib.load()
+        ctx.set_materialize_grads(False)
+        P = _value_pack(params)
+        xs = _slot_addrs(slots, P, "slots")
+        nb, max_rows = int(slots.shape[0]), int(slots.shape[1])
+        xvs = None
+        if v_slots is not None:
+            if v_slots.shape != slots.shape:
+                raise ValueError(f"v_slots {tuple(v_slots.shape)} do not match the slots {tuple(slots.shape)}")
+            xvs = _slot_addrs(v_slots, P, "v_slots")
+        dev = P.device
+        with torch.cuda.device(dev):
+            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+            rows = nb * max_rows
+            classes, A = new(rows, P.C), new(rows, P.C)
+            pred, B = new(nb, P.C), new(nb, P.C, P.D)
+            crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
+            sQ, sV = new(rows, Q_DIM), new(rows, P.D)
+            sH = new(rows, Q_DIM) if P.nonlinear else None
+            ws = _workspace(lib.dsmil_value_forward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
+            rc = lib.dsmil_value_forward_bags_dev(P.ref, _ptr(xs), _ptr(xvs), _ptr(Ns), nb, max_rows, _ptr(classes),
+                                                  _ptr(pred), _ptr(A), _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH),
+                                                  _ptr(sV), _ptr(status), _ptr(ws), ws.numel(), _stream())
+            _lib.check(rc, "dsmil_value_forward_bags_dev")
+        ctx.save_for_backward(xs, xvs, Ns, status, sQ, sH, sV, A, B, crit, *P.tensors)
+        ctx.shape = (nb, max_rows)
+        ctx.mark_non_differentiable(crit)
+        return classes, pred, A, B, crit
+
+    @staticmethod
+    def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or g_A is not None or g_B is not None:
+            raise NotImplementedError("the graph-captured value step takes gradients through the instance scores and "
+                                      "the bag prediction only (no gradient to A, B, the features or value inputs)")
+        lib = _lib.load()
+        xs, xvs, Ns, status, sQ, sH, sV, A, B, crit, *params = ctx.saved_tensors
+        P = ParamPack(*params)
+        nb, max_rows = ctx.shape
+        dev = P.device
+        with torch.cuda.device(dev):
+            out = {nm: (torch.empty_like(t) if t is not None and need else None)
+                   for nm, t, need in zip(PARAM_NAMES, P.tensors, ctx.needs_input_grad[4:])}
+            G = _lib.DsmilGrads(*[_ptr(out[n]) for n in PARAM_NAMES], None)
+            dc, dp = _f32c(g_classes), _f32c(g_pred)
+            ws = _workspace(lib.dsmil_value_backward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
+            rc = lib.dsmil_value_backward_bags_dev(P.ref, _ptr(xs), _ptr(xvs), _ptr(Ns), nb, max_rows, _ptr(sQ),
+                                                   _ptr(sH), _ptr(sV), _ptr(A), _ptr(B), _ptr(crit), _ptr(dc),
+                                                   _ptr(dp), None, None, C.byref(G), _ptr(status), _ptr(ws),
+                                                   ws.numel(), _stream())
+            _lib.check(rc, "dsmil_value_backward_bags_dev")
+        return (None, None, None, None, *[out[n] for n in PARAM_NAMES])
+
+
+@torch.no_grad()
+def mil_forward_value_bags_dev(xs: torch.Tensor, vs: Optional[torch.Tensor], Ns: torch.Tensor, status: torch.Tensor,
+                               max_rows: int, params: Sequence[Optional[torch.Tensor]]):
+    """Inference of a passing_v model over a bag list held on the device (dsmil_value_forward_bags_dev), as
+    mil_forward_bags_dev is for identity v: one call can be recorded into a CUDA graph and replayed over every batch
+    of nb bags of 1..max_rows rows.  xs [nb] int64 (the bags' feature addresses), vs [nb] int64 (their value inputs'
+    addresses, or None: the value inputs are the features), Ns [nb] int64 and status [1] int32 on the device.  Returns
+    the packed (classes, pred, A, B, crit) with nb * max_rows rows of classes and A."""
+    lib = _lib.load()
+    P = _value_pack(params)
+    nb, dev = int(xs.numel()), P.device
+    with torch.cuda.device(dev):
+        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        classes, A = new(nb * max_rows, P.C), new(nb * max_rows, P.C)
+        pred, B = new(nb, P.C), new(nb, P.C, P.D)
+        crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
+        ws = _workspace(lib.dsmil_value_forward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
+        rc = lib.dsmil_value_forward_bags_dev(P.ref, _ptr(xs), _ptr(vs), _ptr(Ns), nb, max_rows, _ptr(classes),
+                                              _ptr(pred), _ptr(A), _ptr(B), _ptr(crit), None, None, None,
+                                              _ptr(status), _ptr(ws), ws.numel(), _stream())
+        _lib.check(rc, "dsmil_value_forward_bags_dev")
+    return classes, pred, A, B, crit
+
+
 @torch.no_grad()
 def _mil_forward_value_bags_infer(bags, params, v_inputs):
     lib = _lib.load()

@@ -35,10 +35,15 @@ class ForwardBagsGraph:
 
     generic=True: also the identity-v shapes off the tensor-core batch (train_graph.step_shape), recorded over the
     generic batched route (dsmil_generic_forward_bags_dev, whose alignment rule refuses a bag of D % 4 == 0 that is not
-    16-byte aligned, and otherwise one that is not 4-byte aligned)."""
+    16-byte aligned, and otherwise one that is not 4-byte aligned).
 
-    def __init__(self, milnet, nb: int, max_rows: int, warmup: int = 1, generic: bool = False):
-        self.D, self.C = step_shape(milnet, generic)
+    value=True: a model with a value network (passing_v), recorded over dsmil_value_forward_bags_dev with the features
+    as value inputs (the generic route's alignment rule), with the bits of forward_bags in eval mode.  A recorded
+    inference draws no dropout mask, so `run` refuses the model in train mode with a dropout_v > 0."""
+
+    def __init__(self, milnet, nb: int, max_rows: int, warmup: int = 1, generic: bool = False, value: bool = False):
+        self.D, self.C = step_shape(milnet, generic, value)
+        self.value = bool(value)
         nb, max_rows = int(nb), int(max_rows)
         if not 1 <= nb <= 65535 or max_rows < 1:
             raise ValueError(f"ForwardBagsGraph: nb={nb} outside [1, 65535] or max_rows={max_rows} < 1")
@@ -76,7 +81,12 @@ class ForwardBagsGraph:
         """Static buffers of a subclass's recorded work beyond the bag list and status."""
 
     def _record(self):
-        self.out = Fn.mil_forward_bags_dev(self.bag_list[0], self.bag_list[1], self.status, self.max_rows, self.params)
+        if self.value:
+            self.out = Fn.mil_forward_value_bags_dev(self.bag_list[0], None, self.bag_list[1], self.status,
+                                                     self.max_rows, self.params)
+        else:
+            self.out = Fn.mil_forward_bags_dev(self.bag_list[0], self.bag_list[1], self.status, self.max_rows,
+                                               self.params)
         self._after(*self.out)
 
     def _after(self, classes, pred, A, B, crit):
@@ -93,6 +103,12 @@ class ForwardBagsGraph:
             raise RuntimeError("ForwardBagsGraph: the model is gone, or a parameter tensor of it was replaced since "
                                "the capture (the graph reads the old one); update parameters in place, or build a new "
                                "graph")
+        if self.value:
+            bc = self._milnet().b_classifier
+            if bc.training and bc._v_params()[2] > 0.0:
+                raise RuntimeError("ForwardBagsGraph: the model is in train mode with dropout_v > 0, and a recorded "
+                                   "inference draws no dropout mask; call milnet.eval(), or train through "
+                                   "TrainStepGraph(value=True)")
         if len(bags) != self.nb:
             raise ValueError(f"ForwardBagsGraph: {len(bags)} bags for a graph of nb={self.nb}")
         Ns = []
@@ -139,9 +155,10 @@ class EvalBagsGraph(ForwardBagsGraph):
     [1, C] rows as feed.eval_epoch computes it, and the sigmoid predictions (average: sigmoid(max) + sigmoid(bag)).
     Fill `labels` [nb, C], then `run(bags)`; `loss` [nb] and `pred` [nb, C] hold the batch's results."""
 
-    def __init__(self, milnet, criterion, nb: int, max_rows: int, average: bool = False, generic: bool = False):
+    def __init__(self, milnet, criterion, nb: int, max_rows: int, average: bool = False, generic: bool = False,
+                 value: bool = False):
         self.criterion, self.average = criterion, bool(average)
-        super().__init__(milnet, nb, max_rows, generic=generic)
+        super().__init__(milnet, nb, max_rows, generic=generic, value=value)
 
     def _buffers(self, dev):
         self.labels = torch.zeros(self.nb, self.C, device=dev)

@@ -94,6 +94,14 @@ class BClassifier(nn.Module):
             return v[1].weight, v[1].bias, float(v[0].p)
         raise TypeError("BClassifier.v must be Identity or Sequential(Dropout, Linear, ReLU) (dsmil.py:35-41)")
 
+    def _v_input(self, feats, out=None):
+        """A bag's value input in a batched step: feats times v's dropout mask, drawn as nn.Dropout draws it in
+        self.forward (dsmil.py:36), into `out` when given; None where no mask is drawn (eval mode, p = 0)."""
+        _, _, p_drop = self._v_params()
+        if not (self.training and p_drop > 0.0):
+            return None
+        return torch.mul(feats, self.v[0](torch.ones_like(feats)), out=out)
+
     def _run(self, feats, i_weight, i_bias, classes_in):
         W1, b1, W2, b2 = self._q_params()
         Wv, bv, p_drop = self._v_params()
@@ -164,14 +172,14 @@ class MILNet(nn.Module):
         ic, bc = self.i_classifier, self.b_classifier
         lin = ic._linear()
         W1, b1, W2, b2 = bc._q_params()
-        Wv, bv, p_drop = bc._v_params()
-        draw = bc.training and p_drop > 0.0
-        feats, v_inputs = [], ([] if draw else None)
+        Wv, bv, _ = bc._v_params()
+        feats, v_inputs = [], []
         for b in bags:   # embedding, then v's dropout mask, bag by bag: the per-bag loop's draws in its order
             f = ic.embed(b) if isinstance(ic, IClassifier) else b
             feats.append(f)
-            if draw:
-                v_inputs.append(f * bc.v[0](torch.ones_like(f)))
+            v_inputs.append(bc._v_input(f))
+        if v_inputs and v_inputs[0] is None:
+            v_inputs = None
         params = (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
         outs, _ = Fn.mil_forward_value_bags(feats, params, v_inputs)
         return outs

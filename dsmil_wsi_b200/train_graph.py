@@ -38,11 +38,12 @@ def check_optimizer(optimizer) -> None:
                      "or Adam / AdamW with capturable=True")
 
 
-def step_shape(milnet, generic: bool = False):
+def step_shape(milnet, generic: bool = False, value: bool = False):
     """(D, C) of a MILNet whose training step the graph can record: FCLayer + BClassifier with identity v, on the
     batched tensor-core shapes (dsmil_shard_bags_supported), or with generic=True also on the generic batched route
     of the other identity-v shapes (dsmil_generic_bags_supported: e.g. D = 166 / 230, linear q, C > 4, D > 2048).
-    Anything else raises ValueError naming the shape."""
+    value=True: a model with a value network (passing_v) instead, on the value calls' shapes
+    (dsmil_value_bags_supported).  Anything else raises ValueError naming the shape."""
     ic, bc = getattr(milnet, "i_classifier", None), getattr(milnet, "b_classifier", None)
     if not (isinstance(ic, FCLayer) and isinstance(bc, BClassifier)):
         raise ValueError("graph-captured training needs MILNet(FCLayer, BClassifier); got "
@@ -52,6 +53,14 @@ def step_shape(milnet, generic: bool = False):
     C, D = int(bc.fcc.weight.shape[0]), int(bc.fcc.weight.shape[2])
     p = _lib.DsmilParams(D, C, int(W2 is not None), int(Wv is not None))
     lib = _lib.load()
+    if value:
+        if Wv is not None:
+            p.Wv = p.bv = 16           # the shape test reads no weights: any non-NULL address will do
+            if lib.dsmil_value_bags_supported(ctypes.byref(p)):
+                return D, C
+        raise ValueError(f"value=True records models with a value network only; D={D}, C={C}, "
+                         f"nonlinear={W2 is not None}, passing_v={Wv is not None} is not one (identity v: "
+                         "value=False)")
     if lib.dsmil_shard_bags_supported(ctypes.byref(p)):
         return D, C
     if generic and lib.dsmil_generic_bags_supported(ctypes.byref(p)):
@@ -150,11 +159,19 @@ class TrainStepGraph:
     freezes the optimizer's hyperparameters (e.g. its learning rate) at construction.  The parameters' .grad become
     the graph's gradient buffers.  generic=True: also the shapes off the tensor-core batch (step_shape), whose step
     records the generic batched route with the bits of its eager step; their bags follow the alignment rule of
-    dsmil_generic_forward_bags_train_dev, which the slots meet."""
+    dsmil_generic_forward_bags_train_dev, which the slots meet.
 
-    def __init__(self, milnet, criterion, optimizer, nb: int, max_rows: int, warmup: int = 1, generic: bool = False):
+    value=True: a model with a value network (passing_v), whose step records MILValueBagsDevFn with the bits of the
+    eager functional.mil_forward_value_bags(grad=True) step.  When the model's dropout_v is > 0 at construction (the
+    p is frozen then, as the other hyperparameters), the value inputs are a static `v_inputs` [nb, max_rows, D]
+    buffer, which the caller fills as it fills `slots` (bag b's features times its dropout mask; see
+    BClassifier._v_input); otherwise `v_inputs` is None and the value inputs are the slots."""
+
+    def __init__(self, milnet, criterion, optimizer, nb: int, max_rows: int, warmup: int = 1, generic: bool = False,
+                 value: bool = False):
         check_optimizer(optimizer)
-        D, C = step_shape(milnet, generic)
+        D, C = step_shape(milnet, generic, value)
+        self.value = bool(value)
         nb, max_rows = int(nb), int(max_rows)
         if not 1 <= nb <= 65535 or max_rows < 1:
             raise ValueError(f"TrainStepGraph: nb={nb} outside [1, 65535] or max_rows={max_rows} < 1")
@@ -164,6 +181,8 @@ class TrainStepGraph:
         dev = milnet.b_classifier.fcc.weight.device
         Fn.require_cuda(milnet.b_classifier.fcc.weight, "the model")
         self.slots = torch.zeros(nb, max_rows, D, device=dev)
+        self.v_inputs = (torch.zeros(nb, max_rows, D, device=dev)
+                         if self.value and milnet.b_classifier._v_params()[2] > 0.0 else None)
         self.Ns = torch.ones(nb, dtype=torch.int64, device=dev)
         self.labels = torch.zeros(nb, C, device=dev)
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -190,11 +209,16 @@ class TrainStepGraph:
         ic, bc = self.milnet.i_classifier, self.milnet.b_classifier
         lin = ic._linear()
         W1, b1, W2, b2 = bc._q_params()
-        return (lin.weight, lin.bias, W1, b1, W2, b2, None, None, bc.fcc.weight, bc.fcc.bias)
+        Wv, bv, _ = bc._v_params() if self.value else (None, None, 0.0)
+        return (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
 
     def _loss(self):
         """The recorded forward and minibatch loss: (loss, ok), ok a device bool that is false for a refused batch."""
-        classes, pred, _, _, crit = Fn.MILBagsDevFn.apply(self.slots, self.Ns, self._step_status, *self._params())
+        if self.value:
+            classes, pred, _, _, crit = Fn.MILValueBagsDevFn.apply(self.slots, self.v_inputs, self.Ns,
+                                                                   self._step_status, *self._params())
+        else:
+            classes, pred, _, _, crit = Fn.MILBagsDevFn.apply(self.slots, self.Ns, self._step_status, *self._params())
         ok = self._step_status[0] == 0
         n = self.Ns.clamp(0, self.max_rows)               # the live sizes (a refused batch's stay in range)
         first = torch.cumsum(n, 0) - n                    # each bag's first packed row

@@ -372,6 +372,43 @@ int dsmil_value_backward_bags(const dsmil_params_t* p, const float* const* Xs, c
                               const float* A, const float* B, const int64_t* crit_idx, const float* d_classes,
                               const float* d_pred, const float* d_A, const float* d_B, const float* v_mask,
                               const dsmil_grads_t* grads, void* workspace, size_t workspace_bytes, void* stream);
+/* The capture-safe forms of the two value calls, as dsmil_generic_forward_bags_train_dev / dsmil_generic_backward_bags_dev
+ * are of the identity-v ones: the bag list Xs_dev / Ns_dev, the value inputs XVs_dev [nb] (device memory, or NULL: the
+ * value inputs are the features) and *status in device memory, every launch sized for nb bags of max_rows rows, no
+ * host<->device copy, allocation or synchronisation, so one call can be recorded into a CUDA graph and replayed over
+ * every batch of nb bags of 1..max_rows rows.  The planner (k_plan_bags_gen) builds the value tables on the device.
+ *  - Per-row outputs and saves (classes, A, save_Q, save_H1 [.,128], save_V [.,D]) are sized for nb * max_rows rows,
+ *    the live rows packed at the live prefix sums.
+ *  - dsmil_value_forward_bags_dev saves as dsmil_value_forward_bags: save_Q, save_V (and save_H1 for a nonlinear q)
+ *    together, or none (inference: Q, H1 and V in the workspace); crit_idx may be NULL without saves.
+ *  - dsmil_value_backward_bags_dev takes gradients through d_classes and d_pred only: d_A, d_B and grads->gX are
+ *    DSMIL_ERR_ARG, so it needs no v mask.
+ *  - Alignment rule: a bag and its value input must be 16-byte aligned when D % 4 == 0 and 4-byte aligned otherwise.
+ *    A bag with N outside [1, max_rows], or whose features or value input are NULL or break the rule, sets *status to
+ *    1 + its index (the first such bag; never cleared) and the call runs the stand-in batch of dsmil_forward_bags_dev
+ *    (every bag one row of zeros, its value input too): every output is finite, every index in range.
+ *  - Bits: on the same bags and value inputs every output and save is dsmil_value_forward_bags's, and every gradient
+ *    dsmil_value_backward_bags's with grads->gX NULL.
+ *  - Identity v (or Wv / bv NULL) is DSMIL_ERR_ARG, as are the sizes the generic dev calls refuse (nb outside
+ *    [1, 65535], max_rows outside [1, 2^32), 2 * nb * ceil(max_rows / 128) > INT_MAX), NULL lists, Ns, status or
+ *    outputs, a partial set of saves, a missing save in the backward, and a batch whose chunk capacity passes 65535
+ *    (the gWv chunks included: rag_splits + nb, rag_splits = max(1, 296 / ceil(D/128)^2)).  A short workspace is
+ *    DSMIL_ERR_WORKSPACE.
+ *  - Workspace: depends on (nb, max_rows) only and is never below the eager value call's (with need_gX = 0 for the
+ *    backward) for nb bags of max_rows rows, so one buffer serves both forms; 0 for every shape or size refused above.
+ *    The backward's gWv partials take (rag_splits + nb) * D^2 floats, besides nb * max_rows * D floats of dzv. */
+size_t dsmil_value_forward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_value_forward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const float* const* XVs_dev,
+                                 const int64_t* Ns_dev, int32_t nb, int64_t max_rows, float* classes, float* pred,
+                                 float* A, float* B, int64_t* crit_idx, float* save_Q, float* save_H1, float* save_V,
+                                 int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+size_t dsmil_value_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
+int dsmil_value_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev, const float* const* XVs_dev,
+                                  const int64_t* Ns_dev, int32_t nb, int64_t max_rows, const float* Q,
+                                  const float* H1, const float* V, const float* A, const float* B,
+                                  const int64_t* crit_idx, const float* d_classes, const float* d_pred,
+                                  const float* d_A, const float* d_B, const dsmil_grads_t* grads, int32_t* status,
+                                  void* workspace, size_t workspace_bytes, void* stream);
 
 /* Call form (2)+(3) of the boundary (SURVEY §8b): the callers in attention_map.py:74,85 /
  * testing_tcga.py:72,83 run the instance classifier and the bag classifier separately.
