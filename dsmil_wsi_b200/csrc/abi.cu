@@ -2275,7 +2275,7 @@ int dsmil_shard_bags_phase2_train(const dsmil_params_t* p, const float* const* X
 }
 
 size_t dsmil_shard_backward_bags_workspace_bytes(const dsmil_params_t* p, const int64_t* Ns, int32_t nb) {
-  if (!dsmil_shard_bags_supported(p) || !Ns || nb < 1) return 0;
+  if (!dsmil_shard_bags_supported(p) || !Ns || nb < 1 || nb > 65535) return 0;
   for (int b = 0; b < nb; ++b)
     if (Ns[b] < 0) return 0;
   bool ok;
@@ -2921,15 +2921,17 @@ int dsmil_shard_bags_phase3_dev(const dsmil_params_t* p, int32_t nb, int64_t max
 }
 
 size_t dsmil_shard_backward_bags_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows) {
-  if (!dev_shape(ROUTE_TC, p) || !dev_sizes(nb, max_rows)) return 0;
+  if (!dev_shape(ROUTE_TC, p) || !dev_sizes(nb, max_rows) || !dev_chunks_ok(ROUTE_TC, p, nb)) return 0;
   bool ok;
   const size_t dev = carve_bwd_bags_dev(p, nb, max_rows, nullptr, 0, &ok).bytes;
   return not_below_eager(dev, dsmil_shard_backward_bags_workspace_bytes, p, nb, max_rows);
 }
 
-// The backward workspace of a sharded dev call, after its checks.
+// The backward workspace of a sharded dev call, after its checks.  Phases 1 and 3 run backward_bags_dev's ragged
+// GEMMs on the same capacities, and phase 2 reads the same workspace, so all three refuse its chunk capacity first.
 static int shard_bwd_bags_dev_ws(const dsmil_params_t* p, int nb, int64_t max_rows, void* workspace,
                                  size_t workspace_bytes, BwdBagsWs* w) {
+  DSMIL_REQUIRE(dev_chunks_ok(ROUTE_TC, p, nb), "nb=%d: the chunk capacity of the ragged GEMMs passes 65535", nb);
   const size_t need = dsmil_shard_backward_bags_dev_workspace_bytes(p, nb, max_rows);
   int rc = need_workspace(need, workspace, workspace_bytes);
   if (rc) return rc;

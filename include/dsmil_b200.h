@@ -535,7 +535,8 @@ int dsmil_shard_bags_phase3(const dsmil_params_t* p, const float* const* Xs, con
  *   phase3: Q-MLP backward over the local rows; the dq_max share goes to the rank that holds row crit_idx[b][k]
  *           (global) - row_offsets[b]; q_max is phase2_train's; local partial gW1/gb1/gW2/gb2
  *                                                                     -> all-reduce the parameter gradients
- * With one rank (identity reductions) the three phases give dsmil_backward_bags's bits.  No gX and no upstream d_A/d_B. */
+ * With one rank (identity reductions) the three phases give dsmil_backward_bags's bits.  No gX and no upstream d_A/d_B.
+ * 1 <= nb <= 65535: another nb is DSMIL_ERR_ARG in every phase, and dsmil_shard_backward_bags_workspace_bytes is 0. */
 int dsmil_shard_bags_phase1_train(const dsmil_params_t* p, const float* const* Xs, const int64_t* Ns, int32_t nb,
                                   const int64_t* row_offsets, float* classes, float* save_Q, float* save_H1,
                                   float* cand_recs, void* workspace, size_t workspace_bytes, void* stream);
@@ -572,8 +573,10 @@ int dsmil_shard_backward_bags_phase3(const dsmil_params_t* p, const float* const
  *   backward: dsmil_shard_backward_bags_phase1_dev -> phase2_dev -> phase3_dev, one workspace of
  *             dsmil_shard_backward_bags_dev_workspace_bytes; phase 3 reads the row offsets from row_offsets_dev
  * Exchanged buffers have the eager calls' fixed sizes for a given nb.  On the same bags each call gives the eager
- * call's bits.  1 <= nb <= 65535; a short workspace is DSMIL_ERR_WORKSPACE.  The workspace sizes depend on
- * (nb, max_rows) only and are never below the eager calls' for nb bags of max_rows rows. */
+ * call's bits.  1 <= nb <= 65535; the backward also needs its ragged GEMMs' chunk capacity within 65535, as
+ * dsmil_backward_bags_dev: past it (only within a few hundred bags of 65535) all three backward phases are DSMIL_ERR_ARG
+ * and dsmil_shard_backward_bags_dev_workspace_bytes is 0.  A short workspace is DSMIL_ERR_WORKSPACE.  The workspace
+ * sizes depend on (nb, max_rows) only and are never below the eager calls' for nb bags of max_rows rows. */
 size_t dsmil_shard_bags_train_dev_workspace_bytes(const dsmil_params_t* p, int32_t nb, int64_t max_rows);
 int dsmil_shard_bags_phase1_train_dev(const dsmil_params_t* p, const float* const* Xs_dev, const int64_t* Ns_dev,
                                       const int64_t* row_offsets_dev, int32_t nb, int64_t max_rows, float* classes,

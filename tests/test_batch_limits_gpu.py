@@ -338,26 +338,30 @@ def test_forward_and_backward_of_65535_bags(case):
     _check_backward(case, bcase, p, pats, _first_outs(o, crit, lay, case.Ns), ups, g, lay, t0)
 
 
-def _check_backward(case, bcase, p, pats, host, ups, g, lay, t0):
-    """First occurrences: the fp64 backward on their own saves (gX row by row); the sums: sum_p w_p g_p."""
+def _check_backward(case, bcase, p, pats, host, ups, g, lay, t0, nb=LIMIT, backward=None):
+    """First occurrences: the fp64 backward on their own saves (gX row by row, when g has one); the sums over the nb
+    bags: sum_p w_p g_p.  backward(X, fo, u) gives a pattern's fp64 gradients (default: orc.backward with gX)."""
     per = []
     for X, h, u in zip([b.X for b in pats], host, ups):
         fo = orc.FwdOut(None, None, h["A"], h["B"], h["crit"], Q=h["Q"], H1=h.get("H1"), V=h.get("V", X))
-        per.append(orc.backward(X, p, fo, u[0], u[1], d_A=u[2], d_B=u[3], need_dX=True))
-    w = signed_counts(LIMIT)
+        per.append(orc.backward(X, p, fo, u[0], u[1], d_A=u[2], d_B=u[3], need_dX=True) if backward is None else
+                   backward(X, fo, u))
+    P = len(per)
+    w = signed_counts(nb, P)
     got = g.host()
     errs = {}
     for k in bcase.names():
         want = sum(wp * gp[k] for wp, gp in zip(w, per))
         if k in ("Wf", "bf"):
             terms = np.stack([gp[k] for gp in per])          # each bag's term: dp_b[k] B_b, or dp_b
-            errs[k] = FW.over(np.abs(got[k] - want), chain_bar(terms, LIMIT))
+            errs[k] = FW.over(np.abs(got[k] - want), chain_bar(terms, nb, P))
         else:                                                 # the chunk and split sums of the other kernels
             terms = np.stack([gp[k] for gp in per])
-            errs[k] = float(np.max(np.abs(got[k] - want))) / ((bcase.bar(k) + C_SUM * U * LIMIT) * chain_max(terms))
-    starts = np.cumsum([0] + list(case.Ns))
-    gX = FW._np(g.gX[:lay.first_rows])
-    errs["X"] = max(rowwise_err(gX[starts[j]:starts[j + 1]], gp["X"]) for j, gp in enumerate(per)) / bcase.bar("X")
+            errs[k] = float(np.max(np.abs(got[k] - want))) / ((bcase.bar(k) + C_SUM * U * nb) * chain_max(terms, P))
+    if g.gX is not None:
+        starts = np.cumsum([0] + list(case.Ns))
+        gX = FW._np(g.gX[:lay.first_rows])
+        errs["X"] = max(rowwise_err(gX[starts[j]:starts[j + 1]], gp["X"]) for j, gp in enumerate(per)) / bcase.bar("X")
     print(f"{case.name} backward, error over bar: " + " ".join(f"{k}={v:.3g}" for k, v in errs.items()))
     _report(case.name, t0)
     bad = {k: v for k, v in errs.items() if not v <= 1.0}
