@@ -12,7 +12,7 @@ from typing import List, Sequence
 import torch
 
 from . import functional as Fn
-from .modules import BClassifier, FCLayer, IClassifier
+from .modules import BClassifier, FCLayer, IClassifier, milnet_params
 
 
 def _member_params(i, milnet):
@@ -20,12 +20,10 @@ def _member_params(i, milnet):
     if not (isinstance(bc, BClassifier) and isinstance(ic, (FCLayer, IClassifier))):
         raise TypeError(f"member {i}: an ensemble forward takes MILNets with an FCLayer or IClassifier and a "
                         "BClassifier")
-    W1, b1, W2, b2 = bc._q_params()
-    Wv, bv, _ = bc._v_params()
-    if Wv is not None:
+    params = milnet_params(milnet)
+    if params[6] is not None:
         raise ValueError(f"member {i}: an ensemble forward takes identity v only (passing_v=False)")
-    lin = ic._linear()
-    return (lin.weight, lin.bias, W1, b1, W2, b2, None, None, bc.fcc.weight, bc.fcc.bias)
+    return params
 
 
 def _shape(params):

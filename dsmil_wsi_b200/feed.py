@@ -17,6 +17,7 @@ import torch
 
 from . import _lib
 from . import functional as Fn
+from .modules import milnet_params
 
 
 def gather_rows(feats: torch.Tensor, idx: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -138,32 +139,21 @@ def train_epoch(milnet, store: DeviceBagStore, criterion, optimizer, dropout_pat
     if graph:
         return _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator,
                                   max(1, bags_per_step), max_rows, generic, value)
-    if value:
-        bc, lin = milnet.b_classifier, milnet.i_classifier._linear()
-        W1, b1, W2, b2 = bc._q_params()
-        Wv, bv, _ = bc._v_params()
-        params = (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
+    if value or bags_per_step > 1:
         k = max(1, bags_per_step)
+        if value:
+            bc, params = milnet.b_classifier, milnet_params(milnet)
         for s in range(0, len(order), k):
             group = order[s:s + k]
             optimizer.zero_grad()
             xs = [dropout_patches(store.bags[i][0], 1 - dropout_patch, generator) for i in group]
-            vs = [bc._v_input(x) for x in xs]
             labels = torch.cat([store.bags[i][1].view(1, -1) for i in group])
-            outs, _ = Fn.mil_forward_value_bags(xs, params, None if vs[0] is None else vs, grad=True)
+            if value:   # each bag's v mask after the group's patch draws, as forward_bags draws them
+                vs = [bc._v_input(x) for x in xs]
+                outs, _ = Fn.mil_forward_value_bags(xs, params, None if vs[0] is None else vs, grad=True)
+            else:
+                outs = milnet.forward_bags(xs, grad=True)
             bag_prediction, max_prediction = _group_predictions(outs)
-            loss = minibatch_loss(criterion, bag_prediction, max_prediction, labels)
-            loss.backward()
-            optimizer.step()
-            total += loss.detach() * len(group)
-        return float(total.item()) / max(1, len(order))
-    if bags_per_step > 1:
-        for s in range(0, len(order), bags_per_step):
-            group = order[s:s + bags_per_step]
-            optimizer.zero_grad()
-            xs = [dropout_patches(store.bags[i][0], 1 - dropout_patch, generator) for i in group]
-            labels = torch.cat([store.bags[i][1].view(1, -1) for i in group])
-            bag_prediction, max_prediction = _group_predictions(milnet.forward_bags(xs, grad=True))
             loss = minibatch_loss(criterion, bag_prediction, max_prediction, labels)
             loss.backward()
             optimizer.step()
@@ -274,18 +264,26 @@ def minibatch_loss(criterion, bag_prediction, max_prediction, labels):
     return 0.5 * criterion(bag_prediction, labels) + 0.5 * criterion(max_prediction, labels)
 
 
+def _graph_rows(store, p, max_rows, bags, what, fold=""):
+    """The row counts of the store's bags `bags` after dropout_patches keeps a fraction p of each, and the row capacity
+    of the `what` graphs: max_rows, by default the store's largest bag.  A bag over the capacity raises ValueError, and
+    one that patch dropout empties IndexError, before any graph is recorded (fold: the prefix naming a bag's fold)."""
+    cap = int(max_rows) if max_rows is not None else max([int(f.shape[0]) for f, _ in store.bags], default=1)
+    keep = [int(int(store.bags[i][0].shape[0]) * p) for i in bags]
+    for i, n in zip(bags, keep):
+        if n > cap:
+            raise ValueError(f"{fold}bag {i}: {n} rows exceed the {what} graph's max_rows={cap}")
+        if n < 1:
+            raise IndexError(f"dsmil_b200: {fold}bag {i} is empty after patch dropout (N == 0)")
+    return keep, cap
+
+
 def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order, generator, k, max_rows, generic,
                        value=False):
     from .train_graph import TrainStepGraph, step_shape
     step_shape(milnet, generic, value)                         # a shape off the batched routes raises here
     p = 1 - dropout_patch
-    keep = [int(int(store.bags[i][0].shape[0]) * p) for i in order]   # dropout_patches' row counts
-    cap = int(max_rows) if max_rows is not None else max([int(f.shape[0]) for f, _ in store.bags], default=1)
-    for i, n in zip(order, keep):
-        if n > cap:
-            raise ValueError(f"bag {i}: {n} rows exceed the training graph's max_rows={cap}")
-        if n < 1:
-            raise IndexError(f"dsmil_b200: bag {i} is empty after patch dropout (N == 0)")
+    keep, cap = _graph_rows(store, p, max_rows, order, "training")
     graphs = {}
     total = torch.zeros((), device=store.device)
     for s in range(0, len(order), k):
@@ -314,14 +312,10 @@ def _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_pat
     from .train_graph import FoldTrainStepGraph, fold_step_shape
     fold_step_shape(milnets)                                   # shapes off the fused fold route raise here
     p = 1 - dropout_patch
-    keep = {i: int(int(store.bags[i][0].shape[0]) * p) for o in orders for i in o}   # dropout_patches' row counts
-    cap = int(max_rows) if max_rows is not None else max([int(f.shape[0]) for f, _ in store.bags], default=1)
+    keep = {}
     for m, o in enumerate(orders):
-        for i in o:
-            if keep[i] > cap:
-                raise ValueError(f"fold {m}, bag {i}: {keep[i]} rows exceed the training graph's max_rows={cap}")
-            if keep[i] < 1:
-                raise IndexError(f"dsmil_b200: fold {m}, bag {i} is empty after patch dropout (N == 0)")
+        rows, cap = _graph_rows(store, p, max_rows, o, "training", f"fold {m}, ")
+        keep.update(zip(o, rows))
     graphs = {}
     totals = [torch.zeros((), device=store.device) for _ in orders]
     bad = torch.zeros(len(orders), dtype=torch.int32, device=store.device)
@@ -367,6 +361,16 @@ def _group_predictions(outs):
             torch.stack([torch.max(ins, 0)[0] for ins, _, _, _ in outs]))
 
 
+def _eval_bag(criterion, ins_prediction, bag_prediction, label, average):
+    """One bag's evaluation loss, 0.5 * criterion(bag) + 0.5 * criterion(max instance), and its sigmoid prediction
+    (average: sigmoid(max) + sigmoid(bag))."""
+    max_prediction, _ = torch.max(ins_prediction, 0)
+    loss = (0.5 * criterion(bag_prediction.view(1, -1), label.view(1, -1)) +
+            0.5 * criterion(max_prediction.view(1, -1), label.view(1, -1)))
+    p = torch.sigmoid(bag_prediction).view(-1)
+    return loss, (torch.sigmoid(max_prediction).view(-1) + p if average else p)
+
+
 def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, bags_per_launch: int = 16,
                dropout_patch: float = 0.0, generator: Optional[torch.Generator] = None, graph: bool = False,
                max_rows: Optional[int] = None, generic: bool = False, value: bool = False):
@@ -410,12 +414,10 @@ def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, 
             xs = [dropout_patches(f, 1 - dropout_patch, generator) if dropout_patch > 0 else f for f, _ in group]
             outs = milnet.forward_bags(xs) if batched else [milnet(x) for x in xs]
             for (ins_prediction, bag_prediction, _, _), (_, label) in zip(outs, group):
-                max_prediction, _ = torch.max(ins_prediction, 0)
-                losses.append(0.5 * criterion(bag_prediction.view(1, -1), label.view(1, -1)) +
-                              0.5 * criterion(max_prediction.view(1, -1), label.view(1, -1)))
+                loss, pred = _eval_bag(criterion, ins_prediction, bag_prediction, label, average)
+                losses.append(loss)
                 labels.append(label.view(-1))
-                p = torch.sigmoid(bag_prediction).view(-1)
-                preds.append(torch.sigmoid(max_prediction).view(-1) + p if average else p)
+                preds.append(pred)
     loss = float(torch.stack([l.reshape(()) for l in losses]).mean().item())
     return loss, torch.stack(labels).cpu().numpy().astype(int), torch.stack(preds).cpu().numpy()
 
@@ -443,11 +445,9 @@ def eval_epoch_models(milnets, store: DeviceBagStore, criterion, average: bool =
             outs = forward_bags_models(milnets, xs) if k > 1 else [[net(x) for x in xs] for net in milnets]
             for m, out in enumerate(outs):
                 for (ins_prediction, bag_prediction, _, _), (_, label) in zip(out, group):
-                    max_prediction, _ = torch.max(ins_prediction, 0)
-                    losses[m].append(0.5 * criterion(bag_prediction.view(1, -1), label.view(1, -1)) +
-                                     0.5 * criterion(max_prediction.view(1, -1), label.view(1, -1)))
-                    p = torch.sigmoid(bag_prediction).view(-1)
-                    preds[m].append(torch.sigmoid(max_prediction).view(-1) + p if average else p)
+                    loss, pred = _eval_bag(criterion, ins_prediction, bag_prediction, label, average)
+                    losses[m].append(loss)
+                    preds[m].append(pred)
         M = len(milnets)
         loss = torch.stack([torch.stack([l.reshape(()) for l in ls]).mean() for ls in losses])
         labels = torch.stack([label.view(-1) for _, label in store.bags])
@@ -471,13 +471,7 @@ def _eval_epoch_graph(milnet, store, criterion, average, k, dropout_patch, gener
     from .train_graph import step_shape
     step_shape(milnet, generic, value)                         # a shape off the batched routes raises here
     p = 1 - dropout_patch
-    keep = [int(int(f.shape[0]) * p) if dropout_patch > 0 else int(f.shape[0]) for f, _ in store.bags]
-    cap = int(max_rows) if max_rows is not None else max(int(f.shape[0]) for f, _ in store.bags)
-    for i, m in enumerate(keep):
-        if m > cap:
-            raise ValueError(f"bag {i}: {m} rows exceed the inference graph's max_rows={cap}")
-        if m < 1:
-            raise IndexError(f"dsmil_b200: bag {i} is empty after patch dropout (N == 0)")
+    _, cap = _graph_rows(store, p, max_rows, range(len(store)), "inference")
     n, C = len(store), int(store.bags[0][1].numel())
     cached = _EVAL_GRAPHS.setdefault(milnet, {})
     graphs = {}

@@ -70,6 +70,16 @@ class ParamPack:
         return C.byref(self.struct)
 
 
+def _warm_up(dev, steps, run):
+    """`run` `steps` times on a side stream, as torch.cuda.graph asks before a capture."""
+    side = torch.cuda.Stream(dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side):
+        for _ in range(max(1, steps)):
+            run()
+    torch.cuda.current_stream(dev).wait_stream(side)
+
+
 def _workspace(nbytes: int, device) -> torch.Tensor:
     return torch.empty(max(int(nbytes), 256), dtype=torch.uint8, device=device)
 
@@ -79,6 +89,48 @@ def _check_feats(feats: torch.Tensor, D: int) -> torch.Tensor:
     if feats.dim() != 2 or feats.shape[1] != D:
         raise ValueError(f"feats must be [N, {D}], got {tuple(feats.shape)}")
     return _f32c(feats)
+
+
+PARAM_NAMES = ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")
+
+
+def _bag_outputs(P: ParamPack, rows: int, nb: int, lead=()):
+    """Empty packed outputs of a bag call on P's device: classes and A [*lead, rows, C], pred [*lead, nb, C],
+    B [*lead, nb, C, D] and crit [*lead, nb, C] int64."""
+    new = lambda *s: torch.empty(*lead, *s, dtype=torch.float32, device=P.device)
+    return (new(rows, P.C), new(nb, P.C), new(rows, P.C), new(nb, P.C, P.D),
+            torch.empty(*lead, nb, P.C, dtype=torch.int64, device=P.device))
+
+
+def _saves(P: ParamPack, rows: int):
+    """Empty activations that a forward saves for its backward: Q [rows, 128], H1 [rows, 128] for a nonlinear q and
+    V [rows, D] for passing_v (None where the model has none)."""
+    new = lambda *s: torch.empty(*s, dtype=torch.float32, device=P.device)
+    return new(rows, Q_DIM), new(rows, Q_DIM) if P.nonlinear else None, new(rows, P.D) if P.passing_v else None
+
+
+def _param_grads(P: ParamPack, needs, gX: Optional[torch.Tensor] = None):
+    """Empty gradients of P's parameters where `needs` (one flag per PARAM_NAMES entry) asks for them, None elsewhere,
+    and the DsmilGrads over them and gX."""
+    out = [torch.empty_like(t) if t is not None and need else None for t, need in zip(P.tensors, needs)]
+    return out, _lib.DsmilGrads(*[_ptr(g) for g in out], _ptr(gX))
+
+
+def _split_rows(gX: Optional[torch.Tensor], Ns, needs):
+    """Each bag's rows of a packed feature gradient where `needs` asks for them, None elsewhere."""
+    out, lo = [], 0
+    for n, need in zip(Ns, needs):
+        out.append(gX[lo:lo + n] if need else None)
+        lo += n
+    return out
+
+
+def _slot_addrs(slots, P: ParamPack, what: str):
+    """The device addresses of the [max_rows, D] slots of a contiguous float32 [nb, max_rows, D] buffer."""
+    if slots.dim() != 3 or slots.shape[2] != P.D or slots.dtype != torch.float32 or not slots.is_contiguous():
+        raise ValueError(f"{what} must be contiguous float32 [nb, max_rows, {P.D}], got {tuple(slots.shape)}")
+    nb, max_rows = int(slots.shape[0]), int(slots.shape[1])
+    return slots.data_ptr() + 4 * max_rows * P.D * torch.arange(nb, dtype=torch.int64, device=slots.device)
 
 
 # --------------------------------------------------------------------------- fused MILNet forward
@@ -114,9 +166,7 @@ class MILForwardFn(torch.autograd.Function):
             classes = new(N, Cc) if cin is None else new(0, Cc)  # bag form: scores are an input, not an output
             pred, A, B = new(1, Cc), new(N, Cc), new(1, Cc, D)
             crit = torch.empty(Cc, dtype=torch.int64, device=X.device)
-            sQ = new(N, Q_DIM) if need_grad else None
-            sH = new(N, Q_DIM) if (need_grad and P.nonlinear) else None
-            sV = new(N, D) if (need_grad and P.passing_v) else None
+            sQ, sH, sV = _saves(P, N) if need_grad else (None, None, None)
             ws = _workspace(lib.dsmil_forward_workspace_bytes(P.ref, N), X.device)
             if cin is None:
                 if Wi is None or bi is None:
@@ -145,16 +195,11 @@ class MILForwardFn(torch.autograd.Function):
         P = ParamPack(*params)
         N, Cc, D = int(X.shape[0]), P.C, P.D
         needs = ctx.needs_input_grad[1:]  # (want_grad,) feats, v_input, v_mask, classes_in, 10 params
-        names = ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")
+        # Wi/bi only get gradient through `classes` in the fused form
+        want = [need and (ctx.fused_scores or nm not in ("Wi", "bi")) for nm, need in zip(PARAM_NAMES, needs[4:])]
         with torch.cuda.device(X.device):
-            out = {}
-            for i, (nm, t) in enumerate(zip(names, P.tensors)):
-                # Wi/bi only get gradient through `classes` in the fused form
-                want = t is not None and needs[4 + i] and not (nm in ("Wi", "bi") and not ctx.fused_scores)
-                out[nm] = torch.empty_like(t) if want else None
             gX = torch.empty_like(X) if needs[0] else None
-            G = _lib.DsmilGrads(*[_ptr(out[n]) for n in ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")],
-                                _ptr(gX))
+            out, G = _param_grads(P, want, gX)
             dc = _f32c(g_classes) if (g_classes is not None and ctx.fused_scores) else None
             dp = _f32c(g_pred.reshape(-1)) if g_pred is not None else None
             dA = _f32c(g_A) if g_A is not None else None
@@ -164,7 +209,7 @@ class MILForwardFn(torch.autograd.Function):
                                     _ptr(crit), _ptr(dc), _ptr(dp), _ptr(dA), _ptr(dB), C.byref(G),
                                     _ptr(v_mask), _ptr(ws), ws.numel(), _stream())
             _lib.check(rc, "dsmil_backward")
-        return (None, gX, None, None, None, *[out[n] for n in names])
+        return (None, gX, None, None, None, *out)
 
 
 # --------------------------------------------------------------------------- instance scores alone
@@ -275,14 +320,10 @@ class MILBagsFn(torch.autograd.Function):
         if P.passing_v:
             raise NotImplementedError("forward_bags(grad=True): passing_v models go through MILNet.forward per bag")
         xs, Ns, c_X, c_N = _bag_table(args[:nb], P)
-        total, Cc, D, dev = sum(Ns), P.C, P.D, P.device
+        total, dev = sum(Ns), P.device
         with torch.cuda.device(dev):
-            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-            classes, A = new(total, Cc), new(total, Cc)
-            pred, B = new(nb, Cc), new(nb, Cc, D)
-            crit = torch.empty(nb, Cc, dtype=torch.int64, device=dev)
-            sQ = new(total, Q_DIM)
-            sH = new(total, Q_DIM) if P.nonlinear else None
+            classes, pred, A, B, crit = _bag_outputs(P, total, nb)
+            sQ, sH, _ = _saves(P, total)
             ws = _workspace(lib.dsmil_forward_bags_train_workspace_bytes(P.ref, c_N, nb), dev)
             rc = lib.dsmil_forward_bags_train(P.ref, c_X, c_N, nb, _ptr(classes), _ptr(pred), _ptr(A), _ptr(B),
                                               _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(ws), ws.numel(), _stream())
@@ -300,24 +341,17 @@ class MILBagsFn(torch.autograd.Function):
         (sQ, sH, A, B, crit), params = saved[nb:nb + 5], saved[nb + 5:]   # saved[:nb]: the bags c_X points at
         P = ParamPack(*params)
         need_bags, need_params = ctx.needs_input_grad[1:1 + nb], ctx.needs_input_grad[1 + nb:]
-        names = ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")
         dev = P.device
         with torch.cuda.device(dev):
-            out = {nm: (torch.empty_like(t) if t is not None and need else None)
-                   for nm, t, need in zip(names, P.tensors, need_params)}
             gX = torch.empty(sum(Ns), P.D, dtype=torch.float32, device=dev) if any(need_bags) else None
-            G = _lib.DsmilGrads(*[_ptr(out[n]) for n in names], _ptr(gX))
+            out, G = _param_grads(P, need_params, gX)
             dc, dp, dA, dB = (_f32c(t) for t in (g_classes, g_pred, g_A, g_B))
             ws = _workspace(lib.dsmil_backward_bags_workspace_bytes(P.ref, c_N, nb, int(gX is not None)), dev)
             rc = lib.dsmil_backward_bags(P.ref, c_X, c_N, nb, _ptr(sQ), _ptr(sH), _ptr(A), _ptr(B), _ptr(crit),
                                          _ptr(dc), _ptr(dp), _ptr(dA), _ptr(dB), C.byref(G), _ptr(ws), ws.numel(),
                                          _stream())
             _lib.check(rc, "dsmil_backward_bags")
-        gxs, lo = [], 0
-        for n, need in zip(Ns, need_bags):
-            gxs.append(gX[lo:lo + n] if need else None)
-            lo += n
-        return (None, *gxs, *[out[n] for n in names])
+        return (None, *_split_rows(gX, Ns, need_bags), *out)
 
 
 def _dev_prefix(lib, P, what):
@@ -345,23 +379,17 @@ class MILBagsDevFn(torch.autograd.Function):
         ctx.set_materialize_grads(False)
         P = ParamPack(*params)
         pre = _dev_prefix(lib, P, "graph-captured training")
-        if slots.dim() != 3 or slots.shape[2] != P.D or slots.dtype != torch.float32 or not slots.is_contiguous():
-            raise ValueError(f"slots must be contiguous float32 [nb, max_rows, {P.D}], got {tuple(slots.shape)}")
+        xs = _slot_addrs(slots, P, "slots")
         nb, max_rows = int(slots.shape[0]), int(slots.shape[1])
         dev = P.device
         with torch.cuda.device(dev):
-            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
             rows = nb * max_rows
-            classes, A = new(rows, P.C), new(rows, P.C)
-            pred, B = new(nb, P.C), new(nb, P.C, P.D)
-            crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
-            sQ, sH = new(rows, Q_DIM), new(rows, Q_DIM)
-            xs = slots.data_ptr() + 4 * max_rows * P.D * torch.arange(nb, dtype=torch.int64, device=dev)
+            classes, pred, A, B, crit = _bag_outputs(P, rows, nb)
+            sQ, sH, _ = _saves(P, rows)
             ws = _workspace(getattr(lib, pre + "forward_bags_train_dev_workspace_bytes")(P.ref, nb, max_rows), dev)
             call = getattr(lib, pre + "forward_bags_train_dev")
-            rc = call(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred),
-                                                  _ptr(A), _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(status),
-                                                  _ptr(ws), ws.numel(), _stream())
+            rc = call(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred), _ptr(A), _ptr(B), _ptr(crit),
+                      _ptr(sQ), _ptr(sH), _ptr(status), _ptr(ws), ws.numel(), _stream())
             _lib.check(rc, pre + "forward_bags_train_dev")
         ctx.save_for_backward(xs, Ns, status, sQ, sH, A, B, crit, *P.tensors)
         ctx.shape, ctx.pre = (nb, max_rows), pre
@@ -377,20 +405,16 @@ class MILBagsDevFn(torch.autograd.Function):
         xs, Ns, status, sQ, sH, A, B, crit, *params = ctx.saved_tensors
         P = ParamPack(*params)
         nb, max_rows = ctx.shape
-        names = ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")
         dev = P.device
         with torch.cuda.device(dev):
-            out = {nm: (torch.empty_like(t) if t is not None and need else None)
-                   for nm, t, need in zip(names, P.tensors, ctx.needs_input_grad[3:])}
-            G = _lib.DsmilGrads(*[_ptr(out[n]) for n in names], None)
+            out, G = _param_grads(P, ctx.needs_input_grad[3:])
             dc, dp = _f32c(g_classes), _f32c(g_pred)
             ws = _workspace(getattr(lib, ctx.pre + "backward_bags_dev_workspace_bytes")(P.ref, nb, max_rows), dev)
             call = getattr(lib, ctx.pre + "backward_bags_dev")
-            rc = call(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(sQ), _ptr(sH), _ptr(A),
-                                             _ptr(B), _ptr(crit), _ptr(dc), _ptr(dp), None, None, C.byref(G),
-                                             _ptr(status), _ptr(ws), ws.numel(), _stream())
+            rc = call(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(sQ), _ptr(sH), _ptr(A), _ptr(B), _ptr(crit),
+                      _ptr(dc), _ptr(dp), None, None, C.byref(G), _ptr(status), _ptr(ws), ws.numel(), _stream())
             _lib.check(rc, ctx.pre + "backward_bags_dev")
-        return (None, None, None, *[out[n] for n in names])
+        return (None, None, None, *out)
 
 
 def mil_forward_bags(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]], *, grad: bool = False):
@@ -421,17 +445,21 @@ def mil_forward_bags_dev(xs: torch.Tensor, Ns: torch.Tensor, status: torch.Tenso
     lib = _lib.load()
     P = ParamPack(*params)
     pre = _dev_prefix(lib, P, "the device bag list")
+    return _infer_bags_dev(P, pre + "forward_bags_dev", xs, None, Ns, status, max_rows)
+
+
+def _infer_bags_dev(P: ParamPack, call: str, xs, vs, Ns, status, max_rows: int):
+    """The body of mil_forward_bags_dev and mil_forward_value_bags_dev: one capture-safe forward `call` without saves.
+    A passing_v model's call also takes the value inputs' addresses vs (None: the features) and the NULL saves."""
+    lib = _lib.load()
     nb, dev = int(xs.numel()), P.device
+    value, saves = ((_ptr(vs),), (None, None, None)) if P.passing_v else ((), ())
     with torch.cuda.device(dev):
-        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-        classes, A = new(nb * max_rows, P.C), new(nb * max_rows, P.C)
-        pred, B = new(nb, P.C), new(nb, P.C, P.D)
-        crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
-        ws = _workspace(getattr(lib, pre + "forward_bags_dev_workspace_bytes")(P.ref, nb, max_rows), dev)
-        call = getattr(lib, pre + "forward_bags_dev")
-        rc = call(P.ref, _ptr(xs), _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred), _ptr(A),
-                                        _ptr(B), _ptr(crit), _ptr(status), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, pre + "forward_bags_dev")
+        classes, pred, A, B, crit = _bag_outputs(P, nb * max_rows, nb)
+        ws = _workspace(getattr(lib, call + "_workspace_bytes")(P.ref, nb, max_rows), dev)
+        rc = getattr(lib, call)(P.ref, _ptr(xs), *value, _ptr(Ns), nb, max_rows, _ptr(classes), _ptr(pred), _ptr(A),
+                                _ptr(B), _ptr(crit), *saves, _ptr(status), _ptr(ws), ws.numel(), _stream())
+        _lib.check(rc, call)
     return classes, pred, A, B, crit
 
 
@@ -457,9 +485,6 @@ def _model_packs(params_list) -> list:
     return packs
 
 
-PARAM_NAMES = ("Wi", "bi", "W1", "b1", "W2", "b2", "Wv", "bv", "Wf", "bf")
-
-
 class MILBagsModelsFn(torch.autograd.Function):
     """MILBagsFn for M members, each over its own bags: dsmil_forward_bags_models_train forward and
     dsmil_backward_bags_models backward, one call each for all members.  args: nbs (each member's bag count), the
@@ -474,16 +499,12 @@ class MILBagsModelsFn(torch.autograd.Function):
         packs = _model_packs([args[ne + 10 * m:ne + 10 * (m + 1)] for m in range(M)])
         P0 = packs[0]
         xs, Ns, c_X, c_N = _bag_table(args[:ne], P0)
-        total, Cc, D, dev = sum(Ns), P0.C, P0.D, P0.device
+        total, dev = sum(Ns), P0.device
         ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
         c_nb = (C.c_int32 * M)(*nbs)
         with torch.cuda.device(dev):
-            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-            classes, A = new(total, Cc), new(total, Cc)
-            pred, B = new(ne, Cc), new(ne, Cc, D)
-            crit = torch.empty(ne, Cc, dtype=torch.int64, device=dev)
-            sQ = new(total, Q_DIM)
-            sH = new(total, Q_DIM) if P0.nonlinear else None
+            classes, pred, A, B, crit = _bag_outputs(P0, total, ne)
+            sQ, sH, _ = _saves(P0, total)
             ws = _workspace(lib.dsmil_forward_bags_models_train_workspace_bytes(ps, M, c_N, c_nb), dev)
             rc = lib.dsmil_forward_bags_models_train(ps, M, c_X, c_N, c_nb, _ptr(classes), _ptr(pred), _ptr(A),
                                                      _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(ws), ws.numel(),
@@ -509,15 +530,13 @@ class MILBagsModelsFn(torch.autograd.Function):
         c_nb = (C.c_int32 * M)(*nbs)
         ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
         with torch.cuda.device(dev):
-            outs = [{nm: (torch.empty_like(t) if t is not None and need else None)
-                     for nm, t, need in zip(PARAM_NAMES, P.tensors, need_params[10 * m:10 * (m + 1)])}
-                    for m, P in enumerate(packs)]
             gX = torch.empty(sum(Ns), P0.D, dtype=torch.float32, device=dev) if any(need_bags) else None
-            grads, lo, b = (_lib.DsmilGrads * M)(), 0, 0
-            for m in range(M):
+            outs, grads, lo, b = [], (_lib.DsmilGrads * M)(), 0, 0
+            for m, P in enumerate(packs):
                 rows = sum(Ns[b:b + nbs[m]])
-                grads[m] = _lib.DsmilGrads(*[_ptr(outs[m][n]) for n in PARAM_NAMES],
-                                           None if gX is None else _ptr(gX[lo:lo + rows]))
+                out, grads[m] = _param_grads(P, need_params[10 * m:10 * (m + 1)],
+                                             None if gX is None else gX[lo:lo + rows])
+                outs += out
                 lo, b = lo + rows, b + nbs[m]
             dc, dp, dA, dB = (_f32c(t) for t in (g_classes, g_pred, g_A, g_B))
             ws = _workspace(lib.dsmil_backward_bags_models_workspace_bytes(ps, M, c_N, c_nb, int(gX is not None)),
@@ -526,11 +545,7 @@ class MILBagsModelsFn(torch.autograd.Function):
                                                 _ptr(crit), _ptr(dc), _ptr(dp), _ptr(dA), _ptr(dB), grads, _ptr(ws),
                                                 ws.numel(), _stream())
             _lib.check(rc, "dsmil_backward_bags_models")
-        gxs, lo = [], 0
-        for n, need in zip(Ns, need_bags):
-            gxs.append(gX[lo:lo + n] if need else None)
-            lo += n
-        return (None, *gxs, *[o[n] for o in outs for n in PARAM_NAMES])
+        return (None, *_split_rows(gX, Ns, need_bags), *outs)
 
 
 class MILBagsModelsDevFn(torch.autograd.Function):
@@ -557,16 +572,13 @@ class MILBagsModelsDevFn(torch.autograd.Function):
         if slots.dim() != 3 or slots.shape[0] != ne or slots.shape[2] != P0.D or slots.dtype != torch.float32 \
                 or not slots.is_contiguous():
             raise ValueError(f"slots must be contiguous float32 [{ne}, max_rows, {P0.D}], got {tuple(slots.shape)}")
+        xs = _slot_addrs(slots, P0, "slots")
         max_rows, dev = int(slots.shape[1]), P0.device
         c_nb = (C.c_int32 * M)(*nbs)
         with torch.cuda.device(dev):
-            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
             rows = ne * max_rows
-            classes, A = new(rows, P0.C), new(rows, P0.C)
-            pred, B = new(ne, P0.C), new(ne, P0.C, P0.D)
-            crit = torch.empty(ne, P0.C, dtype=torch.int64, device=dev)
-            sQ, sH = new(rows, Q_DIM), new(rows, Q_DIM)
-            xs = slots.data_ptr() + 4 * max_rows * P0.D * torch.arange(ne, dtype=torch.int64, device=dev)
+            classes, pred, A, B, crit = _bag_outputs(P0, rows, ne)
+            sQ, sH, _ = _saves(P0, rows)
             ws = _workspace(lib.dsmil_forward_bags_models_train_dev_workspace_bytes(ps, M, c_nb, max_rows), dev)
             rc = lib.dsmil_forward_bags_models_train_dev(ps, M, _ptr(xs), _ptr(Ns), c_nb, max_rows, _ptr(classes),
                                                          _ptr(pred), _ptr(A), _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH),
@@ -592,17 +604,15 @@ class MILBagsModelsDevFn(torch.autograd.Function):
         c_nb = (C.c_int32 * M)(*nbs)
         need = ctx.needs_input_grad[4:]
         with torch.cuda.device(dev):
-            outs = [{nm: (torch.empty_like(t) if t is not None and nd else None)
-                     for nm, t, nd in zip(PARAM_NAMES, P.tensors, need[10 * m:10 * (m + 1)])}
-                    for m, P in enumerate(packs)]
-            grads = (_lib.DsmilGrads * M)(*[_lib.DsmilGrads(*[_ptr(o[n]) for n in PARAM_NAMES], None) for o in outs])
+            outs, grads = zip(*[_param_grads(P, need[10 * m:10 * (m + 1)]) for m, P in enumerate(packs)])
+            grads = (_lib.DsmilGrads * M)(*grads)
             dc, dp = _f32c(g_classes), _f32c(g_pred)
             ws = _workspace(lib.dsmil_backward_bags_models_dev_workspace_bytes(ps, M, c_nb, max_rows), dev)
             rc = lib.dsmil_backward_bags_models_dev(ps, M, _ptr(xs), _ptr(Ns), c_nb, max_rows, _ptr(sQ), _ptr(sH),
                                                     _ptr(A), _ptr(B), _ptr(crit), _ptr(dc), _ptr(dp), None, None,
                                                     grads, _ptr(status), _ptr(ws), ws.numel(), _stream())
             _lib.check(rc, "dsmil_backward_bags_models_dev")
-        return (None, None, None, None, *[o[n] for o in outs for n in PARAM_NAMES])
+        return (None, None, None, None, *[g for out in outs for g in out])
 
 
 def mil_forward_bags_per_model(bag_lists: Sequence[Sequence[torch.Tensor]],
@@ -650,13 +660,10 @@ def mil_forward_bags_models(bags: Sequence[torch.Tensor], params_list: Sequence[
     if nb == 0:
         return [BagOutputs(None, None, None, None, [], None) for _ in range(M)]
     xs, Ns, c_X, c_N = _bag_table(bags, P0)
-    total, Cc, D, dev = sum(Ns), P0.C, P0.D, P0.device
+    dev = P0.device
     ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
     with torch.cuda.device(dev):
-        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-        classes, A = new(M, total, Cc), new(M, total, Cc)
-        pred, B = new(M, nb, Cc), new(M, nb, Cc, D)
-        crit = torch.empty(M, nb, Cc, dtype=torch.int64, device=dev)
+        classes, pred, A, B, crit = _bag_outputs(P0, sum(Ns), nb, lead=(M,))
         ws = _workspace(lib.dsmil_forward_bags_models_workspace_bytes(ps, M, c_N, nb), dev)
         rc = lib.dsmil_forward_bags_models(ps, M, c_X, c_N, nb, _ptr(classes), _ptr(pred), _ptr(A), _ptr(B),
                                            _ptr(crit), _ptr(ws), ws.numel(), _stream())
@@ -713,14 +720,10 @@ class MILValueBagsFn(torch.autograd.Function):
             raise ValueError("v_masks without v_inputs: the masks are the factors of the value inputs")
         if vs is not None and ms is None and any(ctx.needs_input_grad[3:3 + nb]):
             raise ValueError("the bags' gradients through v_inputs need their v_masks (v_inputs == bags * v_masks)")
-        total, Cc, D, dev = sum(Ns), P.C, P.D, P.device
+        total, dev = sum(Ns), P.device
         with torch.cuda.device(dev):
-            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-            classes, A = new(total, Cc), new(total, Cc)
-            pred, B = new(nb, Cc), new(nb, Cc, D)
-            crit = torch.empty(nb, Cc, dtype=torch.int64, device=dev)
-            sQ, sV = new(total, Q_DIM), new(total, D)
-            sH = new(total, Q_DIM) if P.nonlinear else None
+            classes, pred, A, B, crit = _bag_outputs(P, total, nb)
+            sQ, sH, sV = _saves(P, total)
             mask = torch.cat(ms) if ms is not None else None   # packed [sum N, D], as the backward reads it
             ws = _workspace(lib.dsmil_value_forward_bags_workspace_bytes(P.ref, c_N, nb), dev)
             rc = lib.dsmil_value_forward_bags(P.ref, c_X, _ptr_array(vs), c_N, nb, _ptr(classes), _ptr(pred), _ptr(A),
@@ -743,10 +746,8 @@ class MILValueBagsFn(torch.autograd.Function):
         need_bags, need_params = ctx.needs_input_grad[3:3 + nb], ctx.needs_input_grad[3 + nb:]
         dev = P.device
         with torch.cuda.device(dev):
-            out = {nm: (torch.empty_like(t) if t is not None and need else None)
-                   for nm, t, need in zip(PARAM_NAMES, P.tensors, need_params)}
             gX = torch.empty(sum(Ns), P.D, dtype=torch.float32, device=dev) if any(need_bags) else None
-            G = _lib.DsmilGrads(*[_ptr(out[n]) for n in PARAM_NAMES], _ptr(gX))
+            out, G = _param_grads(P, need_params, gX)
             dc, dp, dA, dB = (_f32c(t) for t in (g_classes, g_pred, g_A, g_B))
             ws = _workspace(lib.dsmil_value_backward_bags_workspace_bytes(P.ref, c_N, nb, int(gX is not None)), dev)
             rc = lib.dsmil_value_backward_bags(P.ref, _ptr_array(xs), _ptr_array(vs or None), c_N, nb, _ptr(sQ),
@@ -754,11 +755,7 @@ class MILValueBagsFn(torch.autograd.Function):
                                                _ptr(dA), _ptr(dB), _ptr(mask), C.byref(G), _ptr(ws), ws.numel(),
                                                _stream())
             _lib.check(rc, "dsmil_value_backward_bags")
-        gxs, lo = [], 0
-        for n, need in zip(Ns, need_bags):
-            gxs.append(gX[lo:lo + n] if need else None)
-            lo += n
-        return (None, None, None, *gxs, *[out[n] for n in PARAM_NAMES])
+        return (None, None, None, *_split_rows(gX, Ns, need_bags), *out)
 
 
 def mil_forward_value_bags(bags: Sequence[torch.Tensor], params: Sequence[Optional[torch.Tensor]],
@@ -788,14 +785,6 @@ def mil_forward_value_bags(bags: Sequence[torch.Tensor], params: Sequence[Option
     return _mil_forward_value_bags_infer(bags, params, v_inputs)
 
 
-def _slot_addrs(slots, P: ParamPack, what: str):
-    """The device addresses of the [max_rows, D] slots of a contiguous float32 [nb, max_rows, D] buffer."""
-    if slots.dim() != 3 or slots.shape[2] != P.D or slots.dtype != torch.float32 or not slots.is_contiguous():
-        raise ValueError(f"{what} must be contiguous float32 [nb, max_rows, {P.D}], got {tuple(slots.shape)}")
-    nb, max_rows = int(slots.shape[0]), int(slots.shape[1])
-    return slots.data_ptr() + 4 * max_rows * P.D * torch.arange(nb, dtype=torch.int64, device=slots.device)
-
-
 class MILValueBagsDevFn(torch.autograd.Function):
     """MILValueBagsFn over the capture-safe value calls (dsmil_value_forward_bags_dev / dsmil_value_backward_bags_dev),
     as MILBagsDevFn is MILBagsFn's: the bag list lives on the device, so one recorded call serves every batch of nb
@@ -821,13 +810,9 @@ class MILValueBagsDevFn(torch.autograd.Function):
             xvs = _slot_addrs(v_slots, P, "v_slots")
         dev = P.device
         with torch.cuda.device(dev):
-            new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
             rows = nb * max_rows
-            classes, A = new(rows, P.C), new(rows, P.C)
-            pred, B = new(nb, P.C), new(nb, P.C, P.D)
-            crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
-            sQ, sV = new(rows, Q_DIM), new(rows, P.D)
-            sH = new(rows, Q_DIM) if P.nonlinear else None
+            classes, pred, A, B, crit = _bag_outputs(P, rows, nb)
+            sQ, sH, sV = _saves(P, rows)
             ws = _workspace(lib.dsmil_value_forward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
             rc = lib.dsmil_value_forward_bags_dev(P.ref, _ptr(xs), _ptr(xvs), _ptr(Ns), nb, max_rows, _ptr(classes),
                                                   _ptr(pred), _ptr(A), _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH),
@@ -849,9 +834,7 @@ class MILValueBagsDevFn(torch.autograd.Function):
         nb, max_rows = ctx.shape
         dev = P.device
         with torch.cuda.device(dev):
-            out = {nm: (torch.empty_like(t) if t is not None and need else None)
-                   for nm, t, need in zip(PARAM_NAMES, P.tensors, ctx.needs_input_grad[4:])}
-            G = _lib.DsmilGrads(*[_ptr(out[n]) for n in PARAM_NAMES], None)
+            out, G = _param_grads(P, ctx.needs_input_grad[4:])
             dc, dp = _f32c(g_classes), _f32c(g_pred)
             ws = _workspace(lib.dsmil_value_backward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
             rc = lib.dsmil_value_backward_bags_dev(P.ref, _ptr(xs), _ptr(xvs), _ptr(Ns), nb, max_rows, _ptr(sQ),
@@ -859,7 +842,7 @@ class MILValueBagsDevFn(torch.autograd.Function):
                                                    _ptr(dp), None, None, C.byref(G), _ptr(status), _ptr(ws),
                                                    ws.numel(), _stream())
             _lib.check(rc, "dsmil_value_backward_bags_dev")
-        return (None, None, None, None, *[out[n] for n in PARAM_NAMES])
+        return (None, None, None, None, *out)
 
 
 @torch.no_grad()
@@ -870,20 +853,7 @@ def mil_forward_value_bags_dev(xs: torch.Tensor, vs: Optional[torch.Tensor], Ns:
     of nb bags of 1..max_rows rows.  xs [nb] int64 (the bags' feature addresses), vs [nb] int64 (their value inputs'
     addresses, or None: the value inputs are the features), Ns [nb] int64 and status [1] int32 on the device.  Returns
     the packed (classes, pred, A, B, crit) with nb * max_rows rows of classes and A."""
-    lib = _lib.load()
-    P = _value_pack(params)
-    nb, dev = int(xs.numel()), P.device
-    with torch.cuda.device(dev):
-        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-        classes, A = new(nb * max_rows, P.C), new(nb * max_rows, P.C)
-        pred, B = new(nb, P.C), new(nb, P.C, P.D)
-        crit = torch.empty(nb, P.C, dtype=torch.int64, device=dev)
-        ws = _workspace(lib.dsmil_value_forward_bags_dev_workspace_bytes(P.ref, nb, max_rows), dev)
-        rc = lib.dsmil_value_forward_bags_dev(P.ref, _ptr(xs), _ptr(vs), _ptr(Ns), nb, max_rows, _ptr(classes),
-                                              _ptr(pred), _ptr(A), _ptr(B), _ptr(crit), None, None, None,
-                                              _ptr(status), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, "dsmil_value_forward_bags_dev")
-    return classes, pred, A, B, crit
+    return _infer_bags_dev(_value_pack(params), "dsmil_value_forward_bags_dev", xs, vs, Ns, status, max_rows)
 
 
 @torch.no_grad()
@@ -895,12 +865,9 @@ def _mil_forward_value_bags_infer(bags, params, v_inputs):
         return [], None
     xs, Ns, _, _ = _bag_table(bags, P)
     vs = _per_bag(v_inputs, xs, P, "value input")
-    total, Cc, D, dev = sum(Ns), P.C, P.D, P.device
+    dev = P.device
     with torch.cuda.device(dev):
-        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-        classes, A = new(total, Cc), new(total, Cc)
-        pred, B = new(nb, Cc), new(nb, Cc, D)
-        crit = torch.empty(nb, Cc, dtype=torch.int64, device=dev)
+        classes, pred, A, B, crit = _bag_outputs(P, sum(Ns), nb)
         row = 0
         for s in range(0, nb, MAX_VALUE_BAGS):
             e = min(s + MAX_VALUE_BAGS, nb)
@@ -928,12 +895,8 @@ def _mil_forward_bags_infer(bags: Sequence[torch.Tensor], params: Sequence[Optio
         return [], None
     xs, Ns, c_X, c_N = _bag_table(bags, P)
     dev = P.device
-    total, Cc, D = sum(Ns), P.C, P.D
     with torch.cuda.device(dev):
-        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-        classes, A = new(total, Cc), new(total, Cc)
-        pred, B = new(nb, Cc), new(nb, Cc, D)
-        crit = torch.empty(nb, Cc, dtype=torch.int64, device=dev)
+        classes, pred, A, B, crit = _bag_outputs(P, sum(Ns), nb)
         ws = _workspace(lib.dsmil_forward_bags_workspace_bytes(P.ref, c_N, nb), dev)
         rc = lib.dsmil_forward_bags(P.ref, c_X, c_N, nb, _ptr(classes), _ptr(pred), _ptr(A), _ptr(B), _ptr(crit),
                                     _ptr(ws), ws.numel(), _stream())

@@ -16,7 +16,7 @@ from typing import Sequence
 import torch
 
 from . import functional as Fn
-from .sharded import milnet_params
+from .modules import milnet_params
 from .train_graph import step_shape
 
 
@@ -66,12 +66,7 @@ class ForwardBagsGraph:
         self._scratch = torch.zeros(nb, self.D, device=dev)
         self.bag_list[0] = self._scratch.data_ptr() + 4 * self.D * torch.arange(nb, device=dev)
         self.bag_list[1] = 1
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(max(1, warmup)):
-                self._record()
-        torch.cuda.current_stream(dev).wait_stream(side)
+        Fn._warm_up(dev, warmup, self._record)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self._record()

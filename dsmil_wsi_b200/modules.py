@@ -118,6 +118,16 @@ class BClassifier(nn.Module):
         return pred, A, B
 
 
+def milnet_params(milnet):
+    """The ten parameter tensors of a MILNet(FCLayer|IClassifier, BClassifier) in ABI order (functional.PARAM_NAMES),
+    None where the model has none."""
+    lin = milnet.i_classifier._linear()
+    bc = milnet.b_classifier
+    W1, b1, W2, b2 = bc._q_params()
+    Wv, bv, _ = bc._v_params()
+    return (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
+
+
 class MILNet(nn.Module):
     """dsmil.py:64-74 -- forward(x) -> (classes, prediction_bag, A, B)."""
 
@@ -155,24 +165,19 @@ class MILNet(nn.Module):
         ic, bc = self.i_classifier, self.b_classifier
         if not (isinstance(bc, BClassifier) and isinstance(ic, (FCLayer, IClassifier))):
             return [self.forward(b) for b in bags]
-        if bc._v_params()[0] is not None:
+        params = milnet_params(self)
+        if params[6] is not None:   # Wv: a value network
             if grad:   # autograd through the per-bag forward: the gradients users get from it, bag by bag
                 return [self.forward(b) for b in bags]
-            return self._forward_value_bags(bags)
+            return self._forward_value_bags(bags, params)
         feats = [ic.embed(b) if isinstance(ic, IClassifier) else b for b in bags]
-        lin = ic._linear()
-        W1, b1, W2, b2 = bc._q_params()
-        params = (lin.weight, lin.bias, W1, b1, W2, b2, None, None, bc.fcc.weight, bc.fcc.bias)
         outs, _ = Fn.mil_forward_bags(feats, params, grad=grad)
         return outs
 
-    def _forward_value_bags(self, bags):
+    def _forward_value_bags(self, bags, params):
         """Inference of a passing_v model over the bags in one library call, with the bits and RNG draws of the
         per-bag loop."""
         ic, bc = self.i_classifier, self.b_classifier
-        lin = ic._linear()
-        W1, b1, W2, b2 = bc._q_params()
-        Wv, bv, _ = bc._v_params()
         feats, v_inputs = [], []
         for b in bags:   # embedding, then v's dropout mask, bag by bag: the per-bag loop's draws in its order
             f = ic.embed(b) if isinstance(ic, IClassifier) else b
@@ -180,7 +185,6 @@ class MILNet(nn.Module):
             v_inputs.append(bc._v_input(f))
         if v_inputs and v_inputs[0] is None:
             v_inputs = None
-        params = (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
         outs, _ = Fn.mil_forward_value_bags(feats, params, v_inputs)
         return outs
 

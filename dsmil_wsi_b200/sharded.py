@@ -31,6 +31,7 @@ import torch
 
 from . import _lib
 from . import functional as Fn
+from .modules import milnet_params
 
 
 def shard_bounds(N: int, G: int) -> List[Tuple[int, int]]:
@@ -42,6 +43,24 @@ def shard_bounds(N: int, G: int) -> List[Tuple[int, int]]:
         out.append((lo, hi))
         lo = hi
     return out
+
+
+def _bwd1_shares(ops):
+    """This rank's gWi, gbi, gWf and gbf: the parameter gradients of a backward phase 1."""
+    P = ops.P
+    return ops.new(P.C, P.D), ops.new(P.C), ops.new(P.C, P.C, P.D), ops.new(P.C)
+
+
+def _bwd3_shares(ops):
+    """This rank's gW1, gb1, gW2 and gb2 (None for a linear q): the parameter gradients of a backward phase 3."""
+    P, Q = ops.P, Fn.Q_DIM
+    return (ops.new(Q, P.D), ops.new(Q), ops.new(Q, Q) if P.nonlinear else None,
+            ops.new(Q) if P.nonlinear else None)
+
+
+def _upstream(d_classes, d_pred):
+    """The upstream gradients as a backward phase 1 reads them: contiguous float32, or None."""
+    return tuple(None if d is None else d.to(torch.float32).contiguous() for d in (d_classes, d_pred))
 
 
 class CudaShardOps:
@@ -137,10 +156,8 @@ class CudaShardOps:
         P, N = self.P, int(X.shape[0])
         with torch.cuda.device(self.device):
             dA, t = self.new(N, P.C), self.new(P.C)
-            gWi, gbi = self.new(P.C, P.D), self.new(P.C)
-            gWf, gbf = self.new(P.C, P.C, P.D), self.new(P.C)
-            dc = None if d_classes is None else d_classes.to(torch.float32).contiguous()
-            dp = None if d_pred is None else d_pred.to(torch.float32).contiguous()
+            gWi, gbi, gWf, gbf = _bwd1_shares(self)
+            dc, dp = _upstream(d_classes, d_pred)
             ws = self._bws(N)
             rc = self.lib.dsmil_shard_backward_phase1(P.ref, Fn._ptr(X), N, Fn._ptr(A), Fn._ptr(B.contiguous()),
                                                       Fn._ptr(dc), Fn._ptr(dp), Fn._ptr(dA), Fn._ptr(t), Fn._ptr(gWi),
@@ -162,9 +179,7 @@ class CudaShardOps:
     def bwd3(self, X, row_offset, Q, H1, dL, dqm, qmax, crit):
         P, N = self.P, int(X.shape[0])
         with torch.cuda.device(self.device):
-            gW1, gb1 = self.new(Fn.Q_DIM, P.D), self.new(Fn.Q_DIM)
-            gW2 = self.new(Fn.Q_DIM, Fn.Q_DIM) if P.nonlinear else None
-            gb2 = self.new(Fn.Q_DIM) if P.nonlinear else None
+            gW1, gb1, gW2, gb2 = _bwd3_shares(self)
             ws = self._bws(N)
             rc = self.lib.dsmil_shard_backward_phase3(P.ref, Fn._ptr(X), N, int(row_offset), Fn._ptr(Q), Fn._ptr(H1),
                                                       Fn._ptr(dL), Fn._ptr(dqm.contiguous()), Fn._ptr(qmax.contiguous()),
@@ -301,10 +316,8 @@ class CudaShardBagOps:
         with torch.cuda.device(self.device):
             self.bws = Fn._workspace(self.lib.dsmil_shard_backward_bags_workspace_bytes(P.ref, c_N, nb), self.device)
             dA, t = self.new(total, P.C), self.new(nb, P.C)
-            gWi, gbi = self.new(P.C, P.D), self.new(P.C)
-            gWf, gbf = self.new(P.C, P.C, P.D), self.new(P.C)
-            dc = None if d_classes is None else d_classes.to(torch.float32).contiguous()
-            dp = None if d_pred is None else d_pred.to(torch.float32).contiguous()
+            gWi, gbi, gWf, gbf = _bwd1_shares(self)
+            dc, dp = _upstream(d_classes, d_pred)
             rc = self.lib.dsmil_shard_backward_bags_phase1(P.ref, c_X, c_N, nb, Fn._ptr(A), Fn._ptr(B.contiguous()),
                                                            Fn._ptr(dc), Fn._ptr(dp), Fn._ptr(dA), Fn._ptr(t),
                                                            Fn._ptr(gWi), Fn._ptr(gbi), Fn._ptr(gWf), Fn._ptr(gbf),
@@ -330,8 +343,7 @@ class CudaShardBagOps:
         c_X, c_N, nb = self._table(xs)
         c_off = (C.c_int64 * nb)(*[int(o) for o in row_offsets])
         with torch.cuda.device(self.device):
-            gW1, gb1 = self.new(Fn.Q_DIM, P.D), self.new(Fn.Q_DIM)
-            gW2, gb2 = self.new(Fn.Q_DIM, Fn.Q_DIM), self.new(Fn.Q_DIM)
+            gW1, gb1, gW2, gb2 = _bwd3_shares(self)
             rc = self.lib.dsmil_shard_backward_bags_phase3(P.ref, c_X, c_N, nb, c_off, Fn._ptr(Q), Fn._ptr(H1), Fn._ptr(dL),
                                                            Fn._ptr(dqm.contiguous()), Fn._ptr(qmax.contiguous()),
                                                            Fn._ptr(crit.contiguous()), Fn._ptr(gW1), Fn._ptr(gb1),
@@ -465,13 +477,10 @@ class CudaShardBagDevOps:
     def begin(self, X_locals: Sequence[torch.Tensor], row_offsets: torch.Tensor):
         (slots,) = X_locals
         P = self.P
-        if slots.dim() != 3 or slots.shape[2] != P.D or slots.dtype != torch.float32 or not slots.is_contiguous():
-            raise ValueError(f"slots must be contiguous float32 [nb, max_rows, {P.D}], got {tuple(slots.shape)}")
+        self.xs = Fn._slot_addrs(slots, P, "slots")
         self.nb, self.max_rows = int(slots.shape[0]), int(slots.shape[1])
         self.rows, self.offs = self.nb * self.max_rows, row_offsets
         with torch.cuda.device(self.device):
-            self.xs = slots.data_ptr() + 4 * self.max_rows * P.D * torch.arange(self.nb, dtype=torch.int64,
-                                                                                 device=self.device)
             self.ws = Fn._workspace(self.lib.dsmil_shard_bags_train_dev_workspace_bytes(P.ref, self.nb, self.max_rows),
                                     self.device)
         self.cand_f = int(self.lib.dsmil_cand_floats(P.C))
@@ -520,10 +529,8 @@ class CudaShardBagDevOps:
             self.bws = Fn._workspace(self.lib.dsmil_shard_backward_bags_dev_workspace_bytes(P.ref, self.nb, self.max_rows),
                                      self.device)
             dA, t = self.new(self.rows, P.C), self.new(self.nb, P.C)
-            gWi, gbi = self.new(P.C, P.D), self.new(P.C)
-            gWf, gbf = self.new(P.C, P.C, P.D), self.new(P.C)
-            dc = None if d_classes is None else d_classes.to(torch.float32).contiguous()
-            dp = None if d_pred is None else d_pred.to(torch.float32).contiguous()
+            gWi, gbi, gWf, gbf = _bwd1_shares(self)
+            dc, dp = _upstream(d_classes, d_pred)
             rc = self.lib.dsmil_shard_backward_bags_phase1_dev(P.ref, Fn._ptr(self.xs), Fn._ptr(self.Ns), self.nb,
                                                                self.max_rows, Fn._ptr(A), Fn._ptr(B.contiguous()),
                                                                Fn._ptr(dc), Fn._ptr(dp), Fn._ptr(dA), Fn._ptr(t),
@@ -546,8 +553,7 @@ class CudaShardBagDevOps:
     def bwd3(self, xs, row_offsets, Q, H1, dL, dqm, qmax, crit):
         P = self.P
         with torch.cuda.device(self.device):
-            gW1, gb1 = self.new(Fn.Q_DIM, P.D), self.new(Fn.Q_DIM)
-            gW2, gb2 = self.new(Fn.Q_DIM, Fn.Q_DIM), self.new(Fn.Q_DIM)
+            gW1, gb1, gW2, gb2 = _bwd3_shares(self)
             rc = self.lib.dsmil_shard_backward_bags_phase3_dev(P.ref, self.nb, self.max_rows, Fn._ptr(row_offsets),
                                                                Fn._ptr(Q), Fn._ptr(H1), Fn._ptr(dL),
                                                                Fn._ptr(dqm.contiguous()), Fn._ptr(qmax.contiguous()),
@@ -581,12 +587,8 @@ class ShardedBagsGraph:
 
     def __init__(self, bops: "CudaShardBagOps", X_locals, row_offsets, group=None, warmup: int = 3):
         self.bops, self.xs, self.offs, self.group = bops, list(X_locals), list(row_offsets), group
-        side = torch.cuda.Stream(device=bops.device)
-        side.wait_stream(torch.cuda.current_stream(bops.device))
-        with torch.cuda.stream(side):               # eager warm-up: uploads the bag table, sets NCCL up for these sizes
-            for _ in range(max(1, warmup)):
-                sharded_forward_bags_batched(bops, self.xs, self.offs, group)
-        torch.cuda.current_stream(bops.device).wait_stream(side)
+        # eager warm-up: uploads the bag table, sets NCCL up for these sizes
+        Fn._warm_up(bops.device, warmup, lambda: sharded_forward_bags_batched(bops, self.xs, self.offs, group))
         torch.cuda.synchronize(bops.device)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
@@ -625,15 +627,6 @@ def virtual_sharded_forward(ops, X: torch.Tensor, G: int):
     rec_g = ops.merge_partials(torch.cat([p[1] for p in part]), G)
     outs = [ops.phase3(rec_g, p[0]) for p in part]
     return (torch.cat([l[0] for l in loc]), outs[0][2], torch.cat([o[0] for o in outs]), outs[0][1], crit)
-
-
-def milnet_params(milnet) -> Tuple[Optional[torch.Tensor], ...]:
-    """The ten parameter tensors of a MILNet(FCLayer|IClassifier, BClassifier) in ABI order."""
-    lin = milnet.i_classifier._linear()
-    bc = milnet.b_classifier
-    W1, b1, W2, b2 = bc._q_params()
-    Wv, bv, _ = bc._v_params()
-    return (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
 
 
 def sharded_forward_bags(ops, X_locals: Sequence[torch.Tensor], row_offsets: Sequence[int], group=None):

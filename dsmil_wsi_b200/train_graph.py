@@ -17,7 +17,8 @@ import torch
 from . import _lib
 from . import feed
 from . import functional as Fn
-from .modules import BClassifier, FCLayer
+from .functional import _warm_up
+from .modules import BClassifier, FCLayer, milnet_params
 
 
 def check_optimizer(optimizer) -> None:
@@ -38,6 +39,18 @@ def check_optimizer(optimizer) -> None:
                      "or Adam / AdamW with capturable=True")
 
 
+def _shape_params(D, C, nonlinear, passing_v):
+    """A DsmilParams of this shape for the library's shape tests, which read no weights: every weight the form has
+    gets a stand-in address (any non-NULL one will do)."""
+    p = _lib.DsmilParams(D, C, int(nonlinear), int(passing_v))
+    p.Wi = p.bi = p.W1 = p.b1 = p.Wf = p.bf = 16
+    if nonlinear:
+        p.W2 = p.b2 = 16
+    if passing_v:
+        p.Wv = p.bv = 16
+    return p
+
+
 def step_shape(milnet, generic: bool = False, value: bool = False):
     """(D, C) of a MILNet whose training step the graph can record: FCLayer + BClassifier with identity v, on the
     batched tensor-core shapes (dsmil_shard_bags_supported), or with generic=True also on the generic batched route
@@ -51,13 +64,11 @@ def step_shape(milnet, generic: bool = False, value: bool = False):
     W1, b1, W2, b2 = bc._q_params()
     Wv, _, _ = bc._v_params()
     C, D = int(bc.fcc.weight.shape[0]), int(bc.fcc.weight.shape[2])
-    p = _lib.DsmilParams(D, C, int(W2 is not None), int(Wv is not None))
+    p = _shape_params(D, C, W2 is not None, Wv is not None)
     lib = _lib.load()
     if value:
-        if Wv is not None:
-            p.Wv = p.bv = 16           # the shape test reads no weights: any non-NULL address will do
-            if lib.dsmil_value_bags_supported(ctypes.byref(p)):
-                return D, C
+        if Wv is not None and lib.dsmil_value_bags_supported(ctypes.byref(p)):
+            return D, C
         raise ValueError(f"value=True records models with a value network only; D={D}, C={C}, "
                          f"nonlinear={W2 is not None}, passing_v={Wv is not None} is not one (identity v: "
                          "value=False)")
@@ -84,11 +95,7 @@ def fold_step_shape(milnets):
         if sh != shapes[0]:
             raise ValueError(f"fold {m}: (D, C)={sh} differs from fold 0's {shapes[0]}")
     D, C = shapes[0]
-    ps = (_lib.DsmilParams * len(milnets))()
-    for p in ps:                       # the shape test reads no weights: any non-NULL address will do
-        p.D, p.C, p.nonlinear, p.passing_v = D, C, 1, 0
-        for name in ("Wi", "bi", "W1", "b1", "W2", "b2", "Wf", "bf"):
-            setattr(p, name, 16)
+    ps = (_lib.DsmilParams * len(milnets))(*[_shape_params(D, C, True, False)] * len(milnets))
     if not _lib.load().dsmil_models_supported(ps, len(milnets)):
         raise ValueError(f"the graph-captured fold step runs on the fused fold shapes only; M={len(milnets)}, D={D}, "
                          f"C={C} is not on them: train these folds one at a time (train_epoch(graph=True))")
@@ -135,14 +142,26 @@ def _keep_if(ok, kept, before):
         torch._foreach_copy_(kept, [v.view_as(t) for v, t in zip(new.split([t.numel() for t in kept]), kept)])
 
 
-def _warm_up(dev, steps, run):
-    """`run` `steps` times on a side stream, as torch.cuda.graph asks before a capture."""
-    side = torch.cuda.Stream(dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        for _ in range(max(1, steps)):
-            run()
-    torch.cuda.current_stream(dev).wait_stream(side)
+def _capture_step(dev, optimizers, params, warmup, step):
+    """Records a training step as a CUDA graph.  `step(None)` runs `warmup` times on a side stream; then every
+    optimizer's parameters and state go back in place (so the graph's addresses stay valid; state the warm-up created
+    is reset to zeros) and `step(kept)` is captured, kept holding each optimizer's tensors that a refused step puts
+    back.  Returns (graph, the captured step's result, kept)."""
+    snaps = [_snapshot(o, p) for o, p in zip(optimizers, params)]
+
+    def warm():
+        for o in optimizers:
+            o.zero_grad(set_to_none=True)
+        step(None)
+    _warm_up(dev, warmup, warm)
+    for o, p, snap in zip(optimizers, params, snaps):
+        _restore(o, p, snap)
+        o.zero_grad(set_to_none=True)
+    kept = [_kept_tensors(o, p) for o, p in zip(optimizers, params)]   # the optimizer state exists now
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        out = step(kept)
+    return graph, out, kept
 
 
 class TrainStepGraph:
@@ -188,29 +207,15 @@ class TrainStepGraph:
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
         self._step_status = torch.zeros(1, dtype=torch.int32, device=dev)   # this replay's planners
         self._buffers(dev)
-        snap = _snapshot(optimizer, self.params)
-
-        def warm():
-            optimizer.zero_grad(set_to_none=True)
-            self._step()
-        _warm_up(dev, warmup, warm)
-        _restore(optimizer, self.params, snap)
-        optimizer.zero_grad(set_to_none=True)
-        self._kept = _kept_tensors(optimizer, self.params)   # the optimizer state exists now
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.loss = self._step(guard=True)
+        self.graph, self.loss, (self._kept,) = _capture_step(
+            dev, [optimizer], [self.params], warmup, lambda kept: self._step(None if kept is None else kept[0]))
         self.status.zero_()
 
     def _buffers(self, dev):
         """Static buffers of a subclass's step beyond the slots, sizes, labels and status."""
 
     def _params(self):
-        ic, bc = self.milnet.i_classifier, self.milnet.b_classifier
-        lin = ic._linear()
-        W1, b1, W2, b2 = bc._q_params()
-        Wv, bv, _ = bc._v_params() if self.value else (None, None, 0.0)
-        return (lin.weight, lin.bias, W1, b1, W2, b2, Wv, bv, bc.fcc.weight, bc.fcc.bias)
+        return milnet_params(self.milnet)
 
     def _loss(self):
         """The recorded forward and minibatch loss: (loss, ok), ok a device bool that is false for a refused batch."""
@@ -225,17 +230,18 @@ class TrainStepGraph:
         mx = classes.gather(0, crit + first[:, None])     # the per-bag max instance, as feed._group_predictions
         return feed.minibatch_loss(self.criterion, pred, mx, self.labels), ok
 
-    def _step(self, guard=False):
+    def _step(self, kept=None):
+        """One step; with `kept` (the recorded step) the update stands only for an accepted batch."""
         self._step_status.zero_()
         loss, ok = self._loss()
         # a refused batch: NaN loss and no gradient (where's backward sends none to the unselected side)
         loss = torch.where(ok, loss, torch.full_like(loss, float("nan")))
         loss.backward()
-        if guard:
-            before = _flat(self._kept)
+        if kept is not None:
+            before = _flat(kept)
         self.optimizer.step()
-        if guard:
-            _keep_if(ok, self._kept, before)   # the update stands only for an accepted batch
+        if kept is not None:
+            _keep_if(ok, kept, before)
         self.status.copy_(torch.where(self.status != 0, self.status, self._step_status))
         return loss.detach()
 
@@ -315,24 +321,12 @@ class FoldTrainStepGraph:
         self.labels = torch.zeros(ne, C, device=dev)
         self.status = torch.zeros(M, dtype=torch.int32, device=dev)
         self._step_status = torch.zeros(M, dtype=torch.int32, device=dev)   # this replay's planners
-        snaps = [_snapshot(o, p) for o, p in zip(optimizers, self.params)]
-
-        def warm():
-            for opt in optimizers:
-                opt.zero_grad(set_to_none=True)
-            self._step()
-        _warm_up(dev, warmup, warm)
-        for o, p, snap in zip(optimizers, self.params, snaps):
-            _restore(o, p, snap)
-            o.zero_grad(set_to_none=True)
-        self._kept = [_kept_tensors(o, p) for o, p in zip(optimizers, self.params)]
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.loss = self._step(guard=True)
+        self.graph, self.loss, self._kept = _capture_step(dev, optimizers, self.params, warmup, self._step)
         self.status.zero_()
 
-    def _step(self, guard=False):
-        from .sharded import milnet_params
+    def _step(self, kept=None):
+        """One step; with `kept` (the recorded step, one list per fold) each fold's update stands only if it was
+        accepted."""
         self._step_status.zero_()
         params = [t for net in self.milnets for t in milnet_params(net)]
         classes, pred, _, _, crit = Fn.MILBagsModelsDevFn.apply(self.nbs, self._slots, self.Ns, self._step_status,
@@ -352,13 +346,13 @@ class FoldTrainStepGraph:
         for lm in losses[1:]:
             total = total + lm
         total.backward()
-        if guard:
-            before = [_flat(k) for k in self._kept]
+        if kept is not None:
+            before = [_flat(k) for k in kept]
         for opt in self.optimizers:
             opt.step()
-        if guard:
-            for ok, kept, b in zip(oks, self._kept, before):
-                _keep_if(ok, kept, b)
+        if kept is not None:
+            for ok, k, b in zip(oks, kept, before):
+                _keep_if(ok, k, b)
         self.status.copy_(torch.where(self.status != 0, self.status, self._step_status))
         return torch.stack([lm.detach() for lm in losses])
 
