@@ -528,7 +528,8 @@ static int launch_vproj_b(const dsmil_params_t* p, const sm90::BagDev* vtab, int
                           float* V, cudaStream_t st) {
   const int D = p->D;
 #if DSMIL_VPROJ_LINEAR_B
-  k_linear_b<ACT_RELU><<<dim3(2 * tiles, ceil_div(D, LBN)), 256, 0, st>>>(vtab, nb, tiles_dev, D, p->Wv, p->bv, D, V);
+  k_linear_b<ACT_RELU><<<dim3(2 * tiles, ceil_div(D, LBN)), 256, 0, st>>>(vtab, nb, tiles_dev, D, p->Wv, p->bv, D, V,
+                                                                    nullptr);
   DSMIL_LAUNCH_OK("k_linear_b");
 #else
   k_vproj_b<<<dim3(tiles, ceil_div(D, VBN)), 256, 0, st>>>(vtab, nb, tiles_dev, D, p->Wv, p->bv, D, V);
@@ -537,48 +538,80 @@ static int launch_vproj_b(const dsmil_params_t* p, const sm90::BagDev* vtab, int
   return 0;
 }
 
+// The fold form of the generic forward (dsmil_generic_forward_bags_models_train_dev): w.table lists every model's bags,
+// model-major, as k_plan_bags_models writes it (bag_plan.cuh: FOLD_GEN / FOLD_GEN_QMLP).  The stages that read weights
+// take each entry's model's from `models`; layer 2 of the Q-MLP and a k_qmlp_sm90 phase 1 run one launch per model over
+// that model's block (ps[m]'s weights, its live counts in live[m]), on the grids its one-model dev call sizes.
+struct GenFolds {
+  const dsmil_params_t* ps;       // [M] host
+  const int32_t* nbs;             // [M] host: each model's bags
+  int M;
+  int64_t max_rows;
+  const sm90::ModelDev* models;   // [M] device
+  const ModelsPlan* plan;         // device: the live tiles and records over all models
+  const FoldLive* live;           // device [M]
+};
+
 // The generic forward over w.table: `tiles` and `recs` are the table's 128-row tiles and records and `rows` its packed
-// rows (dev calls: capacities, the live counts in w.plan); max_N bounds the bags' rows.  Q (and H1 for nonlinear q)
-// receive the Q-MLP's outputs row-major.  w.vtab (passing_v, eager only): nb entries of w.table's numbering whose X is
-// each bag's value input, then nb whose X is the bag's packed rows of V; V receives the value projection and the
-// attend pass reads it through the second half.
+// rows (dev calls: capacities, the live counts in w.plan, or in f's for a fold call); max_N bounds the bags' rows.  Q
+// (and H1 for nonlinear q) receive the Q-MLP's outputs row-major.  w.vtab (passing_v, eager only): nb entries of
+// w.table's numbering whose X is each bag's value input, then nb whose X is the bag's packed rows of V; V receives the
+// value projection and the attend pass reads it through the second half.  f: the fold form, p then being model 0's.
 static int gen_forward_run(const dsmil_params_t* p, const GenWs& w, int nb, int64_t rows, int tiles, int recs,
                            int64_t max_N, float* classes, float* pred, float* A, float* B, int64_t* crit, float* Q,
-                           float* H1, float* V, cudaStream_t st) {
+                           float* H1, float* V, cudaStream_t st, const GenFolds* f = nullptr) {
   const int C = p->C, D = p->D;
   const BagsPlan* pl = w.plan;
   const sm90::BagDev* vtab = w.vtab;
+  const int* tiles_dev = f ? &f->plan->tiles : pl ? &pl->tiles : nullptr;
+  const int* recs_dev = f ? &f->plan->recs : pl ? &pl->recs : nullptr;
+  const sm90::ModelDev* models = f ? f->models : nullptr;
   int rc;
   DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * kMaxC * nb, st));
   if (sm90::qmlp_supported(p)) {
-    if ((rc = sm90::launch_prep_wimg(p, w.wimg, st))) return rc;
-    if ((rc = sm90::launch_qmlp(p, w.table, nb, tiles, classes, w.keys, Q, H1, w.wimg, num_sms(), st, false,
-                                pl ? &pl->tiles : nullptr, nullptr)))
-      return rc;
+    if (!f) {
+      if ((rc = sm90::launch_prep_wimg(p, w.wimg, st))) return rc;
+      if ((rc = sm90::launch_qmlp(p, w.table, nb, tiles, classes, w.keys, Q, H1, w.wimg, num_sms(), st, false,
+                                  tiles_dev, nullptr)))
+        return rc;
+    }
+    for (int m = 0, e0 = 0; f && m < f->M; e0 += f->nbs[m], ++m) {   // model m's tiles are numbered from 0
+      const int nbm = f->nbs[m];
+      if ((rc = sm90::launch_prep_wimg(&f->ps[m], w.wimg, st))) return rc;
+      if ((rc = sm90::launch_qmlp(&f->ps[m], w.table + e0, nbm, nbm * tiles_for_bag(f->max_rows), classes,
+                                  w.keys + static_cast<size_t>(e0) * kMaxC, Q, H1, w.wimg, num_sms(), st, false,
+                                  &f->live[m].tiles, nullptr)))
+        return rc;
+    }
   } else {
     const size_t smem = sizeof(float) * C * D;
     if (smem > 48 * 1024)
       DSMIL_CUDA_OK(cudaFuncSetAttribute(k_scores_b, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     prof_begin(PROF_SCORES, st);
-    k_scores_b<<<tiles, 256, smem, st>>>(w.table, nb, pl ? &pl->tiles : nullptr, D, p->Wi, p->bi, C, classes, w.keys);
+    k_scores_b<<<tiles, 256, smem, st>>>(w.table, nb, tiles_dev, D, p->Wi, p->bi, C, classes, w.keys, models);
     prof_end(PROF_SCORES, st);
     DSMIL_LAUNCH_OK("k_scores_b");
     prof_begin(PROF_QMLP, st);
     const dim3 g1(2 * tiles, ceil_div(kQ, LBN));
-    if (p->nonlinear) k_linear_b<ACT_RELU><<<g1, 256, 0, st>>>(w.table, nb, pl ? &pl->tiles : nullptr, D, p->W1, p->b1, kQ, H1);
-    else k_linear_b<ACT_NONE><<<g1, 256, 0, st>>>(w.table, nb, pl ? &pl->tiles : nullptr, D, p->W1, p->b1, kQ, Q);
+    if (p->nonlinear) k_linear_b<ACT_RELU><<<g1, 256, 0, st>>>(w.table, nb, tiles_dev, D, p->W1, p->b1, kQ, H1, models);
+    else k_linear_b<ACT_NONE><<<g1, 256, 0, st>>>(w.table, nb, tiles_dev, D, p->W1, p->b1, kQ, Q, models);
     DSMIL_LAUNCH_OK("k_linear_b");
-    if (p->nonlinear &&
+    if (p->nonlinear && !f &&
         (rc = launch_linear<ACT_TANH, false>(H1, rows, kQ, p->W2, p->b2, kQ, Q, nullptr, 0, st, pl ? &pl->total : nullptr)))
       return rc;
+    for (int m = 0, e0 = 0; p->nonlinear && f && m < f->M; e0 += f->nbs[m], ++m) {   // over model m's block
+      const int64_t r0 = e0 * f->max_rows;
+      if ((rc = launch_linear<ACT_TANH, false>(H1 + r0 * kQ, f->nbs[m] * f->max_rows, kQ, f->ps[m].W2, f->ps[m].b2,
+                                               kQ, Q + r0 * kQ, nullptr, 0, st, &f->live[m].total)))
+        return rc;
+    }
     prof_end(PROF_QMLP, st);
   }
-  if (vtab && (rc = launch_vproj_b(p, vtab, nb, tiles, pl ? &pl->tiles : nullptr, V, st))) return rc;
+  if (vtab && (rc = launch_vproj_b(p, vtab, nb, tiles, tiles_dev, V, st))) return rc;
   k_crit_qmax_b<<<dim3(C, nb), kQ, 0, st>>>(w.table, w.keys, Q, C, w.qmax, crit);
   DSMIL_LAUNCH_OK("k_crit_qmax_b");
   int j = ceil_div(D, 256), J = 1;
   while (J < j) J <<= 1;
-  const int* recs_dev = pl ? &pl->recs : nullptr;
   const sm90::BagDev* atab = vtab ? vtab + nb : w.table;   // the rows the attend pass weighs: V, or the features
   prof_begin(PROF_ATTEND, st);
   if (C == 1) rc = launch_attend_gb_j<1>(J, recs, st, atab, nb, recs_dev, D, C, Q, w.qmax, A, w.recs);
@@ -591,7 +624,7 @@ static int gen_forward_run(const dsmil_params_t* p, const GenWs& w, int nb, int6
   DSMIL_LAUNCH_OK("k_combine_rec_b");
   const int fgrid = static_cast<int>(std::min<int64_t>(std::max<int64_t>(ceil_div(max_N * C, 256), 1), kSplits));
   prof_begin(PROF_FINAL, st);
-  k_finalize_gb<<<dim3(fgrid, nb), 256, 0, st>>>(w.table, w.rec, C, D, p->Wf, p->bf, A, B, pred);
+  k_finalize_gb<<<dim3(fgrid, nb), 256, 0, st>>>(w.table, w.rec, C, D, p->Wf, p->bf, A, B, pred, models);
   prof_end(PROF_FINAL, st);
   DSMIL_LAUNCH_OK("k_finalize_gb");
   return 0;
@@ -2026,6 +2059,7 @@ struct BwdModelsGrid {
   int64_t max_rows;               // rows of the largest model
   bool any_gX;
   const ModelsPlan* live;         // dev call: the planner's counts (device memory); NULL: eager
+  bool linear_q;                  // generic fold calls of a linear q: no layer 2, dz1 is dz2
 };
 static int bwd_models_launch(int C, int D, int M, int ne, const BwdModelsWs& w, const BwdModelsGrid& gr,
                              const float* Q, const float* H1, const float* A, const float* B, const int64_t* crit,
@@ -2077,20 +2111,24 @@ static int bwd_models_launch(int C, int D, int M, int ne, const BwdModelsWs& w, 
   DSMIL_LAUNCH_OK("k_bwd_dL_models");
   k_sum_segments_models<<<dim3(ceil_div(C * kQ, 256), ne), 256, 0, st>>>(w.table, w.dpart, C * kQ, w.dqm);
   DSMIL_LAUNCH_OK("k_sum_segments_models");
-  // phase 3: dz2, back through the Q-MLP
-  k_bwd_dq_b<<<per_entry, 256, 0, st>>>(w.table, C, w.dL, Q, nullptr, w.dqm, crit, nullptr, 1, w.dz2);
+  // phase 3: dz2, back through the Q-MLP (through the tanh and layer 2 for a nonlinear q)
+  k_bwd_dq_b<<<per_entry, 256, 0, st>>>(w.table, C, w.dL, Q, nullptr, w.dqm, crit, nullptr, gr.linear_q ? 0 : 1, w.dz2);
   DSMIL_LAUNCH_OK("k_bwd_dq_b");
-  k_gemm_tn_rag<<<dim3(1, 1, static_cast<unsigned>(gr.nc2)), 256, 0, st>>>(w.dz2, kQ, kQ, w.ch2, w.part,
-                                                                           live ? &live->nc2 : nullptr);
-  DSMIL_LAUNCH_OK("k_gemm_tn_rag");
-  if ((rc = sums(2, static_cast<int64_t>(kQ) * kQ)) || (rc = colsums(w.dz2, kQ, 3))) return rc;
   const unsigned row_tiles = static_cast<unsigned>(ceil_div(gr.max_rows, LBM));
-  k_linear_models<ACT_MASK_POS, true><<<dim3(row_tiles, 1, M), 256, 0, st>>>(w.lin, kQ, kQ);
-  DSMIL_LAUNCH_OK("k_linear_models");
+  const float* dz1 = w.dz2;
+  if (!gr.linear_q) {
+    k_gemm_tn_rag<<<dim3(1, 1, static_cast<unsigned>(gr.nc2)), 256, 0, st>>>(w.dz2, kQ, kQ, w.ch2, w.part,
+                                                                             live ? &live->nc2 : nullptr);
+    DSMIL_LAUNCH_OK("k_gemm_tn_rag");
+    if ((rc = sums(2, static_cast<int64_t>(kQ) * kQ)) || (rc = colsums(w.dz2, kQ, 3))) return rc;
+    k_linear_models<ACT_MASK_POS, true><<<dim3(row_tiles, 1, M), 256, 0, st>>>(w.lin, kQ, kQ);
+    DSMIL_LAUNCH_OK("k_linear_models");
+    dz1 = w.dz1;
+  }
   k_gemm_tn_rag<<<dim3(ceil_div(D, TBM), 1, static_cast<unsigned>(gr.nc1)), 256, 0, st>>>(
-      w.dz1, kQ, D, w.ch1, w.part, live ? &live->nc1 : nullptr);
+      dz1, kQ, D, w.ch1, w.part, live ? &live->nc1 : nullptr);
   DSMIL_LAUNCH_OK("k_gemm_tn_rag");
-  if ((rc = sums(4, static_cast<int64_t>(kQ) * D)) || (rc = colsums(w.dz1, kQ, 5))) return rc;
+  if ((rc = sums(4, static_cast<int64_t>(kQ) * D)) || (rc = colsums(dz1, kQ, 5))) return rc;
   if (gr.any_gX) {
     k_linear_models<ACT_NONE, true><<<dim3(row_tiles, ceil_div(D, LBN), M), 256, 0, st>>>(w.lin + M, kQ, D);
     DSMIL_LAUNCH_OK("k_linear_models");
@@ -2643,12 +2681,19 @@ struct ModelsDevCaps {
   int nci, nc1, nc2, ncs;     // chunk capacities over all models
   int64_t max_model_rows;     // row capacity of the largest model
 };
-static bool models_dev_caps(const dsmil_params_t* ps, int M, const int32_t* nbs, int64_t max_rows, ModelsDevCaps* c) {
-  if (!ps || !nbs || !dsmil_models_supported(ps, M)) return false;
+// gen: the generic fold calls (dsmil_generic_*_models_*), whose k_linear_b grid numbers twice the capacity tiles; why,
+// when given, receives what was out of range.
+static bool models_dev_caps(const dsmil_params_t* ps, int M, const int32_t* nbs, int64_t max_rows, ModelsDevCaps* c,
+                            bool gen = false, const char** why = nullptr) {
+  const char* dummy;
+  if (!why) why = &dummy;
+  *why = "shape";
+  if (!ps || !nbs || !(gen ? dsmil_generic_models_supported(ps, M) : dsmil_models_supported(ps, M))) return false;
   const int C = ps[0].C, D = ps[0].D;
   int64_t ne = 0, nci = 0, nc1 = 0;
   *c = ModelsDevCaps{0, 1, 0, 0, M * kModelSplitsCap, M * kModelSplitsCap, 1};
   for (int m = 0; m < M; ++m) {
+    *why = "a model's nb outside [1, 65535] or max_rows out of range";
     if (!dev_sizes(nbs[m], max_rows)) return false;
     ne += nbs[m];
     nci += rag_chunks_cap(C, D, tn_use_gemv(C, D), nbs[m]);
@@ -2657,8 +2702,10 @@ static bool models_dev_caps(const dsmil_params_t* ps, int M, const int32_t* nbs,
     c->max_model_rows = std::max<int64_t>(c->max_model_rows, nbs[m] * max_rows);
   }
   // every grid within its limits: entries and chunk capacities in 16 bits, the capacity tiles in an int
-  if (ne > 65535 || nci > 65535 || nc1 > 65535 || ne * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) > INT_MAX)
-    return false;
+  *why = "chunk capacity: the bags of all models plus the ragged GEMMs' chunk allowance pass 65535";
+  if (ne > 65535 || nci > 65535 || nc1 > 65535) return false;
+  *why = "max_rows out of range: the capacity tiles pass INT_MAX";
+  if ((gen ? 2 : 1) * ne * ((max_rows + sm90::kTileM - 1) / sm90::kTileM) > INT_MAX) return false;
   c->ne = static_cast<int>(ne);
   c->nci = static_cast<int>(nci);
   c->nc1 = static_cast<int>(nc1);
@@ -2783,10 +2830,14 @@ static BwdModelsWs carve_bwd_models_dev(const dsmil_params_t* ps, int M, const M
   return w;
 }
 
-size_t dsmil_backward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
-                                                      int64_t max_rows) {
+static int check_generic_models_dev(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
+                                    const int32_t* nbs, int64_t max_rows, const int32_t* status, ModelsDevCaps* caps);
+
+// The backward pair's size and body, for the fused tensor-core fold shapes or (gen) the generic ones.
+static size_t backward_bags_models_dev_ws(bool gen, const dsmil_params_t* ps, int M, const int32_t* nbs,
+                                          int64_t max_rows) {
   ModelsDevCaps caps;
-  if (!models_dev_caps(ps, M, nbs, max_rows, &caps)) return 0;
+  if (!models_dev_caps(ps, M, nbs, max_rows, &caps, gen)) return 0;
   bool ok;
   ModelsPlan* plan;
   float* zero_row;
@@ -2794,27 +2845,29 @@ size_t dsmil_backward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, 
   const std::vector<int64_t> Ns(caps.ne, max_rows);
   bytes = std::max(bytes, dsmil_backward_bags_models_workspace_bytes(ps, M, Ns.data(), nbs, 0));
   size_t each = 0;
-  for (int m = 0; m < M; ++m) each += ws_slice(dsmil_backward_bags_dev_workspace_bytes(&ps[m], nbs[m], max_rows));
+  for (int m = 0; m < M; ++m)
+    each += ws_slice(gen ? dsmil_generic_backward_bags_dev_workspace_bytes(&ps[m], nbs[m], max_rows)
+                         : dsmil_backward_bags_dev_workspace_bytes(&ps[m], nbs[m], max_rows));
   return std::max(bytes, each);
 }
 
-int dsmil_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
-                                   const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, const float* Q,
-                                   const float* H1, const float* A, const float* B, const int64_t* crit_idx,
-                                   const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
-                                   const dsmil_grads_t* grads, int32_t* status, void* workspace,
-                                   size_t workspace_bytes, void* stream) {
+static int backward_bags_models_dev(bool gen, const dsmil_params_t* ps, int M, const float* const* Xs_dev,
+                                    const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, const float* Q,
+                                    const float* H1, const float* A, const float* B, const int64_t* crit_idx,
+                                    const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                                    const dsmil_grads_t* grads, int32_t* status, void* workspace,
+                                    size_t workspace_bytes, cudaStream_t st) {
   ModelsDevCaps caps;
-  int rc = check_models_dev(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, &caps);
+  int rc = gen ? check_generic_models_dev(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, &caps)
+               : check_models_dev(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, &caps);
   if (rc) return rc;
-  DSMIL_REQUIRE(Q && H1 && A && B && crit_idx && grads, "NULL pointer");
+  DSMIL_REQUIRE(Q && (H1 || !ps[0].nonlinear) && A && B && crit_idx && grads, "NULL pointer");
   bool gX = false;
   for (int m = 0; m < M; ++m) gX = gX || grads[m].gX != nullptr;
   DSMIL_REQUIRE(!d_A && !d_B && !gX,
                 "the dev backward takes gradients through classes and pred only (no d_A, d_B or gX)");
-  const size_t need = dsmil_backward_bags_models_dev_workspace_bytes(ps, M, nbs, max_rows);
+  const size_t need = backward_bags_models_dev_ws(gen, ps, M, nbs, max_rows);
   if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int C = ps[0].C, D = ps[0].D;
   bool ok;
   ModelsPlan* plan;
@@ -2834,6 +2887,7 @@ int dsmil_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const fl
   pa.dz2 = w.dz2;
   pa.dz1 = w.dz1;
   pa.dc = d_classes != nullptr;
+  pa.gen = gen ? FOLD_GEN : FOLD_TC;
   k_plan_bags_models<<<1, 32 * M, 0, st>>>(pa);
   DSMIL_LAUNCH_OK("k_plan_bags_models");
   if (!d_classes)   // no gradient through the scores: zero instance-classifier gradients, as the eager call
@@ -2841,8 +2895,136 @@ int dsmil_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const fl
       if (grads[m].gWi) DSMIL_CUDA_OK(cudaMemsetAsync(grads[m].gWi, 0, sizeof(float) * C * D, st));
       if (grads[m].gbi) DSMIL_CUDA_OK(cudaMemsetAsync(grads[m].gbi, 0, sizeof(float) * C, st));
     }
-  BwdModelsGrid gr{caps.Gcap, caps.nci, caps.nc1, caps.nc2, caps.ncs, caps.max_model_rows, false, plan};
+  BwdModelsGrid gr{caps.Gcap, caps.nci, caps.nc1, caps.nc2, caps.ncs, caps.max_model_rows, false, plan,
+                   !ps[0].nonlinear};
   return bwd_models_launch(C, D, M, caps.ne, w, gr, Q, H1, A, B, crit_idx, d_classes, d_pred, nullptr, nullptr, st);
+}
+
+size_t dsmil_backward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                      int64_t max_rows) {
+  return backward_bags_models_dev_ws(false, ps, M, nbs, max_rows);
+}
+
+int dsmil_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                   const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, const float* Q,
+                                   const float* H1, const float* A, const float* B, const int64_t* crit_idx,
+                                   const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
+                                   const dsmil_grads_t* grads, int32_t* status, void* workspace,
+                                   size_t workspace_bytes, void* stream) {
+  return backward_bags_models_dev(false, ps, M, Xs_dev, Ns_dev, nbs, max_rows, Q, H1, A, B, crit_idx, d_classes,
+                                  d_pred, d_A, d_B, grads, status, workspace, workspace_bytes,
+                                  static_cast<cudaStream_t>(stream));
+}
+
+// ---- capture-safe fold step on the generic shapes ------------------------------------------------------------------
+// The fold twins of dsmil_generic_forward_bags_train_dev / dsmil_generic_backward_bags_dev: one planner launch
+// (k_plan_bags_models with the generic numbering) for all models, then the generic forward over the table of every
+// model's bags (gen_forward_run's fold form) or the fused fold backward (bwd_models_launch, linear q included).
+int dsmil_generic_models_supported(const dsmil_params_t* ps, int32_t M) {
+  if (!ps || M < 1 || M > sm90::kMaxModels || check_models(ps, M) != 0) return 0;
+  for (int m = 0; m < M; ++m)
+    if (!dsmil_generic_bags_supported(&ps[m])) return 0;
+  return 1;
+}
+
+static int check_generic_models_dev(const dsmil_params_t* ps, int M, const float* const* Xs, const int64_t* Ns,
+                                    const int32_t* nbs, int64_t max_rows, const int32_t* status,
+                                    ModelsDevCaps* caps) {
+  int rc = check_models(ps, M);
+  if (rc) return rc;
+  DSMIL_REQUIRE(!ps[0].passing_v, "the generic fold calls take identity v only (passing_v=1)");
+  DSMIL_REQUIRE(dsmil_generic_models_supported(ps, M),
+                "shape not on the generic batched route, i.e. on the tensor-core fold calls' (D=%d, C=%d, "
+                "nonlinear=%d, M=%d)", ps[0].D, ps[0].C, ps[0].nonlinear, M);
+  DSMIL_REQUIRE(Xs && Ns && nbs && status, "NULL bag list or status");
+  const char* why;
+  DSMIL_REQUIRE(models_dev_caps(ps, M, nbs, max_rows, caps, true, &why), "%s (max_rows=%lld)", why,
+                (long long)max_rows);
+  return 0;
+}
+
+// The forward's carve: the generic forward's for the capacity batch of every model's bags (every bag max_rows rows),
+// then the members, the planner's counts over all models and each model's own.
+struct GenModelsWs {
+  GenWs g;
+  sm90::ModelDev* models;
+  ModelsPlan* plan;
+  FoldLive* live;
+  size_t bytes;
+};
+static GenModelsWs carve_gen_models_dev(const dsmil_params_t* ps, int M, int ne, int64_t max_rows, void* ws,
+                                        size_t cap, bool* ok) {
+  GenModelsWs w;
+  w.g = carve_gen_dev(&ps[0], ne, max_rows, true, ws, cap, ok);
+  Carver c(ws, cap);
+  c.off = w.g.bytes;
+  w.models = c.take<sm90::ModelDev>(M);
+  w.plan = c.take<ModelsPlan>(1);
+  w.live = c.take<FoldLive>(M);
+  w.bytes = c.off;
+  *ok = *ok && c.ok();
+  return w;
+}
+
+size_t dsmil_generic_forward_bags_models_train_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M,
+                                                                   const int32_t* nbs, int64_t max_rows) {
+  ModelsDevCaps caps;
+  if (!models_dev_caps(ps, M, nbs, max_rows, &caps, true)) return 0;
+  bool ok;
+  size_t bytes = carve_gen_models_dev(ps, M, caps.ne, max_rows, nullptr, 0, &ok).bytes;
+  const std::vector<int64_t> Ns(caps.ne, max_rows);
+  bytes = std::max(bytes, dsmil_forward_bags_models_train_workspace_bytes(ps, M, Ns.data(), nbs));
+  size_t each = 0;
+  for (int m = 0; m < M; ++m)
+    each += ws_slice(dsmil_generic_forward_bags_train_dev_workspace_bytes(&ps[m], nbs[m], max_rows));
+  return std::max(bytes, each);
+}
+
+int dsmil_generic_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                                const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows,
+                                                float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                                                float* save_Q, float* save_H1, int32_t* status, void* workspace,
+                                                size_t workspace_bytes, void* stream) {
+  ModelsDevCaps caps;
+  int rc = check_generic_models_dev(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, &caps);
+  if (rc) return rc;
+  DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && (save_H1 || !ps[0].nonlinear),
+                "NULL output pointer");
+  const size_t need = dsmil_generic_forward_bags_models_train_dev_workspace_bytes(ps, M, nbs, max_rows);
+  if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int ne = caps.ne;
+  bool ok;
+  GenModelsWs w = carve_gen_models_dev(ps, M, ne, max_rows, workspace, workspace_bytes, &ok);
+  PlanModelsArgs pa = plan_models_args(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, nullptr);
+  pa.zero_row = w.g.zero_row;
+  pa.plan = w.plan;
+  pa.ftable = w.g.table;
+  pa.fmodels = w.models;
+  pa.gen = sm90::qmlp_supported(&ps[0]) ? FOLD_GEN_QMLP : FOLD_GEN;
+  pa.live = w.live;
+  k_plan_bags_models<<<1, 32 * M, 0, st>>>(pa);
+  DSMIL_LAUNCH_OK("k_plan_bags_models");
+  const GenFolds f{ps, nbs, M, max_rows, w.models, w.plan, w.live};
+  return gen_forward_run(&ps[0], w.g, ne, ne * max_rows, ne * tiles_for_bag(max_rows), ne * attend_ctas(max_rows),
+                         max_rows, classes, pred, A, B, crit_idx, save_Q, ps[0].nonlinear ? save_H1 : nullptr, nullptr,
+                         st, &f);
+}
+
+size_t dsmil_generic_backward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                              int64_t max_rows) {
+  return backward_bags_models_dev_ws(true, ps, M, nbs, max_rows);
+}
+
+int dsmil_generic_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                           const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows,
+                                           const float* Q, const float* H1, const float* A, const float* B,
+                                           const int64_t* crit_idx, const float* d_classes, const float* d_pred,
+                                           const float* d_A, const float* d_B, const dsmil_grads_t* grads,
+                                           int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {
+  return backward_bags_models_dev(true, ps, M, Xs_dev, Ns_dev, nbs, max_rows, Q, H1, A, B, crit_idx, d_classes,
+                                  d_pred, d_A, d_B, grads, status, workspace, workspace_bytes,
+                                  static_cast<cudaStream_t>(stream));
 }
 
 // ---- capture-safe row-sharded batch training: the six calls of the sharded step in dev form -----------------------

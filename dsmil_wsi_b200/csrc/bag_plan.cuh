@@ -8,6 +8,7 @@
 #include "gemm_generic.cuh"
 #include "fwd_sm90.cuh"
 #include "fwd_batched.cuh"
+#include "fwd_generic_b.cuh"
 
 namespace dsmil {
 
@@ -361,6 +362,19 @@ struct ModelsPlan {
   int tiles, recs;
   int nci, nc1, nc2, ncs;
 };
+// One model's live counts in a generic fold forward, for the stages that run one launch per model over its block:
+// its packed rows (layer 2 of the Q-MLP) and its 128-row tiles (k_qmlp_sm90).
+struct FoldLive {
+  long long total;
+  int tiles;
+};
+// The numbering of a fold dev call's forward table (PlanModelsArgs::gen).
+enum FoldTable : int {
+  FOLD_TC = 0,         // the fused tensor-core fold: bag_entry's records, pad_ = the model
+  FOLD_GEN = 1,        // generic: gen_bag_entry's records, pad_ = MODE | model << 2, tiles numbered across the models
+  FOLD_GEN_QMLP = 2    // as FOLD_GEN, but each model's tiles numbered from 0 (its own k_qmlp_sm90 launch)
+};
+
 // What the host knows of model m in a dev call, passed to the planner by value (a dev call uploads nothing).
 struct PlanModel {
   sm90::ModelDev w;
@@ -387,6 +401,8 @@ struct PlanModelsArgs {
   const float* H1;
   float *dz2, *dz1;
   int dc;                     // gradients flow through the scores (d_classes != NULL)
+  int gen;                    // FoldTable: the generic shapes take gen_bag_aligned bags and the generic numbering
+  FoldLive* live;             // generic forward: [M] each model's live counts
   PlanModel m[sm90::kMaxModels];
 };
 
@@ -397,6 +413,10 @@ struct PlanModelsArgs {
 // counts are single numbers and the partial buffer is indexed as in the eager call.  A model with a bad bag (N
 // outside [1, max_rows], features NULL or not 16-byte aligned) sets status[m] = 1 + the bag's index within the model
 // and is planned on its stand-in batch (every bag one row of zeros); the other models' plans do not change.
+// The generic shapes (a.gen != FOLD_TC) take the alignment rule of gen_bag_aligned and the generic forward's table:
+// model m's entries are what k_plan_bags_gen writes for its bags alone, shifted to its capacity block and to the
+// model's first tile and record, with its model beside its MODE in pad_ (fold_pad); FOLD_GEN_QMLP numbers each
+// model's tiles from 0, for phase 1 launched per model.  a.live[m] then receives the model's live rows and tiles.
 __global__ void __launch_bounds__(32 * sm90::kMaxModels)
 k_plan_bags_models(const PlanModelsArgs a) {
   enum { TILES, RECS, NCI, NC1, NC2, NCS, NCNT };
@@ -404,14 +424,15 @@ k_plan_bags_models(const PlanModelsArgs a) {
   const int m = threadIdx.x >> 5, lane = threadIdx.x & 31, M = a.M;
   const int e0 = a.m[m].e0, nb = a.m[m].nb;
   const long long cap0 = a.max_rows * e0;
-  const bool bwd = a.btable != nullptr;
+  const bool bwd = a.btable != nullptr, gen = a.gen != FOLD_TC;
   // the first bad bag and the largest bag, the lanes sharing the list
   int bad = nb + 1;
   long long mx = 0;
   for (int b = lane; b < nb; b += 32) {
     const int64_t N = a.Ns[e0 + b];
     const float* X = a.Xs[e0 + b];
-    if ((N < 1 || N > a.max_rows || X == nullptr || (reinterpret_cast<uintptr_t>(X) & 15) != 0) && b + 1 < bad)
+    const bool misaligned = gen ? !gen_bag_aligned(X, a.D) : (reinterpret_cast<uintptr_t>(X) & 15) != 0;
+    if ((N < 1 || N > a.max_rows || X == nullptr || misaligned) && b + 1 < bad)
       bad = b + 1;
     mx = N > mx ? N : mx;
   }
@@ -435,10 +456,11 @@ k_plan_bags_models(const PlanModelsArgs a) {
       const int64_t N = L.N(b);
       total += N;
       tiles += tiles_for_bag(N);
-      recs += recs_for_bag(N);
+      recs += gen ? attend_ctas(N) : recs_for_bag(N);
     }
     s_cnt[TILES][m] = tiles;
     s_cnt[RECS][m] = recs;
+    if (a.live) a.live[m] = FoldLive{total, tiles};
   }
   total = __shfl_sync(0xffffffffu, total, 0);
   const ModelSplits sp = model_splits(a.C, a.D, nb, total, mx);
@@ -460,10 +482,16 @@ k_plan_bags_models(const PlanModelsArgs a) {
   if (threadIdx.x == 0) *a.plan = ModelsPlan{all[TILES], all[RECS], all[NCI], all[NC1], all[NC2], all[NCS]};
   if (a.ftable && lane == 0) {
     long long row = cap0;
-    int tile = at[TILES], rec = at[RECS];
+    int tile = a.gen == FOLD_GEN_QMLP ? 0 : at[TILES], rec = at[RECS];
     for (int b = 0; b < nb; ++b) {
-      sm90::BagDev e = bag_entry(L.X(b), L.N(b), row, tile, rec);
-      e.pad_ = m;
+      sm90::BagDev e;
+      if (gen) {
+        e = gen_bag_entry(L.X(b), L.N(b), a.D, row, tile, rec);
+        e.pad_ = fold_pad(e.pad_, m);
+      } else {
+        e = bag_entry(L.X(b), L.N(b), row, tile, rec);
+        e.pad_ = m;
+      }
       a.ftable[e0 + b] = e;
     }
     a.fmodels[m] = a.m[m].w;
@@ -485,7 +513,7 @@ k_plan_bags_models(const PlanModelsArgs a) {
     a.segs[3 * M + m] = SumSeg{pm.gb2, at[NCS], sp.cs.S};
     a.segs[4 * M + m] = SumSeg{pm.gW1, at[NC1], s_cnt[NC1][m]};
     a.segs[5 * M + m] = SumSeg{pm.gb1, at[NCS], sp.cs.S};
-    a.lin[m] = LinSeg{a.dz2 + cap0 * kQ, pm.w.W2, a.H1 + cap0 * kQ, a.dz1 + cap0 * kQ, total};
+    a.lin[m] = LinSeg{a.dz2 + cap0 * kQ, pm.w.W2, a.H1 ? a.H1 + cap0 * kQ : nullptr, a.dz1 + cap0 * kQ, total};
     a.lin[M + m] = LinSeg{a.dz1 + cap0 * kQ, pm.w.W1, nullptr, nullptr, total};
   }
   for (int z = lane; z < sp.t2.S; z += 32) a.ch2[at[NC2] + z] = split_chunk(sp.t2, z, cap0, a.H1, kQ);

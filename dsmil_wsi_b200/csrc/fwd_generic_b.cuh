@@ -3,6 +3,10 @@
 // C <= 8, either q form).  Each runs the per-bag kernel's body on its bag's rows, so every bag's outputs are the bits
 // the per-bag forward gives it (DESIGN §4.2h).  The table (bag_plan.cuh: gen_bag_entry) numbers each bag's 128-row
 // tiles (tile_off), its attend_ctas(N) partial records (rec_off, nrec) and carries its k_scores MODE in pad_.
+// The fold form (dsmil_generic_forward_bags_models_train_dev) runs the same launches over every model's bags at once:
+// its table carries each entry's model beside the MODE (bag_plan.cuh: fold_pad), and the stages that read weights
+// (k_scores_b, k_linear_b, k_finalize_gb) take them from `models` [M] by the entry's model.  A one-model table's pad_
+// is its MODE (model 0) and `models` is NULL there, so those stages read the weights they are passed.
 //   k_scores_b       k_scores per 128-row tile of a bag (the bag's MODE), arg-max keys per bag
 //   k_linear_b       layer 1 of the Q-MLP, 64 rows of one bag per CTA (k_linear's tile)
 //   k_crit_qmax_b    q_max and the critical rows per (class, bag), as k_gather_cand + k_merge_cand of one bag
@@ -20,6 +24,11 @@
 namespace dsmil {
 
 static_assert(sm90::kTileM == 2 * LBM, "k_linear_b takes two k_linear tiles per 128-row tile");
+
+// pad_ of a generic table entry: the bag's k_scores MODE in bits 0-1, its model (fold tables; 0 otherwise) above them.
+__host__ __device__ inline int fold_pad(int mode, int m) { return mode | (m << 2); }
+__host__ __device__ inline int fold_pad_mode(int pad) { return pad & 3; }
+__host__ __device__ inline int fold_pad_model(int pad) { return pad >> 2; }
 
 // The per-bag kernels' bodies.  They are copies, not shared with k_scores, k_attend and k_finalize: calling a shared
 // body from those kernels changes their SASS (DESIGN §4.2h), which the per-bag forward keeps as it was.
@@ -258,34 +267,48 @@ __device__ __forceinline__ int bag_of(const sm90::BagDev* __restrict__ bags, int
   return lo;
 }
 
-// grid = tiles (tiles_dev: the live count of a capacity grid); dynamic shared memory C * D floats.
+// grid = tiles (tiles_dev: the live count of a capacity grid); dynamic shared memory C * D floats.  models != NULL:
+// Wi / bi of the entry's model instead of the ones passed.
 __global__ void __launch_bounds__(256)
 k_scores_b(const sm90::BagDev* __restrict__ bags, int nb, const int* __restrict__ tiles_dev, int D,
            const float* __restrict__ Wi, const float* __restrict__ bi, int C, float* __restrict__ classes,
-           unsigned long long* __restrict__ keys) {
+           unsigned long long* __restrict__ keys, const sm90::ModelDev* __restrict__ models) {
   const int t = blockIdx.x;
   if (tiles_dev && t >= *tiles_dev) return;
   const int bag = bag_of(bags, nb, t, false);
   const sm90::BagDev bg = bags[bag];
+  if (models) {
+    const sm90::ModelDev& md = models[fold_pad_model(bg.pad_)];
+    Wi = md.Wi;
+    bi = md.bi;
+  }
+  const int mode = fold_pad_mode(bg.pad_);
   const int64_t tl = t - bg.tile_off;
   const int64_t end = min(static_cast<int64_t>(bg.N), (tl + 1) * sm90::kTileM);
   float* cls = classes + bg.row_off * C;
   unsigned long long* kb = keys + static_cast<size_t>(bag) * kMaxC;
-  if (bg.pad_ == 2) scores_rows<2>(bg.X, end, tl * (sm90::kTileM / 8), 8, D, Wi, bi, C, cls, kb);
-  else if (bg.pad_ == 1) scores_rows<1>(bg.X, end, tl * sm90::kTileM, 8, D, Wi, bi, C, cls, kb);
+  if (mode == 2) scores_rows<2>(bg.X, end, tl * (sm90::kTileM / 8), 8, D, Wi, bi, C, cls, kb);
+  else if (mode == 1) scores_rows<1>(bg.X, end, tl * sm90::kTileM, 8, D, Wi, bi, C, cls, kb);
   else scores_rows<0>(bg.X, end, tl * sm90::kTileM, 8, D, Wi, bi, C, cls, kb);
 }
 
-// Y[packed rows, M] = act(X_b W^T + b) over each bag's own rows.  grid = (2 * tiles, ceil(M / LBN)).
+// Y[packed rows, M] = act(X_b W^T + b) over each bag's own rows.  grid = (2 * tiles, ceil(M / LBN)).  models != NULL:
+// layer 1 of the entry's model (W1 / b1) instead of W / b.
 template <int ACT>
 __global__ void __launch_bounds__(256)
 k_linear_b(const sm90::BagDev* __restrict__ bags, int nb, const int* __restrict__ tiles_dev, int K,
-           const float* __restrict__ W, const float* __restrict__ b, int M, float* __restrict__ Y) {
+           const float* __restrict__ W, const float* __restrict__ b, int M, float* __restrict__ Y,
+           const sm90::ModelDev* __restrict__ models) {
   const int t = blockIdx.x >> 1;
   if (tiles_dev && t >= *tiles_dev) return;
   const sm90::BagDev bg = bags[bag_of(bags, nb, t, false)];
   const int64_t n0 = static_cast<int64_t>(t - bg.tile_off) * sm90::kTileM + (blockIdx.x & 1) * LBM;
   if (n0 >= bg.N) return;
+  if (models) {
+    const sm90::ModelDev& md = models[fold_pad_model(bg.pad_)];
+    W = md.W1;
+    b = md.b1;
+  }
   linear_tile<ACT, false>(bg.X, bg.N, n0, K, W, b, M, Y + bg.row_off * M, nullptr, 0);
 }
 
@@ -330,13 +353,19 @@ k_combine_rec_b(const sm90::BagDev* __restrict__ bags, int C, int D, const float
   combine_recs(recs + bags[blockIdx.z].rec_off * stride, bags[blockIdx.z].nrec, C, D, out + blockIdx.z * stride);
 }
 
-// grid = (any, nb): bag y's A, B [nb, C, D] and pred [nb, C].
-__global__ void __launch_bounds__(256)
+// grid = (any, nb): bag y's A, B [nb, C, D] and pred [nb, C].  models != NULL: Wf / bf of the entry's model.
+// (256, 1): left to its default target ptxas spills the model's two weight pointers to stay within 32 registers.
+__global__ void __launch_bounds__(256, 1)
 k_finalize_gb(const sm90::BagDev* __restrict__ bags, const float* __restrict__ rec, int C, int D,
               const float* __restrict__ Wf, const float* __restrict__ bf, float* __restrict__ A, float* __restrict__ B,
-              float* __restrict__ pred) {
+              float* __restrict__ pred, const sm90::ModelDev* __restrict__ models) {
   const int bag = blockIdx.y;
   const sm90::BagDev bg = bags[bag];
+  if (models) {
+    const sm90::ModelDev& md = models[fold_pad_model(bg.pad_)];
+    Wf = md.Wf;
+    bf = md.bf;
+  }
   finalize_bag(rec + bag * rec_floats(C, D), bg.N, C, D, Wf, bf, A + bg.row_off * C,
                B + static_cast<size_t>(bag) * C * D, pred + static_cast<size_t>(bag) * C, blockIdx.x, gridDim.x);
 }

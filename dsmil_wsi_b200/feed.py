@@ -187,7 +187,8 @@ def fold_steps(sizes: Sequence[int], k: int) -> List[List[Tuple[int, int, int]]]
 def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[int]], criterion,
                        optimizers, dropout_patch: float = 0.0, orders: Optional[Sequence[Sequence[int]]] = None,
                        generators: Optional[Sequence[Optional[torch.Generator]]] = None,
-                       bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None) -> List[float]:
+                       bags_per_step: int = 1, graph: bool = False, max_rows: Optional[int] = None,
+                       generic: bool = False) -> List[float]:
     """One epoch of every fold model of a cross-validation (train_tcga.py:252-288, train_mil.py:164-187), the folds
     taking their steps together; returns each fold's mean loss per bag.  folds[m] lists the store indices of fold m's
     training split; orders[m], when given, is the order fold m visits them in (a permutation of folds[m]), else a
@@ -210,7 +211,9 @@ def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[
     bits.  The bags go through dropout_patches straight into the graph's slots; max_rows is the per-bag row capacity
     (default: the largest bag of the store), and a bag over it raises ValueError before any step.  Needs the fused fold
     shapes (dsmil_models_supported) and capture-safe optimizers, and records its graphs afresh on every call, as
-    train_epoch(graph=True) does."""
+    train_epoch(graph=True) does.  generic=True (with graph=True; the eager step ignores it) also takes folds on the
+    generic batched route (train_graph.fold_step_shape: e.g. the classic-MIL D = 166 / 230, a linear q), each fold's
+    results then the bits of train_epoch(..., graph=True, generic=True)."""
     from .ensemble import forward_bags_per_model
     milnets, M = list(milnets), len(folds)
     if not 1 <= M <= Fn.MAX_MODELS:
@@ -237,7 +240,7 @@ def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[
         net.train()
     if graph:
         return _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_patch, orders, gens,
-                                         bags_per_step, max_rows)
+                                         bags_per_step, max_rows, generic)
     totals = [torch.zeros((), device=store.device) for _ in range(M)]
     for step in fold_steps([len(o) for o in orders], bags_per_step):
         groups = [(m, orders[m][lo:hi]) for m, lo, hi in step]
@@ -308,9 +311,10 @@ def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order
     return loss / max(1, len(order))
 
 
-def _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_patch, orders, gens, k, max_rows):
+def _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_patch, orders, gens, k, max_rows,
+                              generic=False):
     from .train_graph import FoldTrainStepGraph, fold_step_shape
-    fold_step_shape(milnets)                                   # shapes off the fused fold route raise here
+    fold_step_shape(milnets, generic)                          # shapes off the fold routes raise here
     p = 1 - dropout_patch
     keep = {}
     for m, o in enumerate(orders):
@@ -324,7 +328,8 @@ def _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_pat
         g = graphs.get(key)
         if g is None:                                          # the full step, short last groups, fewer folds
             g = graphs[key] = FoldTrainStepGraph([milnets[m] for m, _ in key], criterion,
-                                                 [optimizers[m] for m, _ in key], [n for _, n in key], cap)
+                                                 [optimizers[m] for m, _ in key], [n for _, n in key], cap,
+                                                 generic=generic)
         e = 0
         for j, (m, lo, hi) in enumerate(step):
             group = orders[m][lo:hi]

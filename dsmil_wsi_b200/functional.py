@@ -548,6 +548,70 @@ class MILBagsModelsFn(torch.autograd.Function):
         return (None, *_split_rows(gX, Ns, need_bags), *outs)
 
 
+def _models_dev_forward(ctx, pre, nbs, slots, Ns, status, params):
+    """The body of MILBagsModelsDevFn.forward over the fold dev calls named pre + "forward_bags_models_train_dev"."""
+    lib = _lib.load()
+    ctx.set_materialize_grads(False)
+    M, ne = len(nbs), sum(nbs)
+    packs = _model_packs([params[10 * m:10 * (m + 1)] for m in range(M)])
+    P0 = packs[0]
+    ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
+    if pre == "dsmil_":
+        if min(nbs) < 1 or not lib.dsmil_models_supported(ps, M):
+            raise ValueError(f"the graph-captured fold step runs on the fused fold shapes only; M={M}, D={P0.D}, "
+                             f"C={P0.C}, nonlinear={P0.nonlinear}, group sizes {tuple(nbs)} are not on them")
+    elif min(nbs) < 1 or not lib.dsmil_generic_models_supported(ps, M):
+        raise ValueError(f"the generic graph-captured fold step runs on the generic batched shapes only; M={M}, "
+                         f"D={P0.D}, C={P0.C}, nonlinear={P0.nonlinear}, group sizes {tuple(nbs)} are not on them")
+    if slots.dim() != 3 or slots.shape[0] != ne or slots.shape[2] != P0.D or slots.dtype != torch.float32 \
+            or not slots.is_contiguous():
+        raise ValueError(f"slots must be contiguous float32 [{ne}, max_rows, {P0.D}], got {tuple(slots.shape)}")
+    xs = _slot_addrs(slots, P0, "slots")
+    max_rows, dev = int(slots.shape[1]), P0.device
+    c_nb = (C.c_int32 * M)(*nbs)
+    call = pre + "forward_bags_models_train_dev"
+    with torch.cuda.device(dev):
+        rows = ne * max_rows
+        classes, pred, A, B, crit = _bag_outputs(P0, rows, ne)
+        sQ, sH, _ = _saves(P0, rows)
+        ws = _workspace(getattr(lib, call + "_workspace_bytes")(ps, M, c_nb, max_rows), dev)
+        rc = getattr(lib, call)(ps, M, _ptr(xs), _ptr(Ns), c_nb, max_rows, _ptr(classes), _ptr(pred), _ptr(A),
+                                _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH), _ptr(status), _ptr(ws), ws.numel(),
+                                _stream())
+        _lib.check(rc, call)
+    ctx.save_for_backward(xs, Ns, status, sQ, sH, A, B, crit, *[t for P in packs for t in P.tensors])
+    ctx.nbs, ctx.max_rows, ctx.pre = tuple(nbs), max_rows, pre
+    ctx.mark_non_differentiable(crit)
+    return classes, pred, A, B, crit
+
+
+def _models_dev_backward(ctx, g_classes, g_pred, g_A, g_B):
+    """The body of MILBagsModelsDevFn.backward over the fold dev calls of the forward's prefix."""
+    if ctx.needs_input_grad[1] or g_A is not None or g_B is not None:
+        raise NotImplementedError("the graph-captured fold step takes gradients through the instance scores "
+                                  "and the bag prediction only (no gradient to A, B or the features)")
+    lib = _lib.load()
+    xs, Ns, status, sQ, sH, A, B, crit, *params = ctx.saved_tensors
+    nbs, max_rows = ctx.nbs, ctx.max_rows
+    M = len(nbs)
+    packs = [ParamPack(*params[10 * m:10 * (m + 1)]) for m in range(M)]
+    dev = packs[0].device
+    ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
+    c_nb = (C.c_int32 * M)(*nbs)
+    need = ctx.needs_input_grad[4:]
+    call = ctx.pre + "backward_bags_models_dev"
+    with torch.cuda.device(dev):
+        outs, grads = zip(*[_param_grads(P, need[10 * m:10 * (m + 1)]) for m, P in enumerate(packs)])
+        grads = (_lib.DsmilGrads * M)(*grads)
+        dc, dp = _f32c(g_classes), _f32c(g_pred)
+        ws = _workspace(getattr(lib, call + "_workspace_bytes")(ps, M, c_nb, max_rows), dev)
+        rc = getattr(lib, call)(ps, M, _ptr(xs), _ptr(Ns), c_nb, max_rows, _ptr(sQ), _ptr(sH), _ptr(A), _ptr(B),
+                                _ptr(crit), _ptr(dc), _ptr(dp), None, None, grads, _ptr(status), _ptr(ws),
+                                ws.numel(), _stream())
+        _lib.check(rc, call)
+    return (None, None, None, None, *[g for out in outs for g in out])
+
+
 class MILBagsModelsDevFn(torch.autograd.Function):
     """MILBagsModelsFn over the capture-safe entry points (dsmil_forward_bags_models_train_dev /
     dsmil_backward_bags_models_dev): every member's bag list lives on the device, so one recorded call serves every
@@ -560,59 +624,25 @@ class MILBagsModelsDevFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, nbs, slots, Ns, status, *params):
-        lib = _lib.load()
-        ctx.set_materialize_grads(False)
-        M, ne = len(nbs), sum(nbs)
-        packs = _model_packs([params[10 * m:10 * (m + 1)] for m in range(M)])
-        P0 = packs[0]
-        ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
-        if min(nbs) < 1 or not lib.dsmil_models_supported(ps, M):
-            raise ValueError(f"the graph-captured fold step runs on the fused fold shapes only; M={M}, D={P0.D}, "
-                             f"C={P0.C}, nonlinear={P0.nonlinear}, group sizes {tuple(nbs)} are not on them")
-        if slots.dim() != 3 or slots.shape[0] != ne or slots.shape[2] != P0.D or slots.dtype != torch.float32 \
-                or not slots.is_contiguous():
-            raise ValueError(f"slots must be contiguous float32 [{ne}, max_rows, {P0.D}], got {tuple(slots.shape)}")
-        xs = _slot_addrs(slots, P0, "slots")
-        max_rows, dev = int(slots.shape[1]), P0.device
-        c_nb = (C.c_int32 * M)(*nbs)
-        with torch.cuda.device(dev):
-            rows = ne * max_rows
-            classes, pred, A, B, crit = _bag_outputs(P0, rows, ne)
-            sQ, sH, _ = _saves(P0, rows)
-            ws = _workspace(lib.dsmil_forward_bags_models_train_dev_workspace_bytes(ps, M, c_nb, max_rows), dev)
-            rc = lib.dsmil_forward_bags_models_train_dev(ps, M, _ptr(xs), _ptr(Ns), c_nb, max_rows, _ptr(classes),
-                                                         _ptr(pred), _ptr(A), _ptr(B), _ptr(crit), _ptr(sQ), _ptr(sH),
-                                                         _ptr(status), _ptr(ws), ws.numel(), _stream())
-            _lib.check(rc, "dsmil_forward_bags_models_train_dev")
-        ctx.save_for_backward(xs, Ns, status, sQ, sH, A, B, crit, *[t for P in packs for t in P.tensors])
-        ctx.nbs, ctx.max_rows = tuple(nbs), max_rows
-        ctx.mark_non_differentiable(crit)
-        return classes, pred, A, B, crit
+        return _models_dev_forward(ctx, "dsmil_", nbs, slots, Ns, status, params)
 
     @staticmethod
     def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
-        if ctx.needs_input_grad[1] or g_A is not None or g_B is not None:
-            raise NotImplementedError("the graph-captured fold step takes gradients through the instance scores "
-                                      "and the bag prediction only (no gradient to A, B or the features)")
-        lib = _lib.load()
-        xs, Ns, status, sQ, sH, A, B, crit, *params = ctx.saved_tensors
-        nbs, max_rows = ctx.nbs, ctx.max_rows
-        M = len(nbs)
-        packs = [ParamPack(*params[10 * m:10 * (m + 1)]) for m in range(M)]
-        dev = packs[0].device
-        ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
-        c_nb = (C.c_int32 * M)(*nbs)
-        need = ctx.needs_input_grad[4:]
-        with torch.cuda.device(dev):
-            outs, grads = zip(*[_param_grads(P, need[10 * m:10 * (m + 1)]) for m, P in enumerate(packs)])
-            grads = (_lib.DsmilGrads * M)(*grads)
-            dc, dp = _f32c(g_classes), _f32c(g_pred)
-            ws = _workspace(lib.dsmil_backward_bags_models_dev_workspace_bytes(ps, M, c_nb, max_rows), dev)
-            rc = lib.dsmil_backward_bags_models_dev(ps, M, _ptr(xs), _ptr(Ns), c_nb, max_rows, _ptr(sQ), _ptr(sH),
-                                                    _ptr(A), _ptr(B), _ptr(crit), _ptr(dc), _ptr(dp), None, None,
-                                                    grads, _ptr(status), _ptr(ws), ws.numel(), _stream())
-            _lib.check(rc, "dsmil_backward_bags_models_dev")
-        return (None, None, None, None, *[g for out in outs for g in out])
+        return _models_dev_backward(ctx, g_classes, g_pred, g_A, g_B)
+
+
+class MILBagsModelsGenericDevFn(torch.autograd.Function):
+    """MILBagsModelsDevFn on the generic shapes (dsmil_generic_models_supported: e.g. the classic-MIL D = 166 / 230, a
+    linear q, C > 4, D > 2048): the same arguments and outputs over dsmil_generic_forward_bags_models_train_dev /
+    dsmil_generic_backward_bags_models_dev, member m's slices bit for bit those of MILBagsDevFn on its bags alone."""
+
+    @staticmethod
+    def forward(ctx, nbs, slots, Ns, status, *params):
+        return _models_dev_forward(ctx, "dsmil_generic_", nbs, slots, Ns, status, params)
+
+    @staticmethod
+    def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
+        return _models_dev_backward(ctx, g_classes, g_pred, g_A, g_B)
 
 
 def mil_forward_bags_per_model(bag_lists: Sequence[Sequence[torch.Tensor]],

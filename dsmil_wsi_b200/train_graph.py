@@ -84,22 +84,45 @@ def step_shape(milnet, generic: bool = False, value: bool = False):
                      "(generic=True records the generic batched route of the other identity-v shapes)")
 
 
-def fold_step_shape(milnets):
+def fold_step_shape(milnets, generic: bool = False):
     """(D, C) of MILNets whose fold step the graph can record: each on step_shape's route, all of one D, C and q form,
-    1 to 8 of them, together on the fused fold shapes (dsmil_models_supported).  Else ValueError."""
+    1 to 8 of them, together on the fused fold shapes (dsmil_models_supported).  generic=True also takes folds on the
+    generic batched route (dsmil_generic_models_supported: e.g. the classic-MIL D = 166 / 230, a linear q, C > 4,
+    D > 2048); tensor-core shapes whose folds do not fit the fused fold step stay refused.  Else ValueError."""
+    return _fold_route(milnets, generic)[:2]
+
+
+def _fold_route(milnets, generic):
+    """(D, C, whether the folds take the generic fold calls) of fold_step_shape."""
     milnets = list(milnets)
     if not 1 <= len(milnets) <= Fn.MAX_MODELS:
         raise ValueError(f"a fold step takes 1 to {Fn.MAX_MODELS} folds, got {len(milnets)}")
-    shapes = [step_shape(net) for net in milnets]
+    shapes = [step_shape(net, generic) for net in milnets]
     for m, sh in enumerate(shapes):
         if sh != shapes[0]:
             raise ValueError(f"fold {m}: (D, C)={sh} differs from fold 0's {shapes[0]}")
     D, C = shapes[0]
-    ps = (_lib.DsmilParams * len(milnets))(*[_shape_params(D, C, True, False)] * len(milnets))
-    if not _lib.load().dsmil_models_supported(ps, len(milnets)):
-        raise ValueError(f"the graph-captured fold step runs on the fused fold shapes only; M={len(milnets)}, D={D}, "
+    forms = [milnet_q_nonlinear(net) for net in milnets]
+    for m, nl in enumerate(forms):
+        if nl != forms[0]:
+            raise ValueError(f"fold {m}: nonlinear={nl} differs from fold 0's {forms[0]}")
+    M, lib = len(milnets), _lib.load()
+    ps = (_lib.DsmilParams * M)(*[_shape_params(D, C, forms[0], False)] * M)
+    if lib.dsmil_shard_bags_supported(ctypes.byref(ps[0])):
+        if lib.dsmil_models_supported(ps, M):
+            return D, C, False
+        raise ValueError(f"the graph-captured fold step runs on the fused fold shapes only; M={M}, D={D}, "
                          f"C={C} is not on them: train these folds one at a time (train_epoch(graph=True))")
-    return D, C
+    # off the tensor-core batch: only generic=True gets here (step_shape refuses the shape otherwise)
+    if not lib.dsmil_generic_models_supported(ps, M):
+        raise ValueError(f"the generic graph-captured fold step does not take M={M}, D={D}, C={C}, "
+                         f"nonlinear={forms[0]}")
+    return D, C, True
+
+
+def milnet_q_nonlinear(milnet) -> bool:
+    """Whether a MILNet's q is the nonlinear Linear-ReLU-Linear-Tanh (dsmil.py:31) rather than one Linear (:33)."""
+    return milnet.b_classifier._q_params()[2] is not None
 
 
 def _flat(tensors):
@@ -290,13 +313,15 @@ class FoldTrainStepGraph:
     fold's optimizer.step().  Fill `slots[m][b, :n]` with bag b of fold m, `Ns` [sum nbs] (fold-major) with the row
     counts and `labels` [sum nbs, C], then `step()` replays the graph and returns the M losses (a device tensor,
     overwritten by the next replay).  With the same batches, fold m's losses, gradients and parameters are bit for
-    bit those of its own TrainStepGraph.
+    bit those of its own TrainStepGraph.  generic=True: also folds on the generic batched route (fold_step_shape),
+    whose step records MILBagsModelsGenericDevFn with the bits of each fold's TrainStepGraph(generic=True); fused
+    tensor-core fold shapes keep the fused fold step.
 
     Refusal is per fold: a fold with a bag outside 1..max_rows has `status[m]` set (the first refusal's 1 + bag index
     within the fold; never cleared here), a NaN loss, and its parameters and optimizer state left as they were; the
     other folds step normally.  Warm-up, capture and hyperparameters behave as in TrainStepGraph."""
 
-    def __init__(self, milnets, criterion, optimizers, nbs, max_rows: int, warmup: int = 1):
+    def __init__(self, milnets, criterion, optimizers, nbs, max_rows: int, warmup: int = 1, generic: bool = False):
         milnets, optimizers, nbs = list(milnets), list(optimizers), [int(n) for n in nbs]
         M = len(milnets)
         if len(optimizers) != M or len(nbs) != M:
@@ -304,7 +329,7 @@ class FoldTrainStepGraph:
                              "sizes")
         for opt in optimizers:
             check_optimizer(opt)
-        D, C = fold_step_shape(milnets)
+        D, C, self.generic = _fold_route(milnets, generic)
         ne, max_rows = sum(nbs), int(max_rows)
         if min(nbs) < 1 or ne > 65535 or max_rows < 1:
             raise ValueError(f"FoldTrainStepGraph: group sizes {nbs} outside [1, 65535] or max_rows={max_rows} < 1")
@@ -329,8 +354,8 @@ class FoldTrainStepGraph:
         accepted."""
         self._step_status.zero_()
         params = [t for net in self.milnets for t in milnet_params(net)]
-        classes, pred, _, _, crit = Fn.MILBagsModelsDevFn.apply(self.nbs, self._slots, self.Ns, self._step_status,
-                                                                *params)
+        fn = Fn.MILBagsModelsGenericDevFn if self.generic else Fn.MILBagsModelsDevFn
+        classes, pred, _, _, crit = fn.apply(self.nbs, self._slots, self.Ns, self._step_status, *params)
         n = self.Ns.clamp(0, self.max_rows)                # the live sizes (a refused fold's stay in range)
         losses, oks = [], []
         for m, (e, nb) in enumerate(zip(self._bag0, self.nbs)):

@@ -259,8 +259,8 @@ int dsmil_backward_bags_dev(const dsmil_params_t* p, const float* const* Xs_dev,
  * max_rows * sum_{j<m} nbs[j], and inside that block its live rows are packed at its own live prefix sums: model m's
  * block of every buffer is what the one-model dev call would be given.  classes / A / save_Q / save_H1 / d_classes
  * have max_rows * sum nbs rows; pred, B, crit_idx are [sum nbs, ...].
- * Shapes: dsmil_models_supported(ps, M) must hold (there is no per-model loop route: the one-model dev calls serve
- * the other shapes one fold at a time), 1 <= nbs[m], sum nbs <= 65535 less a chunk allowance of at most 296 per model
+ * Shapes: dsmil_models_supported(ps, M) must hold (there is no per-model loop route: the generic shapes take the
+ * dsmil_generic_*_models_* twins below), 1 <= nbs[m], sum nbs <= 65535 less a chunk allowance of at most 296 per model
  * (the ragged GEMM grids number their chunks in 16 bits), 1 <= max_rows < 2^32 with the capacity tiles in an int.
  * Anything else is DSMIL_ERR_ARG before any CUDA work, and the workspace functions return 0.
  * Refusal is per model: a bag of model m with N outside [1, max_rows], or features NULL or not 16-byte aligned, sets
@@ -286,6 +286,45 @@ int dsmil_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const fl
                                    const float* d_classes, const float* d_pred, const float* d_A, const float* d_B,
                                    const dsmil_grads_t* grads, int32_t* status, void* workspace,
                                    size_t workspace_bytes, void* stream);
+/* The two capture-safe fold calls above on the generic shapes: the fold step of a cross-validation on the shapes off
+ * the tensor-core batch (e.g. the classic-MIL D = 166 / 230, a linear q, C > 4, D > 2048) recorded once as a CUDA
+ * graph.  Arguments, model-major layout, the HOST array nbs, per-model refusal through status[M], the stand-in batch,
+ * the capacity blocks and the workspace rules are those of dsmil_forward_bags_models_train_dev /
+ * dsmil_backward_bags_models_dev, except:
+ *  - Shapes: dsmil_generic_models_supported(ps, M): 1 <= M <= 8 members with the same D, C and q form, identity v,
+ *    each on dsmil_generic_bags_supported.  The tensor-core shapes (dsmil_shard_bags_supported, fused fold or not)
+ *    are DSMIL_ERR_ARG here; passing_v is DSMIL_ERR_ARG ("identity v").
+ *  - Alignment rule: that of the one-model generic dev calls -- a bag must be 16-byte aligned when D % 4 == 0 and
+ *    4-byte aligned otherwise, so [sum nbs, max_rows, D] slots of any D are accepted.  A bag that breaks it refuses
+ *    its model like a bag of a bad size.
+ *  - save_H1 / H1 may be NULL for a linear q.
+ *  - Bits: model m's slices of every output and gradient are, bit for bit, what dsmil_generic_forward_bags_train_dev
+ *    / dsmil_generic_backward_bags_dev give for model m's bags alone; every partial-sum layout follows from model m's
+ *    live sizes alone.
+ *  - Launches: the forward is one planner launch, then one launch per stage for all models, except that layer 2 of
+ *    a nonlinear q (and, on the shapes whose phase 1 is k_qmlp_sm90 -- nonlinear q, D % 128 == 0 -- the weight-image
+ *    prep and phase 1) run once per model over its block.  The backward is the fused fold backward: one planner
+ *    launch and one launch per stage for all models (a linear q has no layer 2).
+ *  - Bounds: sum nbs plus the ragged GEMMs' chunk allowance (rag_splits per model: 148 at D = 166 / 230, C = 1) within
+ *    65535, and 2 * sum nbs * ceil(max_rows / 128) <= INT_MAX; past them DSMIL_ERR_ARG ("chunk capacity" for the
+ *    first) and both workspace sizes are 0.  The workspace sizes are never below the sum of the one-model generic dev
+ *    calls' sizes. */
+int dsmil_generic_models_supported(const dsmil_params_t* ps, int32_t M);
+size_t dsmil_generic_forward_bags_models_train_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M,
+                                                                   const int32_t* nbs, int64_t max_rows);
+int dsmil_generic_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                                const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows,
+                                                float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                                                float* save_Q, float* save_H1, int32_t* status, void* workspace,
+                                                size_t workspace_bytes, void* stream);
+size_t dsmil_generic_backward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                              int64_t max_rows);
+int dsmil_generic_backward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                           const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows,
+                                           const float* Q, const float* H1, const float* A, const float* B,
+                                           const int64_t* crit_idx, const float* d_classes, const float* d_pred,
+                                           const float* d_A, const float* d_B, const dsmil_grads_t* grads,
+                                           int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 /* Capture-safe form of dsmil_forward_bags (inference), under the rules of dsmil_forward_bags_train_dev above: the bag
  * list in device memory, classes and A sized for nb * max_rows rows with the live rows packed at the live prefix sums,
  * no host<->device copy, allocation or synchronisation, the same refusal through *status and the same stand-in batch,
