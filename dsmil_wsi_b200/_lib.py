@@ -194,6 +194,18 @@ SIGNATURES = {
                                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                          C.c_void_p, C.c_void_p, C.POINTER(DsmilGrads), C.c_void_p,
                                                          C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dsmil_forward_bags_models_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32,
+                                                                   C.POINTER(C.c_int32), c_i64]),
+    "dsmil_forward_bags_models_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_int32, C.c_void_p, C.c_void_p,
+                                                C.POINTER(C.c_int32), c_i64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                C.c_void_p]),
+    "dsmil_generic_forward_bags_models_dev_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.c_int32,
+                                                                           C.POINTER(C.c_int32), c_i64]),
+    "dsmil_generic_forward_bags_models_dev": (C.c_int, [C.POINTER(DsmilParams), C.c_int32, C.c_void_p, C.c_void_p,
+                                                        C.POINTER(C.c_int32), c_i64, C.c_void_p, C.c_void_p,
+                                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                        C.c_size_t, C.c_void_p]),
     "dsmil_shard_bags_supported": (C.c_int, [C.POINTER(DsmilParams)]),
     "dsmil_shard_bags_workspace_bytes": (C.c_size_t, [C.POINTER(DsmilParams), C.POINTER(c_i64), C.c_int32]),
     "dsmil_shard_bags_phase1": (C.c_int, [C.POINTER(DsmilParams), C.POINTER(C.c_void_p), C.POINTER(c_i64), C.c_int32,

@@ -2743,10 +2743,11 @@ static PlanModelsArgs plan_models_args(const dsmil_params_t* ps, int M, const fl
 }
 
 // The forward's carve for the capacity batch (every bag max_rows rows), then the planner's counts and the zero row.
-static ModelsWs carve_models_dev(const dsmil_params_t* ps, int M, int ne, int64_t max_rows, void* ws, size_t cap,
-                                 bool* ok, ModelsPlan** plan, float** zero_row) {
+// need_Q: the tile blocks of Q for the capacity tiles (inference); otherwise Q and H1 are the caller's saves.
+static ModelsWs carve_models_dev(const dsmil_params_t* ps, int M, int ne, int64_t max_rows, bool need_Q, void* ws,
+                                 size_t cap, bool* ok, ModelsPlan** plan, float** zero_row) {
   const std::vector<int64_t> Ns(ne, max_rows);
-  ModelsWs w = carve_models(&ps[0], M, Ns.data(), ne, 1, false, ws, cap, ok);
+  ModelsWs w = carve_models(&ps[0], M, Ns.data(), ne, 1, need_Q, ws, cap, ok);
   Carver c(ws, cap);
   c.off = w.bytes;
   *plan = c.take<ModelsPlan>(1);
@@ -2756,39 +2757,46 @@ static ModelsWs carve_models_dev(const dsmil_params_t* ps, int M, int ne, int64_
   return w;
 }
 
-size_t dsmil_forward_bags_models_train_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
-                                                           int64_t max_rows) {
+// The fold forward pair's size (train: dsmil_forward_bags_models_train_dev; inference: dsmil_forward_bags_models_dev,
+// whose Q stays in the workspace as tile blocks): never below the eager fold call's size for the same capacity, nor
+// the one-model dev calls' sizes together.
+static size_t forward_bags_models_dev_ws(bool train, const dsmil_params_t* ps, int M, const int32_t* nbs,
+                                         int64_t max_rows) {
   ModelsDevCaps caps;
   if (!models_dev_caps(ps, M, nbs, max_rows, &caps)) return 0;
   bool ok;
   ModelsPlan* plan;
   float* zero_row;
-  size_t bytes = carve_models_dev(ps, M, caps.ne, max_rows, nullptr, 0, &ok, &plan, &zero_row).bytes;
-  // never below the eager fold call's size for the same capacity, nor the one-model dev calls' sizes together
+  size_t bytes = carve_models_dev(ps, M, caps.ne, max_rows, !train, nullptr, 0, &ok, &plan, &zero_row).bytes;
   const std::vector<int64_t> Ns(caps.ne, max_rows);
   bytes = std::max(bytes, dsmil_forward_bags_models_train_workspace_bytes(ps, M, Ns.data(), nbs));
   size_t each = 0;
-  for (int m = 0; m < M; ++m) each += ws_slice(dsmil_forward_bags_train_dev_workspace_bytes(&ps[m], nbs[m], max_rows));
+  for (int m = 0; m < M; ++m)
+    each += ws_slice(train ? dsmil_forward_bags_train_dev_workspace_bytes(&ps[m], nbs[m], max_rows)
+                           : dsmil_forward_bags_dev_workspace_bytes(&ps[m], nbs[m], max_rows));
   return std::max(bytes, each);
 }
 
-int dsmil_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
-                                        const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, float* classes,
-                                        float* pred, float* A, float* B, int64_t* crit_idx, float* save_Q,
-                                        float* save_H1, int32_t* status, void* workspace, size_t workspace_bytes,
-                                        void* stream) {
+// The fold forward pair's body.  train: as dsmil_forward_bags_train_dev, phase 1 writes the caller's row-major save_Q
+// and save_H1 and the attend pass is a plain launch.  Inference: as dsmil_forward_bags_dev, Q stays in the workspace
+// as tile blocks, and the attend pass is a programmatic dependent of phase 1 (also under stream capture), each entry
+// gated on its tiles' releases in w.done (DESIGN §4.2k); only kernel timing keeps the plain launch.  Either way the
+// weight images are rebuilt on every call and the grids are the capacity's, their live counts the planner's.
+static int forward_bags_models_dev(bool train, const dsmil_params_t* ps, int M, const float* const* Xs_dev,
+                                   const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, float* classes,
+                                   float* pred, float* A, float* B, int64_t* crit_idx, float* save_Q, float* save_H1,
+                                   int32_t* status, void* workspace, size_t workspace_bytes, cudaStream_t st) {
   ModelsDevCaps caps;
   int rc = check_models_dev(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, &caps);
   if (rc) return rc;
-  DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && save_H1, "NULL output pointer");
-  const size_t need = dsmil_forward_bags_models_train_dev_workspace_bytes(ps, M, nbs, max_rows);
+  DSMIL_REQUIRE(classes && pred && A && B && (!train || (crit_idx && save_Q && save_H1)), "NULL output pointer");
+  const size_t need = forward_bags_models_dev_ws(train, ps, M, nbs, max_rows);
   if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int C = ps[0].C, D = ps[0].D, ne = caps.ne;
   bool ok;
   ModelsPlan* plan;
   float* zero_row;
-  ModelsWs w = carve_models_dev(ps, M, ne, max_rows, workspace, workspace_bytes, &ok, &plan, &zero_row);
+  ModelsWs w = carve_models_dev(ps, M, ne, max_rows, !train, workspace, workspace_bytes, &ok, &plan, &zero_row);
   PlanModelsArgs pa = plan_models_args(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, nullptr);
   pa.zero_row = zero_row;
   pa.plan = plan;
@@ -2796,18 +2804,49 @@ int dsmil_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, con
   pa.fmodels = w.models;
   k_plan_bags_models<<<1, 32 * M, 0, st>>>(pa);
   DSMIL_LAUNCH_OK("k_plan_bags_models");
-  // as dsmil_forward_bags_train_dev: the weight images rebuilt on every call, phase 1 on the capacity grid of tiles,
-  // the attend pass a plain launch on the capacity grid of records
+  const bool overlap = !train && !g_prof_on;
+  float* Q = train ? save_Q : w.Q;
+  const int tiles = ne * tiles_for_bag(max_rows);
   DSMIL_CUDA_OK(cudaMemsetAsync(w.keys, 0, sizeof(unsigned long long) * (kMaxC + 1) * ne, st));
   if ((rc = sm90::launch_prep_wimg_models(w.models, M, D, w.wimg, st))) return rc;
-  if ((rc = sm90::launch_qmlp_models(w.models, M, D, C, w.table, ne, ne * tiles_for_bag(max_rows), classes, w.keys,
-                                     save_Q, save_H1, false, w.wimg, num_sms(), st, nullptr, &plan->tiles)))
+  if ((rc = sm90::launch_qmlp_models(w.models, M, D, C, w.table, ne, tiles, classes, w.keys, Q,
+                                     train ? save_H1 : nullptr, !train, w.wimg,
+                                     overlap ? overlap_phase1_ctas(tiles) : num_sms(), st,
+                                     overlap ? w.done : nullptr, &plan->tiles)))
     return rc;
-  sm90::AttendArgs aa{w.table, ne, D, C, save_Q, false, w.keys, A, w.recs, nullptr, &plan->recs, nullptr};
+  sm90::AttendArgs aa{w.table, ne, D, C, Q, !train, w.keys, A, w.recs, nullptr, &plan->recs,
+                      overlap ? w.done : nullptr};
   if ((rc = sm90::launch_attend_b(aa, ne * recs_for_bag(max_rows), st))) return rc;
   sm90::FinalizeArgs fa{w.table, D, C, w.recs, w.keys, nullptr, nullptr, A, B, pred,
                         reinterpret_cast<long long*>(crit_idx), w.pred_part, w.counters, nullptr, 0, 0, w.models, 1, 0};
   return sm90::launch_finalize_b(fa, ne, st);
+}
+
+size_t dsmil_forward_bags_models_train_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                           int64_t max_rows) {
+  return forward_bags_models_dev_ws(true, ps, M, nbs, max_rows);
+}
+
+int dsmil_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                        const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, float* classes,
+                                        float* pred, float* A, float* B, int64_t* crit_idx, float* save_Q,
+                                        float* save_H1, int32_t* status, void* workspace, size_t workspace_bytes,
+                                        void* stream) {
+  return forward_bags_models_dev(true, ps, M, Xs_dev, Ns_dev, nbs, max_rows, classes, pred, A, B, crit_idx, save_Q,
+                                 save_H1, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+size_t dsmil_forward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                     int64_t max_rows) {
+  return forward_bags_models_dev_ws(false, ps, M, nbs, max_rows);
+}
+
+int dsmil_forward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                  const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, float* classes,
+                                  float* pred, float* A, float* B, int64_t* crit_idx, int32_t* status, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  return forward_bags_models_dev(false, ps, M, Xs_dev, Ns_dev, nbs, max_rows, classes, pred, A, B, crit_idx, nullptr,
+                                 nullptr, status, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 // The backward's carve at the capacities, then the planner's counts and the zero row.
@@ -2944,7 +2983,8 @@ static int check_generic_models_dev(const dsmil_params_t* ps, int M, const float
 }
 
 // The forward's carve: the generic forward's for the capacity batch of every model's bags (every bag max_rows rows),
-// then the members, the planner's counts over all models and each model's own.
+// then the members, the planner's counts over all models and each model's own.  saves: the caller keeps Q and H1
+// (the training form); inference keeps them, and the critical rows if the caller wants none, in the workspace.
 struct GenModelsWs {
   GenWs g;
   sm90::ModelDev* models;
@@ -2952,10 +2992,10 @@ struct GenModelsWs {
   FoldLive* live;
   size_t bytes;
 };
-static GenModelsWs carve_gen_models_dev(const dsmil_params_t* ps, int M, int ne, int64_t max_rows, void* ws,
-                                        size_t cap, bool* ok) {
+static GenModelsWs carve_gen_models_dev(const dsmil_params_t* ps, int M, int ne, int64_t max_rows, bool saves,
+                                        void* ws, size_t cap, bool* ok) {
   GenModelsWs w;
-  w.g = carve_gen_dev(&ps[0], ne, max_rows, true, ws, cap, ok);
+  w.g = carve_gen_dev(&ps[0], ne, max_rows, saves, ws, cap, ok);
   Carver c(ws, cap);
   c.off = w.g.bytes;
   w.models = c.take<sm90::ModelDev>(M);
@@ -2966,36 +3006,41 @@ static GenModelsWs carve_gen_models_dev(const dsmil_params_t* ps, int M, int ne,
   return w;
 }
 
-size_t dsmil_generic_forward_bags_models_train_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M,
-                                                                   const int32_t* nbs, int64_t max_rows) {
+// The generic fold forward pair's size (train: the _train_dev call; inference: Q, H1 and the critical rows in the
+// workspace), never below the eager fold call's size for the same capacity, nor the one-model generic dev calls'
+// sizes together.
+static size_t generic_forward_bags_models_dev_ws(bool train, const dsmil_params_t* ps, int M, const int32_t* nbs,
+                                                 int64_t max_rows) {
   ModelsDevCaps caps;
   if (!models_dev_caps(ps, M, nbs, max_rows, &caps, true)) return 0;
   bool ok;
-  size_t bytes = carve_gen_models_dev(ps, M, caps.ne, max_rows, nullptr, 0, &ok).bytes;
+  size_t bytes = carve_gen_models_dev(ps, M, caps.ne, max_rows, train, nullptr, 0, &ok).bytes;
   const std::vector<int64_t> Ns(caps.ne, max_rows);
   bytes = std::max(bytes, dsmil_forward_bags_models_train_workspace_bytes(ps, M, Ns.data(), nbs));
   size_t each = 0;
   for (int m = 0; m < M; ++m)
-    each += ws_slice(dsmil_generic_forward_bags_train_dev_workspace_bytes(&ps[m], nbs[m], max_rows));
+    each += ws_slice(train ? dsmil_generic_forward_bags_train_dev_workspace_bytes(&ps[m], nbs[m], max_rows)
+                           : dsmil_generic_forward_bags_dev_workspace_bytes(&ps[m], nbs[m], max_rows));
   return std::max(bytes, each);
 }
 
-int dsmil_generic_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
-                                                const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows,
-                                                float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
-                                                float* save_Q, float* save_H1, int32_t* status, void* workspace,
-                                                size_t workspace_bytes, void* stream) {
+// The generic fold forward pair's body: one planner launch, then gen_forward_run's fold form.  Inference differs
+// from training only in where Q, H1 and the critical rows go (the generic forward has no phase-1 overlap).
+static int generic_forward_bags_models_dev(bool train, const dsmil_params_t* ps, int M, const float* const* Xs_dev,
+                                           const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows,
+                                           float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                                           float* save_Q, float* save_H1, int32_t* status, void* workspace,
+                                           size_t workspace_bytes, cudaStream_t st) {
   ModelsDevCaps caps;
   int rc = check_generic_models_dev(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, &caps);
   if (rc) return rc;
-  DSMIL_REQUIRE(classes && pred && A && B && crit_idx && save_Q && (save_H1 || !ps[0].nonlinear),
+  DSMIL_REQUIRE(classes && pred && A && B && (!train || (crit_idx && save_Q && (save_H1 || !ps[0].nonlinear))),
                 "NULL output pointer");
-  const size_t need = dsmil_generic_forward_bags_models_train_dev_workspace_bytes(ps, M, nbs, max_rows);
+  const size_t need = generic_forward_bags_models_dev_ws(train, ps, M, nbs, max_rows);
   if ((rc = need_workspace(need, workspace, workspace_bytes))) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int ne = caps.ne;
   bool ok;
-  GenModelsWs w = carve_gen_models_dev(ps, M, ne, max_rows, workspace, workspace_bytes, &ok);
+  GenModelsWs w = carve_gen_models_dev(ps, M, ne, max_rows, train, workspace, workspace_bytes, &ok);
   PlanModelsArgs pa = plan_models_args(ps, M, Xs_dev, Ns_dev, nbs, max_rows, status, nullptr);
   pa.zero_row = w.g.zero_row;
   pa.plan = w.plan;
@@ -3006,9 +3051,39 @@ int dsmil_generic_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_
   k_plan_bags_models<<<1, 32 * M, 0, st>>>(pa);
   DSMIL_LAUNCH_OK("k_plan_bags_models");
   const GenFolds f{ps, nbs, M, max_rows, w.models, w.plan, w.live};
+  float* H1 = ps[0].nonlinear ? (train ? save_H1 : w.g.H1) : nullptr;
   return gen_forward_run(&ps[0], w.g, ne, ne * max_rows, ne * tiles_for_bag(max_rows), ne * attend_ctas(max_rows),
-                         max_rows, classes, pred, A, B, crit_idx, save_Q, ps[0].nonlinear ? save_H1 : nullptr, nullptr,
-                         st, &f);
+                         max_rows, classes, pred, A, B, crit_idx ? crit_idx : w.g.crit, train ? save_Q : w.g.Q, H1,
+                         nullptr, st, &f);
+}
+
+size_t dsmil_generic_forward_bags_models_train_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M,
+                                                                   const int32_t* nbs, int64_t max_rows) {
+  return generic_forward_bags_models_dev_ws(true, ps, M, nbs, max_rows);
+}
+
+int dsmil_generic_forward_bags_models_train_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                                const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows,
+                                                float* classes, float* pred, float* A, float* B, int64_t* crit_idx,
+                                                float* save_Q, float* save_H1, int32_t* status, void* workspace,
+                                                size_t workspace_bytes, void* stream) {
+  return generic_forward_bags_models_dev(true, ps, M, Xs_dev, Ns_dev, nbs, max_rows, classes, pred, A, B, crit_idx,
+                                         save_Q, save_H1, status, workspace, workspace_bytes,
+                                         static_cast<cudaStream_t>(stream));
+}
+
+size_t dsmil_generic_forward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                             int64_t max_rows) {
+  return generic_forward_bags_models_dev_ws(false, ps, M, nbs, max_rows);
+}
+
+int dsmil_generic_forward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                          const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, float* classes,
+                                          float* pred, float* A, float* B, int64_t* crit_idx, int32_t* status,
+                                          void* workspace, size_t workspace_bytes, void* stream) {
+  return generic_forward_bags_models_dev(false, ps, M, Xs_dev, Ns_dev, nbs, max_rows, classes, pred, A, B, crit_idx,
+                                         nullptr, nullptr, status, workspace, workspace_bytes,
+                                         static_cast<cudaStream_t>(stream));
 }
 
 size_t dsmil_generic_backward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,

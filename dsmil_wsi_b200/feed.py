@@ -213,11 +213,16 @@ def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[
     shapes (dsmil_models_supported) and capture-safe optimizers, and records its graphs afresh on every call, as
     train_epoch(graph=True) does.  generic=True (with graph=True; the eager step ignores it) also takes folds on the
     generic batched route (train_graph.fold_step_shape: e.g. the classic-MIL D = 166 / 230, a linear q), each fold's
-    results then the bits of train_epoch(..., graph=True, generic=True)."""
+    results then the bits of train_epoch(..., graph=True, generic=True).
+
+    criterion: one criterion for every fold, or one per fold (e.g. each fold's BCEWithLogitsLoss with the pos_weight
+    of its own training split, train_mil.py:172-173); fold m's minibatch_loss then uses criterion[m], and its results
+    are those of its own train_epoch with that criterion."""
     from .ensemble import forward_bags_per_model
     milnets, M = list(milnets), len(folds)
     if not 1 <= M <= Fn.MAX_MODELS:
         raise ValueError(f"a fold step takes 1 to {Fn.MAX_MODELS} folds, got {M}")
+    criteria = fold_criteria(criterion, M)
     for what, seq in (("milnets", milnets), ("optimizers", optimizers), ("orders", orders),
                       ("generators", generators)):
         if seq is not None and len(seq) != M:
@@ -240,7 +245,7 @@ def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[
         net.train()
     if graph:
         return _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_patch, orders, gens,
-                                         bags_per_step, max_rows, generic)
+                                         bags_per_step, max_rows, generic, criteria)
     totals = [torch.zeros((), device=store.device) for _ in range(M)]
     for step in fold_steps([len(o) for o in orders], bags_per_step):
         groups = [(m, orders[m][lo:hi]) for m, lo, hi in step]
@@ -252,7 +257,7 @@ def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[
         for (m, group), out in zip(groups, outs):
             labels = torch.cat([store.bags[i][1].view(1, -1) for i in group])
             bag_prediction, max_prediction = _group_predictions(out)
-            lm = minibatch_loss(criterion, bag_prediction, max_prediction, labels)
+            lm = minibatch_loss(criteria[m], bag_prediction, max_prediction, labels)
             totals[m] += lm.detach() * len(group)
             loss = lm if loss is None else loss + lm
         loss.backward()
@@ -260,6 +265,16 @@ def train_epoch_models(milnets, store: DeviceBagStore, folds: Sequence[Sequence[
             optimizers[m].step()
     host = torch.stack(totals).double().tolist()    # the epoch's one host sync
     return [t / len(o) for t, o in zip(host, orders)]
+
+
+def fold_criteria(criterion, M: int) -> list:
+    """The M folds' criteria: `criterion` itself for every fold, or, given a list or tuple, one per fold (ValueError
+    for another count)."""
+    if isinstance(criterion, (list, tuple)):
+        if len(criterion) != M:
+            raise ValueError(f"{len(criterion)} criteria for {M} folds: give one criterion, or one per fold")
+        return list(criterion)
+    return [criterion] * M
 
 
 def minibatch_loss(criterion, bag_prediction, max_prediction, labels):
@@ -312,7 +327,7 @@ def _train_epoch_graph(milnet, store, criterion, optimizer, dropout_patch, order
 
 
 def _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_patch, orders, gens, k, max_rows,
-                              generic=False):
+                              generic, criteria):
     from .train_graph import FoldTrainStepGraph, fold_step_shape
     fold_step_shape(milnets, generic)                          # shapes off the fold routes raise here
     p = 1 - dropout_patch
@@ -327,7 +342,9 @@ def _train_epoch_models_graph(milnets, store, criterion, optimizers, dropout_pat
         key = tuple((m, hi - lo) for m, lo, hi in step)
         g = graphs.get(key)
         if g is None:                                          # the full step, short last groups, fewer folds
-            g = graphs[key] = FoldTrainStepGraph([milnets[m] for m, _ in key], criterion,
+            # one criterion for all folds stays one object; per-fold criteria go with their folds
+            crit = [criteria[m] for m, _ in key] if isinstance(criterion, (list, tuple)) else criterion
+            g = graphs[key] = FoldTrainStepGraph([milnets[m] for m, _ in key], crit,
                                                  [optimizers[m] for m, _ in key], [n for _, n in key], cap,
                                                  generic=generic)
         e = 0
@@ -427,12 +444,19 @@ def eval_epoch(milnet, store: DeviceBagStore, criterion, average: bool = False, 
     return loss, torch.stack(labels).cpu().numpy().astype(int), torch.stack(preds).cpu().numpy()
 
 
-def eval_epoch_models(milnets, store: DeviceBagStore, criterion, average: bool = False, bags_per_launch: int = 16):
+def eval_epoch_models(milnets, store: DeviceBagStore, criterion, average: bool = False, bags_per_launch: int = 16,
+                      graph: bool = False, max_rows: Optional[int] = None):
     """eval_epoch for an ensemble (the fold models of train_tcga.py:395-404) over the same bags: one (loss, labels,
     preds) per model, each bit for bit `eval_epoch(milnets[m], store, criterion, average, bags_per_launch)` without
     patch dropout.  Each group of bags_per_launch > 1 bags is one ensemble.forward_bags_models call, and the whole
     call makes one host sync.  The thresholds and the vote over the models (train_tcga.py:113-124, 401-404) are the
-    caller's, on these arrays."""
+    caller's, on these arrays.
+
+    graph=True: each group of bags_per_launch bags (and a short last group) replays an infer_graph.EvalBagsModelsGraph
+    in which every model is given the group's bags, cached as eval_epoch_folds caches its graphs; max_rows as
+    eval_epoch's.  The results are the eager call's bits.  The members and shapes are those of
+    train_graph.fold_step_shape.  Each model reads the group's bags in a pass of its own, so the members' passes over
+    a bag do not follow each other in L2 as the eager fused ensemble's do."""
     from .ensemble import forward_bags_models
     milnets = list(milnets)
     for m in milnets:
@@ -440,6 +464,10 @@ def eval_epoch_models(milnets, store: DeviceBagStore, criterion, average: bool =
     n, k = len(store), max(1, bags_per_launch)
     if n == 0:
         raise ValueError("eval_epoch_models over an empty store")
+    if graph:
+        M = len(milnets)
+        return _eval_folds_graph(milnets, store, [list(range(n))] * M, [criterion] * M, average, k, max_rows, False,
+                                 "eval_epoch_models")
     losses = [[] for _ in milnets]
     preds = [[] for _ in milnets]
     with torch.no_grad():
@@ -463,6 +491,137 @@ def eval_epoch_models(milnets, store: DeviceBagStore, criterion, average: bool =
     lab = host[M:M + n * C].reshape(n, C).astype(int)
     pr = host[M + n * C:].reshape(M, n, C).astype(np.float32)
     return [(float(host[m]), lab.copy(), pr[m]) for m in range(M)]
+
+
+def eval_epoch_folds(milnets, store: DeviceBagStore, folds: Sequence[Sequence[int]], criterion, average: bool = False,
+                     bags_per_launch: int = 16, graph: bool = False, max_rows: Optional[int] = None,
+                     generic: bool = False):
+    """The validation half of a fold epoch (train_tcga.py:272-287, train_mil.py:177-184): every fold model over its
+    own held-out bags, the folds taking their steps together.  folds[m] lists fold m's held-out store indices in the
+    order they are evaluated; criterion is one criterion, or one per fold (fold_criteria).  Returns one (loss,
+    labels, preds) per fold, fold m's bit for bit `eval_epoch(milnets[m], <a store of folds[m]'s bags in that order>,
+    criteria[m], average, bags_per_launch, graph=graph)`.  No patch dropout, as eval_epoch_models.
+
+    The steps follow fold_steps: each step, every fold that still has bags takes its next group of k =
+    bags_per_launch.  Eager, each fold model runs its group as eval_epoch does: one forward_bags call (k = 1: one
+    milnet(x)).  It does not use ensemble.forward_bags_per_model: that is the training form, whose bag predictions can
+    differ from the inference forward's in the last bits.  graph=True: a step replays an infer_graph.EvalBagsModelsGraph, one per (folds
+    in the step, their group sizes), with the capacity max_rows (default: the largest bag of the store; a bag over it
+    raises ValueError before any launch).  The graphs stay cached with the first model of their step (held weakly), and
+    later calls replay them: a call over 50 epochs records on its first only.  A graph is recorded again when one of
+    its models' parameter tensors, or its criteria, changed.  Needs the members and shapes of
+    train_graph.fold_step_shape (generic=True: also the generic fold shapes).
+
+    One host sync per call; a fold with a bag the library refused raises RuntimeError naming the fold."""
+    milnets, M = list(milnets), len(folds)
+    if not 1 <= M <= Fn.MAX_MODELS:
+        raise ValueError(f"eval_epoch_folds takes 1 to {Fn.MAX_MODELS} folds, got {M}")
+    if len(milnets) != M:
+        raise ValueError(f"{len(milnets)} milnets for {M} folds")
+    criteria = fold_criteria(criterion, M)
+    folds = [list(f) for f in folds]
+    for m, fold in enumerate(folds):
+        if len(fold) == 0:
+            raise ValueError(f"fold {m} has no held-out bags")
+        bad = [i for i in fold if not 0 <= i < len(store)]
+        if bad:
+            raise IndexError(f"fold {m}: store index {bad[0]} outside [0, {len(store)})")
+    for net in milnets:
+        net.eval()
+    k = max(1, bags_per_launch)
+    if graph:
+        return _eval_folds_graph(milnets, store, folds, criteria, average, k, max_rows, generic, "eval_epoch_folds")
+    losses = [[] for _ in range(M)]
+    preds = [[] for _ in range(M)]
+    with torch.no_grad():
+        for step in fold_steps([len(f) for f in folds], k):
+            groups = [(m, folds[m][lo:hi]) for m, lo, hi in step]
+            for m, group in groups:
+                net, xs = milnets[m], [store.bags[i][0] for i in group]
+                out = net.forward_bags(xs) if k > 1 and hasattr(net, "forward_bags") else [net(x) for x in xs]
+                for (ins_prediction, bag_prediction, _, _), i in zip(out, group):
+                    loss, pred = _eval_bag(criteria[m], ins_prediction, bag_prediction, store.bags[i][1], average)
+                    losses[m].append(loss)
+                    preds[m].append(pred)
+        loss = torch.stack([torch.stack([l.reshape(()) for l in ls]).mean() for ls in losses])
+        return _fold_results(store, folds, loss, [torch.stack(ps) for ps in preds], None)
+
+
+def _fold_results(store, folds, loss, preds, status):
+    """Each fold's (loss, labels, preds) from the device: loss [M], preds[m] [n_m, C] and (graphs) each fold's planner
+    status [M], in one host sync (float32 and the integer labels are exact in float64).  RuntimeError naming the first
+    fold with a refused bag."""
+    M = len(folds)
+    labels = torch.stack([store.bags[i][1].view(-1) for f in folds for i in f])
+    parts = [loss.double().view(-1)] + ([status.double().view(-1)] if status is not None else [])
+    host = torch.cat(parts + [labels.double().view(-1)] + [p.double().view(-1) for p in preds]).cpu().numpy()
+    at = M
+    if status is not None:
+        for m, st in enumerate(host[M:2 * M]):
+            if st:
+                raise RuntimeError(f"inference graph: fold {m} held a bag the library refused (planner status "
+                                   f"{int(st)})")
+        at = 2 * M
+    C = int(labels.shape[1])
+    out = []
+    lab = host[at:at + labels.numel()].reshape(-1, C).astype(int)
+    at += labels.numel()
+    row = 0
+    for m, f in enumerate(folds):
+        n = len(f)
+        out.append((float(host[m]), lab[row:row + n].copy(), host[at:at + n * C].reshape(n, C).astype(np.float32)))
+        row, at = row + n, at + n * C
+    return out
+
+
+# first model of a step -> {(the step's models, their group sizes, max_rows, average, generic): EvalBagsModelsGraph},
+# as _EVAL_GRAPHS keeps EvalBagsGraph: weakly, off the models themselves
+_FOLD_EVAL_GRAPHS = weakref.WeakKeyDictionary()
+
+
+def _fold_eval_graph(nets, crits, nbs, cap, average, generic):
+    """The cached EvalBagsModelsGraph of these models, criteria and group sizes, recorded if there is none or if a
+    model's parameter tensors or a criterion changed since."""
+    from .infer_graph import EvalBagsModelsGraph
+    cached = _FOLD_EVAL_GRAPHS.setdefault(nets[0], {})
+    key = (tuple(id(net) for net in nets), tuple(nbs), cap, bool(average), bool(generic))
+    g = cached.get(key)
+    if (g is None or not g.current() or any(a is not b for a, b in zip(g.members(), nets))
+            or any(a is not b for a, b in zip(g.criteria, crits))):
+        g = cached[key] = EvalBagsModelsGraph(nets, list(crits), nbs, cap, average, generic=generic)
+    return g
+
+
+def _eval_folds_graph(milnets, store, folds, criteria, average, k, max_rows, generic, what):
+    from .train_graph import fold_step_shape
+    fold_step_shape(milnets, generic)                          # shapes off the fold routes raise here
+    cap = None
+    for m, f in enumerate(folds):
+        _, cap = _graph_rows(store, 1.0, max_rows, f, "inference", f"fold {m}, ")
+    M = len(folds)
+    losses = [torch.empty(len(f), device=store.device) for f in folds]
+    preds = [torch.empty(len(f), int(store.bags[0][1].numel()), device=store.device) for f in folds]
+    status = torch.zeros(M, dtype=torch.int32, device=store.device)
+    used = []
+    for step in fold_steps([len(f) for f in folds], k):
+        nets = [milnets[m] for m, _, _ in step]
+        g = _fold_eval_graph(nets, [criteria[m] for m, _, _ in step], [hi - lo for _, lo, hi in step], cap, average,
+                             generic)
+        groups = [folds[m][lo:hi] for m, lo, hi in step]
+        torch.cat([store.bags[i][1].view(1, -1) for group in groups for i in group], out=g.labels)
+        g.run([[store.bags[i][0] for i in group] for group in groups])
+        e = 0
+        for j, (m, lo, hi) in enumerate(step):
+            losses[m][lo:hi] = g.loss[e:e + hi - lo]
+            preds[m][lo:hi] = g.pred[e:e + hi - lo]
+            status[m] = torch.where(status[m] != 0, status[m], g.status[j])
+            e += hi - lo
+        used.append(g)
+    out = _fold_results(store, folds, torch.stack([l.mean() for l in losses]), preds, status)
+    for g in used:
+        g.status.zero_()
+        g.release()
+    return out
 
 
 # model -> {(bags per graph, max_rows, average): EvalBagsGraph}: later epochs replay the graphs of earlier ones (the

@@ -548,21 +548,31 @@ class MILBagsModelsFn(torch.autograd.Function):
         return (None, *_split_rows(gX, Ns, need_bags), *outs)
 
 
-def _models_dev_forward(ctx, pre, nbs, slots, Ns, status, params):
-    """The body of MILBagsModelsDevFn.forward over the fold dev calls named pre + "forward_bags_models_train_dev"."""
+def _fold_packs(pre, nbs, params, what="the graph-captured fold step"):
+    """The M members' ParamPacks and their DsmilParams array for the fold dev calls of prefix pre ("dsmil_": the fused
+    tensor-core fold shapes, "dsmil_generic_": the generic ones); ValueError off them."""
     lib = _lib.load()
-    ctx.set_materialize_grads(False)
-    M, ne = len(nbs), sum(nbs)
+    M = len(nbs)
     packs = _model_packs([params[10 * m:10 * (m + 1)] for m in range(M)])
     P0 = packs[0]
     ps = (_lib.DsmilParams * M)(*[P.struct for P in packs])
     if pre == "dsmil_":
         if min(nbs) < 1 or not lib.dsmil_models_supported(ps, M):
-            raise ValueError(f"the graph-captured fold step runs on the fused fold shapes only; M={M}, D={P0.D}, "
+            raise ValueError(f"{what} runs on the fused fold shapes only; M={M}, D={P0.D}, "
                              f"C={P0.C}, nonlinear={P0.nonlinear}, group sizes {tuple(nbs)} are not on them")
     elif min(nbs) < 1 or not lib.dsmil_generic_models_supported(ps, M):
-        raise ValueError(f"the generic graph-captured fold step runs on the generic batched shapes only; M={M}, "
+        raise ValueError(f"the generic {what.removeprefix('the ')} runs on the generic batched shapes only; M={M}, "
                          f"D={P0.D}, C={P0.C}, nonlinear={P0.nonlinear}, group sizes {tuple(nbs)} are not on them")
+    return packs, ps
+
+
+def _models_dev_forward(ctx, pre, nbs, slots, Ns, status, params):
+    """The body of MILBagsModelsDevFn.forward over the fold dev calls named pre + "forward_bags_models_train_dev"."""
+    lib = _lib.load()
+    ctx.set_materialize_grads(False)
+    M, ne = len(nbs), sum(nbs)
+    packs, ps = _fold_packs(pre, nbs, params)
+    P0 = packs[0]
     if slots.dim() != 3 or slots.shape[0] != ne or slots.shape[2] != P0.D or slots.dtype != torch.float32 \
             or not slots.is_contiguous():
         raise ValueError(f"slots must be contiguous float32 [{ne}, max_rows, {P0.D}], got {tuple(slots.shape)}")
@@ -643,6 +653,39 @@ class MILBagsModelsGenericDevFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_classes, g_pred, g_A, g_B, _g_crit):
         return _models_dev_backward(ctx, g_classes, g_pred, g_A, g_B)
+
+
+@torch.no_grad()
+def mil_forward_bags_models_dev(nbs: Sequence[int], xs: torch.Tensor, Ns: torch.Tensor, status: torch.Tensor,
+                                max_rows: int, params_list: Sequence[Sequence[Optional[torch.Tensor]]],
+                                generic: bool = False):
+    """Inference of M members, each over its OWN bag list held on the device (dsmil_forward_bags_models_dev): the fold
+    models' validation, with no host work that depends on the bags, so one call can be recorded into a CUDA graph and
+    replayed over every batch of the same group sizes.
+
+    nbs: each member's bag count (host); xs [sum nbs] int64 (the bags' feature addresses, member-major), Ns [sum nbs]
+    int64 and status [M] int32 on the device.  Returns the packed (classes, pred, A, B, crit): classes and A have
+    sum(nbs) * max_rows rows, member m's block starting at row max_rows * sum(nbs[:m]) with its live rows packed at the
+    prefix sums of its own Ns; pred, B and crit are [sum nbs, ...].  Member m's slices are bit for bit those of
+    mil_forward_bags_dev on its bags alone.  A member with a refused bag sets status[m] (see the header) and only its
+    slices are a stand-in.  generic=True: the generic fold shapes (dsmil_generic_forward_bags_models_dev)."""
+    nbs = tuple(int(n) for n in nbs)
+    pre = "dsmil_generic_" if generic else "dsmil_"
+    packs, ps = _fold_packs(pre, nbs, [t for p in params_list for t in p], "the fold models' inference")
+    M, ne, P0 = len(nbs), sum(nbs), packs[0]
+    if xs.numel() != ne or Ns.numel() != ne or status.numel() != M:
+        raise ValueError(f"xs and Ns need {ne} entries and status {M}; got {xs.numel()}, {Ns.numel()} and "
+                         f"{status.numel()}")
+    lib = _lib.load()
+    c_nb = (C.c_int32 * M)(*nbs)
+    call = pre + "forward_bags_models_dev"
+    with torch.cuda.device(P0.device):
+        classes, pred, A, B, crit = _bag_outputs(P0, ne * max_rows, ne)
+        ws = _workspace(getattr(lib, call + "_workspace_bytes")(ps, M, c_nb, max_rows), P0.device)
+        rc = getattr(lib, call)(ps, M, _ptr(xs), _ptr(Ns), c_nb, max_rows, _ptr(classes), _ptr(pred), _ptr(A),
+                                _ptr(B), _ptr(crit), _ptr(status), _ptr(ws), ws.numel(), _stream())
+        _lib.check(rc, call)
+    return classes, pred, A, B, crit
 
 
 def mil_forward_bags_per_model(bag_lists: Sequence[Sequence[torch.Tensor]],

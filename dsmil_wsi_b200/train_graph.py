@@ -319,7 +319,10 @@ class FoldTrainStepGraph:
 
     Refusal is per fold: a fold with a bag outside 1..max_rows has `status[m]` set (the first refusal's 1 + bag index
     within the fold; never cleared here), a NaN loss, and its parameters and optimizer state left as they were; the
-    other folds step normally.  Warm-up, capture and hyperparameters behave as in TrainStepGraph."""
+    other folds step normally.  Warm-up, capture and hyperparameters behave as in TrainStepGraph.
+
+    criterion: one for every fold, or a list or tuple of one per fold (feed.fold_criteria), fold m's minibatch_loss
+    then using criterion[m]."""
 
     def __init__(self, milnets, criterion, optimizers, nbs, max_rows: int, warmup: int = 1, generic: bool = False):
         milnets, optimizers, nbs = list(milnets), list(optimizers), [int(n) for n in nbs]
@@ -334,6 +337,7 @@ class FoldTrainStepGraph:
         if min(nbs) < 1 or ne > 65535 or max_rows < 1:
             raise ValueError(f"FoldTrainStepGraph: group sizes {nbs} outside [1, 65535] or max_rows={max_rows} < 1")
         self.milnets, self.criterion, self.optimizers = milnets, criterion, optimizers
+        self.criteria = feed.fold_criteria(criterion, M)
         self.nbs, self.max_rows = tuple(nbs), max_rows
         self.params = [[p for g in opt.param_groups for p in g["params"]] for opt in optimizers]
         dev = milnets[0].b_classifier.fcc.weight.device
@@ -362,7 +366,7 @@ class FoldTrainStepGraph:
             nm = n[e:e + nb]
             first = torch.cumsum(nm, 0) - nm + e * self.max_rows          # each bag's first packed row
             mx = classes.gather(0, crit[e:e + nb] + first[:, None])
-            lm = feed.minibatch_loss(self.criterion, pred[e:e + nb], mx, self.labels[e:e + nb])
+            lm = feed.minibatch_loss(self.criteria[m], pred[e:e + nb], mx, self.labels[e:e + nb])
             ok = self._step_status[m] == 0
             # a refused fold: NaN loss and no gradient (where's backward sends none to the unselected side)
             losses.append(torch.where(ok, lm, torch.full_like(lm, float("nan"))))

@@ -368,6 +368,35 @@ int dsmil_generic_forward_bags_dev(const dsmil_params_t* p, const float* const* 
                                    int32_t nb, int64_t max_rows, float* classes, float* pred, float* A, float* B,
                                    int64_t* crit_idx, int32_t* status, void* workspace, size_t workspace_bytes,
                                    void* stream);
+/* Capture-safe inference over the fold models of a cross-validation, each over its OWN bags: the validation half of
+ * a fold epoch (each fold model over its held-out bags) recorded once as a CUDA graph.  dsmil_forward_bags_models_dev
+ * is dsmil_forward_bags_models_train_dev without saves, under every rule of that call: model-major device lists, nbs
+ * a HOST array fixed per call, model m's rows in the capacity block from max_rows * sum_{j<m} nbs[j] packed at its own
+ * live prefix sums, per-model refusal through status[M] with the refused model alone on the stand-in batch, the
+ * shapes of dsmil_models_supported and the same bounds, no host<->device copy, allocation or synchronisation, the W1/W2
+ * images rebuilt on every call.  Q stays in the workspace as tile blocks and there is no H1.  crit_idx [sum nbs, C] may
+ * be NULL.  As in dsmil_forward_bags_dev, the attend pass is a programmatic dependent of phase 1, each entry gated on
+ * its own tiles, also under stream capture (a programmatic edge in the graph); only dsmil_profile_enable(1) keeps the
+ * plain launch.  Model m's slices are, bit for bit, what dsmil_forward_bags(&ps[m], ...) and the one-model
+ * dsmil_forward_bags_dev give on model m's bags.  Its classes and crit_idx are also model m's slices of
+ * dsmil_forward_bags_models_train_dev; that training form's pred, A and B can differ from them in the last bits.
+ * dsmil_generic_forward_bags_models_dev: the same on dsmil_generic_models_supported (the rules, alignment, launches and
+ * bounds of dsmil_generic_forward_bags_models_train_dev, without saves); model m's slices are
+ * dsmil_generic_forward_bags_dev's on its bags.  Each call refuses the other's shapes (DSMIL_ERR_ARG).
+ * The workspace sizes depend on (M, nbs, max_rows) only and are never below the eager fold call's size for nbs bags of
+ * max_rows rows, nor below the sum of the one-model dev calls' sizes; 0 for invalid arguments. */
+size_t dsmil_forward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                     int64_t max_rows);
+int dsmil_forward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                  const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, float* classes,
+                                  float* pred, float* A, float* B, int64_t* crit_idx, int32_t* status, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+size_t dsmil_generic_forward_bags_models_dev_workspace_bytes(const dsmil_params_t* ps, int32_t M, const int32_t* nbs,
+                                                             int64_t max_rows);
+int dsmil_generic_forward_bags_models_dev(const dsmil_params_t* ps, int32_t M, const float* const* Xs_dev,
+                                          const int64_t* Ns_dev, const int32_t* nbs, int64_t max_rows, float* classes,
+                                          float* pred, float* A, float* B, int64_t* crit_idx, int32_t* status,
+                                          void* workspace, size_t workspace_bytes, void* stream);
 
 /* The batched forward of a model with a value network (passing_v: v = Dropout-Linear(D,D)-ReLU, dsmil.py:35-39), which
  * dsmil_forward_bags also takes with the features as value inputs.  dsmil_value_bags_supported: passing_v with Wv/bv, 1 <= D <= 4096,
